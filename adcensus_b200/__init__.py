@@ -1,6 +1,6 @@
-"""adcensus_b200 -- B200-native AD-Census stereo matching behind the reference's ADCensusStereo API.
+"""adcensus_b200 -- H100-native AD-Census stereo matching behind the reference's ADCensusStereo API.
 
-The compute path is the hand-written sm_100a CUDA library ``adcensus_b200/lib/libadcensus_b200.so``
+The compute path is the hand-written sm_90a CUDA library ``adcensus_b200/lib/libadcensus_b200.so``
 (sources in ``adcensus_b200/csrc``), reached through its C ABI (``include/adcensus_b200.h``).
 This package is the Python mirror of the reference's interface for that path
 (``ADCensusOption`` and ``ADCensusStereo.Initialize / Match / Reset``, reference

@@ -1,4 +1,4 @@
-"""Builds the CUDA library in-tree with nvcc for sm_100a (no JIT cache, so the .so travels with the repo)."""
+"""Builds the CUDA library in-tree with nvcc for sm_90a (no JIT cache, so the .so travels with the repo)."""
 from __future__ import annotations
 
 import os
@@ -20,7 +20,7 @@ def _stale() -> bool:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> Path:
-    """nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo ... (see csrc/Makefile)."""
+    """nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo ... (see csrc/Makefile)."""
     if force or _stale():
         nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
         if not Path(nvcc).exists():

@@ -1,4 +1,4 @@
-// adc_common.cuh -- shared declarations for the sm_100a AD-Census kernels.
+// adc_common.cuh -- shared declarations for the sm_90a AD-Census kernels.
 //
 // Data layout in HBM (per wave of S stereo pairs; every array is [S][...], pair index outermost):
 //   bgr      u8  [S][2][H][W][3]   left, right packed BGR exactly as the caller passes them
@@ -72,6 +72,14 @@ inline void adc_once_done(AdcOnce& o) {
     int dev = 0;
     cudaGetDevice(&dev);
     o.done[dev & 63].store(1, std::memory_order_release);
+}
+
+// SMs of the current device (grid sizes of the grid-stride and look-ahead launches scale with it)
+inline int adc_sm_count() {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n > 0 ? n : 1;
 }
 
 // TMA descriptors (CUtensorMap, 128 bytes each) of a lane's two cost volumes for the two axes of the fused aggregation kernel

@@ -1,4 +1,4 @@
-// engine.cu -- host side of the B200 AD-Census engine and its C ABI (include/adcensus_b200.h).
+// engine.cu -- host side of the H100 AD-Census engine and its C ABI (include/adcensus_b200.h).
 //
 // An engine owns `lanes` independent pipelines.  A lane = one CUDA stream + a device arena for a
 // wave of up to `wave_pairs` stereo pairs (two cost volumes per pair dominate: 2*4*N*Dp bytes) +
@@ -452,7 +452,7 @@ int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, cons
 extern "C" {
 
 const char* adc_last_error(void) { return g_err.c_str(); }
-const char* adc_version(void) { return "adcensus_b200 0.1 (sm_100a)"; }
+const char* adc_version(void) { return "adcensus_b200 0.1 (sm_90a)"; }
 
 void adc_default_option(adc_option* o) {
     if (!o) return;
@@ -521,8 +521,8 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
     auto bail = [&](int rc) { adc_destroy(e); return rc; };
     if (cudaSetDevice(e->cfg.device) != cudaSuccess) return bail(fail(ADC_ERR_CUDA, "cudaSetDevice failed"));
 
-    // wave size: enough scanlines in flight for the line-per-lane-group scanline kernels (measured on Cone: 32 pairs
-    // per wave x 4 lanes beats 16 x 6; the scanline passes only have W or H lines per pair to spread over 148 SMs)
+    // wave size: enough scanlines in flight for the line-per-lane-group scanline kernels (32 pairs per wave
+    // x 4 lanes for Cone: the scanline passes only have W or H lines per pair to spread over the SMs)
     int S = e->cfg.wave_pairs;
     if (S <= 0) S = std::min(32, std::max(2, (12288 + std::min(width, height) - 1) / std::min(width, height)));
     int nl = e->cfg.lanes > 0 ? e->cfg.lanes : 4;

@@ -14,8 +14,8 @@
 #define CT_HX 3
 #define CT_HY 4
 
-// (A table of the 3 x 256 possible products, which leaves two double adds per pixel, was measured: the per-CTA copy of the
-//  table into shared memory costs more than the three multiplies it saves -- 220 us against 201 us per wave of 32 pairs.)
+// (A table of the 3 x 256 possible products, which leaves two double adds per pixel, was tried: the per-CTA copy of the
+//  table into shared memory costs more than the three multiplies it saves.)
 __device__ __forceinline__ uint8_t gray_of(const uint8_t* __restrict__ px) {
     const double b = (double)__ldg(px), g = (double)__ldg(px + 1), r = (double)__ldg(px + 2);
     const double v = __dadd_rn(__dadd_rn(__dmul_rn(r, 0.299), __dmul_rn(g, 0.587)), __dmul_rn(b, 0.114));
@@ -88,10 +88,10 @@ void adc_launch_gray_census(const AdcParams& P, const AdcWave& w, cudaStream_t s
 // one needs 4.9.  A CTA computes four consecutive rows of its segment; the tables are staged once per CTA, replicated (x32 for the 64-entry census table: conflict-free;
 // x16 for the 766-entry AD table: two lanes per replica) so that the data-dependent look-ups of a warp spread over the
 // banks.
-// (Measured and rejected in round 2: lanes = 32 consecutive disparities of one pixel -- half the index arithmetic, but
-//  32-bit stores and table addresses that differ in every lane: 631 us against 486 us per wave of 32 Cone pairs; one pixel x
-//  four disparities per thread with a single 128-bit load per array out of four shifted copies of the row: half the
-//  instructions of version 3 and exactly its time, 482 us -- same shared-memory wavefronts.)
+// (Tried and rejected: lanes = 32 consecutive disparities of one pixel -- half the index arithmetic, but 32-bit stores
+//  and table addresses that differ in every lane, slower; one pixel x four disparities per thread with a single 128-bit
+//  load per array out of four shifted copies of the row: half the instructions of version 3 and no faster -- same
+//  shared-memory wavefronts.)
 // ---------------------------------------------------------------------------------------------
 #define CV_AD_REP 16
 #define CV_SEG_COLS 928       // columns per CTA at most: longer rows are cut into segments (multiple of 4)

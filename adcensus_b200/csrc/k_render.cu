@@ -74,7 +74,7 @@ int adc_launch_render(const AdcDims& dm, const float* d_disp, unsigned* d_mm, ui
         adc_once_done(g_jet_uploaded);
     }
     k_render_init<<<1, 1, 0, st>>>(d_mm, dm.W);
-    k_render_minmax<<<148, 256, 0, st>>>(dm.N, d_disp, d_mm);
+    k_render_minmax<<<adc_sm_count(), 256, 0, st>>>(dm.N, d_disp, d_mm);
     k_render_gray_jet<<<(dm.N + 255) / 256, 256, 0, st>>>(dm.N, d_disp, d_mm, d_gray, d_jet, d_mm_out);
     *launches += 3;
     return 0;

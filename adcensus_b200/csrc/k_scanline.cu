@@ -386,10 +386,7 @@ static int launch_scanline_kf(const AdcParams& P, const AdcWave& w, const float*
     return 0;
 }
 
-// Which way a pass fills its ring.  Measured on B200 per pass of a wave (x / y direction), cp.async vs bulk:
-//   8 lanes per line  (Cone, D = 64):        582 / 521 us  vs  592 / 537 us
-//   16 lanes per line (1242x375, D = 128):   2.67 / 2.44 ms vs 2.68 / 2.46 ms
-//   32 lanes per line (1920x1080, D = 192):  6.61 / 6.86 ms vs 6.44 / 6.32 ms
+// Which way a pass fills its ring: cp.async for 8 and 16 lanes per line, bulk copies for a whole warp per line.
 // A bulk copy costs ~20 issue slots (uniform-register set-up, lane election) and every refill needs a proxy fence; it pays
 // when one copy moves a whole warp's step (a single line of D > 128 disparities), not when a warp steps four short lines.
 template <int K, int LPS>

@@ -572,7 +572,7 @@ bool adc_launch_vote_push(const AdcParams& P, const AdcWave& w, cudaStream_t st,
     dim3 sgrid(64, w.S);
     k_vote_slots<<<sgrid, 256, 0, st>>>(dm, w.vlist, w.counters, w.vote_state, w.vote_pslotT, w.sup_h);
     unsigned* hist = w.vote_hist;
-    int gx = (148 * 8 + w.S - 1) / w.S;
+    int gx = (adc_sm_count() * 8 + w.S - 1) / w.S;
     if (gx < 1) gx = 1;
     dim3 igrid(gx, w.S);
     k_vote_scan<<<igrid, VI_WARPS * 32, 0, st>>>(P, w.arms, w.vote_alr, w.vote_state, w.sup_h, w.vlist, w.counters, hist,

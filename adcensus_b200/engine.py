@@ -73,7 +73,7 @@ def load_library() -> ctypes.CDLL:
     p = lib_path()
     if not p.exists():
         raise AdcError(f"{p} is missing: build it with adcensus_b200.build_library() "
-                       "(nvcc, sm_100a).  This package has no CPU fallback.")
+                       "(nvcc, sm_90a).  This package has no CPU fallback.")
     L = ctypes.CDLL(str(p))
     vp, i32, u8p, f32p = ctypes.c_void_p, ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p
     L.adc_default_option.argtypes = [ctypes.POINTER(ADCensusOption)]

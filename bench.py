@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the contract benchmark of the B200 AD-Census engine.
+"""bench.py -- the benchmark of the H100 AD-Census engine.
 
 Metric (BASELINE.json): disparity-maps/sec on Cone 450x375x64, batch 256 per GPU (configs[1]).
 A "step" = one pass of the whole hot path (ADCensusStereo::Match for every pair) over one batch of
@@ -10,13 +10,18 @@ replicated 256x (SURVEY.md 8d, config 2); every output therefore has to equal th
   e2e   : the same through the host-buffer C-ABI call (pinned host memory, H2D + D2H inside the
           timed region, adc_match_batch_pinned_async + synchronise)
   roofline     : the dominant kernel timed in isolation (CUDA events on the engine's stream)
-  cpu_baseline : the reference's own CPU implementation (oracle/_ref) on this box's host cores
+  cpu_baseline : the reference's own CPU implementation (oracle/_ref) on the host's cores
 
 `--impl reference` times the reference CPU path (oracle/_ref when it was built, else the oracle
 port) with one independent instance per host core, on the same workload/metric.
 
 Multi-GPU: independent pairs shard over the ranks (weak scaling, 256 pairs per rank per step);
 NCCL carries only the job descriptor broadcast, the timing max and a result checksum.
+
+`--dump-outputs DIR` writes, after the timed steps, what the timed call returned in its last step: the left disparity
+maps of a fixed, seeded sample of the batch's pairs (DIR/disp_left.npy, float32 [pairs, H, W], at most 64 MB) and the
+batch indices of those pairs (DIR/disp_left_pairs.npy, float64).  The inputs are fixed (Cone, or seeded synthetic
+pairs), so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -38,6 +43,8 @@ sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
 WORKLOAD = "cone_450x375_d64_batch256"
+DUMP_BYTES = 64 * 10**6
+HBM_PEAK_GBS = 3350.0      # H100 SXM data sheet (HBM3); not a measured figure
 PAIRS_PER_STEP = 256
 METRIC = "disparity-maps/sec (450x375x64)"
 
@@ -162,11 +169,11 @@ class ClockSampler(threading.Thread):
 
 
 def _config_dict(wl_name, n, w, h, D, eng=None, world=1, pipelined=True, sharded=False):
-    """The `config` object of the JSON line -- built the same way by both arms so that the driver can compare them."""
+    """The `config` object of the JSON line -- built the same way by both arms so that their lines can be compared."""
     c = {"workload": wl_name, "pairs_per_step_per_gpu": n, "width": w, "height": h, "disparities": D}
     if eng is not None:
         c.update({"wave_pairs": eng.wave_pairs, "lanes": eng.lanes, "steps_pipelined": pipelined,
-                  "l2_policy": "no flush needed: each step streams the whole batch of images and several GB of cost volumes per wave, far beyond the 126 MB L2",
+                  "l2_policy": "no flush needed: each step streams the whole batch of images and several GB of cost volumes per wave, far beyond the 50 MB L2",
                   "parallelism": (f"dp{world}, one batch owned by rank 0: NCCL scatter of the inputs, per-rank Match, NCCL gather of the maps"
                                   if sharded else f"dp{world} (independent pairs, no data-path collective)")})
     return c
@@ -213,6 +220,17 @@ def reference_single_instance(left, right, dmax):
     eng.close()
     return {"kind": kind, "cores": 1, "s_per_map_median_of_5": round(statistics.median(tot), 4),
             "stage_s": {k: round(v, 4) for k, v in split.items()}}
+
+
+def dump_outputs(out_dir, d_disp):
+    """The maps of a fixed, seeded sample of the batch (all of it when it fits in DUMP_BYTES) as float32 .npy files."""
+    n = d_disp.shape[0]
+    k = max(1, min(n, DUMP_BYTES // (d_disp[0].numel() * 4)))
+    idx = np.arange(n) if k == n else np.sort(np.random.default_rng(0).choice(n, k, replace=False))
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    np.save(out / "disp_left.npy", d_disp[idx].cpu().numpy().astype(np.float32))
+    np.save(out / "disp_left_pairs.npy", idx.astype(np.float64))
 
 
 def run_gpu_arm(args):
@@ -310,6 +328,8 @@ def run_gpu_arm(args):
         sampler.start()
     ms_dev, launches = timed(dev_step, args.steps)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_disp)
     for _ in range(2):
         e2e_step()
     eng.join(st.cuda_stream)
@@ -356,12 +376,8 @@ def run_gpu_arm(args):
                   "note": "adc_match: pageable host pointers in, host map out, synchronous; stage times from CUDA events"}
         eng.set_pipelined(not args.no_pipeline)
 
-        peaks = {}
-        pk = ROOT / "MEASURED_PEAKS.json"
-        if pk.exists():
-            peaks = json.loads(pk.read_text())
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        hbm_peak = HBM_PEAK_GBS
+        peak_src = "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
         V, Nf = 4.0 * N * (dmax - dmin), float(N)
         kern = {}
         names = ["cost_volume", "arm_sum_h", "arm_sum2_v", "arm_sum2_h", "arm_sum_h_div", "arm_sum_v_div", "scanline_x", "scanline_y", "wta"]
@@ -396,21 +412,12 @@ def run_gpu_arm(args):
         else:
             share = {"arm_sum_v_div": agg_ms / 2, "arm_sum_h": agg_ms / 2, "scanline_x": so_ms / 2, "scanline_y": so_ms / 2}
         dom = max(share, key=share.get)
-        # measured DRAM bytes of that kernel (ncu --set full capture summarised in profiles/; per pair there, per launch here)
-        traffic, tsrc = None, None
-        tf = ROOT / "profiles" / "traffic.json"
-        if tf.exists():
-            tj = json.loads(tf.read_text())
-            per_pair = tj.get(dom, {}).get("dram_bytes_per_pair")
-            tsrc = tj.get("_source")
-            if per_pair:
-                traffic = round(per_pair * eng.wave_pairs)
         roof = {"kernel": dom, "bound": "hbm", "achieved": kern[dom]["achieved_gbs"], "peak": hbm_peak, "unit": "GB/s",
-                "frac": kern[dom]["frac"], "traffic": traffic, "peak_source": peak_src,
+                "frac": kern[dom]["frac"], "peak_source": peak_src,
                 "note": "algorithmic bytes per launch = (2V + 6N) per pair x pairs per launch, V = 4*H*W*D: the kernel reads one volume and "
                         "writes one (a fused double pass keeps its intermediate in shared memory; it does one iteration's worth of work per "
-                        "launch, SURVEY 8d); traffic = dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu capture "
-                        f"({tsrc}); kernel timed alone with CUDA events on the engine's stream; 'aggregation' below is the whole stage on the 8(d) model"}
+                        "launch, SURVEY 8d); kernel timed alone with CUDA events on the engine's stream; 'aggregation' below is the whole "
+                        "stage on the 8(d) model"}
         total_maps = world * n * args.steps
         value = total_maps / (ms_dev * 1e-3)
         e2e_v = total_maps / (ms_e2e * 1e-3)
@@ -469,6 +476,8 @@ def run_sharded_arm(args, eng, dev, rank, world, n, w, h, D, wl_name, np_left, n
     clocks = sampler.stop() if sampler else None
     if "resolve" in phases:
         phases["resolve"]()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, d_out)
     ok, check = True, {}
     if rank == 0:
         golden = _golden_final_sha(args.workload)
@@ -520,6 +529,9 @@ def main():
     ap.add_argument("--pairs", type=int, default=0, help="pairs per step per GPU (default: the BASELINE batch of the workload)")
     ap.add_argument("--sharded", action="store_true",
                     help="BASELINE configs[4] form: one batch of pairs x gpus owned by rank 0, NCCL scatter -> Match -> NCCL gather")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the disparity maps of the last step (a fixed, seeded sample of at most "
+                         "64 MB) to DIR as .npy files")
     ap.add_argument("--workload", default="cone", choices=["cone", "kitti", "1080p"],
                     help="cone = BASELINE configs[1] (the contract metric); kitti / 1080p = configs[2] / configs[3] (extra lines)")
     args = ap.parse_args()

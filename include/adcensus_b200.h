@@ -1,6 +1,6 @@
-/* include/adcensus_b200.h -- the drop-in boundary of the B200-native AD-Census engine.
+/* include/adcensus_b200.h -- the drop-in boundary of the H100-native AD-Census engine.
  *
- * A plain C ABI (extern "C", raw pointers and sizes, no torch / CUDA types) over the sm_100a
+ * A plain C ABI (extern "C", raw pointers and sizes, no torch / CUDA types) over the sm_90a
  * kernels in adcensus_b200/csrc.  The reference (ethan-li-coding/AD-Census) has no FFI of its
  * own: its boundary is the C++ class ADCensusStereo (ADCensusStereo.h:14-95) compiled into the
  * caller.  include/ADCensusStereo.h in this repo is the header-compatible shim of that class and

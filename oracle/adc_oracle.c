@@ -2,7 +2,7 @@
  *
  * A plain-C, single-threaded restatement of the reference's AD-Census pipeline, written from the
  * algorithm's description stage by stage.  Every function names the reference lines it follows
- * (paths relative to /root/reference/AD-Census).  It keeps the reference's *sequential in-place*
+ * (paths relative to the reference's AD-Census/ directory).  It keeps the reference's *sequential in-place*
  * semantics everywhere (LR check, region voting, median) because those define the answer.
  *
  * Arithmetic conventions that matter for bit-exactness (SURVEY.md section 8c):

@@ -5,7 +5,7 @@
  * load this; the product library (adcensus_b200/csrc) never does.
  *
  * Parity status: PINNED.  tests/test_oracle_vs_ref.py compares every stage of this restatement
- * bit-for-bit with the real reference (oracle/_ref, built from /root/reference by oracle/Makefile)
+ * bit-for-bit with the real reference (oracle/_ref, built from a checkout of the reference by oracle/Makefile)
  * on Cone and on synthetic pairs, and tests/test_oracle_golden.py compares it with the committed
  * golden vectors in tests/golden/ that were produced by the real reference (tools/make_golden.py).
  */

@@ -1,6 +1,6 @@
 // oracle/ref_harness.cpp -- TEST INFRASTRUCTURE ONLY (never linked into the product library).
 //
-// Thin C-ABI harness around the UNMODIFIED reference sources under /root/reference/AD-Census.
+// Thin C-ABI harness around the UNMODIFIED reference sources (AD-Census/ of a checkout of the reference).
 // It is compiled together with the reference's six algorithm .cpp files (where they lie, nothing
 // is copied into this repo) into oracle/_ref/libadcensus_ref.so by oracle/Makefile.  It exists to
 //   (1) pin oracle/adc_oracle.c (our own restatement) against the real reference, stage by stage,

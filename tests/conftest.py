@@ -10,7 +10,7 @@ for p in (str(ROOT), str(ROOT / "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

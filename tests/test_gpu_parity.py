@@ -341,7 +341,7 @@ def test_real_pairs_vs_reference_goldens(name):
 def test_baseline_configs_vs_reference_goldens(name):
     """BASELINE.json configs 3 and 4 (synthetic 1242x375x128, 1920x1080x192): the aggregated volume, the optimised
     volume, both WTA maps, the outlier lists and the final map against the unmodified reference's hashes
-    (one 115 s reference run per 1080p pair, done once in the build container: tools/make_golden_big.py)."""
+    (one long reference run per 1080p pair, done once by tools/make_golden_big.py)."""
     g = _big()[name]
     w, h, D = g["width"], g["height"], g["max_disparity"]
     seed = int(name.rsplit("_s", 1)[1])
@@ -404,7 +404,7 @@ if world > 1:
 @pytest.mark.parametrize("world", [1, 2])
 def test_sharded_batch_real_engine(tmp_path, world):
     """adcensus_b200.parallel.run_sharded_device (BASELINE configs[4] form) with the REAL engine: rank 0 owns the batch,
-    NCCL scatter -> Match -> NCCL gather, order and bits against the oracle.  world = 2 needs two GPUs (gpurun --gpus 2)."""
+    NCCL scatter -> Match -> NCCL gather, order and bits against the oracle.  world = 2 needs two GPUs."""
     import os, socket, subprocess, sys
     import torch
     if torch.cuda.device_count() < world:

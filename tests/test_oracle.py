@@ -1,5 +1,5 @@
-"""CPU tests of the oracle (test infrastructure): pinned against the real reference (oracle/_ref,
-where it exists) and against the committed golden vectors produced by the real reference."""
+"""CPU tests of the oracle (test infrastructure): pinned against the committed golden vectors produced by the
+real reference."""
 import json
 import sys
 from pathlib import Path
@@ -51,29 +51,19 @@ def test_oracle_cone_final_matches_golden(cone):
     assert np.array_equal(disp.view(np.uint32), z["MEDIAN__DISP_L"].view(np.uint32))
 
 
-@pytest.mark.skipif(not T.have_ref(), reason="oracle/_ref not built (needs /root/reference)")
-@pytest.mark.parametrize("case", [(70, 50, 20, {}, 21), (64, 40, 16, {"min_disparity": 0, "do_lr_check": 0}, 22),
-                                  (90, 64, 40, {"do_filling": 0}, 23), (33, 30, 48, {}, 24), (9, 9, 8, {}, 25),
-                                  (80, 60, 32, {"min_disparity": 2, "max_disparity": 34}, 31),
-                                  (80, 60, 32, {"min_disparity": -4, "max_disparity": 28}, 32)])
+@pytest.mark.parametrize("case", G.REF_CASES)
 def test_oracle_vs_live_reference(case):
-    w, h, D, over, seed = case
-    opt = T.default_option(**{"max_disparity": D, **over})
-    left, right = T.synthetic_pair(w, h, D, seed)
-    orc, ref = T.Oracle(w, h, opt), T.Reference(w, h, opt)
+    """Every tap after every stage against the sha256 the unmodified reference produced for the same synthetic input,
+    recorded from a live reference build by tools/make_golden.py (tests/golden/golden_ref_cases.json)."""
+    want = json.loads((T.GOLDEN_DIR / "golden_ref_cases.json").read_text())[G.ref_case_id(case)]
+    left, right, opt = G.ref_case_inputs(case)
+    h, w, _ = left.shape
+    orc = T.Oracle(w, h, opt)
     orc.begin(left, right)
-    ref.begin(left, right)
     for st in T.STAGES:
         orc.step()
-        ref.step()
         for tap in T.STAGE_TAPS[st]:
-            a, b = orc.tap(tap), ref.tap(tap)
-            if tap == "DISP_R" and opt.min_disparity > 0:
-                # right pixels x >= W - dmin have no candidate column at all: the reference then runs its parabola on an
-                # uninitialised cost_local[] (ADCensusStereo.cpp:271-300, SURVEY 8a A10) -- whatever the heap held; the
-                # restatement writes the integer 0 there.  Undefined in the reference, so not compared.
-                a, b = a[:, :w - opt.min_disparity], b[:, :w - opt.min_disparity]
-            assert a.shape == b.shape and np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8)), f"{st}/{tap}"
+            assert T.sha(G.ref_case_tap(opt, tap, orc.tap(tap))) == want[f"{st}/{tap}"], f"{st}/{tap}"
 
 
 def test_gray_exhaustive():

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Generates tests/golden/golden_*.npz from the UNMODIFIED reference (oracle/_ref built from
-/root/reference by oracle/Makefile).  Run in the build container; the fixtures are committed so the
-GPU box (no /root/reference) can check against the real reference's outputs.
+"""Generates tests/golden/golden_*.npz from the UNMODIFIED reference (oracle/_ref, built by oracle/Makefile from the
+checkout ADC_REFERENCE_DIR names).  The fixtures are committed, so the tests check against the real reference's outputs
+without the reference itself.
 
 For every case: sha256 of every tap after every stage (bit-exact pin for all intermediates,
 including the cost volumes) plus the full arrays of the small per-pixel maps and the final map.
@@ -28,6 +28,32 @@ CASES = {
     "synth_disc": ("synth", 80, 60, {"max_disparity": 32, "do_discontinuity_adjustment": 1}, 10),
 }
 FULL_TAPS = {"ARMS", "SUPCNT_H", "SUPCNT_V", "DISP_L", "DISP_R", "MISMATCHES", "OCCLUSIONS", "CENSUS_L"}
+# synthetic cases (W, H, D, option overrides, seed) whose every tap after every stage is pinned by sha256 in
+# tests/golden/golden_ref_cases.json: small sizes, option switches, dmin > 0 and dmin < 0
+REF_CASES = [(70, 50, 20, {}, 21), (64, 40, 16, {"min_disparity": 0, "do_lr_check": 0}, 22),
+             (90, 64, 40, {"do_filling": 0}, 23), (33, 30, 48, {}, 24), (9, 9, 8, {}, 25),
+             (80, 60, 32, {"min_disparity": 2, "max_disparity": 34}, 31),
+             (80, 60, 32, {"min_disparity": -4, "max_disparity": 28}, 32)]
+
+
+def ref_case_id(case):
+    return f"{case[0]}x{case[1]}x{case[2]}-s{case[4]}"
+
+
+def ref_case_tap(opt, tap, a):
+    """The part of a tap the reference defines.  Right pixels x >= W - dmin have no candidate column at all: the reference
+    then runs its parabola on an uninitialised cost_local[] (ADCensusStereo.cpp:271-300, SURVEY 8a A10) -- whatever the
+    heap held; the restatement writes the integer 0 there.  Undefined in the reference, so not pinned."""
+    if tap == "DISP_R" and opt.min_disparity > 0:
+        a = a[:, :a.shape[1] - opt.min_disparity]
+    return a
+
+
+def ref_case_inputs(case):
+    w, h, D, over, seed = case
+    opt = T.default_option(**{"max_disparity": D, **over})
+    left, right = T.synthetic_pair(w, h, D, seed)
+    return left, right, opt
 
 
 def case_inputs(name):
@@ -43,7 +69,7 @@ def case_inputs(name):
 
 
 def main():
-    assert T.have_ref() or (T.build_oracle() or T.have_ref()), "oracle/_ref is required (build container only)"
+    assert T.have_ref() or (T.build_oracle() or T.have_ref()), "oracle/_ref is required: set ADC_REFERENCE_DIR to a checkout of the reference"
     out_dir = T.GOLDEN_DIR
     for name in CASES:
         left, right, opt = case_inputs(name)
@@ -62,6 +88,20 @@ def main():
         assert T.sha(stock) == hashes["MEDIAN/DISP_L"], "staged runner and stock Match disagree"
         np.savez_compressed(out_dir / f"golden_{name}.npz", hashes=json.dumps(hashes), **arrays)
         print(name, w, h, "final sha", hashes["MEDIAN/DISP_L"][:16], "arrays", len(arrays))
+    ref_cases = {}
+    for case in REF_CASES:
+        left, right, opt = ref_case_inputs(case)
+        h, w, _ = left.shape
+        ref = T.Reference(w, h, opt)
+        ref.begin(left, right)
+        hashes = {}
+        for st in T.STAGES:
+            ref.step()
+            for tap in T.STAGE_TAPS[st]:
+                hashes[f"{st}/{tap}"] = T.sha(ref_case_tap(opt, tap, ref.tap(tap)))
+        ref_cases[ref_case_id(case)] = hashes
+        print(ref_case_id(case), "final sha", hashes["MEDIAN/DISP_L"][:16])
+    (out_dir / "golden_ref_cases.json").write_text(json.dumps(ref_cases, indent=1, sort_keys=True) + "\n")
 
 
 if __name__ == "__main__":

@@ -11,8 +11,8 @@
                                    those pairs and for the BASELINE.json configs 3 / 4 inputs: synthetic 1242x375x128
                                    seeds 1-2, synthetic 1920x1080x192 seed 1
 
-Run in the build container only (needs /root/reference and oracle/_ref); the fixtures are committed so that the
-GPU box, which has neither, can compare the CUDA path with the real reference's outputs.
+Needs a checkout of the reference (ADC_REFERENCE_DIR) and oracle/_ref built from it; the fixtures are committed so that
+the tests, which have neither, can compare the CUDA path with the real reference's outputs.
 """
 import json
 import sys
@@ -59,7 +59,7 @@ def run_case(name, left, right, dmax, out):
 def main():
     import cv2
     T.build_oracle()
-    assert T.have_ref(), "oracle/_ref is required (build container only)"
+    assert T.have_ref(), "oracle/_ref is required: set ADC_REFERENCE_DIR to a checkout of the reference"
     only = set(sys.argv[1:])
     jpath = T.GOLDEN_DIR / "golden_big.json"
     out = json.loads(jpath.read_text()) if jpath.exists() else {}

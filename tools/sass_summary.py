@@ -1,13 +1,13 @@
 #!/usr/bin/env python
 """Per-kernel SASS opcode summary of the product library (cuobjdump -sass): total instructions and the counts of the
-mnemonics that show which hardware path a kernel uses (B200_PROFILING.md: UTMALDG / UBLKCP = TMA, SYNCS = mbarrier,
-LDGSTS = cp.async, FADD2 = packed f32x2 add, R2P = register-to-predicates).  usage: sass_summary.py lib.so > out.txt"""
+mnemonics that show which hardware path a kernel uses (UTMALDG / UBLKCP = TMA, SYNCS = mbarrier,
+LDGSTS = cp.async, R2P = register-to-predicates).  usage: sass_summary.py lib.so > out.txt"""
 import collections
 import re
 import subprocess
 import sys
 
-KEY = ["UTMALDG", "UBLKCP", "SYNCS", "LDGSTS", "FADD2", "R2P", "LDG", "STG", "LDS", "STS", "ATOMS", "ATOMG", "RED", "SHFL", "REDUX", "MUFU", "BAR", "UCGABAR"]
+KEY = ["UTMALDG", "UBLKCP", "SYNCS", "LDGSTS", "R2P", "LDG", "STG", "LDS", "STS", "ATOMS", "ATOMG", "RED", "SHFL", "REDUX", "MUFU", "BAR", "UCGABAR"]
 out = subprocess.run(["cuobjdump", "-sass", sys.argv[1]], capture_output=True, text=True).stdout
 kern, cur = collections.OrderedDict(), None
 for line in out.splitlines():
