@@ -128,6 +128,11 @@ struct AdcWave {            // device pointers of one wave (S pairs)
 
 void adc_launch_gray_census(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_cost(const AdcParams& P, const AdcWave& w, float* vol, cudaStream_t st, unsigned long long* launches);
+// cost-input mode (k_ingest.cu): the wave's caller volumes at `src` (pair stride N*D elements, layout ADC_COST_HWD /
+// ADC_COST_DHW, element type ADC_COST_F32 / F16 / BF16) -> `vol`, clamped to the documented value domain
+void adc_launch_cost_ingest(const AdcParams& P, const AdcWave& w, const void* src, int layout, int dtype, float* vol,
+                            cudaStream_t st, unsigned long long* launches);
+size_t adc_cost_elem_bytes(int dtype);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

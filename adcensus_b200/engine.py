@@ -53,6 +53,13 @@ class _Config(ctypes.Structure):
 # adc_config.debug_flags (test hooks)
 DBG_NO_RAY_TABLE, DBG_VOTE_ENUM, DBG_VOTE_GLOBAL_STATE, DBG_UNFUSED_AGG = 1, 2, 4, 8
 
+# cost-input mode (adc_match_cost*): volume layouts, element types and the value domain's ceiling
+COST_HWD, COST_DHW = 0, 1
+COST_F32, COST_F16, COST_BF16 = 0, 1, 2
+COST_MAX = 65536.0
+COST_LAYOUTS = {"hwd": COST_HWD, "dhw": COST_DHW}
+COST_DTYPES = {"f32": COST_F32, "f16": COST_F16, "bf16": COST_BF16}
+
 
 class AdcError(RuntimeError):
     pass
@@ -104,6 +111,9 @@ def load_library() -> ctypes.CDLL:
     L.adc_last_error.restype = ctypes.c_char_p
     L.adc_version.restype = ctypes.c_char_p
     L.adc_debug_run.argtypes = [vp, u8p, u8p, i32]
+    L.adc_match_cost.argtypes = [vp, u8p, u8p, vp, i32, i32, f32p]
+    L.adc_match_cost_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, vp]
+    L.adc_debug_run_cost.argtypes = [vp, u8p, u8p, vp, i32, i32, i32]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -121,6 +131,14 @@ def _img(a, shape) -> np.ndarray:
     if a.shape != shape:
         raise ValueError(f"expected packed BGR uint8 array of shape {shape}, got {a.shape}")
     return a
+
+
+def _code(table, v, what):
+    if isinstance(v, str):
+        if v not in table:
+            raise ValueError(f"unknown cost {what} {v!r} (one of {sorted(table)})")
+        return table[v]
+    return int(v)
 
 
 class Engine:
@@ -165,6 +183,44 @@ class Engine:
         _check(self._L.adc_get_right_disparity(self._h, disp.ctypes.data))
         return disp
 
+    # ---- matching from a caller's cost volume (adc_match_cost*) -------------------------------
+    def _cost(self, cost, layout, dtype):
+        """(contiguous numpy volume, layout code, dtype code) for a host cost volume of one pair.  numpy has no bfloat16:
+        a bf16 volume is passed as its uint16 bit patterns with dtype="bf16"."""
+        lay = _code(COST_LAYOUTS, layout, "layout")
+        cost = np.ascontiguousarray(cost)
+        want_np = {COST_F32: np.float32, COST_F16: np.float16, COST_BF16: np.uint16}
+        if dtype is None:
+            dt = {np.dtype(np.float32): COST_F32, np.dtype(np.float16): COST_F16}.get(cost.dtype)
+            if dt is None:
+                raise ValueError(f"cost volume must be float32 or float16 (or uint16 bits with dtype='bf16'), got {cost.dtype}")
+        else:
+            dt = _code(COST_DTYPES, dtype, "dtype")
+            if cost.dtype != want_np.get(dt):
+                raise ValueError(f"dtype {dtype!r} expects a numpy {np.dtype(want_np.get(dt, np.float32)).name} array, got {cost.dtype}")
+        H, W, D = self.height, self.width, self.D
+        want = (H, W, D) if lay == COST_HWD else (D, H, W)
+        if cost.shape != want:
+            raise ValueError(f"expected a cost volume of shape {want} for layout {layout!r}, got {cost.shape}")
+        return cost, lay, dt
+
+    def match_cost(self, left, right, cost, layout="hwd", dtype=None) -> np.ndarray:
+        """Match with the given matching cost instead of the AD-census cost: `cost` is one pair's volume, float32 or
+        float16, [H][W][D] (layout "hwd") or [D][H][W] ("dhw"); lower = better.  Values are clamped to [0, COST_MAX]."""
+        left = _img(left, (self.height, self.width, 3))
+        right = _img(right, (self.height, self.width, 3))
+        cost, lay, dt = self._cost(cost, layout, dtype)
+        disp = np.empty((self.height, self.width), np.float32)
+        _check(self._L.adc_match_cost(self._h, left.ctypes.data, right.ctypes.data, cost.ctypes.data, lay, dt, disp.ctypes.data))
+        return disp
+
+    def match_cost_batch_device(self, n: int, d_left: int, d_right: int, d_cost: int, d_disp: int,
+                                layout="dhw", dtype="f32", stream: int = 0):
+        """Device pointers (ints): n pairs of images, n cost volumes of H*W*D elements each (layout "hwd" / "dhw", dtype
+        "f32" / "f16" / "bf16"), n maps out; enqueued on `stream` without synchronising, like match_batch_device."""
+        _check(self._L.adc_match_cost_batch_device(self._h, n, d_left, d_right, d_cost, _code(COST_LAYOUTS, layout, "layout"),
+                                                   _code(COST_DTYPES, dtype, "dtype"), d_disp, stream))
+
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
         lefts = np.ascontiguousarray(lefts, np.uint8)
@@ -207,7 +263,7 @@ class Engine:
         return list(out)
 
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
-                       "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9}
+                       "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""
@@ -247,6 +303,13 @@ class Engine:
         left = _img(left, (self.height, self.width, 3))
         right = _img(right, (self.height, self.width, 3))
         _check(self._L.adc_debug_run(self._h, left.ctypes.data, right.ctypes.data, STAGE[last_stage]))
+
+    def debug_run_cost(self, left, right, cost, layout, last_stage: str, dtype=None):
+        left = _img(left, (self.height, self.width, 3))
+        right = _img(right, (self.height, self.width, 3))
+        cost, lay, dt = self._cost(cost, layout, dtype)
+        _check(self._L.adc_debug_run_cost(self._h, left.ctypes.data, right.ctypes.data, cost.ctypes.data, lay, dt,
+                                          STAGE[last_stage]))
 
     def counters(self):
         out = (ctypes.c_int32 * 16)()

@@ -132,6 +132,43 @@ int adc_match_batch_pinned_async(adc_engine* e, int32_t n, const uint8_t* left, 
 int adc_set_pipelined(adc_engine* e, int32_t on);
 int adc_join(adc_engine* e, void* stream);
 
+/* ---- matching from a caller-supplied cost volume ------------------------------------------------
+ * The entry points below replace stage 1 (gray, census, AD-census cost) by the caller's own matching cost -- from a
+ * network, another census variant, a fusion of cues -- and run everything after it unchanged: cross-based aggregation,
+ * scanline optimisation, left/right WTA with the parabola, LR check, region voting, interpolation, discontinuity
+ * adjustment and the median.  The images are still required: the cross arms, the scanline penalties and the refinement
+ * read them.
+ *
+ * Layout of one pair's volume, contiguous, d = disparity - min_disparity in [0, D), D = max_disparity - min_disparity:
+ *   ADC_COST_HWD  [H][W][D]  element (y * W + x) * D + d        (the reference's cost_init_ layout)
+ *   ADC_COST_DHW  [D][H][W]  element (d * H + y) * W + x        (a network's [N, D, H, W] cost tensor, one pair)
+ * Pairs follow each other with a stride of H*W*D elements.  Element types: ADC_COST_F32, ADC_COST_F16 (IEEE half) and
+ * ADC_COST_BF16 (bfloat16), converted to float exactly.
+ * Value domain, applied to every element on the way in: NaN, +inf and values >= ADC_COST_MAX become ADC_COST_MAX;
+ * negative values, -0.0 and -inf become +0.0.  (The engine treats columns outside the image as cost 99999, never the
+ * minimum; aggregation and scanline optimisation never exceed their largest input by more than rounding, so inputs up
+ * to 65536 keep that ordering.  -0.0 would let equal minima tie-break differently from the reference's comparisons.)
+ * Lower cost = better match, as in the AD-census cost.  lambda_ad and lambda_census are ignored; every other option
+ * applies.  After a cost call, adc_get_right_disparity, adc_last_stage_ms (out[0] = uploads + ingestion),
+ * adc_launch_count and the VOL_* / DISP_* / list debug taps behave as after the image calls; the GRAY_* / CENSUS_* taps
+ * are not meaningful.  An unknown layout or element type, or a NULL pointer, fails with ADC_ERR_ARG before any
+ * device work. */
+enum { ADC_COST_HWD = 0, ADC_COST_DHW = 1 };
+enum { ADC_COST_F32 = 0, ADC_COST_F16 = 1, ADC_COST_BF16 = 2 };
+#define ADC_COST_MAX 65536.0f
+
+/* adc_match with the cost volume of the pair given: host pointers (images as for adc_match, `cost` one pair's volume),
+ * synchronous. */
+int adc_match_cost(adc_engine* e, const uint8_t* img_left, const uint8_t* img_right,
+                   const void* cost, int32_t layout, int32_t dtype, float* disp_left);
+
+/* adc_match_batch_device with one cost volume per pair: d_cost holds n volumes in device memory (pair i at element
+ * i*H*W*D), read straight from there by the ingestion kernel of each wave.  Stream, fork/join and pipelined-mode
+ * behaviour (adc_set_pipelined / adc_join) as for adc_match_batch_device; the caller's buffers must stay untouched
+ * until the work is joined. */
+int adc_match_cost_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                const void* d_cost, int32_t layout, int32_t dtype, float* d_disp, void* stream);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
@@ -149,7 +186,9 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * wave of wave_pairs pairs: kernel_id 0 = cost volume, 1 = horizontal arm sum, 2 = vertical arm sum
  * with division, 3 = scanline pass along x, 4 = scanline pass along y, 5 = WTA left+right, 6 / 7 = the fused
  * vertical / horizontal double pass of the aggregation (divide + sum, intermediate in shared memory), 8 = horizontal
- * arm sum with division, 9 = vertical arm sum without division.
+ * arm sum with division, 9 = vertical arm sum without division, 10 = cost-volume ingestion (layout and element type of
+ * the engine's last cost call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*D*sizeof(element) + N*Dp*4 bytes per
+ * pair, Dp = D rounded up to a multiple of 4).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 
@@ -194,6 +233,9 @@ enum {
     ADC_TAP_COUNT = 13
 };
 int adc_debug_run(adc_engine* e, const uint8_t* img_left, const uint8_t* img_right, int32_t last_stage);
+/* adc_debug_run with a caller-supplied cost volume (host pointer, layouts and domain as for adc_match_cost) */
+int adc_debug_run_cost(adc_engine* e, const uint8_t* img_left, const uint8_t* img_right,
+                       const void* cost, int32_t layout, int32_t dtype, int32_t last_stage);
 /* region-voting statistics of pair 0 of the last run: out[0],out[1] = remaining mismatch / occlusion
  * list sizes, out[2] = fixed-point rounds, out[3] = vote evaluations, out[12..15] = microseconds one warp spent
  * evaluating / waiting at round barriers / committing / compacting lists */

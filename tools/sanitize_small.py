@@ -26,4 +26,31 @@ for (w, h, D, seed, over) in cases:
     c = eng.disparity_cloud(left, a)
     eng.close()
     print("ok", w, h, D, mm, c.shape, flush=True)
+
+# cost-input mode: both layouts, a bf16 volume and the batched device entry point
+import cost_testlib as CT
+for (w, h, D, seed, over) in [(97, 61, 22, 2, {}), (80, 60, 32, 42, {"min_disparity": -4, "max_disparity": 28})]:
+    kw = dict(max_disparity=D); kw.update(over)
+    dmin = kw.get("min_disparity", 0)
+    D = kw["max_disparity"] - dmin
+    left, right = T.synthetic_pair(w, h, D, seed)
+    cost = CT.synthetic_cost(w, h, D, seed, dmin)
+    eng = A.Engine(w, h, A.ADCensusOption(**kw), wave_pairs=2, lanes=2)
+    a = eng.match_cost(left, right, cost, "hwd")
+    dhw = np.ascontiguousarray(cost.transpose(2, 0, 1))
+    assert eng.match_cost(left, right, dhw, "dhw").tobytes() == a.tobytes()
+    assert eng.match_cost(left, right, CT.to_bf16_bits(cost), "hwd", dtype="bf16").tobytes() == a.tobytes()
+    import torch
+    dev = torch.device("cuda", 0)
+    n = 5
+    d_l = torch.from_numpy(np.stack([left] * n)).to(dev)
+    d_r = torch.from_numpy(np.stack([right] * n)).to(dev)
+    d_c = torch.from_numpy(np.stack([CT.to_bf16_bits(dhw)] * n)).to(dev)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_cost_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), d_c.data_ptr(), d_o.data_ptr(), "dhw", "bf16",
+                                torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    assert (d_o.cpu().numpy().view(np.uint32) == a.view(np.uint32)[None]).all()
+    eng.close()
+    print("cost ok", w, h, D, flush=True)
 print("all ok")
