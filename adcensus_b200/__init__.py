@@ -8,9 +8,10 @@ This package is the Python mirror of the reference's interface for that path
 works anywhere, but creating an engine without the CUDA library or without a GPU raises.
 """
 from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TAP, lib_path,  # noqa: F401
-                     load_library, Invalid_Float, COST_HWD, COST_DHW, COST_F32, COST_F16, COST_BF16, COST_MAX)
+                     load_library, Invalid_Float, COST_HWD, COST_DHW, COST_F32, COST_F16, COST_BF16, COST_MAX,
+                     VOL_COST, VOL_AGGR, VOL_OPT)
 from .build import build_library  # noqa: F401
 
 __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "TAP", "lib_path",
            "load_library", "build_library", "Invalid_Float", "COST_HWD", "COST_DHW", "COST_F32", "COST_F16", "COST_BF16",
-           "COST_MAX"]
+           "COST_MAX", "VOL_COST", "VOL_AGGR", "VOL_OPT"]

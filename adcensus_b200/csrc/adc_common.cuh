@@ -133,6 +133,10 @@ void adc_launch_cost(const AdcParams& P, const AdcWave& w, float* vol, cudaStrea
 void adc_launch_cost_ingest(const AdcParams& P, const AdcWave& w, const void* src, int layout, int dtype, float* vol,
                             cudaStream_t st, unsigned long long* launches);
 size_t adc_cost_elem_bytes(int dtype);
+// volume export (k_ingest.cu): the wave's [S][N][Dp] f32 volume `vol` -> `dst` (pair stride N*D elements, layout
+// ADC_COST_HWD / ADC_COST_DHW, element type ADC_COST_F32 / F16 / BF16 rounded to nearest even); dst aligned to its element
+void adc_launch_cost_export(const AdcParams& P, const AdcWave& w, const float* vol, void* dst, int layout, int dtype,
+                            cudaStream_t st, unsigned long long* launches);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

@@ -60,6 +60,17 @@ COST_MAX = 65536.0
 COST_LAYOUTS = {"hwd": COST_HWD, "dhw": COST_DHW}
 COST_DTYPES = {"f32": COST_F32, "f16": COST_F16, "bf16": COST_BF16}
 
+# volume export (adc_match_volumes*): which volume a request names
+VOL_COST, VOL_AGGR, VOL_OPT = 0, 1, 2
+VOL_STAGES = {"cost": VOL_COST, "aggr": VOL_AGGR, "opt": VOL_OPT}
+_VOL_NP = {COST_F32: np.float32, COST_F16: np.float16, COST_BF16: np.uint16}
+
+
+class VolumeOut(ctypes.Structure):
+    """adc_volume_out: one exported volume (destination, ADC_VOL_* stage, layout, element type)."""
+    _fields_ = [("dst", ctypes.c_void_p), ("stage", ctypes.c_int32), ("layout", ctypes.c_int32),
+                ("dtype", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
 
 class AdcError(RuntimeError):
     pass
@@ -114,6 +125,8 @@ def load_library() -> ctypes.CDLL:
     L.adc_match_cost.argtypes = [vp, u8p, u8p, vp, i32, i32, f32p]
     L.adc_match_cost_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, vp]
     L.adc_debug_run_cost.argtypes = [vp, u8p, u8p, vp, i32, i32, i32]
+    L.adc_match_volumes.argtypes = [vp, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32]
+    L.adc_match_volumes_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -139,6 +152,15 @@ def _code(table, v, what):
             raise ValueError(f"unknown cost {what} {v!r} (one of {sorted(table)})")
         return table[v]
     return int(v)
+
+
+def _volume_outs(outs):
+    """ctypes array of adc_volume_out from (ptr, stage, layout, dtype) tuples (names or ADC_* codes)."""
+    arr = (VolumeOut * max(1, len(outs)))()
+    for i, (ptr, stage, layout, dtype) in enumerate(outs):
+        arr[i] = VolumeOut(ptr, _code(VOL_STAGES, stage, "volume stage"), _code(COST_LAYOUTS, layout, "layout"),
+                           _code(COST_DTYPES, dtype, "dtype"), 0)
+    return arr
 
 
 class Engine:
@@ -221,6 +243,40 @@ class Engine:
         _check(self._L.adc_match_cost_batch_device(self._h, n, d_left, d_right, d_cost, _code(COST_LAYOUTS, layout, "layout"),
                                                    _code(COST_DTYPES, dtype, "dtype"), d_disp, stream))
 
+    # ---- exporting the cost volumes (adc_match_volumes*) --------------------------------------
+    def match_volumes(self, left, right, stages, layout="hwd", dtype="f32", cost=None, cost_layout="hwd", cost_dtype=None,
+                      disparity=True):
+        """(disparity map or None, {stage: volume}) of one pair.  `stages`: one or more of "cost", "aggr", "opt" (the
+        matching cost, the cross-aggregated cost, the scanline-optimised cost).  Volumes come back [H][W][D] ("hwd") or
+        [D][H][W] ("dhw") as float32, float16 or -- numpy has no bfloat16 -- uint16 bit patterns for "bf16".  `cost`: a
+        caller's matching cost instead of the AD-census cost, as for match_cost.  disparity=False stops the pipeline after
+        the latest requested volume."""
+        left = _img(left, (self.height, self.width, 3))
+        right = _img(right, (self.height, self.width, 3))
+        if isinstance(stages, (str, int)):
+            stages = [stages]
+        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
+        H, W, D = self.height, self.width, self.D
+        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
+        vols = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in stages}
+        outs = _volume_outs([(v.ctypes.data, s, lay, dt) for s, v in vols.items()])
+        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
+        disp = np.empty((H, W), np.float32) if disparity else None
+        _check(self._L.adc_match_volumes(self._h, left.ctypes.data, right.ctypes.data, None if c is None else c.ctypes.data,
+                                         clay, cdt, None if disp is None else disp.ctypes.data, outs, len(vols)))
+        return disp, vols
+
+    def match_volumes_batch_device(self, n: int, d_left: int, d_right: int, outs, d_disp: int = 0, d_cost: int = 0,
+                                   cost_layout="dhw", cost_dtype="f32", stream: int = 0):
+        """Device pointers (ints): n pairs of images, optional n cost volumes, optional n maps (d_disp 0 = volumes only);
+        `outs` a list of (ptr, stage, layout, dtype), each ptr n volumes of H*W*D elements.  Enqueued on `stream` without
+        synchronising, like match_batch_device."""
+        arr = _volume_outs(outs)
+        _check(self._L.adc_match_volumes_batch_device(self._h, n, d_left, d_right, d_cost or None,
+                                                      _code(COST_LAYOUTS, cost_layout, "layout"),
+                                                      _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, arr,
+                                                      len(outs), stream))
+
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
         lefts = np.ascontiguousarray(lefts, np.uint8)
@@ -263,7 +319,8 @@ class Engine:
         return list(out)
 
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
-                       "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10}
+                       "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10,
+                       "cost_export": 11}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""

@@ -169,6 +169,44 @@ int adc_match_cost(adc_engine* e, const uint8_t* img_left, const uint8_t* img_ri
 int adc_match_cost_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
                                 const void* d_cost, int32_t layout, int32_t dtype, float* d_disp, void* stream);
 
+/* ---- exporting the cost volumes ------------------------------------------------------------------
+ * The entry points below hand out up to three volumes of every pair next to (or instead of) the disparity map:
+ *   ADC_VOL_COST  the matching cost: the reference's cost_init_ after ComputeCost; with a caller's cost (d_cost / cost
+ *                 non-NULL), the ingested volume after the value domain above
+ *   ADC_VOL_AGGR  the cross-aggregated cost after the 4 iterations: cost_aggr_ after Aggregate
+ *   ADC_VOL_OPT   the scanline-optimised cost after the 4 passes, the volume the WTA reads: cost_aggr_ after Optimize
+ * in the layouts and element types of cost input (ADC_COST_HWD / ADC_COST_DHW, ADC_COST_F32 / F16 / BF16), pair i of
+ * `dst` at element i*H*W*D, the padding disparities and the right view never included.  f32 is the engine's values bit
+ * for bit; f16 is IEEE round-to-nearest-even (values >= 65520 become +inf: torch's .half(), numpy's astype(float16));
+ * bf16 is round-to-nearest-even.  The volumes hold no NaN.  Each volume is written by one extra pass over it, enqueued
+ * where the volume is live; the disparity map of a call that exports is bit-identical to the same call without export.
+ * disp NULL = volumes only: the pipeline stops after the latest exported stage (no WTA, no refinement).
+ * Fails with ADC_ERR_ARG before any device work, naming the field: n_outs outside 0..3; outs NULL with n_outs > 0; a
+ * stage requested twice; an unknown stage, layout or dtype; a NULL dst (on the device entry also a dst not aligned to its
+ * element size); a non-zero reserved; n_outs == 0 with disp NULL; an unknown cost layout or dtype when a cost is given. */
+enum { ADC_VOL_COST = 0, ADC_VOL_AGGR = 1, ADC_VOL_OPT = 2 };
+typedef struct adc_volume_out {
+    void*   dst;      /* n volumes of H*W*D elements, pair i at element i*H*W*D */
+    int32_t stage;    /* ADC_VOL_* */
+    int32_t layout;   /* ADC_COST_HWD / ADC_COST_DHW */
+    int32_t dtype;    /* ADC_COST_F32 / ADC_COST_F16 / ADC_COST_BF16 */
+    int32_t reserved; /* must be zero */
+} adc_volume_out;
+
+/* adc_match_batch_device / adc_match_cost_batch_device plus volume export.  d_cost NULL = the AD-census cost
+ * (cost_layout / cost_dtype ignored).  d_disp NULL = stop after the latest exported stage.  Device pointers; stream,
+ * fork/join and pipelined-mode behaviour as for adc_match_batch_device. */
+int adc_match_volumes_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                   const void* d_cost, int32_t cost_layout, int32_t cost_dtype, float* d_disp,
+                                   const adc_volume_out* outs, int32_t n_outs, void* stream);
+/* One pair, host pointers (images, optional cost, optional disp, outs[i].dst), synchronous.  The volumes pass through
+ * device staging that the engine allocates on first use, grows when a call needs more and frees in adc_destroy
+ * (ADC_ERR_NOMEM, before any work, if that allocation fails).  With disp: adc_last_stage_ms (each export counted in the
+ * stage that produced its volume) and adc_get_right_disparity behave as after adc_match; after a volumes-only call
+ * (disp NULL) neither is meaningful. */
+int adc_match_volumes(adc_engine* e, const uint8_t* left, const uint8_t* right, const void* cost, int32_t cost_layout,
+                      int32_t cost_dtype, float* disp, const adc_volume_out* outs, int32_t n_outs);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
@@ -188,7 +226,8 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * vertical / horizontal double pass of the aggregation (divide + sum, intermediate in shared memory), 8 = horizontal
  * arm sum with division, 9 = vertical arm sum without division, 10 = cost-volume ingestion (layout and element type of
  * the engine's last cost call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*D*sizeof(element) + N*Dp*4 bytes per
- * pair, Dp = D rounded up to a multiple of 4).
+ * pair, Dp = D rounded up to a multiple of 4), 11 = volume export (layout and element type of the engine's last export
+ * call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*Dp*4 + N*D*sizeof(element) bytes per pair).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 

@@ -53,4 +53,33 @@ for (w, h, D, seed, over) in [(97, 61, 22, 2, {}), (80, 60, 32, 42, {"min_dispar
     assert (d_o.cpu().numpy().view(np.uint32) == a.view(np.uint32)[None]).all()
     eng.close()
     print("cost ok", w, h, D, flush=True)
+
+# volume export: every stage, both layouts, 2-byte types, D % 4 != 0 and odd H*W (odd pair offsets), volumes only,
+# the batched device entry point at an odd destination offset
+for (w, h, D, seed) in [(97, 61, 22, 2), (71, 47, 23, 5)]:
+    left, right = T.synthetic_pair(w, h, D, seed)
+    eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+    a = eng.match(left, right)
+    for layout in ("hwd", "dhw"):
+        for dtype in ("f32", "bf16", "f16"):
+            disp, vols = eng.match_volumes(left, right, ["cost", "aggr", "opt"], layout, dtype)
+            assert disp.tobytes() == a.tobytes()
+            none, only = eng.match_volumes(left, right, ["opt"], layout, dtype, disparity=False)
+            assert none is None and only["opt"].tobytes() == vols["opt"].tobytes()
+    import torch
+    dev = torch.device("cuda", 0)
+    n, ND = 5, h * w * D
+    d_l = torch.from_numpy(np.stack([left] * n)).to(dev)
+    d_r = torch.from_numpy(np.stack([right] * n)).to(dev)
+    d_v = torch.empty(n * ND + 1, dtype=torch.bfloat16, device=dev)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_volumes_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), [(d_v[1:].data_ptr(), "aggr", "dhw", "bf16")],
+                                   d_disp=d_o.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    assert (d_o.cpu().numpy().view(np.uint32) == a.view(np.uint32)[None]).all()
+    _, want = eng.match_volumes(left, right, "aggr", "dhw", "bf16")
+    got = d_v[1:].view(torch.int16).cpu().numpy().view(np.uint16).reshape(n, -1)
+    assert (got == want["aggr"].reshape(1, -1)).all()
+    eng.close()
+    print("export ok", w, h, D, flush=True)
 print("all ok")
