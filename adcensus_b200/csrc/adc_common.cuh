@@ -158,6 +158,10 @@ size_t adc_so_bitrow_bytes(const AdcDims& dm);
 int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
                         cudaStream_t st, unsigned long long* launches);
 int adc_launch_wta(const AdcParams& P, const AdcWave& w, const float* vol, cudaStream_t st, unsigned long long* launches);
+// cost-curve confidence (k_confidence.cu): per pixel of the wave's volume `vol`, c1 = C(d1) -> min_cost and c1 / c2 ->
+// peak_ratio (either may be NULL; pair i at element i*N, 4-byte aligned)
+void adc_launch_confidence(const AdcParams& P, const AdcWave& w, const float* vol, float* min_cost, float* peak_ratio,
+                           cudaStream_t st, unsigned long long* launches);
 void adc_launch_outlier(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_build_lists(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_voting(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);

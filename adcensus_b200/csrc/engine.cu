@@ -254,11 +254,27 @@ struct VolOuts {
     int n = 0;
 };
 
+// Side maps a call requests (adc_map_out), indexed by ADC_MAP_* kind, with the wave's destinations; nullptr = not requested.
+struct MapOuts {
+    void* dst[5] = {};
+};
+
+size_t map_elem_bytes(int kind) { return kind == ADC_MAP_OUTLIERS ? 1 : sizeof(float); }
+
 // The stage a volumes-only run stops after: the latest exported volume's.
 int last_export_stage(const adc_volume_out* outs, int n_outs) {
     static const int stop_after[3] = {ADC_STAGE_COST, ADC_STAGE_AGG4, ADC_STAGE_SO4};
     int last = ADC_STAGE_COST;
     for (int i = 0; i < n_outs; i++) last = std::max(last, stop_after[outs[i].stage]);
+    return last;
+}
+
+// The stage a run without a final map stops after: the latest requested volume's or map's (the outlier map is taken
+// after the LR check, every other map right after the WTA).
+int last_output_stage(const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps) {
+    int last = last_export_stage(vols, n_vols);
+    for (int i = 0; i < n_maps; i++)
+        last = std::max(last, maps[i].kind == ADC_MAP_OUTLIERS ? (int)ADC_STAGE_OUTLIER : (int)ADC_STAGE_WTA);
     return last;
 }
 
@@ -272,9 +288,11 @@ bool agg_fused_for(const adc_engine* e, int last_stage) {
 // stage boundaries the reference times in Match (ADCensusStereo.cpp:81-129).  `outs` (optional) are exported at the one
 // point where their volume is live (DESIGN.md section 11): COST in C0 right after stage 1, before the first aggregation
 // launch (the fused passes overwrite volB); AGGR in volA after the last aggregation pass, before scanline pass 2 writes volA;
-// OPT in volA after scanline pass 4, which nothing later writes.
+// OPT in volA after scanline pass 4, which nothing later writes.  `maps` (optional) likewise (DESIGN.md section 12): the
+// WTA maps and the confidence right after the WTA (disp_l is overwritten by the LR check), the outlier map right after
+// the LR check (region voting changes label).
 int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_t* ev, const CostSrc& cost = CostSrc(),
-                     const VolOuts& outs = VolOuts()) {
+                     const VolOuts& outs = VolOuts(), const MapOuts& maps = MapOuts()) {
     const AdcParams& P = e->P;
     const AdcWave w = wave_view(e, ln, nS);
     cudaStream_t st = ln.st;
@@ -359,6 +377,13 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
 
     // ---- stage 4: left + right disparity (ADCensusStereo.cpp:108-109)
     if (adc_launch_wta(P, w, A, st, L)) return fail(ADC_ERR_UNSUPPORTED, "WTA launch failed");
+    if (maps.dst[ADC_MAP_WTA_LEFT])
+        CK(cudaMemcpyAsync(maps.dst[ADC_MAP_WTA_LEFT], w.disp_l, mapN * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (maps.dst[ADC_MAP_WTA_RIGHT])
+        CK(cudaMemcpyAsync(maps.dst[ADC_MAP_WTA_RIGHT], w.disp_r, mapN * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (maps.dst[ADC_MAP_MIN_COST] || maps.dst[ADC_MAP_PEAK_RATIO])
+        adc_launch_confidence(P, w, A, static_cast<float*>(maps.dst[ADC_MAP_MIN_COST]),
+                              static_cast<float*>(maps.dst[ADC_MAP_PEAK_RATIO]), st, L);
     if ((rc = launched("winner-takes-all"))) return rc;
     if (ev) CK(cudaEventRecord(ev[4], st));
     if (stop(ADC_STAGE_WTA)) return ADC_OK;
@@ -371,6 +396,7 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
         CK(cudaMemsetAsync(w.label, 0, mapN, st));
         CK(cudaMemcpyAsync(w.disp_t, w.disp_l, mapN * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
+    if (maps.dst[ADC_MAP_OUTLIERS]) CK(cudaMemcpyAsync(maps.dst[ADC_MAP_OUTLIERS], w.label, mapN, cudaMemcpyDeviceToDevice, st));
     if (stop(ADC_STAGE_OUTLIER)) return launched("outlier detection");
     if (e->opt.do_filling) {  // gates voting AND interpolation (ADCensusStereo.cpp:183)
         CK(cudaMemsetAsync(w.counters, 0, (size_t)nS * ADC_CNT * sizeof(int), st));
@@ -424,7 +450,7 @@ enum SrcKind { SRC_HOST_PTRS, SRC_HOST_STRIDED, SRC_DEVICE_STRIDED };
 int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, const uint8_t* const* rp,
               float* const* dp, const uint8_t* ls, const uint8_t* rs, float* ds, cudaStream_t user, bool pinned,
               bool force_join = false, const CostSrc& cost = CostSrc(), int last_stage = ADC_STAGE_MEDIAN,
-              const adc_volume_out* outs = nullptr, int n_outs = 0) {
+              const adc_volume_out* outs = nullptr, int n_outs = 0, const adc_map_out* maps = nullptr, int n_maps = 0) {
     const size_t N = (size_t)e->P.dm.N, IMG = N * 3;
     const int S = e->S, nl = (int)e->lanes.size();
     CK(cudaEventRecord(e->ev_fork, user));
@@ -473,9 +499,12 @@ int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, cons
             wave_outs.o[i] = outs[i];
             wave_outs.o[i].dst = static_cast<char*>(outs[i].dst) + (size_t)first * N * e->P.dm.D * adc_cost_elem_bytes(outs[i].dtype);
         }
-        int rc = enqueue_pipeline(e, ln, nS, last_stage, nullptr, wave_cost, wave_outs);
+        MapOuts wave_maps;
+        for (int i = 0; i < n_maps; i++)
+            wave_maps.dst[maps[i].kind] = static_cast<char*>(maps[i].dst) + (size_t)first * N * map_elem_bytes(maps[i].kind);
+        int rc = enqueue_pipeline(e, ln, nS, last_stage, nullptr, wave_cost, wave_outs, wave_maps);
         if (rc) return rc;
-        // ---- outputs (a device call without a map output exports volumes only)
+        // ---- outputs (a device call without a map output gives exported volumes / side maps only)
         if (kind == SRC_DEVICE_STRIDED) {
             if (ds) CK(cudaMemcpyAsync(ds + (size_t)first * N, io.disp_l, (size_t)nS * N * sizeof(float), cudaMemcpyDeviceToDevice, rst));
         } else if (pinned) {
@@ -511,30 +540,55 @@ int check_cost_args(const char* fn, int layout, int dtype) {
 }
 
 // The argument rules of adc_match_volumes*, checked before any device work.  `device`: the destinations are the caller's
-// device buffers, written by the export kernel directly, and must be aligned to their element size.
-int check_volume_args(const char* fn, const adc_volume_out* outs, int n_outs, bool have_disp, bool have_cost, int cost_layout,
-                      int cost_dtype, bool device) {
-    if (n_outs < 0 || n_outs > 3) return fail(ADC_ERR_ARG, "%s: n_outs %d outside 0..3", fn, n_outs);
-    if (n_outs > 0 && !outs) return fail(ADC_ERR_ARG, "%s: outs is NULL with n_outs %d", fn, n_outs);
-    if (n_outs == 0 && !have_disp) return fail(ADC_ERR_ARG, "%s: disp is NULL and no volume is requested (n_outs 0)", fn);
+// device buffers, written by the export kernel directly, and must be aligned to their element size.  `what`: the name of
+// the request array in the entry point's signature ("outs" / "vols").  `need_output`: no final map is requested, so a
+// volume must be.
+int check_volume_args(const char* fn, const char* what, const adc_volume_out* outs, int n_outs, bool need_output, bool have_cost,
+                      int cost_layout, int cost_dtype, bool device) {
+    if (n_outs < 0 || n_outs > 3) return fail(ADC_ERR_ARG, "%s: n_%s %d outside 0..3", fn, what, n_outs);
+    if (n_outs > 0 && !outs) return fail(ADC_ERR_ARG, "%s: %s is NULL with n_%s %d", fn, what, what, n_outs);
+    if (n_outs == 0 && need_output) return fail(ADC_ERR_ARG, "%s: disp is NULL and no volume is requested (n_%s 0)", fn, what);
     for (int i = 0; i < n_outs; i++) {
         const adc_volume_out& o = outs[i];
-        if (o.stage < ADC_VOL_COST || o.stage > ADC_VOL_OPT) return fail(ADC_ERR_ARG, "%s: outs[%d].stage %d unknown", fn, i, o.stage);
+        if (o.stage < ADC_VOL_COST || o.stage > ADC_VOL_OPT) return fail(ADC_ERR_ARG, "%s: %s[%d].stage %d unknown", fn, what, i, o.stage);
         for (int j = 0; j < i; j++)
-            if (outs[j].stage == o.stage) return fail(ADC_ERR_ARG, "%s: outs[%d].stage %d requested twice", fn, i, o.stage);
-        if (o.layout != ADC_COST_HWD && o.layout != ADC_COST_DHW) return fail(ADC_ERR_ARG, "%s: outs[%d].layout %d unknown", fn, i, o.layout);
+            if (outs[j].stage == o.stage) return fail(ADC_ERR_ARG, "%s: %s[%d].stage %d requested twice", fn, what, i, o.stage);
+        if (o.layout != ADC_COST_HWD && o.layout != ADC_COST_DHW) return fail(ADC_ERR_ARG, "%s: %s[%d].layout %d unknown", fn, what, i, o.layout);
         if (o.dtype != ADC_COST_F32 && o.dtype != ADC_COST_F16 && o.dtype != ADC_COST_BF16)
-            return fail(ADC_ERR_ARG, "%s: outs[%d].dtype %d unknown", fn, i, o.dtype);
-        if (o.reserved != 0) return fail(ADC_ERR_ARG, "%s: outs[%d].reserved must be zero", fn, i);
-        if (!o.dst) return fail(ADC_ERR_ARG, "%s: outs[%d].dst is NULL", fn, i);
+            return fail(ADC_ERR_ARG, "%s: %s[%d].dtype %d unknown", fn, what, i, o.dtype);
+        if (o.reserved != 0) return fail(ADC_ERR_ARG, "%s: %s[%d].reserved must be zero", fn, what, i);
+        if (!o.dst) return fail(ADC_ERR_ARG, "%s: %s[%d].dst is NULL", fn, what, i);
         if (device && (uintptr_t)o.dst % adc_cost_elem_bytes(o.dtype))
-            return fail(ADC_ERR_ARG, "%s: outs[%d].dst is not aligned to its element size", fn, i);
+            return fail(ADC_ERR_ARG, "%s: %s[%d].dst is not aligned to its element size", fn, what, i);
     }
     if (have_cost) {
         if (cost_layout != ADC_COST_HWD && cost_layout != ADC_COST_DHW) return fail(ADC_ERR_ARG, "%s: unknown cost_layout %d", fn, cost_layout);
         if (cost_dtype != ADC_COST_F32 && cost_dtype != ADC_COST_F16 && cost_dtype != ADC_COST_BF16)
             return fail(ADC_ERR_ARG, "%s: unknown cost_dtype %d", fn, cost_dtype);
     }
+    return ADC_OK;
+}
+
+// The argument rules of adc_match_outputs*: those of the volume entries for vols, then the maps', then "some output".
+// `device`: f32 map destinations are written by kernels and device copies directly and must be 4-byte aligned.
+int check_output_args(const char* fn, const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps,
+                      bool have_disp, bool have_cost, int cost_layout, int cost_dtype, bool device) {
+    int rc = check_volume_args(fn, "vols", vols, n_vols, false, have_cost, cost_layout, cost_dtype, device);
+    if (rc) return rc;
+    if (n_maps < 0 || n_maps > 5) return fail(ADC_ERR_ARG, "%s: n_maps %d outside 0..5", fn, n_maps);
+    if (n_maps > 0 && !maps) return fail(ADC_ERR_ARG, "%s: maps is NULL with n_maps %d", fn, n_maps);
+    for (int i = 0; i < n_maps; i++) {
+        const adc_map_out& m = maps[i];
+        if (m.kind < ADC_MAP_WTA_LEFT || m.kind > ADC_MAP_PEAK_RATIO) return fail(ADC_ERR_ARG, "%s: maps[%d].kind %d unknown", fn, i, m.kind);
+        for (int j = 0; j < i; j++)
+            if (maps[j].kind == m.kind) return fail(ADC_ERR_ARG, "%s: maps[%d].kind %d requested twice", fn, i, m.kind);
+        if (m.reserved != 0) return fail(ADC_ERR_ARG, "%s: maps[%d].reserved must be zero", fn, i);
+        if (!m.dst) return fail(ADC_ERR_ARG, "%s: maps[%d].dst is NULL", fn, i);
+        if (device && (uintptr_t)m.dst % map_elem_bytes(m.kind))
+            return fail(ADC_ERR_ARG, "%s: maps[%d].dst is not 4-byte aligned", fn, i);
+    }
+    if (!have_disp && n_vols == 0 && n_maps == 0)
+        return fail(ADC_ERR_ARG, "%s: disp is NULL and no volume or map is requested (n_vols 0, n_maps 0)", fn);
     return ADC_OK;
 }
 
@@ -552,6 +606,102 @@ int upload_cost_pair(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t
     src->dtype = dtype;
     e->cost_layout = layout;
     e->cost_dtype = dtype;
+    return ADC_OK;
+}
+
+// The batched device driver of adc_match_volumes_batch_device and adc_match_outputs_batch_device (arguments checked).
+int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_left, const uint8_t* d_right, const void* d_cost,
+                         int cost_layout, int cost_dtype, float* d_disp, const adc_volume_out* vols, int n_vols,
+                         const adc_map_out* maps, int n_maps, cudaStream_t stream) {
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if (n < 0 || (n > 0 && (!d_left || !d_right))) return fail(ADC_ERR_ARG, "%s: bad arguments", fn);
+    if (n == 0) return ADC_OK;
+    CK(cudaSetDevice(e->cfg.device));
+    CostSrc src;
+    if (d_cost) {
+        src.p = d_cost;
+        src.layout = cost_layout;
+        src.dtype = cost_dtype;
+        e->cost_layout = cost_layout;
+        e->cost_dtype = cost_dtype;
+    }
+    if (n_vols > 0) {
+        e->export_layout = vols[n_vols - 1].layout;
+        e->export_dtype = vols[n_vols - 1].dtype;
+    }
+    const int last = d_disp ? ADC_STAGE_MEDIAN : last_output_stage(vols, n_vols, maps, n_maps);
+    return run_batch(e, n, SRC_DEVICE_STRIDED, nullptr, nullptr, nullptr, d_left, d_right, d_disp, stream, true, false, src,
+                     last, vols, n_vols, maps, n_maps);
+}
+
+// The one-pair host driver of adc_match_volumes and adc_match_outputs (arguments checked): volumes and maps go to device
+// staging first (one after the other), then to the caller's host buffers.
+int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const uint8_t* right, const void* cost, int cost_layout,
+                       int cost_dtype, float* disp, const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps) {
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if (!left || !right) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    Lane& ln = e->lanes[0];
+    const size_t N = (size_t)e->P.dm.N, IMG = N * 3, ND = N * e->P.dm.D;
+    int rc;
+    if ((rc = drain_lane(e, ln))) return rc;
+    CK(cudaStreamSynchronize(ln.st));
+    size_t need = 0;
+    for (int i = 0; i < n_vols; i++) need += align_up(ND * adc_cost_elem_bytes(vols[i].dtype), 256);
+    for (int i = 0; i < n_maps; i++) need += align_up(N * map_elem_bytes(maps[i].kind), 256);
+    if (need > e->vol_stage_bytes) {
+        if (e->vol_stage) CK(cudaFree(e->vol_stage));
+        e->vol_stage = nullptr;
+        e->vol_stage_bytes = 0;
+        if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
+            cudaGetLastError();
+            e->vol_stage = nullptr;
+            return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for the exported volumes and maps", fn, need);
+        }
+        e->vol_stage_bytes = need;
+    }
+    VolOuts dev;
+    dev.n = n_vols;
+    size_t off = 0;
+    for (int i = 0; i < n_vols; i++) {
+        dev.o[i] = vols[i];
+        dev.o[i].dst = static_cast<char*>(e->vol_stage) + off;
+        off += align_up(ND * adc_cost_elem_bytes(vols[i].dtype), 256);
+    }
+    MapOuts dev_maps;
+    for (int i = 0; i < n_maps; i++) {
+        dev_maps.dst[maps[i].kind] = static_cast<char*>(e->vol_stage) + off;
+        off += align_up(N * map_elem_bytes(maps[i].kind), 256);
+    }
+    if (n_vols > 0) {
+        e->export_layout = vols[n_vols - 1].layout;
+        e->export_dtype = vols[n_vols - 1].dtype;
+    }
+    const int last = disp ? ADC_STAGE_MEDIAN : last_output_stage(vols, n_vols, maps, n_maps);
+    cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
+    if (ev) CK(cudaEventRecord(ev[0], ln.st));
+    CostSrc src;
+    if (cost) {
+        if ((rc = upload_cost_pair(e, ln, left, right, cost, cost_layout, cost_dtype, last, &src))) return rc;
+    } else {
+        memcpy(ln.pin_in, left, IMG);
+        memcpy(ln.pin_in + IMG, right, IMG);
+        CK(cudaMemcpyAsync(ln.w.bgr, ln.pin_in, 2 * IMG, cudaMemcpyHostToDevice, ln.st));
+    }
+    if ((rc = enqueue_pipeline(e, ln, 1, last, ev, src, dev, dev_maps))) return rc;
+    if (disp) {
+        CK(cudaMemcpyAsync(ln.pin_out, ln.w.disp_l, N * sizeof(float), cudaMemcpyDeviceToHost, ln.st));
+        CK(cudaEventRecord(ev[6], ln.st));
+    }
+    CK(cudaStreamSynchronize(ln.st));
+    if (disp) {
+        memcpy(disp, ln.pin_out, N * sizeof(float));
+        for (int i = 0; i < 6; i++) CK(cudaEventElapsedTime(&e->stage_ms[i], ev[i], ev[i + 1]));
+    }
+    for (int i = 0; i < n_vols; i++)
+        CK(cudaMemcpy(vols[i].dst, dev.o[i].dst, ND * adc_cost_elem_bytes(vols[i].dtype), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n_maps; i++)
+        CK(cudaMemcpy(maps[i].dst, dev_maps.dst[maps[i].kind], N * map_elem_bytes(maps[i].kind), cudaMemcpyDeviceToHost));
     return ADC_OK;
 }
 
@@ -797,91 +947,37 @@ int adc_match_volumes_batch_device(adc_engine* e, int32_t n, const uint8_t* d_le
                                    int32_t cost_layout, int32_t cost_dtype, float* d_disp, const adc_volume_out* outs,
                                    int32_t n_outs, void* stream) {
     const char* fn = "adc_match_volumes_batch_device";
-    int rc = check_volume_args(fn, outs, n_outs, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
+    int rc = check_volume_args(fn, "outs", outs, n_outs, d_disp == nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
     if (rc) return rc;
-    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
-    if (n < 0 || (n > 0 && (!d_left || !d_right))) return fail(ADC_ERR_ARG, "%s: bad arguments", fn);
-    if (n == 0) return ADC_OK;
-    CK(cudaSetDevice(e->cfg.device));
-    CostSrc src;
-    if (d_cost) {
-        src.p = d_cost;
-        src.layout = cost_layout;
-        src.dtype = cost_dtype;
-        e->cost_layout = cost_layout;
-        e->cost_dtype = cost_dtype;
-    }
-    if (n_outs > 0) {
-        e->export_layout = outs[n_outs - 1].layout;
-        e->export_dtype = outs[n_outs - 1].dtype;
-    }
-    const int last = d_disp ? ADC_STAGE_MEDIAN : last_export_stage(outs, n_outs);
-    return run_batch(e, n, SRC_DEVICE_STRIDED, nullptr, nullptr, nullptr, d_left, d_right, d_disp, (cudaStream_t)stream, true,
-                     false, src, last, outs, n_outs);
+    return match_outputs_device(e, fn, n, d_left, d_right, d_cost, cost_layout, cost_dtype, d_disp, outs, n_outs, nullptr, 0,
+                                (cudaStream_t)stream);
 }
 
 int adc_match_volumes(adc_engine* e, const uint8_t* left, const uint8_t* right, const void* cost, int32_t cost_layout,
                       int32_t cost_dtype, float* disp, const adc_volume_out* outs, int32_t n_outs) {
     const char* fn = "adc_match_volumes";
-    int rc = check_volume_args(fn, outs, n_outs, disp != nullptr, cost != nullptr, cost_layout, cost_dtype, false);
+    int rc = check_volume_args(fn, "outs", outs, n_outs, disp == nullptr, cost != nullptr, cost_layout, cost_dtype, false);
     if (rc) return rc;
-    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
-    if (!left || !right) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
-    CK(cudaSetDevice(e->cfg.device));
-    Lane& ln = e->lanes[0];
-    const size_t N = (size_t)e->P.dm.N, IMG = N * 3, ND = N * e->P.dm.D;
-    if ((rc = drain_lane(e, ln))) return rc;
-    CK(cudaStreamSynchronize(ln.st));
-    // the exports go to device staging first (one volume after the other), then to the caller's host buffers
-    size_t need = 0;
-    for (int i = 0; i < n_outs; i++) need += align_up(ND * adc_cost_elem_bytes(outs[i].dtype), 256);
-    if (need > e->vol_stage_bytes) {
-        if (e->vol_stage) CK(cudaFree(e->vol_stage));
-        e->vol_stage = nullptr;
-        e->vol_stage_bytes = 0;
-        if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
-            cudaGetLastError();
-            e->vol_stage = nullptr;
-            return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for the exported volumes", fn, need);
-        }
-        e->vol_stage_bytes = need;
-    }
-    VolOuts dev;
-    dev.n = n_outs;
-    size_t off = 0;
-    for (int i = 0; i < n_outs; i++) {
-        dev.o[i] = outs[i];
-        dev.o[i].dst = static_cast<char*>(e->vol_stage) + off;
-        off += align_up(ND * adc_cost_elem_bytes(outs[i].dtype), 256);
-    }
-    if (n_outs > 0) {
-        e->export_layout = outs[n_outs - 1].layout;
-        e->export_dtype = outs[n_outs - 1].dtype;
-    }
-    const int last = disp ? ADC_STAGE_MEDIAN : last_export_stage(outs, n_outs);
-    cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
-    if (ev) CK(cudaEventRecord(ev[0], ln.st));
-    CostSrc src;
-    if (cost) {
-        if ((rc = upload_cost_pair(e, ln, left, right, cost, cost_layout, cost_dtype, last, &src))) return rc;
-    } else {
-        memcpy(ln.pin_in, left, IMG);
-        memcpy(ln.pin_in + IMG, right, IMG);
-        CK(cudaMemcpyAsync(ln.w.bgr, ln.pin_in, 2 * IMG, cudaMemcpyHostToDevice, ln.st));
-    }
-    if ((rc = enqueue_pipeline(e, ln, 1, last, ev, src, dev))) return rc;
-    if (disp) {
-        CK(cudaMemcpyAsync(ln.pin_out, ln.w.disp_l, N * sizeof(float), cudaMemcpyDeviceToHost, ln.st));
-        CK(cudaEventRecord(ev[6], ln.st));
-    }
-    CK(cudaStreamSynchronize(ln.st));
-    if (disp) {
-        memcpy(disp, ln.pin_out, N * sizeof(float));
-        for (int i = 0; i < 6; i++) CK(cudaEventElapsedTime(&e->stage_ms[i], ev[i], ev[i + 1]));
-    }
-    for (int i = 0; i < n_outs; i++)
-        CK(cudaMemcpy(outs[i].dst, dev.o[i].dst, ND * adc_cost_elem_bytes(outs[i].dtype), cudaMemcpyDeviceToHost));
-    return ADC_OK;
+    return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, outs, n_outs, nullptr, 0);
+}
+
+int adc_match_outputs_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right, const void* d_cost,
+                                   int32_t cost_layout, int32_t cost_dtype, float* d_disp, const adc_volume_out* vols,
+                                   int32_t n_vols, const adc_map_out* maps, int32_t n_maps, void* stream) {
+    const char* fn = "adc_match_outputs_batch_device";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
+    if (rc) return rc;
+    return match_outputs_device(e, fn, n, d_left, d_right, d_cost, cost_layout, cost_dtype, d_disp, vols, n_vols, maps, n_maps,
+                                (cudaStream_t)stream);
+}
+
+int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, const void* cost, int32_t cost_layout,
+                      int32_t cost_dtype, float* disp, const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps,
+                      int32_t n_maps) {
+    const char* fn = "adc_match_outputs";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, disp != nullptr, cost != nullptr, cost_layout, cost_dtype, false);
+    if (rc) return rc;
+    return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps);
 }
 
 void* adc_host_alloc(size_t bytes) {
@@ -1015,6 +1111,10 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
             case 11:    // volA's volumes exported into volB (N*D elements of at most 4 bytes fit in N*Dp floats)
                 adc_launch_cost_export(P, w, w.volA, w.volB, e->export_layout, e->export_dtype, ln.st, &e->launches);
                 bytes = N * P.dm.Dp * 4.0 + N * P.dm.D * (double)adc_cost_elem_bytes(e->export_dtype);
+                break;
+            case 12:    // both confidence maps of volA into volB (2*N floats of a pair fit in its N*Dp, Dp >= 4)
+                adc_launch_confidence(P, w, w.volA, w.volB, w.volB + (size_t)e->S * P.dm.N, ln.st, &e->launches);
+                bytes = N * P.dm.Dp * 4.0 + 2 * 4.0 * N;
                 break;
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);
         }

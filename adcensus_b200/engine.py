@@ -72,6 +72,19 @@ class VolumeOut(ctypes.Structure):
                 ("dtype", ctypes.c_int32), ("reserved", ctypes.c_int32)]
 
 
+# per-pixel side maps (adc_match_outputs*): which map a request names, and its element type
+MAP_WTA_LEFT, MAP_WTA_RIGHT, MAP_OUTLIERS, MAP_MIN_COST, MAP_PEAK_RATIO = 0, 1, 2, 3, 4
+MAP_KINDS = {"wta_left": MAP_WTA_LEFT, "wta_right": MAP_WTA_RIGHT, "outliers": MAP_OUTLIERS, "min_cost": MAP_MIN_COST,
+             "peak_ratio": MAP_PEAK_RATIO}
+_MAP_NP = {MAP_WTA_LEFT: np.float32, MAP_WTA_RIGHT: np.float32, MAP_OUTLIERS: np.uint8, MAP_MIN_COST: np.float32,
+           MAP_PEAK_RATIO: np.float32}
+
+
+class MapOut(ctypes.Structure):
+    """adc_map_out: one requested side map (destination, ADC_MAP_* kind)."""
+    _fields_ = [("dst", ctypes.c_void_p), ("kind", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -127,6 +140,10 @@ def load_library() -> ctypes.CDLL:
     L.adc_debug_run_cost.argtypes = [vp, u8p, u8p, vp, i32, i32, i32]
     L.adc_match_volumes.argtypes = [vp, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32]
     L.adc_match_volumes_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32, vp]
+    L.adc_match_outputs.argtypes = [vp, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32,
+                                    ctypes.POINTER(MapOut), i32]
+    L.adc_match_outputs_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32,
+                                                 ctypes.POINTER(MapOut), i32, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -160,6 +177,14 @@ def _volume_outs(outs):
     for i, (ptr, stage, layout, dtype) in enumerate(outs):
         arr[i] = VolumeOut(ptr, _code(VOL_STAGES, stage, "volume stage"), _code(COST_LAYOUTS, layout, "layout"),
                            _code(COST_DTYPES, dtype, "dtype"), 0)
+    return arr
+
+
+def _map_outs(maps):
+    """ctypes array of adc_map_out from (ptr, kind) tuples (names or ADC_MAP_* codes)."""
+    arr = (MapOut * max(1, len(maps)))()
+    for i, (ptr, kind) in enumerate(maps):
+        arr[i] = MapOut(ptr, _code(MAP_KINDS, kind, "map kind"), 0)
     return arr
 
 
@@ -277,6 +302,45 @@ class Engine:
                                                       _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, arr,
                                                       len(outs), stream))
 
+    # ---- per-pixel side maps, with or without volumes (adc_match_outputs*) -----------------------
+    def match_outputs(self, left, right, maps=(), volumes=(), layout="hwd", dtype="f32", cost=None, cost_layout="hwd",
+                      cost_dtype=None, disparity=True):
+        """(disparity map or None, {name: array}) of one pair from one pipeline pass.  `maps`: any of "wta_left",
+        "wta_right" (float32 [H][W], the WTA's maps before refinement), "outliers" (uint8 [H][W], 0 kept / 1 mismatch /
+        2 occlusion before region voting), "min_cost", "peak_ratio" (float32 [H][W], the cost-curve confidence).
+        `volumes`: any of "cost", "aggr", "opt" in `layout` / `dtype`, as for match_volumes.  `cost`: a caller's matching
+        cost, as for match_cost.  disparity=False stops the pipeline after the latest requested output."""
+        left = _img(left, (self.height, self.width, 3))
+        right = _img(right, (self.height, self.width, 3))
+        maps = [maps] if isinstance(maps, (str, int)) else list(maps)
+        volumes = [volumes] if isinstance(volumes, (str, int)) else list(volumes)
+        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
+        H, W, D = self.height, self.width, self.D
+        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
+        out = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in volumes}
+        vouts = _volume_outs([(out[s].ctypes.data, s, lay, dt) for s in volumes])
+        for m in maps:
+            out[m] = np.empty((H, W), _MAP_NP.get(_code(MAP_KINDS, m, "map kind"), np.float32))
+        mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
+        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
+        disp = np.empty((H, W), np.float32) if disparity else None
+        _check(self._L.adc_match_outputs(self._h, left.ctypes.data, right.ctypes.data, None if c is None else c.ctypes.data,
+                                         clay, cdt, None if disp is None else disp.ctypes.data, vouts, len(volumes),
+                                         mouts, len(maps)))
+        return disp, out
+
+    def match_outputs_batch_device(self, n: int, d_left: int, d_right: int, maps=(), volumes=(), d_disp: int = 0,
+                                   d_cost: int = 0, cost_layout="dhw", cost_dtype="f32", stream: int = 0):
+        """Device pointers (ints): n pairs of images, optional n cost volumes, optional n maps (d_disp 0 = no final map);
+        `maps` a list of (ptr, kind), each ptr n maps of H*W elements (float32, uint8 for "outliers"); `volumes` a list
+        of (ptr, stage, layout, dtype) as for match_volumes_batch_device.  Enqueued on `stream` without synchronising,
+        like match_batch_device."""
+        varr, marr = _volume_outs(volumes), _map_outs(maps)
+        _check(self._L.adc_match_outputs_batch_device(self._h, n, d_left, d_right, d_cost or None,
+                                                      _code(COST_LAYOUTS, cost_layout, "layout"),
+                                                      _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
+                                                      len(volumes), marr, len(maps), stream))
+
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
         lefts = np.ascontiguousarray(lefts, np.uint8)
@@ -320,7 +384,7 @@ class Engine:
 
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
                        "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10,
-                       "cost_export": 11}
+                       "cost_export": 11, "confidence": 12}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""

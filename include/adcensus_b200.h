@@ -207,6 +207,55 @@ int adc_match_volumes_batch_device(adc_engine* e, int32_t n, const uint8_t* d_le
 int adc_match_volumes(adc_engine* e, const uint8_t* left, const uint8_t* right, const void* cost, int32_t cost_layout,
                       int32_t cost_dtype, float* disp, const adc_volume_out* outs, int32_t n_outs);
 
+/* ---- per-pixel side maps ---------------------------------------------------------------------------
+ * The entry points below hand out, for every pair and in the same pipeline pass, up to five [H][W] maps next to (or
+ * instead of) the final disparity map and the exported volumes (pair i at element i*H*W of its destination):
+ *   ADC_MAP_WTA_LEFT    f32  the left map right after the WTA, before any refinement: disp_left_ after ComputeDisparity
+ *   ADC_MAP_WTA_RIGHT   f32  the right-view map: disp_right_ (what adc_get_right_disparity gives for one pair)
+ *   ADC_MAP_OUTLIERS    u8   0 = kept, 1 = mismatch, 2 = occlusion, as the LR check classified the pixel BEFORE region
+ *                            voting (the pixels of mismatches_ / occlusions_ after OutlierDetection); all 0 when
+ *                            do_lr_check is off
+ *   ADC_MAP_MIN_COST    f32  c1 = C(d1)
+ *   ADC_MAP_PEAK_RATIO  f32  c1 / c2 in [0, 1]; 0 = unique minimum, 1 = ambiguous
+ * Confidence definitions.  C is the scanline-optimised volume, the one the WTA reads and ADC_VOL_OPT exports; d runs
+ * over [0, D).
+ *   d1 = the smallest d where C(d) is minimal.  This is the index the left WTA picks: it scans with a strict '>' from
+ *        99999, and every cost is below that.  It is defined for every pixel, including pixels whose WTA value is
+ *        Invalid because d1 lies at either end of the range.
+ *   c2 = min of C(d) over |d - d1| >= 2.  The immediate neighbours are excluded, as in OpenCV's uniqueness check.
+ *   PEAK_RATIO = c1 / c2, an IEEE round-to-nearest f32 division (__fdiv_rn).  It is 1.0f when no d with |d - d1| >= 2
+ *        exists (D <= 2, or D = 3 with d1 = 1) or when c2 == 0; in that case c1 == 0 too, because the costs are
+ *        non-negative.
+ * The WTA maps and the confidence are enqueued right after the WTA (counted in its stage by adc_last_stage_ms), the
+ * outlier map right after the LR check (counted in refinement).  The confidence costs one extra read of the optimised
+ * volume; the other maps are copies.  The final map of a call with side maps is bit-identical to the same call without.
+ * disp NULL = no final map: the pipeline stops after the latest requested output (the WTA for the WTA and confidence
+ * maps, the LR check for ADC_MAP_OUTLIERS, the stage of the latest exported volume), so no voting, interpolation or
+ * median runs.
+ * Fails with ADC_ERR_ARG before any device work, naming the field: every rule of the volume entries above for vols /
+ * n_vols; n_maps outside 0..5; maps NULL with n_maps > 0; a kind requested twice or unknown; a NULL dst; a non-zero
+ * reserved; on the device entry an f32 map's dst not 4-byte aligned (u8 maps may start at any byte); no map, no volume
+ * and no disp. */
+enum { ADC_MAP_WTA_LEFT = 0, ADC_MAP_WTA_RIGHT = 1, ADC_MAP_OUTLIERS = 2, ADC_MAP_MIN_COST = 3, ADC_MAP_PEAK_RATIO = 4 };
+typedef struct adc_map_out {
+    void*   dst;      /* n maps of H*W elements (f32, or u8 for ADC_MAP_OUTLIERS), pair i at element i*H*W */
+    int32_t kind;     /* ADC_MAP_* */
+    int32_t reserved; /* must be zero */
+} adc_map_out;
+
+/* adc_match_volumes_batch_device plus side maps: one pipeline pass gives the final map (d_disp), the exported volumes
+ * (vols) and the maps (maps), any of them optional but not all.  Device pointers; stream, fork/join and pipelined-mode
+ * behaviour as for adc_match_batch_device. */
+int adc_match_outputs_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                   const void* d_cost, int32_t cost_layout, int32_t cost_dtype, float* d_disp,
+                                   const adc_volume_out* vols, int32_t n_vols,
+                                   const adc_map_out* maps, int32_t n_maps, void* stream);
+/* One pair, host pointers, synchronous; volumes and maps pass through the device staging of adc_match_volumes.  With
+ * disp: adc_last_stage_ms and adc_get_right_disparity behave as after adc_match; without, neither is meaningful. */
+int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, const void* cost,
+                      int32_t cost_layout, int32_t cost_dtype, float* disp,
+                      const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
@@ -227,7 +276,8 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * arm sum with division, 9 = vertical arm sum without division, 10 = cost-volume ingestion (layout and element type of
  * the engine's last cost call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*D*sizeof(element) + N*Dp*4 bytes per
  * pair, Dp = D rounded up to a multiple of 4), 11 = volume export (layout and element type of the engine's last export
- * call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*Dp*4 + N*D*sizeof(element) bytes per pair).
+ * call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*Dp*4 + N*D*sizeof(element) bytes per pair), 12 = confidence
+ * (MIN_COST and PEAK_RATIO of the left view; N*Dp*4 + 2*4*N bytes per pair).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 

@@ -38,6 +38,49 @@ from bench_cost_input import card  # noqa: E402
 GOLDEN_TAP = {"cost": "COST/VOL_INIT", "aggr": "AGG4/VOL_AGGR", "opt": "SO4/VOL_AGGR"}
 
 
+def alternating_windows(eng, st, paths, steps, warmup, rounds):
+    """{path name: [ms per window]}: each path (a function that enqueues one step on `st`) is warmed up, then the paths
+    are timed in `rounds` alternating windows of `steps` steps each, CUDA events around a window joined on `st`."""
+    def timed(fn):
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(st)
+        for _ in range(steps):
+            fn()
+        eng.join(st.cuda_stream)
+        e1.record(st)
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1)
+
+    for fn in paths:
+        for _ in range(max(2, warmup)):
+            fn()
+        eng.join(st.cuda_stream)
+    ms = {fn.__name__: [] for fn in paths}
+    for _ in range(rounds):
+        for fn in paths:
+            ms[fn.__name__].append(timed(fn))
+    torch.cuda.synchronize()
+    return ms
+
+
+def d2d_copy(src, nbytes, reps):
+    """(ms, GB/s with read + write counted) of a device-to-device copy (torch copy_, cudaMemcpyAsync) of the first
+    `nbytes` bytes of the uint8 device tensor `src`, CUDA events over `reps` copies."""
+    src = src[:nbytes]
+    dst = torch.empty(nbytes, dtype=torch.uint8, device=src.device)
+    dst.copy_(src)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        dst.copy_(src)
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1) / reps
+    return ms, 2 * nbytes / (ms * 1e-3) / 1e9
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--export", required=True,
@@ -85,27 +128,7 @@ def main():
             eng.match_volumes_batch_device(min(ring_pairs, n - j), d_left[j:].data_ptr(), d_right[j:].data_ptr(),
                                            [(ring_v.data_ptr(), stage, layout, dtype)], stream=st.cuda_stream)
 
-    def timed(fn):
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(st)
-        for _ in range(args.steps):
-            fn()
-        eng.join(st.cuda_stream)
-        e1.record(st)
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1)
-
-    paths = (regular, export, volumes_only)
-    for fn in paths:
-        for _ in range(max(2, args.warmup)):
-            fn()
-        eng.join(st.cuda_stream)
-    ms = {fn.__name__: [] for fn in paths}
-    for _ in range(args.rounds):
-        for fn in paths:
-            ms[fn.__name__].append(timed(fn))
-    torch.cuda.synchronize()
+    ms = alternating_windows(eng, st, (regular, export, volumes_only), args.steps, args.warmup, args.rounds)
     reg, exp = d_disp.cpu().numpy(), d_disp_x.cpu().numpy()
     reg_ok = all(T.sha(reg[i]) == golden for i in range(n))
     exp_maps_ok = all(T.sha(exp[i]) == golden for i in range(n))
@@ -124,19 +147,8 @@ def main():
     reps = 50
     k_ms, k_bytes = eng.profile_kernel("cost_export", reps=reps)
     cp_bytes = int(k_bytes // 2)                         # a copy of B bytes reads B and writes B
-    src = ring_x.view(torch.uint8).reshape(-1)[:cp_bytes]
-    dst = torch.empty(cp_bytes, dtype=torch.uint8, device=dev)
-    dst.copy_(src)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        dst.copy_(src)
-    e1.record()
-    torch.cuda.synchronize()
-    cp_ms = e0.elapsed_time(e1) / reps
+    cp_ms, cp_gbs = d2d_copy(ring_x.view(torch.uint8).reshape(-1), cp_bytes, reps)
     k_gbs = k_bytes / (k_ms * 1e-3) / 1e9
-    cp_gbs = 2 * cp_bytes / (cp_ms * 1e-3) / 1e9
     rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
     checked = "every timed map: sha256 of the unmodified reference's map"
     vol_checked = "every ring volume of the last call: the single-pair adc_match_volumes export" + \
