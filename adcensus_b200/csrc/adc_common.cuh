@@ -1,7 +1,8 @@
 // adc_common.cuh -- shared declarations for the sm_90a AD-Census kernels.
 //
 // Data layout in HBM (per wave of S stereo pairs; every array is [S][...], pair index outermost):
-//   bgr      u8  [S][2][H][W][3]   left, right packed BGR exactly as the caller passes them
+//   bgr      u8  [S][2][H][W][3]   left, right packed BGR: copied as the caller passes them, or written by the image
+//                                  ingestion kernel (k_image.cu) from another format / pitch
 //   gray     u8  [S][2][H][W]
 //   census   u64 [S][2][H][W]
 //   volA/B   f32 [S][H][W][Dp]     the two cost volumes, d fastest, Dp = D rounded up to 4 so that
@@ -137,6 +138,15 @@ size_t adc_cost_elem_bytes(int dtype);
 // ADC_COST_HWD / ADC_COST_DHW, element type ADC_COST_F32 / F16 / BF16 rounded to nearest even); dst aligned to its element
 void adc_launch_cost_export(const AdcParams& P, const AdcWave& w, const float* vol, void* dst, int layout, int dtype,
                             cudaStream_t st, unsigned long long* launches);
+// image ingestion (k_image.cu): the wave's views at left / right (pair i at byte i*image_stride, format ADC_IMG_*, pitches
+// resolved: no zero defaults left) -> w.bgr as packed BGR
+struct AdcImageGeom {
+    int format;
+    long long row_pitch, plane_pitch, image_stride;
+};
+void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
+                             const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches);
+int adc_image_bytes_per_pixel(int format);   // per plane for ADC_IMG_RGB_PLANAR
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

@@ -27,6 +27,9 @@ static_assert(sizeof(adc_option) == 60, "adc_option must match the reference's A
 static_assert(offsetof(adc_option, so_p1) == 32 && offsetof(adc_option, irv_th) == 48 &&
               offsetof(adc_option, do_lr_check) == 56 && offsetof(adc_option, do_discontinuity_adjustment) == 58,
               "adc_option field offsets must match adcensus_types.h:45-75");
+static_assert(sizeof(adc_image_desc) == 32 && offsetof(adc_image_desc, reserved) == 4 &&
+              offsetof(adc_image_desc, row_pitch) == 8 && offsetof(adc_image_desc, plane_pitch) == 16 &&
+              offsetof(adc_image_desc, image_stride) == 24, "adc_image_desc layout (include/adcensus_b200.h)");
 
 namespace {
 
@@ -93,6 +96,8 @@ struct adc_engine {
     int cost_layout = ADC_COST_DHW, cost_dtype = ADC_COST_F32;
     // layout / element type of the last volume export (adc_profile_kernel's export timing)
     int export_layout = ADC_COST_DHW, export_dtype = ADC_COST_F32;
+    // image format of the last adc_match_images* call (adc_profile_kernel's ingestion timing)
+    int img_format = ADC_IMG_RGB_PLANAR;
     // device staging of adc_match_volumes' exported volumes: allocated on first use, grown when needed
     void* vol_stage = nullptr;
     size_t vol_stage_bytes = 0;
@@ -447,10 +452,13 @@ enum SrcKind { SRC_HOST_PTRS, SRC_HOST_STRIDED, SRC_DEVICE_STRIDED };
 // Common batch driver.  `user` = stream to fork from / join to.
 // `force_join`: the call is one of the synchronous entry points, whose results must be complete on return whatever the
 // engine's pipelined setting (adc_set_pipelined only changes the asynchronous entry points).
+// `img` (SRC_DEVICE_STRIDED only): the resolved geometry of images that are not tight packed BGR, converted by the
+// ingestion kernel; nullptr = tight packed BGR, copied.
 int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, const uint8_t* const* rp,
               float* const* dp, const uint8_t* ls, const uint8_t* rs, float* ds, cudaStream_t user, bool pinned,
               bool force_join = false, const CostSrc& cost = CostSrc(), int last_stage = ADC_STAGE_MEDIAN,
-              const adc_volume_out* outs = nullptr, int n_outs = 0, const adc_map_out* maps = nullptr, int n_maps = 0) {
+              const adc_volume_out* outs = nullptr, int n_outs = 0, const adc_map_out* maps = nullptr, int n_maps = 0,
+              const AdcImageGeom* img = nullptr) {
     const size_t N = (size_t)e->P.dm.N, IMG = N * 3;
     const int S = e->S, nl = (int)e->lanes.size();
     CK(cudaEventRecord(e->ev_fork, user));
@@ -461,7 +469,10 @@ int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, cons
         const int first = wv * S, nS = std::min(S, n - first);
         const AdcWave& io = ln.w;   // where the images go in and the map comes out
         // ---- inputs -> io.bgr  ([S][2][IMG])
-        if (kind == SRC_DEVICE_STRIDED) {
+        if (kind == SRC_DEVICE_STRIDED && img) {
+            const long long off = (long long)first * img->image_stride;
+            adc_launch_image_ingest(e->P, wave_view(e, ln, nS), ls + off, rs + off, *img, ln.st, &e->launches);
+        } else if (kind == SRC_DEVICE_STRIDED) {
             CK(cudaMemcpy2DAsync(io.bgr, 2 * IMG, ls + (size_t)first * IMG, IMG, IMG, nS, cudaMemcpyDeviceToDevice, ln.st));
             CK(cudaMemcpy2DAsync(io.bgr + IMG, 2 * IMG, rs + (size_t)first * IMG, IMG, IMG, nS, cudaMemcpyDeviceToDevice, ln.st));
         } else if (pinned) {
@@ -592,14 +603,83 @@ int check_output_args(const char* fn, const adc_volume_out* vols, int n_vols, co
     return ADC_OK;
 }
 
+// The rules of an image descriptor that need no image size (adc_match_images*, checked before the engine).
+int check_image_desc(const char* fn, const adc_image_desc* img) {
+    if (!img) return ADC_OK;
+    if (img->format < ADC_IMG_BGR || img->format > ADC_IMG_RGB_PLANAR) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
+    if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
+    if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
+    if (img->plane_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is negative", fn, (long long)img->plane_pitch);
+    if (img->image_stride < 0) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld is negative", fn, (long long)img->image_stride);
+    if (img->format != ADC_IMG_RGB_PLANAR && img->plane_pitch != 0)
+        return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format that is not ADC_IMG_RGB_PLANAR", fn);
+    return ADC_OK;
+}
+
+// The size-dependent rules of an image descriptor (NULL = tight packed BGR); `g` receives the geometry with every zero
+// default replaced.
+int resolve_image(const adc_engine* e, const char* fn, const adc_image_desc* img, AdcImageGeom* g) {
+    const adc_image_desc d = img ? *img : adc_image_desc{};
+    const long long W = e->W, H = e->H, bpp = adc_image_bytes_per_pixel(d.format);
+    g->format = d.format;
+    g->row_pitch = d.row_pitch ? (long long)d.row_pitch : W * bpp;
+    if (g->row_pitch < W * bpp)
+        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is less than W * bytes per pixel (%lld)", fn, g->row_pitch, W * bpp);
+    long long foot = 0;
+    if (__builtin_mul_overflow(H, g->row_pitch, &foot)) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is too large", fn, g->row_pitch);
+    g->plane_pitch = 0;
+    if (d.format == ADC_IMG_RGB_PLANAR) {
+        g->plane_pitch = d.plane_pitch ? (long long)d.plane_pitch : foot;
+        if (g->plane_pitch < foot)
+            return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is less than H * row_pitch (%lld)", fn, g->plane_pitch, foot);
+        if (__builtin_mul_overflow(3ll, g->plane_pitch, &foot))
+            return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is too large", fn, g->plane_pitch);
+    }
+    g->image_stride = d.image_stride ? (long long)d.image_stride : foot;
+    if (g->image_stride < foot)
+        return fail(ADC_ERR_ARG, "%s: img->image_stride %lld is less than the view's footprint (%lld)", fn, g->image_stride, foot);
+    return ADC_OK;
+}
+
+bool tight_bgr(const adc_engine* e, const AdcImageGeom& g) {
+    return g.format == ADC_IMG_BGR && g.row_pitch == 3ll * e->W && g.image_stride == 3ll * e->W * e->H;
+}
+
+// One pair of the host entry's images (geometry g) -> ln.w.bgr.  Packed BGR rows go straight into bgr (the 2D copy
+// drops any row padding).  Every other format is uploaded tightly, view after view, into the lane volume that stage 1
+// writes, and converted from there by the ingestion kernel: nothing reads that volume before stage 1 overwrites it, the
+// cost-input staging of upload_cost_pair is the other volume, and the export / map staging is a separate allocation.
+int upload_images(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g, int last_stage) {
+    const size_t W = (size_t)e->W, H = (size_t)e->H, N = W * H, IMG = N * 3;
+    const size_t bpp = (size_t)adc_image_bytes_per_pixel(g.format);
+    if (g.format == ADC_IMG_BGR) {
+        CK(cudaMemcpy2DAsync(ln.w.bgr, 3 * W, left, (size_t)g.row_pitch, 3 * W, H, cudaMemcpyHostToDevice, ln.st));
+        CK(cudaMemcpy2DAsync(ln.w.bgr + IMG, 3 * W, right, (size_t)g.row_pitch, 3 * W, H, cudaMemcpyHostToDevice, ln.st));
+        return ADC_OK;
+    }
+    uint8_t* stage = reinterpret_cast<uint8_t*>(agg_fused_for(e, last_stage) ? ln.w.volB : ln.w.volA);
+    const bool planar = g.format == ADC_IMG_RGB_PLANAR;
+    const size_t foot = planar ? 3 * N : bpp * N;
+    for (int v = 0; v < 2; v++)
+        for (int c = 0; c < (planar ? 3 : 1); c++)
+            CK(cudaMemcpy2DAsync(stage + v * foot + c * N, bpp * W, (v ? right : left) + c * g.plane_pitch, (size_t)g.row_pitch,
+                                 bpp * W, H, cudaMemcpyHostToDevice, ln.st));
+    const AdcImageGeom tight{g.format, (long long)(bpp * W), planar ? (long long)N : 0, (long long)foot};
+    adc_launch_image_ingest(e->P, wave_view(e, ln, 1), stage, stage + foot, tight, ln.st, &e->launches);
+    return ADC_OK;
+}
+
 // Host entry points of cost-input mode: the raw volume of one pair (at most N*D*4 bytes) goes into the lane's volume
-// that stage 1 does NOT write, and is ingested from there.  Also uploads the images.
+// that stage 1 does NOT write, and is ingested from there.  Also uploads the images, unless left is NULL (the caller
+// uploaded them with upload_images).
 int upload_cost_pair(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t* right, const void* cost, int layout,
                      int dtype, int last_stage, CostSrc* src) {
     const size_t N = (size_t)e->P.dm.N, IMG = N * 3;
     void* staging = agg_fused_for(e, last_stage) ? (void*)ln.w.volA : (void*)ln.w.volB;
-    CK(cudaMemcpyAsync(ln.w.bgr, left, IMG, cudaMemcpyHostToDevice, ln.st));
-    CK(cudaMemcpyAsync(ln.w.bgr + IMG, right, IMG, cudaMemcpyHostToDevice, ln.st));
+    if (left) {
+        CK(cudaMemcpyAsync(ln.w.bgr, left, IMG, cudaMemcpyHostToDevice, ln.st));
+        CK(cudaMemcpyAsync(ln.w.bgr + IMG, right, IMG, cudaMemcpyHostToDevice, ln.st));
+    }
     CK(cudaMemcpyAsync(staging, cost, N * e->P.dm.D * adc_cost_elem_bytes(dtype), cudaMemcpyHostToDevice, ln.st));
     src->p = staging;
     src->layout = layout;
@@ -609,10 +689,11 @@ int upload_cost_pair(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t
     return ADC_OK;
 }
 
-// The batched device driver of adc_match_volumes_batch_device and adc_match_outputs_batch_device (arguments checked).
+// The batched device driver of adc_match_volumes_batch_device, adc_match_outputs_batch_device and
+// adc_match_images_batch_device (arguments checked; img = resolved geometry of images that are not tight packed BGR).
 int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_left, const uint8_t* d_right, const void* d_cost,
                          int cost_layout, int cost_dtype, float* d_disp, const adc_volume_out* vols, int n_vols,
-                         const adc_map_out* maps, int n_maps, cudaStream_t stream) {
+                         const adc_map_out* maps, int n_maps, cudaStream_t stream, const AdcImageGeom* img = nullptr) {
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if (n < 0 || (n > 0 && (!d_left || !d_right))) return fail(ADC_ERR_ARG, "%s: bad arguments", fn);
     if (n == 0) return ADC_OK;
@@ -631,13 +712,15 @@ int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_
     }
     const int last = d_disp ? ADC_STAGE_MEDIAN : last_output_stage(vols, n_vols, maps, n_maps);
     return run_batch(e, n, SRC_DEVICE_STRIDED, nullptr, nullptr, nullptr, d_left, d_right, d_disp, stream, true, false, src,
-                     last, vols, n_vols, maps, n_maps);
+                     last, vols, n_vols, maps, n_maps, img);
 }
 
-// The one-pair host driver of adc_match_volumes and adc_match_outputs (arguments checked): volumes and maps go to device
-// staging first (one after the other), then to the caller's host buffers.
+// The one-pair host driver of adc_match_volumes, adc_match_outputs and adc_match_images (arguments checked): volumes and
+// maps go to device staging first (one after the other), then to the caller's host buffers.  img = the images' resolved
+// geometry, nullptr = tight packed BGR.
 int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const uint8_t* right, const void* cost, int cost_layout,
-                       int cost_dtype, float* disp, const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps) {
+                       int cost_dtype, float* disp, const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps,
+                       const AdcImageGeom* img = nullptr) {
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if (!left || !right) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
     CK(cudaSetDevice(e->cfg.device));
@@ -681,7 +764,10 @@ int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const
     cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
     if (ev) CK(cudaEventRecord(ev[0], ln.st));
     CostSrc src;
-    if (cost) {
+    if (img) {
+        if ((rc = upload_images(e, ln, left, right, *img, last))) return rc;
+        if (cost && (rc = upload_cost_pair(e, ln, nullptr, nullptr, cost, cost_layout, cost_dtype, last, &src))) return rc;
+    } else if (cost) {
         if ((rc = upload_cost_pair(e, ln, left, right, cost, cost_layout, cost_dtype, last, &src))) return rc;
     } else {
         memcpy(ln.pin_in, left, IMG);
@@ -980,6 +1066,39 @@ int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, 
     return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps);
 }
 
+int adc_match_images_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                  const adc_image_desc* img, const void* d_cost, int32_t cost_layout, int32_t cost_dtype,
+                                  float* d_disp, const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps,
+                                  int32_t n_maps, void* stream) {
+    const char* fn = "adc_match_images_batch_device";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
+    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcImageGeom g;
+    if ((rc = resolve_image(e, fn, img, &g))) return rc;
+    long long last_view = 0;
+    if (n > 1 && __builtin_mul_overflow((long long)(n - 1), g.image_stride, &last_view))
+        return fail(ADC_ERR_ARG, "%s: img->image_stride %lld * (n - 1) overflows", fn, g.image_stride);
+    e->img_format = g.format;
+    return match_outputs_device(e, fn, n, d_left, d_right, d_cost, cost_layout, cost_dtype, d_disp, vols, n_vols, maps, n_maps,
+                                (cudaStream_t)stream, tight_bgr(e, g) ? nullptr : &g);
+}
+
+int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img, const void* cost,
+                     int32_t cost_layout, int32_t cost_dtype, float* disp, const adc_volume_out* vols, int32_t n_vols,
+                     const adc_map_out* maps, int32_t n_maps) {
+    const char* fn = "adc_match_images";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, disp != nullptr, cost != nullptr, cost_layout, cost_dtype, false);
+    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcImageGeom g;
+    if ((rc = resolve_image(e, fn, img, &g))) return rc;
+    e->img_format = g.format;
+    const bool bgr_rows = g.format == ADC_IMG_BGR && g.row_pitch == 3ll * e->W;   // one pair: the image stride plays no part
+    return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps,
+                              bgr_rows ? nullptr : &g);
+}
+
 void* adc_host_alloc(size_t bytes) {
     void* p = nullptr;
     if (cudaHostAlloc(&p, bytes, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return nullptr; }
@@ -1116,6 +1235,16 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 adc_launch_confidence(P, w, w.volA, w.volB, w.volB + (size_t)e->S * P.dm.N, ln.st, &e->launches);
                 bytes = N * P.dm.Dp * 4.0 + 2 * 4.0 * N;
                 break;
+            case 13: {  // volA's bytes taken as the wave's tight images (at most 2*4*N bytes a pair: they fit in its N*Dp floats)
+                const int bpp = adc_image_bytes_per_pixel(e->img_format);
+                const bool planar = e->img_format == ADC_IMG_RGB_PLANAR;
+                const long long foot = (long long)P.dm.N * (planar ? 3 : bpp);
+                const AdcImageGeom g{e->img_format, (long long)P.dm.W * bpp, planar ? (long long)P.dm.N : 0, 2 * foot};
+                const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
+                adc_launch_image_ingest(P, w, src, src + foot, g, ln.st, &e->launches);
+                bytes = 2.0 * foot + 2 * 3.0 * N;
+                break;
+            }
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);
         }
     }

@@ -85,6 +85,55 @@ class MapOut(ctypes.Structure):
     _fields_ = [("dst", ctypes.c_void_p), ("kind", ctypes.c_int32), ("reserved", ctypes.c_int32)]
 
 
+# image input formats (adc_match_images*): u8 pixels, packed or planar, matched exactly as the same pixels packed as BGR
+IMG_BGR, IMG_RGB, IMG_BGRA, IMG_RGBA, IMG_GRAY, IMG_RGB_PLANAR = 0, 1, 2, 3, 4, 5
+IMG_FORMATS = {"bgr": IMG_BGR, "rgb": IMG_RGB, "bgra": IMG_BGRA, "rgba": IMG_RGBA, "gray": IMG_GRAY,
+               "rgb_planar": IMG_RGB_PLANAR}
+IMG_CHANNELS = {IMG_BGR: 3, IMG_RGB: 3, IMG_BGRA: 4, IMG_RGBA: 4, IMG_GRAY: 1, IMG_RGB_PLANAR: 1}   # bytes per pixel (plane)
+
+
+class ImageDesc(ctypes.Structure):
+    """adc_image_desc: format (IMG_*) and byte pitches of the images of one call; zero pitches mean tight."""
+    _fields_ = [("format", ctypes.c_int32), ("reserved", ctypes.c_int32), ("row_pitch", ctypes.c_int64),
+                ("plane_pitch", ctypes.c_int64), ("image_stride", ctypes.c_int64)]
+
+
+assert ctypes.sizeof(ImageDesc) == 32
+
+
+def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> ImageDesc:
+    """An ImageDesc from a format name or IMG_* code and byte pitches (0 = tight)."""
+    return ImageDesc(_img_format(format), 0, int(row_pitch), int(plane_pitch), int(image_stride))
+
+
+def _img_format(v) -> int:
+    if isinstance(v, str):
+        if v not in IMG_FORMATS:
+            raise ValueError(f"unknown image format {v!r} (one of {sorted(IMG_FORMATS)})")
+        return IMG_FORMATS[v]
+    return int(v)
+
+
+def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
+    """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray) or [3][H][W] (planar R, G, B)
+    with the pixels / channels of a row contiguous; the pitches come from the view's strides, so slices of a larger
+    frame (crops, side-by-side halves) need no copy."""
+    if a.dtype != np.uint8:
+        raise ValueError(f"images must be uint8, got {a.dtype}")
+    C = IMG_CHANNELS[fmt]
+    if fmt == IMG_RGB_PLANAR:
+        shape, inner, pitches = (3, H, W), (1,), (0, a.strides[1], a.strides[0])
+    elif fmt == IMG_GRAY:
+        shape, inner, pitches = (H, W), (1,), (0, a.strides[0], 0)
+    else:
+        shape, inner, pitches = (H, W, C), (C, 1), (0, a.strides[0], 0)
+    if a.shape != shape:
+        raise ValueError(f"expected an image of shape {shape} for format {fmt}, got {a.shape}")
+    if tuple(a.strides[-len(inner):]) != inner or min(a.strides) < 0:
+        raise ValueError(f"the pixels of an image row must be contiguous (strides {a.strides})")
+    return ImageDesc(fmt, 0, pitches[1], pitches[2], 0)
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -144,6 +193,10 @@ def load_library() -> ctypes.CDLL:
                                     ctypes.POINTER(MapOut), i32]
     L.adc_match_outputs_batch_device.argtypes = [vp, i32, u8p, u8p, vp, i32, i32, f32p, ctypes.POINTER(VolumeOut), i32,
                                                  ctypes.POINTER(MapOut), i32, vp]
+    L.adc_match_images.argtypes = [vp, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
+                                   ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32]
+    L.adc_match_images_batch_device.argtypes = [vp, i32, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
+                                                ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -341,6 +394,47 @@ class Engine:
                                                       _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
                                                       len(volumes), marr, len(maps), stream))
 
+    # ---- image input formats (adc_match_images*) -----------------------------------------------
+    def match_images(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
+                     cost_layout="hwd", cost_dtype=None, disparity=True):
+        """match_outputs for images in any IMG_* format, read in place: `left` / `right` are uint8 numpy views of shape
+        [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray) or [3][H][W] (rgb_planar) whose rows may be pitched, e.g.
+        frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.  The result is
+        what match_outputs gives for the same pixels packed as BGR."""
+        fmt = _img_format(format)
+        H, W, D = self.height, self.width, self.D
+        desc = _image_view_desc(left, fmt, H, W)
+        if _image_view_desc(right, fmt, H, W).row_pitch != desc.row_pitch or \
+                (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
+            raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
+        maps = [maps] if isinstance(maps, (str, int)) else list(maps)
+        volumes = [volumes] if isinstance(volumes, (str, int)) else list(volumes)
+        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
+        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
+        out = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in volumes}
+        vouts = _volume_outs([(out[s].ctypes.data, s, lay, dt) for s in volumes])
+        for m in maps:
+            out[m] = np.empty((H, W), _MAP_NP.get(_code(MAP_KINDS, m, "map kind"), np.float32))
+        mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
+        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
+        disp = np.empty((H, W), np.float32) if disparity else None
+        _check(self._L.adc_match_images(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc),
+                                        None if c is None else c.ctypes.data, clay, cdt,
+                                        None if disp is None else disp.ctypes.data, vouts, len(volumes), mouts, len(maps)))
+        return disp, out
+
+    def match_images_batch_device(self, n: int, d_left: int, d_right: int, image=None, maps=(), volumes=(),
+                                  d_disp: int = 0, d_cost: int = 0, cost_layout="dhw", cost_dtype="f32", stream: int = 0):
+        """match_outputs_batch_device for images described by `image` (an ImageDesc, e.g. from image_desc(); None = tight
+        packed BGR): device pointers (ints) to the first pair's left and right view, pair i at i * image_stride bytes.
+        Enqueued on `stream` without synchronising, like match_batch_device."""
+        varr, marr = _volume_outs(volumes), _map_outs(maps)
+        _check(self._L.adc_match_images_batch_device(self._h, n, d_left, d_right,
+                                                     None if image is None else ctypes.byref(image), d_cost or None,
+                                                     _code(COST_LAYOUTS, cost_layout, "layout"),
+                                                     _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
+                                                     len(volumes), marr, len(maps), stream))
+
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
         lefts = np.ascontiguousarray(lefts, np.uint8)
@@ -384,7 +478,7 @@ class Engine:
 
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
                        "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10,
-                       "cost_export": 11, "confidence": 12}
+                       "cost_export": 11, "confidence": 12, "image_ingest": 13}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""

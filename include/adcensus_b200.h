@@ -256,6 +256,60 @@ int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, 
                       int32_t cost_layout, int32_t cost_dtype, float* disp,
                       const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
 
+/* ---- image input formats ----------------------------------------------------------------------------
+ * The entry points below read the caller's images in place, in any of these u8 formats, with any row, plane and image
+ * pitch, instead of requiring packed BGR with rows exactly 3*W bytes and pairs exactly 3*H*W bytes apart:
+ *   ADC_IMG_BGR         3 bytes per pixel, packed, B G R       (OpenCV, the reference's main.cpp)
+ *   ADC_IMG_RGB         3 bytes per pixel, packed, R G B       (PIL / imageio / numpy loaders, channels-last torch)
+ *   ADC_IMG_BGRA        4 bytes per pixel, packed, B G R A     (OpenCV 4-channel Mat, ZED SDK)
+ *   ADC_IMG_RGBA        4 bytes per pixel, packed, R G B A     (PIL RGBA, GL / capture buffers)
+ *   ADC_IMG_GRAY        1 byte per pixel, one plane            (mono stereo cameras)
+ *   ADC_IMG_RGB_PLANAR  1 byte per pixel in each of three planes R, G, B   (torchvision [N, 3, H, W])
+ * Semantics: an image in any format is matched exactly as if the caller had packed the same pixels as BGR u8 and called
+ * the corresponding packed-BGR entry point.  The channel order is resolved, alpha is ignored, and a gray pixel v is the
+ * BGR pixel (v, v, v).  A gray image therefore goes through the engine's gray conversion like any other: the reference's
+ * fp64 luma of (v, v, v), truncated, is not always v (gray(128, 128, 128) = 127), and the AD term and the arm / scanline
+ * colour distances see three equal channels.
+ * Geometry (shared by both views; each view has its own base pointer).  Offsets are bytes, 64-bit:
+ *   pixel (x, y) of pair i, packed / gray:  base + i*image_stride + y*row_pitch + x*bytes_per_pixel
+ *   channel c (0 = R, 1 = G, 2 = B) of a planar pixel:  base + i*image_stride + c*plane_pitch + y*row_pitch + x
+ * Zero-initialised means tight packed BGR, i.e. the packed-BGR entry points' contract.  Rules: none of the pitches may be
+ * negative; row_pitch (0 = tight: W * bytes per pixel, W for gray / planar) must be at least W * bytes per pixel;
+ * plane_pitch must be 0 for every format but ADC_IMG_RGB_PLANAR, where 0 = H * row_pitch and it must be at least
+ * H * row_pitch; image_stride (0 = tight: the view's footprint) must be at least the view's footprint, H * row_pitch or,
+ * planar, 3 * plane_pitch; reserved must be zero.  Base pointers and pitches may have any byte alignment (a side-by-side
+ * right view starts W * 4 bytes into a BGRA frame; a crop starts at an arbitrary x).  The engine reads only the pixels
+ * themselves: nothing past the last pixel of a view's last row, and never an alpha byte.
+ * Rule violations fail with ADC_ERR_ARG naming the field: the rules that need no image size before the engine is
+ * checked, the size-dependent ones before any device work.
+ * Cost: tight packed BGR takes the packed-BGR entry points' copies; every other format or geometry runs one ingestion
+ * kernel per wave that writes the wave's packed BGR in one pass. */
+enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC_IMG_GRAY = 4, ADC_IMG_RGB_PLANAR = 5 };
+typedef struct adc_image_desc {
+    int32_t format;        /* ADC_IMG_* */
+    int32_t reserved;      /* must be zero */
+    int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / planar) */
+    int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; other formats: must be 0 */
+    int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch) */
+} adc_image_desc;          /* 32 bytes */
+
+/* adc_match_outputs_batch_device with the images described by `img` (NULL = tight packed BGR, the same call as
+ * adc_match_outputs_batch_device).  Device pointers; stream, fork/join and pipelined-mode behaviour, cost input, volume
+ * export, side maps and their argument rules as for adc_match_outputs_batch_device.  A NULL descriptor, or one that
+ * describes tight packed BGR, issues exactly the launches of adc_match_outputs_batch_device; any other adds one
+ * ingestion launch per wave.  The caller's images must stay untouched until the work is joined. */
+int adc_match_images_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                  const adc_image_desc* img, const void* d_cost, int32_t cost_layout, int32_t cost_dtype,
+                                  float* d_disp, const adc_volume_out* vols, int32_t n_vols,
+                                  const adc_map_out* maps, int32_t n_maps, void* stream);
+/* One pair, host pointers, synchronous: adc_match_outputs with the images described by `img` (image_stride is not used),
+ * e.g. an OpenCV gray Mat's data and step.  Each view's pixels are uploaded into device memory the engine already owns
+ * (the lane volume that stage 1 writes) and converted there.  With disp: adc_last_stage_ms (out[0] = uploads + ingestion
+ * + stage 1) and adc_get_right_disparity behave as after adc_match. */
+int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img,
+                     const void* cost, int32_t cost_layout, int32_t cost_dtype, float* disp,
+                     const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
@@ -277,7 +331,9 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * the engine's last cost call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*D*sizeof(element) + N*Dp*4 bytes per
  * pair, Dp = D rounded up to a multiple of 4), 11 = volume export (layout and element type of the engine's last export
  * call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*Dp*4 + N*D*sizeof(element) bytes per pair), 12 = confidence
- * (MIN_COST and PEAK_RATIO of the left view; N*Dp*4 + 2*4*N bytes per pair).
+ * (MIN_COST and PEAK_RATIO of the left view; N*Dp*4 + 2*4*N bytes per pair), 13 = image ingestion (format of the
+ * engine's last adc_match_images* call, ADC_IMG_RGB_PLANAR if there was none, tight pitches; the source bytes of both
+ * views + 2*3*N written per pair).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 

@@ -82,4 +82,46 @@ for (w, h, D, seed) in [(97, 61, 22, 2), (71, 47, 23, 5)]:
     assert (got == want["aggr"].reshape(1, -1)).all()
     eng.close()
     print("export ok", w, h, D, flush=True)
+
+# image input: odd-x crops in every format, the right view of each ending exactly at the end of its own cudaMalloc
+# allocation (torch's caching allocator would hide an over-read inside a larger block), through the batched entry
+import ctypes
+import images_testlib as IT
+cudart = ctypes.CDLL("libcudart.so.12")       # already loaded by the engine library
+cudart.cudaMalloc.argtypes = [ctypes.POINTER(ctypes.c_void_p), ctypes.c_size_t]
+cudart.cudaMemcpy.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int]
+cudart.cudaFree.argtypes = [ctypes.c_void_p]
+w, h, D, n = 71, 47, 23, 3
+left, right = T.synthetic_pair(w, h, D, 8)
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+want = eng.match(left, right)
+for fmt in IT.FORMATS:
+    l, r = (IT.gray_to_bgr(left[:, :, 1]), IT.gray_to_bgr(right[:, :, 1])) if fmt == "gray" else (left, right)
+    bpp, x0 = IT.BPP[fmt], 3
+    rp = (w + x0) * bpp
+    pp = h * rp if fmt == "rgb_planar" else 0
+    stride = IT.footprint(fmt, h, rp, pp)
+    ptrs = []
+    for img in (l, r):
+        host = np.zeros(n * stride, np.uint8)
+        for i in range(n):
+            IT.write_view(host[i * stride:], IT.from_bgr(img, fmt), fmt, rp, pp, x0 * bpp)
+        # the allocation ends with the last pixel of the last row of the last view: drop the row's unused tail
+        size = n * stride - (rp - (x0 + w) * bpp)
+        p = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(p), size) == 0
+        assert cudart.cudaMemcpy(p, host.ctypes.data, size, 1) == 0
+        ptrs.append(p.value)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_images_batch_device(n, ptrs[0] + x0 * bpp, ptrs[1] + x0 * bpp, image=A.image_desc(fmt, rp, pp, stride),
+                                  d_disp=d_o.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(l, r)
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), fmt
+    if fmt != "gray":
+        assert single.tobytes() == want.tobytes(), fmt
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("images ok", fmt, flush=True)
+eng.close()
 print("all ok")
