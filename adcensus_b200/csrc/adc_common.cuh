@@ -2,7 +2,8 @@
 //
 // Data layout in HBM (per wave of S stereo pairs; every array is [S][...], pair index outermost):
 //   bgr      u8  [S][2][H][W][3]   left, right packed BGR: copied as the caller passes them, or written by the image
-//                                  ingestion kernel (k_image.cu) from another format / pitch
+//                                  ingestion kernel (k_image.cu) from another format / pitch, or by the rectified
+//                                  ingestion kernel (k_rectify.cu) from raw frames
 //   gray     u8  [S][2][H][W]
 //   census   u64 [S][2][H][W]
 //   volA/B   f32 [S][H][W][Dp]     the two cost volumes, d fastest, Dp = D rounded up to 4 so that
@@ -147,6 +148,18 @@ struct AdcImageGeom {
 void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
                              const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches);
 int adc_image_bytes_per_pixel(int format);   // per plane for ADC_IMG_RGB_PLANAR
+// rectified ingestion (k_rectify.cu).  The engine's internal form of a view's remap table: one uint2 per output pixel,
+// .x = (u16)x0 | (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
+struct AdcRectGeom {
+    const uint2* map[2];   // left, right: [H][W] each
+    int src_w, src_h;      // raw frame size
+};
+// a view's adc_remap (map1 / map2 with byte pitches, device-readable, ADC_REMAP_F32 / ADC_REMAP_FIXED) -> out [H][W]
+void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1, long long pitch1, const void* map2,
+                              long long pitch2, uint2* out, cudaStream_t st);
+// the wave's raw views at left / right (geometry g over src_w x src_h frames, pitches resolved) -> w.bgr, resampled
+void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
+                               const AdcImageGeom& g, const AdcRectGeom& r, cudaStream_t st, unsigned long long* launches);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

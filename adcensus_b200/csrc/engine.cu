@@ -30,6 +30,11 @@ static_assert(offsetof(adc_option, so_p1) == 32 && offsetof(adc_option, irv_th) 
 static_assert(sizeof(adc_image_desc) == 32 && offsetof(adc_image_desc, reserved) == 4 &&
               offsetof(adc_image_desc, row_pitch) == 8 && offsetof(adc_image_desc, plane_pitch) == 16 &&
               offsetof(adc_image_desc, image_stride) == 24, "adc_image_desc layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_remap) == 32 && offsetof(adc_remap, map2) == 8 && offsetof(adc_remap, map1_pitch) == 16 &&
+              offsetof(adc_remap, map2_pitch) == 24, "adc_remap layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_rectification) == 80 && offsetof(adc_rectification, src_height) == 4 &&
+              offsetof(adc_rectification, map_type) == 8 && offsetof(adc_rectification, reserved) == 12 &&
+              offsetof(adc_rectification, view) == 16, "adc_rectification layout (include/adcensus_b200.h)");
 
 namespace {
 
@@ -98,6 +103,11 @@ struct adc_engine {
     int export_layout = ADC_COST_DHW, export_dtype = ADC_COST_F32;
     // image format of the last adc_match_images* call (adc_profile_kernel's ingestion timing)
     int img_format = ADC_IMG_RGB_PLANAR;
+    // rectification (adc_set_rectification): both views' maps in the internal form, [2][N]; nullptr = none set
+    uint2* rect_map = nullptr;
+    int rect_src_w = 0, rect_src_h = 0;
+    // raw frame format of the last adc_match_rectified* call (adc_profile_kernel's rectified ingestion timing)
+    int rect_format = ADC_IMG_BGR;
     // device staging of adc_match_volumes' exported volumes: allocated on first use, grown when needed
     void* vol_stage = nullptr;
     size_t vol_stage_bytes = 0;
@@ -453,12 +463,13 @@ enum SrcKind { SRC_HOST_PTRS, SRC_HOST_STRIDED, SRC_DEVICE_STRIDED };
 // `force_join`: the call is one of the synchronous entry points, whose results must be complete on return whatever the
 // engine's pipelined setting (adc_set_pipelined only changes the asynchronous entry points).
 // `img` (SRC_DEVICE_STRIDED only): the resolved geometry of images that are not tight packed BGR, converted by the
-// ingestion kernel; nullptr = tight packed BGR, copied.
+// ingestion kernel; nullptr = tight packed BGR, copied.  `rect` (with img): the views are raw frames, resampled
+// through these maps by the rectified ingestion kernel.
 int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, const uint8_t* const* rp,
               float* const* dp, const uint8_t* ls, const uint8_t* rs, float* ds, cudaStream_t user, bool pinned,
               bool force_join = false, const CostSrc& cost = CostSrc(), int last_stage = ADC_STAGE_MEDIAN,
               const adc_volume_out* outs = nullptr, int n_outs = 0, const adc_map_out* maps = nullptr, int n_maps = 0,
-              const AdcImageGeom* img = nullptr) {
+              const AdcImageGeom* img = nullptr, const AdcRectGeom* rect = nullptr) {
     const size_t N = (size_t)e->P.dm.N, IMG = N * 3;
     const int S = e->S, nl = (int)e->lanes.size();
     CK(cudaEventRecord(e->ev_fork, user));
@@ -469,7 +480,10 @@ int run_batch(adc_engine* e, int n, SrcKind kind, const uint8_t* const* lp, cons
         const int first = wv * S, nS = std::min(S, n - first);
         const AdcWave& io = ln.w;   // where the images go in and the map comes out
         // ---- inputs -> io.bgr  ([S][2][IMG])
-        if (kind == SRC_DEVICE_STRIDED && img) {
+        if (kind == SRC_DEVICE_STRIDED && rect) {
+            const long long off = (long long)first * img->image_stride;
+            adc_launch_rectify_ingest(e->P, wave_view(e, ln, nS), ls + off, rs + off, *img, *rect, ln.st, &e->launches);
+        } else if (kind == SRC_DEVICE_STRIDED && img) {
             const long long off = (long long)first * img->image_stride;
             adc_launch_image_ingest(e->P, wave_view(e, ln, nS), ls + off, rs + off, *img, ln.st, &e->launches);
         } else if (kind == SRC_DEVICE_STRIDED) {
@@ -616,11 +630,11 @@ int check_image_desc(const char* fn, const adc_image_desc* img) {
     return ADC_OK;
 }
 
-// The size-dependent rules of an image descriptor (NULL = tight packed BGR); `g` receives the geometry with every zero
-// default replaced.
-int resolve_image(const adc_engine* e, const char* fn, const adc_image_desc* img, AdcImageGeom* g) {
+// The size-dependent rules of an image descriptor (NULL = tight packed BGR) for views of w x h pixels (the engine's
+// size, or the raw frame size of the rectified entries); `g` receives the geometry with every zero default replaced.
+int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, AdcImageGeom* g) {
     const adc_image_desc d = img ? *img : adc_image_desc{};
-    const long long W = e->W, H = e->H, bpp = adc_image_bytes_per_pixel(d.format);
+    const long long W = w, H = h, bpp = adc_image_bytes_per_pixel(d.format);
     g->format = d.format;
     g->row_pitch = d.row_pitch ? (long long)d.row_pitch : W * bpp;
     if (g->row_pitch < W * bpp)
@@ -645,27 +659,44 @@ bool tight_bgr(const adc_engine* e, const AdcImageGeom& g) {
     return g.format == ADC_IMG_BGR && g.row_pitch == 3ll * e->W && g.image_stride == 3ll * e->W * e->H;
 }
 
+// Bytes stage_views writes for views of geometry g over w x h frames.
+size_t staged_bytes(const AdcImageGeom& g, int w, int h) {
+    const size_t N = (size_t)w * h;
+    return 2 * N * (g.format == ADC_IMG_RGB_PLANAR ? 3 : adc_image_bytes_per_pixel(g.format));
+}
+
+// Uploads one pair of host views (geometry g over w x h frames) tightly, view after view, to the device memory at
+// `stage`; `tight` receives their geometry there (image_stride = the right view's offset).
+int stage_views(Lane& ln, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g, int w, int h, uint8_t* stage,
+                AdcImageGeom* tight) {
+    const size_t W = (size_t)w, H = (size_t)h, N = W * H;
+    const size_t bpp = (size_t)adc_image_bytes_per_pixel(g.format);
+    const bool planar = g.format == ADC_IMG_RGB_PLANAR;
+    const size_t foot = staged_bytes(g, w, h) / 2;
+    for (int v = 0; v < 2; v++)
+        for (int c = 0; c < (planar ? 3 : 1); c++)
+            CK(cudaMemcpy2DAsync(stage + v * foot + c * N, bpp * W, (v ? right : left) + c * g.plane_pitch, (size_t)g.row_pitch,
+                                 bpp * W, H, cudaMemcpyHostToDevice, ln.st));
+    *tight = AdcImageGeom{g.format, (long long)(bpp * W), planar ? (long long)N : 0, (long long)foot};
+    return ADC_OK;
+}
+
 // One pair of the host entry's images (geometry g) -> ln.w.bgr.  Packed BGR rows go straight into bgr (the 2D copy
 // drops any row padding).  Every other format is uploaded tightly, view after view, into the lane volume that stage 1
 // writes, and converted from there by the ingestion kernel: nothing reads that volume before stage 1 overwrites it, the
 // cost-input staging of upload_cost_pair is the other volume, and the export / map staging is a separate allocation.
 int upload_images(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g, int last_stage) {
     const size_t W = (size_t)e->W, H = (size_t)e->H, N = W * H, IMG = N * 3;
-    const size_t bpp = (size_t)adc_image_bytes_per_pixel(g.format);
     if (g.format == ADC_IMG_BGR) {
         CK(cudaMemcpy2DAsync(ln.w.bgr, 3 * W, left, (size_t)g.row_pitch, 3 * W, H, cudaMemcpyHostToDevice, ln.st));
         CK(cudaMemcpy2DAsync(ln.w.bgr + IMG, 3 * W, right, (size_t)g.row_pitch, 3 * W, H, cudaMemcpyHostToDevice, ln.st));
         return ADC_OK;
     }
     uint8_t* stage = reinterpret_cast<uint8_t*>(agg_fused_for(e, last_stage) ? ln.w.volB : ln.w.volA);
-    const bool planar = g.format == ADC_IMG_RGB_PLANAR;
-    const size_t foot = planar ? 3 * N : bpp * N;
-    for (int v = 0; v < 2; v++)
-        for (int c = 0; c < (planar ? 3 : 1); c++)
-            CK(cudaMemcpy2DAsync(stage + v * foot + c * N, bpp * W, (v ? right : left) + c * g.plane_pitch, (size_t)g.row_pitch,
-                                 bpp * W, H, cudaMemcpyHostToDevice, ln.st));
-    const AdcImageGeom tight{g.format, (long long)(bpp * W), planar ? (long long)N : 0, (long long)foot};
-    adc_launch_image_ingest(e->P, wave_view(e, ln, 1), stage, stage + foot, tight, ln.st, &e->launches);
+    AdcImageGeom tight;
+    int rc = stage_views(ln, left, right, g, e->W, e->H, stage, &tight);
+    if (rc) return rc;
+    adc_launch_image_ingest(e->P, wave_view(e, ln, 1), stage, stage + tight.image_stride, tight, ln.st, &e->launches);
     return ADC_OK;
 }
 
@@ -689,11 +720,13 @@ int upload_cost_pair(adc_engine* e, Lane& ln, const uint8_t* left, const uint8_t
     return ADC_OK;
 }
 
-// The batched device driver of adc_match_volumes_batch_device, adc_match_outputs_batch_device and
-// adc_match_images_batch_device (arguments checked; img = resolved geometry of images that are not tight packed BGR).
+// The batched device driver of adc_match_volumes_batch_device, adc_match_outputs_batch_device,
+// adc_match_images_batch_device and adc_match_rectified_batch_device (arguments checked; img = resolved geometry of
+// images that are not tight packed BGR, or of the raw frames that rect resamples).
 int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_left, const uint8_t* d_right, const void* d_cost,
                          int cost_layout, int cost_dtype, float* d_disp, const adc_volume_out* vols, int n_vols,
-                         const adc_map_out* maps, int n_maps, cudaStream_t stream, const AdcImageGeom* img = nullptr) {
+                         const adc_map_out* maps, int n_maps, cudaStream_t stream, const AdcImageGeom* img = nullptr,
+                         const AdcRectGeom* rect = nullptr) {
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if (n < 0 || (n > 0 && (!d_left || !d_right))) return fail(ADC_ERR_ARG, "%s: bad arguments", fn);
     if (n == 0) return ADC_OK;
@@ -712,15 +745,17 @@ int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_
     }
     const int last = d_disp ? ADC_STAGE_MEDIAN : last_output_stage(vols, n_vols, maps, n_maps);
     return run_batch(e, n, SRC_DEVICE_STRIDED, nullptr, nullptr, nullptr, d_left, d_right, d_disp, stream, true, false, src,
-                     last, vols, n_vols, maps, n_maps, img);
+                     last, vols, n_vols, maps, n_maps, img, rect);
 }
 
-// The one-pair host driver of adc_match_volumes, adc_match_outputs and adc_match_images (arguments checked): volumes and
-// maps go to device staging first (one after the other), then to the caller's host buffers.  img = the images' resolved
-// geometry, nullptr = tight packed BGR.
+// The one-pair host driver of adc_match_volumes, adc_match_outputs, adc_match_images and adc_match_rectified (arguments
+// checked): volumes and maps go to device staging first (one after the other), then to the caller's host buffers.
+// img = the images' resolved geometry, nullptr = tight packed BGR.  rect (with img): the views are raw frames, uploaded
+// tightly into the lane volume that stage 1 writes when both fit in it, and otherwise behind the volumes and maps in the
+// device staging, then resampled into ln.w.bgr.
 int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const uint8_t* right, const void* cost, int cost_layout,
                        int cost_dtype, float* disp, const adc_volume_out* vols, int n_vols, const adc_map_out* maps, int n_maps,
-                       const AdcImageGeom* img = nullptr) {
+                       const AdcImageGeom* img = nullptr, const AdcRectGeom* rect = nullptr) {
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if (!left || !right) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
     CK(cudaSetDevice(e->cfg.device));
@@ -732,6 +767,9 @@ int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const
     size_t need = 0;
     for (int i = 0; i < n_vols; i++) need += align_up(ND * adc_cost_elem_bytes(vols[i].dtype), 256);
     for (int i = 0; i < n_maps; i++) need += align_up(N * map_elem_bytes(maps[i].kind), 256);
+    const size_t raw = rect ? staged_bytes(*img, rect->src_w, rect->src_h) : 0;
+    const bool raw_in_volume = raw <= (size_t)e->S * e->P.dm.vol_stride * sizeof(float);
+    if (!raw_in_volume) need += raw;
     if (need > e->vol_stage_bytes) {
         if (e->vol_stage) CK(cudaFree(e->vol_stage));
         e->vol_stage = nullptr;
@@ -764,7 +802,15 @@ int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const
     cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
     if (ev) CK(cudaEventRecord(ev[0], ln.st));
     CostSrc src;
-    if (img) {
+    if (rect) {
+        uint8_t* stage = raw_in_volume ? reinterpret_cast<uint8_t*>(agg_fused_for(e, last) ? ln.w.volB : ln.w.volA)
+                                       : static_cast<uint8_t*>(e->vol_stage) + off;
+        AdcImageGeom tight;
+        if ((rc = stage_views(ln, left, right, *img, rect->src_w, rect->src_h, stage, &tight))) return rc;
+        adc_launch_rectify_ingest(e->P, wave_view(e, ln, 1), stage, stage + tight.image_stride, tight, *rect, ln.st,
+                                  &e->launches);
+        if (cost && (rc = upload_cost_pair(e, ln, nullptr, nullptr, cost, cost_layout, cost_dtype, last, &src))) return rc;
+    } else if (img) {
         if ((rc = upload_images(e, ln, left, right, *img, last))) return rc;
         if (cost && (rc = upload_cost_pair(e, ln, nullptr, nullptr, cost, cost_layout, cost_dtype, last, &src))) return rc;
     } else if (cost) {
@@ -788,6 +834,18 @@ int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const
         CK(cudaMemcpy(vols[i].dst, dev.o[i].dst, ND * adc_cost_elem_bytes(vols[i].dtype), cudaMemcpyDeviceToHost));
     for (int i = 0; i < n_maps; i++)
         CK(cudaMemcpy(maps[i].dst, dev_maps.dst[maps[i].kind], N * map_elem_bytes(maps[i].kind), cudaMemcpyDeviceToHost));
+    return ADC_OK;
+}
+
+// The rules the rectified entries add to the image entries' (after the engine check): a rectification is set, and
+// the descriptor's size-dependent rules hold for the raw frame size.
+int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, AdcImageGeom* g, AdcRectGeom* r) {
+    if (!e->rect_map) return fail(ADC_ERR_ARG, "%s: no rectification is set (adc_set_rectification)", fn);
+    int rc = resolve_image(fn, e->rect_src_w, e->rect_src_h, img, g);
+    if (rc) return rc;
+    const size_t N = (size_t)e->P.dm.N;
+    *r = AdcRectGeom{{e->rect_map, e->rect_map + N}, e->rect_src_w, e->rect_src_h};
+    e->rect_format = g->format;
     return ADC_OK;
 }
 
@@ -830,6 +888,7 @@ void adc_destroy(adc_engine* e) {
     if (e->d_rays) cudaFree(e->d_rays);
     if (e->d_ray_off) cudaFree(e->d_ray_off);
     if (e->vol_stage) cudaFree(e->vol_stage);
+    if (e->rect_map) cudaFree(e->rect_map);
     if (e->ev_fork) cudaEventDestroy(e->ev_fork);
     for (auto& ev : e->ev_stage) if (ev) cudaEventDestroy(ev);
     if (e->main_st) cudaStreamDestroy(e->main_st);
@@ -1075,7 +1134,7 @@ int adc_match_images_batch_device(adc_engine* e, int32_t n, const uint8_t* d_lef
     if (rc || (rc = check_image_desc(fn, img))) return rc;
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     AdcImageGeom g;
-    if ((rc = resolve_image(e, fn, img, &g))) return rc;
+    if ((rc = resolve_image(fn, e->W, e->H, img, &g))) return rc;
     long long last_view = 0;
     if (n > 1 && __builtin_mul_overflow((long long)(n - 1), g.image_stride, &last_view))
         return fail(ADC_ERR_ARG, "%s: img->image_stride %lld * (n - 1) overflows", fn, g.image_stride);
@@ -1092,11 +1151,135 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
     if (rc || (rc = check_image_desc(fn, img))) return rc;
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     AdcImageGeom g;
-    if ((rc = resolve_image(e, fn, img, &g))) return rc;
+    if ((rc = resolve_image(fn, e->W, e->H, img, &g))) return rc;
     e->img_format = g.format;
     const bool bgr_rows = g.format == ADC_IMG_BGR && g.row_pitch == 3ll * e->W;   // one pair: the image stride plays no part
     return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps,
                               bgr_rows ? nullptr : &g);
+}
+
+int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
+    const char* fn = "adc_set_rectification";
+    const bool f32 = r && r->map_type == ADC_REMAP_F32;
+    const long long e1 = 4, e2 = f32 ? 4 : 2;   // bytes per element of map1 (float, int16 pair) and map2 (float, uint16)
+    if (r) {
+        if (r->src_width < 1 || r->src_width > 32767) return fail(ADC_ERR_ARG, "%s: r->src_width %d outside 1..32767", fn, r->src_width);
+        if (r->src_height < 1 || r->src_height > 32767) return fail(ADC_ERR_ARG, "%s: r->src_height %d outside 1..32767", fn, r->src_height);
+        if (r->map_type != ADC_REMAP_F32 && r->map_type != ADC_REMAP_FIXED) return fail(ADC_ERR_ARG, "%s: r->map_type %d unknown", fn, r->map_type);
+        if (r->reserved != 0) return fail(ADC_ERR_ARG, "%s: r->reserved must be zero", fn);
+        for (int v = 0; v < 2; v++) {
+            const adc_remap& m = r->view[v];
+            if (!m.map1) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1 is NULL", fn, v);
+            if (!m.map2) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2 is NULL", fn, v);
+            if (m.map1_pitch < 0) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1_pitch %lld is negative", fn, v, (long long)m.map1_pitch);
+            if (m.map2_pitch < 0) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2_pitch %lld is negative", fn, v, (long long)m.map2_pitch);
+            if ((uintptr_t)m.map1 % (f32 ? 4 : 2) || m.map1_pitch % (f32 ? 4 : 2))
+                return fail(ADC_ERR_ARG, "%s: r->view[%d].map1 or map1_pitch is not aligned to its element", fn, v);
+            if ((uintptr_t)m.map2 % e2 || m.map2_pitch % e2)
+                return fail(ADC_ERR_ARG, "%s: r->view[%d].map2 or map2_pitch is not aligned to its element", fn, v);
+        }
+    }
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    const long long W = e->W, H = e->H;
+    long long p1[2] = {0, 0}, p2[2] = {0, 0};
+    if (r) {
+        for (int v = 0; v < 2; v++) {
+            const adc_remap& m = r->view[v];
+            p1[v] = m.map1_pitch ? (long long)m.map1_pitch : W * e1;
+            p2[v] = m.map2_pitch ? (long long)m.map2_pitch : W * e2;
+            long long foot = 0;
+            if (p1[v] < W * e1) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1_pitch %lld is less than a row (%lld bytes)", fn, v, p1[v], W * e1);
+            if (p2[v] < W * e2) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2_pitch %lld is less than a row (%lld bytes)", fn, v, p2[v], W * e2);
+            if (__builtin_mul_overflow(H, p1[v], &foot)) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1_pitch %lld is too large", fn, v, p1[v]);
+            if (__builtin_mul_overflow(H, p2[v], &foot)) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2_pitch %lld is too large", fn, v, p2[v]);
+        }
+    }
+    CK(cudaSetDevice(e->cfg.device));
+    const size_t N = (size_t)e->P.dm.N;
+    uint2* maps = nullptr;
+    void* tmp = nullptr;
+    bool host[2][2] = {};
+    if (r) {
+        bool any_host = false;
+        for (int v = 0; v < 2; v++)
+            for (int k = 0; k < 2; k++) {
+                cudaPointerAttributes at{};
+                const void* p = k ? r->view[v].map2 : r->view[v].map1;
+                if (cudaPointerGetAttributes(&at, p) != cudaSuccess) cudaGetLastError();
+                host[v][k] = at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged;
+                any_host |= host[v][k];
+            }
+        // the maps in the internal form, and (host maps) device staging of one view's tight maps
+        if (cudaMalloc(&maps, 2 * N * sizeof(uint2)) != cudaSuccess ||
+            (any_host && cudaMalloc(&tmp, N * (size_t)(e1 + e2)) != cudaSuccess)) {
+            cudaGetLastError();
+            if (maps) cudaFree(maps);
+            return fail(ADC_ERR_NOMEM, "%s: device memory for the maps (%zu bytes)", fn, 2 * N * sizeof(uint2) + N * (size_t)(e1 + e2));
+        }
+    }
+    // join the engine's outstanding work (and whatever work of the caller's wrote device maps)
+    cudaError_t err = cudaDeviceSynchronize();
+    for (int v = 0; r && v < 2 && err == cudaSuccess; v++) {
+        const adc_remap& m = r->view[v];
+        const void* s1 = m.map1;
+        const void* s2 = m.map2;
+        long long q1 = p1[v], q2 = p2[v];
+        uint8_t* t = static_cast<uint8_t*>(tmp);
+        if (host[v][0] && err == cudaSuccess) {
+            err = cudaMemcpy2DAsync(t, W * e1, s1, q1, W * e1, H, cudaMemcpyDefault, e->main_st);
+            s1 = t, q1 = W * e1;
+        }
+        if (host[v][1] && err == cudaSuccess) {
+            err = cudaMemcpy2DAsync(t + N * e1, W * e2, s2, q2, W * e2, H, cudaMemcpyDefault, e->main_st);
+            s2 = t + N * e1, q2 = W * e2;
+        }
+        if (err == cudaSuccess) {
+            adc_launch_remap_convert(e->P.dm, r->map_type, s1, q1, s2, q2, maps + v * N, e->main_st);
+            err = cudaGetLastError();
+        }
+        if (err == cudaSuccess) err = cudaStreamSynchronize(e->main_st);   // the staging is reused by the next view
+    }
+    if (tmp) cudaFree(tmp);
+    if (err != cudaSuccess) {
+        if (maps) cudaFree(maps);
+        return fail(ADC_ERR_CUDA, "%s: %s", fn, cudaGetErrorString(err));
+    }
+    if (e->rect_map) CK(cudaFree(e->rect_map));
+    e->rect_map = maps;
+    e->rect_src_w = r ? r->src_width : 0;
+    e->rect_src_h = r ? r->src_height : 0;
+    return ADC_OK;
+}
+
+int adc_match_rectified_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                     const adc_image_desc* img, const void* d_cost, int32_t cost_layout,
+                                     int32_t cost_dtype, float* d_disp, const adc_volume_out* vols, int32_t n_vols,
+                                     const adc_map_out* maps, int32_t n_maps, void* stream) {
+    const char* fn = "adc_match_rectified_batch_device";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
+    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcImageGeom g;
+    AdcRectGeom r;
+    if ((rc = resolve_rectified(e, fn, img, &g, &r))) return rc;
+    long long last_view = 0;
+    if (n > 1 && __builtin_mul_overflow((long long)(n - 1), g.image_stride, &last_view))
+        return fail(ADC_ERR_ARG, "%s: img->image_stride %lld * (n - 1) overflows", fn, g.image_stride);
+    return match_outputs_device(e, fn, n, d_left, d_right, d_cost, cost_layout, cost_dtype, d_disp, vols, n_vols, maps, n_maps,
+                                (cudaStream_t)stream, &g, &r);
+}
+
+int adc_match_rectified(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img, const void* cost,
+                        int32_t cost_layout, int32_t cost_dtype, float* disp, const adc_volume_out* vols, int32_t n_vols,
+                        const adc_map_out* maps, int32_t n_maps) {
+    const char* fn = "adc_match_rectified";
+    int rc = check_output_args(fn, vols, n_vols, maps, n_maps, disp != nullptr, cost != nullptr, cost_layout, cost_dtype, false);
+    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcImageGeom g;
+    AdcRectGeom r;
+    if ((rc = resolve_rectified(e, fn, img, &g, &r))) return rc;
+    return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps, &g, &r);
 }
 
 void* adc_host_alloc(size_t bytes) {
@@ -1243,6 +1426,20 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
                 adc_launch_image_ingest(P, w, src, src + foot, g, ln.st, &e->launches);
                 bytes = 2.0 * foot + 2 * 3.0 * N;
+                break;
+            }
+            case 14: {  // volA's bytes taken as the wave's tight raw frames, resampled through the engine's maps
+                if (!e->rect_map) return fail(ADC_ERR_ARG, "adc_profile_kernel: no rectification is set (adc_set_rectification)");
+                const int bpp = adc_image_bytes_per_pixel(e->rect_format);
+                const bool planar = e->rect_format == ADC_IMG_RGB_PLANAR;
+                const long long sN = (long long)e->rect_src_w * e->rect_src_h, foot = sN * (planar ? 3 : bpp);
+                if (2 * foot > P.dm.vol_stride * 4)
+                    return fail(ADC_ERR_UNSUPPORTED, "adc_profile_kernel: a pair's raw frames (%lld bytes) exceed its share of a lane volume", 2 * foot);
+                const AdcImageGeom g{e->rect_format, (long long)e->rect_src_w * bpp, planar ? sN : 0, 2 * foot};
+                const AdcRectGeom rg{{e->rect_map, e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h};
+                const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
+                adc_launch_rectify_ingest(P, w, src, src + foot, g, rg, ln.st, &e->launches);
+                bytes = 2.0 * foot + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
                 break;
             }
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);

@@ -134,6 +134,62 @@ def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
     return ImageDesc(fmt, 0, pitches[1], pitches[2], 0)
 
 
+# rectification on the way in (adc_set_rectification, adc_match_rectified*): remap tables as cv2.initUndistortRectifyMap
+# returns them, float32 x / y planes or int16 (x, y) pairs + uint16 fractions
+REMAP_F32, REMAP_FIXED = 0, 1
+
+
+class Remap(ctypes.Structure):
+    """adc_remap: one view's map1 / map2 (host or device pointers) and their row pitches in bytes (0 = tight)."""
+    _fields_ = [("map1", ctypes.c_void_p), ("map2", ctypes.c_void_p), ("map1_pitch", ctypes.c_int64),
+                ("map2_pitch", ctypes.c_int64)]
+
+
+class Rectification(ctypes.Structure):
+    """adc_rectification: raw frame size, REMAP_* map type and both views' maps."""
+    _fields_ = [("src_width", ctypes.c_int32), ("src_height", ctypes.c_int32), ("map_type", ctypes.c_int32),
+                ("reserved", ctypes.c_int32), ("view", Remap * 2)]
+
+
+assert ctypes.sizeof(Remap) == 32 and ctypes.sizeof(Rectification) == 80
+
+
+def _map_plane(a, H: int, W: int, pair: bool):
+    """(pointer, row pitch in bytes, dtype name) of one remap plane: a numpy array or a torch tensor (CPU or CUDA) of
+    shape [H][W] ([H][W][2] for the int16 pairs) whose rows are contiguous; the pitch comes from the row stride."""
+    if hasattr(a, "data_ptr"):   # torch
+        if not a.is_cuda:
+            a = a.numpy()
+        else:
+            name = str(a.dtype).replace("torch.", "")
+            es = a.element_size()
+            shape, strides, ptr = tuple(a.shape), tuple(x * es for x in a.stride()), a.data_ptr()
+    if isinstance(a, np.ndarray):
+        name, es = a.dtype.name, a.dtype.itemsize
+        shape, strides, ptr = a.shape, a.strides, a.ctypes.data
+    want = (H, W, 2) if pair else (H, W)
+    if shape != want:
+        raise ValueError(f"expected a map of shape {want}, got {shape}")
+    inner = (2 * es, es) if pair else (es,)
+    if tuple(strides[1:]) != inner or strides[0] < 0:
+        raise ValueError(f"the elements of a map row must be contiguous (strides {strides})")
+    return ptr, strides[0], name
+
+
+def _remap(maps, H: int, W: int):
+    """(map type, Remap) of one view's (map1, map2) as cv2.initUndistortRectifyMap returns them: float32 [H][W] x and
+    y, or int16 [H][W][2] and uint16 [H][W] (int16 accepted for a CUDA tensor, as the same bits)."""
+    map1, map2 = maps
+    pair = len(getattr(map1, "shape", ())) == 3
+    p1, q1, t1 = _map_plane(map1, H, W, pair)
+    p2, q2, t2 = _map_plane(map2, H, W, False)
+    if not pair and (t1, t2) == ("float32", "float32"):
+        return REMAP_F32, Remap(p1, p2, q1, q2)
+    if pair and t1 == "int16" and t2 in ("uint16", "int16"):
+        return REMAP_FIXED, Remap(p1, p2, q1, q2)
+    raise ValueError(f"maps must be float32 [H][W] x2 or int16 [H][W][2] + uint16 [H][W], got {t1} and {t2}")
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -197,6 +253,11 @@ def load_library() -> ctypes.CDLL:
                                    ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32]
     L.adc_match_images_batch_device.argtypes = [vp, i32, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
                                                 ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32, vp]
+    L.adc_set_rectification.argtypes = [vp, ctypes.POINTER(Rectification)]
+    L.adc_match_rectified.argtypes = [vp, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
+                                      ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32]
+    L.adc_match_rectified_batch_device.argtypes = [vp, i32, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
+                                                   ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -257,6 +318,7 @@ class Engine:
         got = _Config()
         self._L.adc_get_config(self._h, ctypes.byref(got))
         self.wave_pairs, self.lanes, self.device = got.wave_pairs, got.lanes, got.device
+        self.rect_src_size = None   # (width, height) of the raw frames while a rectification is set
 
     def close(self):
         if getattr(self, "_h", None):
@@ -401,10 +463,17 @@ class Engine:
         [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray) or [3][H][W] (rgb_planar) whose rows may be pitched, e.g.
         frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.  The result is
         what match_outputs gives for the same pixels packed as BGR."""
+        return self._match_views(self._L.adc_match_images, self.height, self.width, left, right, format, maps, volumes,
+                                 layout, dtype, cost, cost_layout, cost_dtype, disparity)
+
+    def _match_views(self, call, vh, vw, left, right, format, maps, volumes, layout, dtype, cost, cost_layout,
+                     cost_dtype, disparity):
+        """The host entries that take views in an IMG_* format: adc_match_images (views of H x W) and
+        adc_match_rectified (raw frames of vh x vw)."""
         fmt = _img_format(format)
         H, W, D = self.height, self.width, self.D
-        desc = _image_view_desc(left, fmt, H, W)
-        if _image_view_desc(right, fmt, H, W).row_pitch != desc.row_pitch or \
+        desc = _image_view_desc(left, fmt, vh, vw)
+        if _image_view_desc(right, fmt, vh, vw).row_pitch != desc.row_pitch or \
                 (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
             raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
         maps = [maps] if isinstance(maps, (str, int)) else list(maps)
@@ -418,9 +487,8 @@ class Engine:
         mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
         c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
         disp = np.empty((H, W), np.float32) if disparity else None
-        _check(self._L.adc_match_images(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc),
-                                        None if c is None else c.ctypes.data, clay, cdt,
-                                        None if disp is None else disp.ctypes.data, vouts, len(volumes), mouts, len(maps)))
+        _check(call(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc), None if c is None else c.ctypes.data,
+                    clay, cdt, None if disp is None else disp.ctypes.data, vouts, len(volumes), mouts, len(maps)))
         return disp, out
 
     def match_images_batch_device(self, n: int, d_left: int, d_right: int, image=None, maps=(), volumes=(),
@@ -434,6 +502,51 @@ class Engine:
                                                      _code(COST_LAYOUTS, cost_layout, "layout"),
                                                      _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
                                                      len(volumes), marr, len(maps), stream))
+
+    # ---- rectification on the way in (adc_set_rectification, adc_match_rectified*) --------------------
+    def set_rectification(self, left_maps, right_maps=None, src_size=None):
+        """Sets the remap tables the rectified entries resample each raw view through: `left_maps` / `right_maps` are
+        (map1, map2) exactly as cv2.initUndistortRectifyMap returns them for this engine's (width, height) -- float32
+        [H][W] x and y, or int16 [H][W][2] and uint16 [H][W] -- as numpy arrays or CUDA tensors (row pitches from the
+        strides); `src_size` = (width, height) of the raw frames.  The maps are copied: the caller's may be freed.
+        set_rectification(None) clears them."""
+        if left_maps is None:
+            _check(self._L.adc_set_rectification(self._h, None))
+            self.rect_src_size = None
+            return
+        sw, sh = (int(v) for v in src_size)
+        t0, left = _remap(left_maps, self.height, self.width)
+        t1, right = _remap(right_maps, self.height, self.width)
+        if t0 != t1:
+            raise ValueError("both views' maps must be of the same type")
+        r = Rectification(sw, sh, t0, 0, (Remap * 2)(left, right))
+        _check(self._L.adc_set_rectification(self._h, ctypes.byref(r)))
+        self.rect_src_size = (sw, sh)
+
+    def match_rectified(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
+                        cost_layout="hwd", cost_dtype=None, disparity=True):
+        """match_images for raw frames: `left` / `right` are uint8 numpy views of the src_size frames given to
+        set_rectification, in any IMG_* format and pitch, resampled through the maps on the way in.  The result is what
+        match_outputs gives for cv2.remap(view, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) of each view packed as
+        BGR."""
+        if self.rect_src_size is None:
+            raise AdcError("no rectification is set (set_rectification)")
+        sw, sh = self.rect_src_size
+        return self._match_views(self._L.adc_match_rectified, sh, sw, left, right, format, maps, volumes, layout, dtype,
+                                 cost, cost_layout, cost_dtype, disparity)
+
+    def match_rectified_batch_device(self, n: int, d_left: int, d_right: int, image=None, maps=(), volumes=(),
+                                     d_disp: int = 0, d_cost: int = 0, cost_layout="dhw", cost_dtype="f32",
+                                     stream: int = 0):
+        """match_images_batch_device for raw frames: `image` (an ImageDesc, None = tight packed BGR) describes the raw
+        views of the src_size given to set_rectification; pair i at i * image_stride bytes.  Enqueued on `stream`
+        without synchronising, like match_batch_device."""
+        varr, marr = _volume_outs(volumes), _map_outs(maps)
+        _check(self._L.adc_match_rectified_batch_device(self._h, n, d_left, d_right,
+                                                        None if image is None else ctypes.byref(image), d_cost or None,
+                                                        _code(COST_LAYOUTS, cost_layout, "layout"),
+                                                        _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
+                                                        len(volumes), marr, len(maps), stream))
 
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
@@ -478,7 +591,8 @@ class Engine:
 
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
                        "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10,
-                       "cost_export": 11, "confidence": 12, "image_ingest": 13}
+                       "cost_export": 11, "confidence": 12, "image_ingest": 13,
+                       "rectify": 14}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""

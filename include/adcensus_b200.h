@@ -310,6 +310,69 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
                      const void* cost, int32_t cost_layout, int32_t cost_dtype, float* disp,
                      const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
 
+/* ---- rectification on the way in ---------------------------------------------------------------------
+ * The rectified entry points take raw camera frames and resample each view through a per-view remap table (as from
+ * cv::initUndistortRectifyMap) while they ingest it: one gather pass per view writes the wave's packed BGR, and
+ * everything after that is the pipeline of the image entry points.
+ * Semantics: a raw pair matched through adc_match_rectified* gives exactly what this two-step path gives -- the final
+ * map, the exported volumes and the side maps, bit for bit:
+ *   cv::remap(view, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) on each view, then the same call through
+ *   adc_match_outputs* with the rectified images packed as BGR.
+ * Channels are resampled independently; formats are resolved as for adc_match_images (gray v -> (v, v, v)), which
+ * commutes with the resampling.  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
+ * the 5-bit fractions:
+ *   ADC_REMAP_F32 (map1 = float x [H][W], map2 = float y [H][W], CV_32FC1 each):
+ *     X = round_half_even(x * 32) saturated to int32, where NaN and values outside int32 give INT_MIN;
+ *     x0 = sat_int16(X >> 5) (arithmetic shift), ax = X & 31; likewise Y, y0, ay.
+ *   ADC_REMAP_FIXED (map1 = int16 (x, y) pairs [H][W][2], CV_16SC2; map2 = uint16 [H][W], CV_16UC1, as from
+ *   initUndistortRectifyMap(..., CV_16SC2) or cv::convertMaps):
+ *     (x0, y0) = map1; a = map2 & 1023, ax = a & 31, ay = a >> 5 (the high bits of map2 are ignored).
+ *   out = (sum over dx, dy in {0, 1} of w * s + 512) >> 10, with w = (dx ? ax : 32 - ax) * (dy ? ay : 32 - ay) and s
+ *   the source byte at (x0 + dx, y0 + dy), or 0 for a neighbour outside the src_width x src_height frame.
+ * Every map is [H][W] over the engine's output size; each map's rows may be pitched (bytes, 0 = tight).  The maps of
+ * an F32 set and the map2 of a FIXED set are as cv::remap takes them; both map types are pinned to what cv::remap does
+ * with that map (initUndistortRectifyMap's CV_16SC2 output is not convertMaps of its float output everywhere). */
+enum { ADC_REMAP_F32 = 0, ADC_REMAP_FIXED = 1 };
+typedef struct adc_remap {
+    const void* map1;      /* F32: float x [H][W]; FIXED: int16 (x, y) [H][W][2] */
+    const void* map2;      /* F32: float y [H][W]; FIXED: uint16 [H][W] */
+    int64_t map1_pitch;    /* bytes from one row of map1 to the next, 0 = tight (W * 4) */
+    int64_t map2_pitch;    /* bytes from one row of map2 to the next, 0 = tight (W * 4, FIXED: W * 2) */
+} adc_remap;               /* 32 bytes */
+typedef struct adc_rectification {
+    int32_t src_width;     /* raw frame size, each 1..32767 (OpenCV's coordinates are int16) */
+    int32_t src_height;
+    int32_t map_type;      /* ADC_REMAP_* */
+    int32_t reserved;      /* must be zero */
+    adc_remap view[2];     /* left, right */
+} adc_rectification;       /* 80 bytes */
+
+/* Sets (r != NULL) or clears (r == NULL) the engine's rectification.  Both views' maps are copied and converted into
+ * device memory the engine owns (8 bytes per output pixel and view; the caller's maps may be freed on return).  Map
+ * pointers may be host memory (pageable or pinned) or device memory; device maps must be complete when the call is
+ * made.  Synchronous: before the maps are replaced the device is synchronised, so that every earlier call, pipelined
+ * or not, runs with the maps that were set when it was made.  Rules (each violation fails with ADC_ERR_ARG naming the
+ * field; those that need no output size before the engine is checked): src_width and src_height in 1..32767;
+ * map_type one of ADC_REMAP_*; reserved zero; no map pointer NULL; pitches not negative and, when not 0, at least a
+ * row's bytes; map pointers and pitches aligned to their element (4 bytes for float, 2 for int16 / uint16).  A failed
+ * allocation fails with ADC_ERR_NOMEM before anything changes.  adc_destroy frees the maps. */
+int adc_set_rectification(adc_engine* e, const adc_rectification* r);
+
+/* adc_match_images_batch_device / adc_match_images on raw frames: `img` (NULL = tight packed BGR) describes the raw
+ * views, and its size-dependent rules are checked against src_width x src_height instead of W x H.  Each view is
+ * resampled through the maps set with adc_set_rectification (semantics above) by one ingestion launch per wave, in
+ * place of the image ingestion; cost input, volume export, side maps, streams and pipelined mode as for the image entry
+ * points.  Without a rectification set they fail with ADC_ERR_ARG.  The host entry uploads the raw views tightly into
+ * the lane volume that stage 1 writes when they fit there, and otherwise into the device staging the exported volumes
+ * use (allocated on first use, grown when needed), so it runs for every source size adc_set_rectification accepts. */
+int adc_match_rectified_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                     const adc_image_desc* img, const void* d_cost, int32_t cost_layout,
+                                     int32_t cost_dtype, float* d_disp, const adc_volume_out* vols, int32_t n_vols,
+                                     const adc_map_out* maps, int32_t n_maps, void* stream);
+int adc_match_rectified(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img,
+                        const void* cost, int32_t cost_layout, int32_t cost_dtype, float* disp,
+                        const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
@@ -333,7 +396,9 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * call, ADC_COST_DHW / ADC_COST_F32 if there was none; N*Dp*4 + N*D*sizeof(element) bytes per pair), 12 = confidence
  * (MIN_COST and PEAK_RATIO of the left view; N*Dp*4 + 2*4*N bytes per pair), 13 = image ingestion (format of the
  * engine's last adc_match_images* call, ADC_IMG_RGB_PLANAR if there was none, tight pitches; the source bytes of both
- * views + 2*3*N written per pair).
+ * views + 2*3*N written per pair), 14 = rectified ingestion (format of the engine's last adc_match_rectified* call,
+ * ADC_IMG_BGR if there was none, tight raw frames; needs a rectification set; per pair the bytes of both raw frames +
+ * 2*3*N written, plus both views' internal maps, 2*8*N, once per wave).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 

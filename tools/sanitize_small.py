@@ -124,4 +124,49 @@ for fmt in IT.FORMATS:
         cudart.cudaFree(p)
     print("images ok", fmt, flush=True)
 eng.close()
+
+# rectified input: raw odd-x crops in every format, the right view of each ending exactly at the end of its own
+# cudaMalloc allocation, with maps that sample the last row and column, half a pixel and more beyond them
+import rectify_testlib as R
+w, h, D, n, sw, sh = 71, 47, 23, 3, 83, 53
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+rng = np.random.default_rng(5)
+edge = np.array([sw - 1, sw - 1.5, sw - 0.5, sw - 1 / 64, sw, sw + 0.5, -0.5, -1 / 64], np.float32)
+for k, fmt in enumerate(IT.FORMATS):
+    maps = []
+    for v in range(2):
+        mx, my = R.warp_maps(w, h, sw, sh, 70 + v, specials=False)
+        mx[:, -8:] = edge
+        my[-8:, :] = (edge * sh / sw).astype(np.float32)[:, None]
+        my[-1, :] = sh - 1
+        mx[-1, ::2] = sw - 1
+        maps.append(R.convert_maps(mx, my) if k % 2 else (mx, my))
+    eng.set_rectification(maps[0], maps[1], (sw, sh))
+    raw = [rng.integers(0, 256, (sh, sw, 3), dtype=np.uint8) for _ in range(2)]
+    if fmt == "gray":
+        raw = [IT.gray_to_bgr(x[:, :, 1]) for x in raw]
+    bpp, x0 = IT.BPP[fmt], 3
+    rp = (sw + x0) * bpp
+    pp = sh * rp if fmt == "rgb_planar" else 0
+    stride = IT.footprint(fmt, sh, rp, pp)
+    ptrs = []
+    for img in raw:
+        host = np.zeros(n * stride, np.uint8)
+        for i in range(n):
+            IT.write_view(host[i * stride:], IT.from_bgr(img, fmt), fmt, rp, pp, x0 * bpp)
+        size = n * stride - (rp - (x0 + sw) * bpp)
+        p = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(p), size) == 0
+        assert cudart.cudaMemcpy(p, host.ctypes.data, size, 1) == 0
+        ptrs.append(p.value)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_rectified_batch_device(n, ptrs[0] + x0 * bpp, ptrs[1] + x0 * bpp, image=A.image_desc(fmt, rp, pp, stride),
+                                     d_disp=d_o.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(R.remap(raw[0], *maps[0]), R.remap(raw[1], *maps[1]))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), fmt
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("rectified ok", fmt, flush=True)
+eng.close()
 print("all ok")
