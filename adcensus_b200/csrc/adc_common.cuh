@@ -14,6 +14,7 @@
 //   disp_*   f32 [S][H][W]
 //   label    u8  [S][H][W]         0 = valid, 1 = mismatch list, 2 = occlusion list
 #pragma once
+#include <cuda.h>     // CUtensorMap and its enums only
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -86,6 +87,14 @@ inline int adc_sm_count() {
 
 // TMA descriptors (CUtensorMap, 128 bytes each) of a lane's two cost volumes for the two axes of the fused aggregation kernel
 struct alignas(64) AdcArmTmaps { unsigned char map[2][2][128]; int ok; };
+// TMA descriptors of the scanline passes, per axis (0: +-x, 1: +-y): the two volumes and the penalty records, with the boxes
+// of that axis's launch plan (T steps per ring slot, NS slots per warp, dynamic shared memory per CTA; so_plan.h)
+struct alignas(64) AdcSoTmaps { unsigned char cost[2][2][128]; unsigned char rec[2][128]; int T[2], NS[2]; unsigned smem[2]; };
+// cuTensorMapEncodeTiled, fetched through the runtime (no link-time libcuda dependency); NULL when the driver lacks it
+typedef CUresult (*AdcTmapEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+AdcTmapEncodeFn adc_tmap_encoder();
 
 // ---- launchers (defined in the k_*.cu files; all asynchronous on `st`) -------------------------
 struct AdcWave {            // device pointers of one wave (S pairs)
@@ -108,6 +117,7 @@ struct AdcWave {            // device pointers of one wave (S pairs)
     int* rowcnt;            // [S][2][H] per-row list counts / offsets
     unsigned* so_bitrows;   // [S][4][H][row words] mirrored per-row bit vectors of the right image (scanline optimiser)
     unsigned* so_rec;       // [S][4][N][rec words] per-pixel penalty records of the four pass directions
+    const AdcSoTmaps* so_tm;     // host memory, owned by the lane: tensor maps of the scanline passes
     int* tile_stamp;        // [S][tiles] region voting: epoch of the last change near a 16x16 tile
     int* last_eval;         // [S][N]     region voting: epoch of a pixel's (or tile's) last evaluation
     unsigned long long* wta_key;  // [S][N] right-view WTA keys (ordered cost << 32 | disparity index)
@@ -177,7 +187,9 @@ size_t adc_arm_overread_floats(const AdcDims& dm);     // padding the arena keep
 void adc_launch_so_bitrows(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 size_t adc_so_rec_bytes(const AdcDims& dm);
 size_t adc_so_bitrow_bytes(const AdcDims& dm);
-// one scanline pass: (sx,sy) in {(1,0),(-1,0),(0,1),(0,-1)}
+// tensor maps and launch plans of the scanline passes over a lane of capacity S (false: they cannot be encoded)
+bool adc_so_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, unsigned* so_rec, AdcSoTmaps* out);
+// one scanline pass: (sx,sy) in {(1,0),(-1,0),(0,1),(0,-1)}, src = w.volA or w.volB; non-zero: not launched
 int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
                         cudaStream_t st, unsigned long long* launches);
 int adc_launch_wta(const AdcParams& P, const AdcWave& w, const float* vol, cudaStream_t st, unsigned long long* launches);

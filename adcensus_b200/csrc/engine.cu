@@ -64,6 +64,7 @@ struct Lane {
     void* arena = nullptr;
     AdcWave w{};                       // device pointers, capacity S pairs
     AdcArmTmaps arm_tm{};              // TMA descriptors of this lane's volumes (fused aggregation kernel)
+    AdcSoTmaps so_tm{};                // TMA descriptors of this lane's volumes and penalty records (scanline passes)
     uint8_t* pin_in = nullptr;         // [S][2][N*3] pinned staging (pageable callers only)
     float* pin_out = nullptr;          // [S][N]
     // pending copy-out of a staged wave (pageable callers)
@@ -382,7 +383,7 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
         const float* src = (ps % 2 == 0) ? A : B;
         float* dst = (ps % 2 == 0) ? B : A;
         if (adc_launch_scanline(P, w, src, dst, dirs[ps][0], dirs[ps][1], st, L))
-            return fail(ADC_ERR_UNSUPPORTED, "disparity range %d exceeds the scanline kernel's limit of 256", P.dm.D);
+            return fail(ADC_ERR_UNSUPPORTED, "scanline pass not launched (disparity range %d, limit 256)", P.dm.D);
         if (ps % 2 == 0) e->dbg_init = B; else e->dbg_aggr = A;
         if (ps == 3) export_vol(ADC_VOL_OPT, A);
         if (stop(ADC_STAGE_SO1 + ps)) return launched("scanline optimisation");
@@ -957,6 +958,9 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
         if (cudaMalloc(&ln.arena, bytes) != cudaSuccess) { cudaGetLastError(); return bail(fail(ADC_ERR_NOMEM, "device arena of %zu bytes", bytes)); }
         carve_lane(ln.arena, e->P.dm, e->P.L1, S, &ln.w);
         if (adc_arm_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, &ln.arm_tm)) ln.w.arm_tm = &ln.arm_tm;
+        if (!adc_so_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, ln.w.so_rec, &ln.so_tm))
+            return bail(fail(ADC_ERR_CUDA, "adc_create: the scanline passes' tensor maps could not be encoded (cuTensorMapEncodeTiled)"));
+        ln.w.so_tm = &ln.so_tm;
         if (cudaMemsetAsync(ln.arena, 0, bytes, ln.st) != cudaSuccess) return bail(fail(ADC_ERR_CUDA, "memset failed"));
         if (cudaHostAlloc((void**)&ln.pin_in, (size_t)S * 2 * N * 3, cudaHostAllocDefault) != cudaSuccess ||
             cudaHostAlloc((void**)&ln.pin_out, (size_t)S * N * sizeof(float), cudaHostAllocDefault) != cudaSuccess) {
