@@ -181,6 +181,12 @@ void adc_launch_arm_sum(const AdcParams& P, const AdcWave& w, const float* src, 
 bool adc_arm_sum2_available(const AdcParams& P);
 bool adc_launch_arm_sum2(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int dir,
                          const uint16_t* sup_mid, cudaStream_t st, unsigned long long* launches);
+// the AD-census cost computed in place of the cost volume and summed as the first horizontal pass (no division) into
+// `dst`; cost_out (nullable) also receives the cost volume, padding disparities included, as adc_launch_cost writes it.
+// false = not applicable for these parameters (ca_plan.h), nothing launched
+bool adc_cost_arm_sum_h_available(const AdcParams& P);
+bool adc_launch_cost_arm_sum_h(const AdcParams& P, const AdcWave& w, float* dst, float* cost_out, cudaStream_t st,
+                               unsigned long long* launches);
 size_t adc_arm_rec_bytes(const AdcDims& dm, int L1);   // window records of one pair
 bool adc_arm_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, AdcArmTmaps* out);   // false: TMA path not available
 size_t adc_arm_overread_floats(const AdcDims& dm);     // padding the arena keeps behind the two volumes

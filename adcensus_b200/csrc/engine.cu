@@ -22,6 +22,7 @@
 
 #include "../../include/adcensus_b200.h"
 #include "adc_common.cuh"
+#include "ca_plan.h"
 
 static_assert(sizeof(adc_option) == 60, "adc_option must match the reference's ADCensusOption (60 bytes)");
 static_assert(offsetof(adc_option, so_p1) == 32 && offsetof(adc_option, irv_th) == 48 &&
@@ -303,7 +304,8 @@ bool agg_fused_for(const adc_engine* e, int last_stage) {
 // `last_stage` (ADC_STAGE_MEDIAN = everything).  ev[] (optional, 6 events) are recorded at the
 // stage boundaries the reference times in Match (ADCensusStereo.cpp:81-129).  `outs` (optional) are exported at the one
 // point where their volume is live (DESIGN.md section 11): COST in C0 right after stage 1, before the first aggregation
-// launch (the fused passes overwrite volB); AGGR in volA after the last aggregation pass, before scanline pass 2 writes volA;
+// launch (the fused passes overwrite volB) -- or, where the cost is computed inside the first aggregation pass, right after
+// that kernel, which then also stores the cost volume to C0; AGGR in volA after the last aggregation pass, before scanline pass 2 writes volA;
 // OPT in volA after scanline pass 4, which nothing later writes.  `maps` (optional) likewise (DESIGN.md section 12): the
 // WTA maps and the confidence right after the WTA (disp_l is overwritten by the LR check), the outlier map right after
 // the LR check (region voting changes label).
@@ -322,7 +324,14 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
     float* A = w.volA;
     float* B = w.volB;
     float* C0 = fused ? B : A;          // where the cost volume is written
-    e->dbg_init = C0;
+    // The fused path computes the AD-census cost inside iteration 0's horizontal pass (k_cost_arm_sum_h): the cost volume
+    // is not materialised, C0 is written only for a COST export.  The host staging of images, rectified frames and cost
+    // inputs that goes through "the lane volume that stage 1 writes" (volB here) stays valid: volB is first written by the
+    // first fused vertical double pass, after the ingestion kernels have read it.
+    const bool cost_in_agg = fused && last_stage > ADC_STAGE_ARMS && !cost.p && adc_cost_arm_sum_h_available(P);
+    bool cost_exported = false;
+    for (int i = 0; i < outs.n; i++) cost_exported |= outs.o[i].stage == ADC_VOL_COST;
+    e->dbg_init = cost_in_agg && !cost_exported ? nullptr : C0;   // no tap of a cost volume that was never written
     e->dbg_aggr = C0;
     auto stop = [&](int stage) { e->dbg_stage = stage; return stage >= last_stage; };
     // launch errors surface where they happen: a stage boundary reports the first failed launch since the previous one
@@ -342,8 +351,8 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
     // kernels after this stage read the packed pixels (bgrx) the census kernel writes.
     adc_launch_gray_census(P, w, st, L);
     if (cost.p) adc_launch_cost_ingest(P, w, cost.p, cost.layout, cost.dtype, C0, st, L);
-    else adc_launch_cost(P, w, C0, st, L);
-    export_vol(ADC_VOL_COST, C0);
+    else if (!cost_in_agg) adc_launch_cost(P, w, C0, st, L);
+    if (!cost_in_agg) export_vol(ADC_VOL_COST, C0);
     if ((rc = launched("cost volume"))) return rc;
     if (ev) CK(cudaEventRecord(ev[1], st));
     if (stop(ADC_STAGE_COST)) return ADC_OK;
@@ -353,7 +362,13 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
     if ((rc = launched("cross arms"))) return rc;
     if (stop(ADC_STAGE_ARMS)) return ADC_OK;
     if (fused) {
-        adc_launch_arm_sum(P, w, B, A, 0, nullptr, st, L);                       // it 0: H
+        if (cost_in_agg) {                                                       // cost + it 0: H
+            if (!adc_launch_cost_arm_sum_h(P, w, A, cost_exported ? C0 : nullptr, st, L))
+                return fail(ADC_ERR_UNSUPPORTED, "fused cost and aggregation pass not applicable");
+            export_vol(ADC_VOL_COST, C0);
+        } else {
+            adc_launch_arm_sum(P, w, B, A, 0, nullptr, st, L);                   // it 0: H
+        }
         if (!adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L) ||               // it 0: V /   + it 1: V
             !adc_launch_arm_sum2(P, w, B, A, 0, w.sup_v, st, L) ||               // it 1: H /   + it 2: H
             !adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L))                 // it 2: V /   + it 3: V
@@ -1446,6 +1461,11 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 bytes = 2.0 * foot + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
                 break;
             }
+            case 15:    // the cost computed from the wave's images and census words, summed as iteration 0's H pass into volA
+                if (!adc_launch_cost_arm_sum_h(P, w, w.volA, nullptr, ln.st, &e->launches))
+                    return fail(ADC_ERR_UNSUPPORTED, "fused cost and horizontal arm sums not applicable");
+                bytes = V + 24 * N + (double)P.dm.H * ((P.dm.W + 3) / 4) * arm_rec_words(P.L1) * 4.0;   // + horizontal records
+                break;
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);
         }
     }
@@ -1526,6 +1546,10 @@ size_t adc_debug_get(adc_engine* e, int32_t tap, void* dst, size_t cap) {
         case ADC_TAP_VOL_AGGR: {
             const float* v = tap == ADC_TAP_VOL_INIT ? e->dbg_init : e->dbg_aggr;
             bytes = N * dm.D * sizeof(float);
+            if (dst && cap >= bytes && !v) {
+                fail(ADC_ERR_ARG, "adc_debug_get: no such volume: no run yet, or the last run computed the cost inside the aggregation");
+                return 0;
+            }
             if (!dst || cap < bytes || !v) return bytes;
             // strip the Dp padding: [N][Dp] -> [N][D]
             if (cudaMemcpy2D(dst, (size_t)dm.D * 4, v, (size_t)dm.Dp * 4, (size_t)dm.D * 4, N, cudaMemcpyDeviceToHost) != cudaSuccess) {
