@@ -1,5 +1,6 @@
-// ca_plan.h -- window-record sizes and the launch plan of the fused cost + first horizontal arm sum (k_cost_arm_sum_h,
-// k_aggregate.cu).  Plain C++ with no CUDA dependency, so that tests/test_cost_fused_agg.py can check the plan on the CPU.
+// ca_plan.h -- window-record sizes and the launch plans of the fused aggregation kernels of k_aggregate.cu: the fused cost +
+// first horizontal arm sum (k_cost_arm_sum_h) and the double passes (k_arm_sum2t, k_arm_sum2).  Plain C++ with no CUDA
+// dependency, so that tests/test_cost_fused_agg.py and tests/test_kernel_sweep.py can check the plans on the CPU.
 #pragma once
 #include <stddef.h>
 
@@ -61,4 +62,81 @@ inline CaPlan ca_plan(int W, int Dp, int L1) {
     if (p.threads > CA_MAX_THREADS) p.threads = CA_MAX_THREADS;
     p.ok = true;
     return p;
+}
+
+// Plan of the TMA-staged double pass (k_arm_sum2t, k_aggregate.cu) for one axis (dir 0 = rows, 1 = columns): quads per
+// CTA, box length, segment length, lines per CTA, shared-memory sizes.
+struct ArmSum2tPlan { int qc, BR, Ls, nseg, nchunks, rows_s_cap, threads, lpc; size_t smem; bool ok; };
+inline ArmSum2tPlan plan_arm_sum2t(int W, int H, int Dp, int L1, int dir) {
+    const int budget_kb = 104;            // shared memory per CTA (two CTAs per SM); 72 and 130 KB measured slower or equal
+    const int qc_env[2] = {0, 0};         // quads per CTA: 8, or 4 when that makes a whole line fit (chosen below)
+    ArmSum2tPlan pl{};
+    const int Q = Dp / 4, L = dir ? H : W, L1c = arm_L1c(L1);
+    if (Q < 4) { pl.ok = false; return pl; }                      // (tiny disparity ranges take the LDG kernel)
+    const int BR = 64;
+    auto need = [&](int qc, int ls, bool whole, int* rows_s_cap) {
+        const int rows_m = (whole ? L : ls + 2 * L1c + 3) + 13;   // + 8 over-read rows, + rounding, + the row that holds the mbarrier
+        const int rows_s = whole ? L : ls + 4 * L1c + 3;
+        *rows_s_cap = (rows_s + BR - 1) / BR * BR + 8;
+        return (size_t)(*rows_s_cap + rows_m) * qc * 16 + 16 + (size_t)(rows_m / 4 + 1) * arm_rec_words(L1) * 4 + (size_t)rows_m * 4 + 64;   // tiles | mid | mbarrier | records | divisors
+    };
+    const size_t budget = (size_t)budget_kb * 1024;
+    int qc = qc_env[dir] ? qc_env[dir] : 8;
+    if (qc > Q) qc = 4;
+    int cap = 0;
+    if (!qc_env[dir] && need(8, 0, true, &cap) > budget && need(4, 0, true, &cap) <= budget) qc = 4;   // a whole line with 4 quads beats segments with 8
+    pl.qc = qc; pl.BR = BR;
+    if (need(qc, 0, true, &cap) <= budget) { pl.Ls = (L + 3) & ~3; pl.nseg = 1; }
+    else {
+        int ls = (L + 3) & ~3;
+        while (ls > 64 && need(qc, ls, false, &cap) > budget) ls -= 4;
+        if (need(qc, ls, false, &cap) > budget) { pl.ok = false; return pl; }
+        const int nseg = (L + ls - 1) / ls;
+        pl.Ls = ((L + nseg - 1) / nseg + 3) & ~3;
+        pl.nseg = (L + pl.Ls - 1) / pl.Ls;
+    }
+    pl.smem = need(qc, pl.Ls, pl.nseg == 1, &pl.rows_s_cap);
+    pl.nchunks = (Q + qc - 1) / qc;
+    // threads: as few whole warps as give every thread the same number of groups
+    const int groups = ((pl.nseg == 1 ? L : pl.Ls) + 3) / 4, slots = 256 / qc;
+    const int iters = (groups + slots - 1) / slots;
+    pl.threads = (((groups + iters - 1) / iters) * qc + 31) / 32 * 32;
+    if (pl.threads > 256) pl.threads = 256;
+    // lines per CTA: each line after the first loads while the previous one finishes.  A line cut into segments keeps one
+    // per CTA (1920x1080x192's vertical pass measured 3 % slower with two or four).
+    pl.lpc = pl.nseg > 1 ? 1 : 4;
+    pl.ok = true;
+    return pl;
+}
+
+// Segment length / chunk width of the LDG double pass (k_arm_sum2, k_aggregate.cu) for one axis: the largest segment whose `mid` rows fit the
+// shared-memory budget; a whole line when it fits.  ok = false: not applicable (arms too long for the budget).
+struct ArmSum2Plan { int Ls, qc_log2, nseg, nchunks, rows_m_cap; size_t smem; bool ok; };
+inline ArmSum2Plan plan_arm_sum2(int W, int H, int Dp, int L1, int dir) {
+    const int budget_kb = 60;    // shared memory per CTA the plan may use (40 KB: 8 % slower on Cone; 75 / 100 KB: no faster)
+    ArmSum2Plan pl{};
+    const int Q = Dp / 4, L = dir ? H : W, L1c = arm_L1c(L1);
+    int ql = 0;
+    while ((1 << ql) < Q && ql < 3) ql++;                 // Qc = min(8, Q rounded up to a power of two); 4 quads measured 4-25 % slower
+    const int Qc = 1 << ql;
+    size_t budget = (size_t)budget_kb * 1024;
+    const size_t need_min = (size_t)(2 * L1c + 16 + 64) * Qc * 16;    // a segment of at least 64 outputs
+    if (budget < need_min) budget = need_min;
+    if (budget > 200 * 1024) { pl.ok = false; return pl; }
+    const int rows_max = (int)(budget / ((size_t)Qc * 16));
+    int Ls;
+    if (L + 12 <= rows_max) Ls = (L + 3) & ~3;             // the whole line
+    else {
+        const int ls_max = (rows_max - 2 * L1c - 16) & ~3;
+        const int nseg = (L + ls_max - 1) / ls_max;
+        Ls = ((L + nseg - 1) / nseg + 3) & ~3;
+    }
+    pl.Ls = Ls; pl.qc_log2 = ql;
+    pl.nseg = (L + Ls - 1) / Ls;
+    pl.nchunks = (Q + Qc - 1) / Qc;
+    const int rows = (pl.nseg == 1 ? L : Ls + 2 * L1c + 3) + 4 + 8;   // + the rows the last trip of a walk may touch
+    pl.rows_m_cap = (rows + 3) & ~3;
+    pl.smem = (size_t)pl.rows_m_cap * Qc * 16 + (size_t)(pl.rows_m_cap / 4 + 1) * arm_rec_words(L1) * 4 + (size_t)pl.rows_m_cap * 4 + 16;   // mid | records | divisors
+    pl.ok = true;
+    return pl;
 }

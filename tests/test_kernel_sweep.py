@@ -1,0 +1,342 @@
+"""Parity sweep over the kernel instantiations and launch-plan branches that the disparity range and the shape select.
+
+The scanline, fused-cost and fused-aggregation kernels are templates whose instantiation follows from the disparity
+range, and their launch plans (adcensus_b200/csrc/so_plan.h, ca_plan.h) cut rows and columns differently per shape.
+
+CPU: the instantiations compiled into the library (cuobjdump -symbols), the instantiations every GPU case of this file
+reaches by the launch rules, and the assertion that together they reach every one; the plan branch each plan-branch case
+is meant to take; the oracle against the reference's hashes of the sweep cases (tests/golden/golden_sweep_ref.json).
+GPU: for every disparity range 1..256 and every plan-branch case, one batched call over five distinct pairs (three waves
+of two, the last partial; a flat and a white-noise pair between textured ones) that exports every volume and side map,
+each pair compared bit for bit with its own oracle run.
+"""
+import json
+import os
+import re
+import subprocess
+import sys
+from concurrent.futures import ThreadPoolExecutor
+from pathlib import Path
+
+import numpy as np
+import pytest
+
+import adc_testlib as T
+import maps_testlib as MT
+from test_gpu_parity import _engine, _same
+
+ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT / "tools"))
+import make_golden_sweep as GS  # noqa: E402  (case definitions shared with the fixture generator)
+
+SMEM_RESERVED_PER_CTA = 1024     # shared memory the driver reserves per CTA on sm_90
+
+
+# ---- cases ----------------------------------------------------------------------------------------------------------
+class Case:
+    """One batched GPU run: W x H x D with `opt`, n pairs in waves of `wave_pairs` over `lanes` lanes."""
+
+    def __init__(self, name, W, H, opt, seed, wave_pairs=2, lanes=2, n=5):
+        self.name, self.W, self.H, self.opt, self.seed = name, W, H, opt, seed
+        self.D = opt.max_disparity - opt.min_disparity
+        self.Dp = (self.D + 3) // 4 * 4
+        self.L1 = opt.cross_L1
+        self.wave_pairs, self.lanes, self.n = wave_pairs, lanes, n
+
+
+def _sweep_case(D):
+    W, H, opt, seed = GS.sweep_case(D)
+    return Case(f"D{D}", W, H, opt, seed)
+
+
+def _opt(D, **kw):
+    return T.default_option(max_disparity=D, **kw)
+
+
+LONG_ARMS = dict(cross_L1=255, cross_L2=120, cross_t1=50, cross_t2=25)
+# name -> (case, what its plans must be).  Shapes found with the plan executables; test_plan_branch_cases checks them.
+PLAN_CASES = {
+    # fused cost + first horizontal pass (ca_plan): rows in 2 and 3 segments at L1 = 34, qc = 8, exact and not
+    "cost_rows_2seg": (Case("cost_rows_2seg", 501, 23, _opt(45), 61), dict(ca_nseg=2, ca_qc=8)),
+    "cost_rows_3seg": (Case("cost_rows_3seg", 861, 19, _opt(64), 62), dict(ca_nseg=3, ca_qc=8)),
+    # L1 = 130: 3 segments of 164 outputs, shorter than 2 L1, so a segment's halos span a whole neighbouring segment
+    "cost_rows_l1_130": (Case("cost_rows_l1_130", 486, 17, _opt(61, cross_L1=130, cross_L2=40, cross_t1=60, cross_t2=30), 63),
+                         dict(ca_nseg=3, ca_qc=8, ca_short=True)),
+    # D < 32: four quads per CTA, D not a multiple of 4, rows in 2 segments
+    "cost_rows_qc4": (Case("cost_rows_qc4", 825, 13, _opt(23), 64), dict(ca_nseg=2, ca_qc=4)),
+    # arms too long for the fused cost plan: the separate cost kernel, exact and padded D; at W = 701 the row does not
+    # fit k_arm_sum2t's plan either, so both axes take the LDG double pass with eight quads
+    "cost_volume_exact": (Case("cost_volume_exact", 509, 13, _opt(32, **LONG_ARMS), 65), dict(ca_ok=False)),
+    "cost_volume_padded_ldg": (Case("cost_volume_padded_ldg", 701, 13, _opt(37, **LONG_ARMS), 66),
+                               dict(ca_ok=False, tmaps=False)),
+    # k_arm_sum2t down columns cut into segments, one line per CTA, eight and four quads
+    "cols_seg_qc8": (Case("cols_seg_qc8", 21, 709, _opt(64), 67), dict(t1_nseg=3, t1_qc=8, t1_lpc=1)),
+    "cols_seg_qc4": (Case("cols_seg_qc4", 13, 809, _opt(23), 68), dict(t1_nseg=2, t1_qc=4, t1_lpc=1)),
+    # the LDG double pass on rows in segments: Q = 4 (generic QC) and Q = 3 (no TMA plan at all, Q < 4)
+    "ldg_rows_q4": (Case("ldg_rows_q4", 1001, 13, _opt(14), 69), dict(ldg0_nseg=2, ldg0_qc=0, t0_nseg=2)),
+    "ldg_rows_q3": (Case("ldg_rows_q3", 1001, 13, _opt(11), 70), dict(ldg0_nseg=2, ldg0_qc=0, tmaps=False)),
+    # scanline slots of T = 2 steps on the row passes, for 8, 16 and 32 lanes per line, K not FULL, an odd step count
+    "so_t2_lps8": (Case("so_t2_lps8", 33, 1057, _opt(61), 71, wave_pairs=8, lanes=1), dict(so_T0=2, lps=8)),
+    "so_t2_lps16": (Case("so_t2_lps16", 33, 659, _opt(93), 72, wave_pairs=8, lanes=1), dict(so_T0=2, lps=16)),
+    "so_t2_lps32": (Case("so_t2_lps32", 33, 329, _opt(200), 73, wave_pairs=8, lanes=1), dict(so_T0=2, lps=32)),
+}
+
+SWEEP_DS = list(range(1, 257))
+
+
+def _all_cases():
+    return [_sweep_case(D) for D in SWEEP_DS] + [c for c, _ in PLAN_CASES.values()]
+
+
+# ---- plans (tests/c/*_plan_main.cpp print the plans of the headers the kernels are launched with) ---------------------
+@pytest.fixture(scope="module")
+def plans(tmp_path_factory):
+    d = tmp_path_factory.mktemp("plans")
+    for name in ("ca_plan_main", "so_plan_main"):
+        subprocess.run(["g++", "-O2", "-std=c++17", "-o", str(d / name), str(ROOT / "tests" / "c" / f"{name}.cpp")], check=True)
+    return Plans(d)
+
+
+def _device_figures():
+    """(SM count, shared memory per SM, reserved per CTA) of device 0, or an H100 SXM's where there is no GPU."""
+    import torch
+    if torch.cuda.is_available():
+        p = torch.cuda.get_device_properties(0)
+        return p.multi_processor_count, p.shared_memory_per_multiprocessor, SMEM_RESERVED_PER_CTA
+    return 132, 228 * 1024, SMEM_RESERVED_PER_CTA
+
+
+class Plans:
+    def __init__(self, d):
+        self.d = d
+        self.dev = _device_figures()
+
+    def _run(self, exe, *args):
+        r = subprocess.run([str(self.d / exe), *map(str, args)], capture_output=True, text=True)
+        assert r.returncode == 0, (exe, args, r.stdout, r.stderr)
+        return r.stdout
+
+    def ca(self, c):
+        v = list(map(int, self._run("ca_plan_main", c.W, c.Dp, c.L1).split("\n")[0].split()))
+        return dict(zip(("qc", "Ls", "nseg", "nchunks", "gm", "lpc", "threads", "smem", "ok", "budget"), v))
+
+    def arm(self, c):
+        out = []
+        for line in self._run("ca_plan_main", "arm", c.W, c.H, c.Dp, c.L1).strip().split("\n"):
+            v = list(map(int, line.split()))
+            out.append(dict(zip(("dir", "t_ok", "t_qc", "t_Ls", "t_nseg", "t_nchunks", "t_lpc", "t_threads", "t_smem",
+                                 "ldg_ok", "ldg_qc_log2", "ldg_Ls", "ldg_nseg", "ldg_smem"), v)))
+        return out
+
+    def so(self, c, axis):
+        v = list(map(int, self._run("so_plan_main", c.W, c.H, c.Dp, c.wave_pairs, axis, *self.dev).split()))
+        return dict(zip(("T", "NS", "smem", "ctas", "ctas_per_sm", "waves"), v))
+
+
+def so_lanes_per_line(Dp):
+    return 8 if Dp <= 64 else (16 if Dp <= 128 else 32)
+
+
+def reached(c, plans):
+    """The instantiations of the five templates one batched run of case c launches, by the launch rules of
+    k_aggregate.cu, k_cost.cu and k_scanline.cu (a run that matches, so every stage runs, with the fused aggregation):
+      cost:      k_cost_arm_sum_h<D == Dp, ca_plan.qc> where ca_plan is ok, else k_cost_volume<D == Dp>;
+      axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok (the tensor maps are encoded for both) and,
+                 on rows, the row is one segment; else k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC);
+      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp)."""
+    out = set()
+    exact = c.D == c.Dp
+    ca = plans.ca(c)
+    out.add(("k_cost_arm_sum_h", exact, ca["qc"]) if ca["ok"] else ("k_cost_volume", exact))
+    arm = plans.arm(c)
+    assert arm[0]["ldg_ok"] and arm[1]["ldg_ok"], (c.name, arm)       # the fused aggregation runs on every shape
+    tmaps = bool(arm[0]["t_ok"] and arm[1]["t_ok"])
+    for a in arm:
+        if tmaps and not (a["dir"] == 0 and a["t_nseg"] > 1):
+            out.add(("k_arm_sum2t", a["dir"] == 1, a["t_qc"]))
+        else:
+            out.add(("k_arm_sum2", a["dir"] == 1, 8 if a["ldg_qc_log2"] == 3 else 0))
+    lps = so_lanes_per_line(c.Dp)
+    K = -(-c.Dp // lps)
+    out.add(("k_scanline", K, lps, c.D == K * lps))
+    return out
+
+
+# ---- CPU ------------------------------------------------------------------------------------------------------------
+_SYMBOLS = {
+    "k_scanline": re.compile(r"_Z10k_scanlineILi(\d+)ELi(\d+)ELb([01])EE"),
+    "k_cost_volume": re.compile(r"_Z13k_cost_volumeILb([01])EE"),
+    "k_cost_arm_sum_h": re.compile(r"_Z16k_cost_arm_sum_hILb([01])ELi(\d+)EE"),
+    "k_arm_sum2t": re.compile(r"_Z11k_arm_sum2tILb([01])ELi(\d+)EE"),
+    "k_arm_sum2": re.compile(r"_Z10k_arm_sum2ILb([01])ELi(\d+)EE"),
+}
+
+
+def library_instantiations():
+    """{(template, args...)} of the five templates, read from the built library's device symbols."""
+    from adcensus_b200.build import build_library
+    cuobjdump = Path(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")).parent / "cuobjdump"
+    if not cuobjdump.exists():
+        pytest.skip(f"cuobjdump not found at {cuobjdump}")
+    r = subprocess.run([str(cuobjdump), "-symbols", str(build_library())], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-2000:]
+    found = set()
+    for name, rx in _SYMBOLS.items():
+        for m in rx.finditer(r.stdout):
+            args = tuple(int(g) for g in m.groups())
+            if name == "k_scanline":
+                found.add((name, args[0], args[1], bool(args[2])))
+            else:
+                found.add((name, bool(args[0]), *args[1:]))
+    return found
+
+
+def test_every_instantiation_is_reached(plans):
+    """Every instantiation of k_scanline, k_cost_volume, k_cost_arm_sum_h, k_arm_sum2t and k_arm_sum2 in the library is
+    launched by at least one GPU case of this file; one that no case reaches fails here."""
+    lib = library_instantiations()
+    assert sum(1 for i in lib if i[0] == "k_scanline") == 32, sorted(lib)
+    assert {i[0] for i in lib} == set(_SYMBOLS), sorted(lib)
+    by_case = {c.name: reached(c, plans) for c in _all_cases()}
+    union = set().union(*by_case.values())
+    assert union <= lib, sorted(union - lib)           # the launch rules name only instantiations that exist
+    missing = sorted(lib - union)
+    assert not missing, f"instantiations no GPU case reaches: {missing}"
+    for inst in sorted(lib, key=str):
+        print(inst, "reached by", sorted((n for n, r in by_case.items() if inst in r), key=len)[:4])
+
+
+def test_plan_branch_cases(plans):
+    """Each plan-branch case takes the branch it is there for (so that a plan change cannot drop the coverage quietly)."""
+    for name, (c, want) in PLAN_CASES.items():
+        ca, arm = plans.ca(c), plans.arm(c)
+        tmaps = bool(arm[0]["t_ok"] and arm[1]["t_ok"])
+        got = dict(ca_ok=bool(ca["ok"]), ca_nseg=ca["nseg"], ca_qc=ca["qc"], ca_short=ca["Ls"] < 2 * min(max(c.L1, 0), 255),
+                   tmaps=tmaps, t0_nseg=arm[0]["t_nseg"], t1_nseg=arm[1]["t_nseg"], t1_qc=arm[1]["t_qc"],
+                   t1_lpc=arm[1]["t_lpc"], ldg0_nseg=arm[0]["ldg_nseg"], ldg0_qc=8 if arm[0]["ldg_qc_log2"] == 3 else 0,
+                   so_T0=plans.so(c, 0)["T"], lps=so_lanes_per_line(c.Dp))
+        for k, v in want.items():
+            assert got[k] == v, f"{name}: {k} = {got[k]}, expected {v} (plans: ca {ca}, arm {arm})"
+        if "t1_lpc" in want:           # k_arm_sum2t takes the columns, one segment's worth per CTA
+            assert tmaps and arm[1]["t_nseg"] > 1, (name, arm)
+        if "ldg0_nseg" in want:        # the rows take the LDG double pass
+            assert not tmaps or arm[0]["t_nseg"] > 1, (name, arm)
+        if "so_T0" in want:            # ... with K not FULL and an odd number of steps along the row pass
+            K = -(-c.Dp // want["lps"])
+            assert c.D != K * want["lps"] and c.W % 2 == 1 and c.H % 2 == 1, name
+
+
+def test_sweep_case_shapes(plans):
+    """The sweep's shapes: W and H not multiples of 4, H not a multiple of either pass's T, W < D on a few ranges,
+    min_disparity != 0 on every seventh, both signs; whole-line plans whose line counts are not multiples of lpc."""
+    narrow, dmins = 0, set()
+    for D in SWEEP_DS:
+        c = _sweep_case(D)
+        assert c.D == D and c.W % 4 and c.H % 4, (D, c.W, c.H)
+        for axis in (0, 1):
+            assert c.H % plans.so(c, axis)["T"], (D, c.H)
+        narrow += c.W < D
+        if c.opt.min_disparity:
+            dmins.add(np.sign(c.opt.min_disparity))
+        if D == 64:
+            arm = plans.arm(c)
+            assert arm[0]["t_lpc"] == arm[1]["t_lpc"] == 4 and c.H % 4 and c.W % 4, arm
+    assert narrow >= 4 and dmins == {-1, 1}
+    assert sum(1 for D in SWEEP_DS if _sweep_case(D).opt.min_disparity) >= len(SWEEP_DS) // 8
+
+
+@pytest.mark.parametrize("D", GS.GOLDEN_DS)
+def test_sweep_oracle_vs_reference(D):
+    """The oracle on the sweep cases the other fixtures do not reach (D = 1, 2, 96, 161, 253, ...): every tap after every
+    stage of the first pair against the unmodified reference's sha256 (tools/make_golden_sweep.py)."""
+    want = json.loads((T.GOLDEN_DIR / "golden_sweep_ref.json").read_text())[str(D)]
+    W, H, opt, seed = GS.sweep_case(D)
+    left, right = GS.sweep_pairs(W, H, D, seed)[0]
+    orc = T.Oracle(W, H, opt)
+    got = GS.staged_hashes(orc, opt, left, right)
+    orc.close()
+    bad = [k for k in want if got[k] != want[k]]
+    assert not bad and set(got) == set(want), f"D={D}: taps differing from the reference: {bad}"
+
+
+# ---- GPU ------------------------------------------------------------------------------------------------------------
+def _oracle_taps(W, H, opt, left, right):
+    """The taps the batched run's outputs are compared with, from one oracle run of one pair."""
+    want = {("COST", "VOL_INIT"): "cost", ("AGG4", "VOL_AGGR"): "aggr", ("SO4", "VOL_AGGR"): "opt",
+            ("WTA", "DISP_L"): "wta_left", ("WTA", "DISP_R"): "wta_right", ("OUTLIER", "MISMATCHES"): "mismatches",
+            ("OUTLIER", "OCCLUSIONS"): "occlusions", ("MEDIAN", "DISP_L"): "final"}
+    orc = T.Oracle(W, H, opt)
+    orc.begin(left, right)
+    out = {}
+    for st in T.STAGES:
+        orc.step()
+        for tap in T.STAGE_TAPS[st]:
+            if (st, tap) in want:
+                out[want[(st, tap)]] = orc.tap(tap).copy()
+    orc.close()
+    return out
+
+
+def _run_batched(c, pairs):
+    """One match_outputs_batch_device call over all pairs: the three volumes (f32, [H][W][D]), the WTA maps, the outlier
+    map and the final map of every pair, as numpy arrays."""
+    import torch
+    dev = torch.device("cuda", 0)
+    n, H, W, D = len(pairs), c.H, c.W, c.D
+    d_l = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev)
+    d_r = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev)
+    vols = {s: torch.full((n, H, W, D), float("nan"), dtype=torch.float32, device=dev) for s in ("cost", "aggr", "opt")}
+    maps = {"wta_left": torch.full((n, H, W), -7.0, device=dev), "wta_right": torch.full((n, H, W), -7.0, device=dev),
+            "outliers": torch.full((n, H, W), 0xee, dtype=torch.uint8, device=dev)}
+    d_disp = torch.full((n, H, W), -7.0, device=dev)
+    eng = _engine(W, H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes)
+    assert (eng.wave_pairs, eng.lanes) == (c.wave_pairs, c.lanes), (eng.wave_pairs, eng.lanes)
+    st = torch.cuda.current_stream()
+    eng.match_outputs_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), maps=[(t.data_ptr(), k) for k, t in maps.items()],
+                                   volumes=[(t.data_ptr(), s, "hwd", "f32") for s, t in vols.items()],
+                                   d_disp=d_disp.data_ptr(), stream=st.cuda_stream)
+    torch.cuda.synchronize()
+    eng.close()
+    got = {k: t.cpu().numpy() for k, t in {**vols, **maps}.items()}
+    got["final"] = d_disp.cpu().numpy()
+    return got
+
+
+def _check_case(c):
+    # the oracle runs overlap in threads (ctypes releases the GIL during the call) while the GPU runs the batch
+    pairs = GS.sweep_pairs(c.W, c.H, c.D, c.seed)[:c.n]
+    with ThreadPoolExecutor(len(pairs)) as ex:
+        futs = [ex.submit(_oracle_taps, c.W, c.H, c.opt, l, r) for l, r in pairs]
+        got = _run_batched(c, pairs)
+        want = [f.result() for f in futs]
+    for i, w in enumerate(want):
+        tag = f"{c.name} ({c.W}x{c.H}x{c.D}, dmin {c.opt.min_disparity}) pair {i}"
+        _same(f"{tag} COST/VOL_INIT", got["cost"][i], w["cost"])
+        _same(f"{tag} AGG4/VOL_AGGR", got["aggr"][i], w["aggr"])
+        _same(f"{tag} SO4/VOL_AGGR", got["opt"][i], w["opt"])
+        _same(f"{tag} WTA/DISP_L", got["wta_left"][i], w["wta_left"])
+        _same(f"{tag} WTA/DISP_R", got["wta_right"][i], w["wta_right"])
+        mis, occ = MT.outlier_lists(got["outliers"][i])
+        _same(f"{tag} OUTLIER/MISMATCHES", mis, w["mismatches"].reshape(-1, 2))
+        _same(f"{tag} OUTLIER/OCCLUSIONS", occ, w["occlusions"].reshape(-1, 2))
+        _same(f"{tag} MEDIAN/DISP_L", got["final"][i], w["final"])
+    return got
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("D", SWEEP_DS)
+def test_disparity_sweep(D):
+    """Disparity range D through one batched call (five distinct pairs, waves of two, the last partial) against the
+    oracle, every exported volume and side map bit for bit; the ranges pinned to the reference also by the final map's
+    sha256."""
+    got = _check_case(_sweep_case(D))
+    if D in GS.GOLDEN_DS:
+        want = json.loads((T.GOLDEN_DIR / "golden_sweep_ref.json").read_text())[str(D)]
+        assert T.sha(got["final"][0]) == want["MEDIAN/DISP_L"], f"D={D}: final map differs from the reference's hash"
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", sorted(PLAN_CASES))
+def test_plan_branch(name):
+    """A shape that sends a kernel down a plan branch the sweep's small shapes do not take, checked as the sweep is."""
+    _check_case(PLAN_CASES[name][0])
