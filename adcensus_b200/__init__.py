@@ -11,11 +11,13 @@ from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TA
                      load_library, Invalid_Float, COST_HWD, COST_DHW, COST_F32, COST_F16, COST_BF16, COST_MAX,
                      VOL_COST, VOL_AGGR, VOL_OPT, MAP_WTA_LEFT, MAP_WTA_RIGHT, MAP_OUTLIERS, MAP_MIN_COST,
                      MAP_PEAK_RATIO, IMG_BGR, IMG_RGB, IMG_BGRA, IMG_RGBA, IMG_GRAY, IMG_RGB_PLANAR, ImageDesc,
-                     image_desc, REMAP_F32, REMAP_FIXED, Remap, Rectification)
+                     image_desc, REMAP_F32, REMAP_FIXED, Remap, Rectification, REPROJ_POINTS, REPROJ_DEPTH,
+                     REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut)
 from .build import build_library  # noqa: F401
 
 __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "TAP", "lib_path",
            "load_library", "build_library", "Invalid_Float", "COST_HWD", "COST_DHW", "COST_F32", "COST_F16", "COST_BF16",
            "COST_MAX", "VOL_COST", "VOL_AGGR", "VOL_OPT", "MAP_WTA_LEFT", "MAP_WTA_RIGHT", "MAP_OUTLIERS", "MAP_MIN_COST",
            "MAP_PEAK_RATIO", "IMG_BGR", "IMG_RGB", "IMG_BGRA", "IMG_RGBA", "IMG_GRAY", "IMG_RGB_PLANAR", "ImageDesc",
-           "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification"]
+           "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
+           "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut"]

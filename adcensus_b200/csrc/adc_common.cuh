@@ -170,6 +170,11 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
 // the wave's raw views at left / right (geometry g over src_w x src_h frames, pitches resolved) -> w.bgr, resampled
 void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
                                const AdcImageGeom& g, const AdcRectGeom& r, cudaStream_t st, unsigned long long* launches);
+// reprojection to 3-D (k_reproject.cu): n maps of dm.N pixels at disp -> the outputs whose pointer is not NULL (map i
+// at pixel i*N of each), Q row-major; s16_invalid = the DISP_S16 value of a +inf pixel.  One launch.
+struct AdcReprojQ { double q[16]; };
+void adc_launch_reproject(const AdcDims& dm, long long n, const float* disp, const AdcReprojQ& Q, float* points,
+                          float* depth, int16_t* s16, int16_t s16_invalid, cudaStream_t st, unsigned long long* launches);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

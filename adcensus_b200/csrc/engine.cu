@@ -36,6 +36,8 @@ static_assert(sizeof(adc_remap) == 32 && offsetof(adc_remap, map2) == 8 && offse
 static_assert(sizeof(adc_rectification) == 80 && offsetof(adc_rectification, src_height) == 4 &&
               offsetof(adc_rectification, map_type) == 8 && offsetof(adc_rectification, reserved) == 12 &&
               offsetof(adc_rectification, view) == 16, "adc_rectification layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_reproject_out) == 16 && offsetof(adc_reproject_out, kind) == 8 &&
+              offsetof(adc_reproject_out, reserved) == 12, "adc_reproject_out layout (include/adcensus_b200.h)");
 
 namespace {
 
@@ -764,6 +766,22 @@ int match_outputs_device(adc_engine* e, const char* fn, int n, const uint8_t* d_
                      last, vols, n_vols, maps, n_maps, img, rect);
 }
 
+// Makes the device staging of the host entries (e->vol_stage) at least `need` bytes: freed and re-allocated when it is
+// smaller, ADC_ERR_NOMEM if that fails.
+int grow_stage(adc_engine* e, const char* fn, size_t need, const char* what) {
+    if (need <= e->vol_stage_bytes) return ADC_OK;
+    if (e->vol_stage) CK(cudaFree(e->vol_stage));
+    e->vol_stage = nullptr;
+    e->vol_stage_bytes = 0;
+    if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
+        cudaGetLastError();
+        e->vol_stage = nullptr;
+        return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for %s", fn, need, what);
+    }
+    e->vol_stage_bytes = need;
+    return ADC_OK;
+}
+
 // The one-pair host driver of adc_match_volumes, adc_match_outputs, adc_match_images and adc_match_rectified (arguments
 // checked): volumes and maps go to device staging first (one after the other), then to the caller's host buffers.
 // img = the images' resolved geometry, nullptr = tight packed BGR.  rect (with img): the views are raw frames, uploaded
@@ -786,17 +804,7 @@ int match_outputs_host(adc_engine* e, const char* fn, const uint8_t* left, const
     const size_t raw = rect ? staged_bytes(*img, rect->src_w, rect->src_h) : 0;
     const bool raw_in_volume = raw <= (size_t)e->S * e->P.dm.vol_stride * sizeof(float);
     if (!raw_in_volume) need += raw;
-    if (need > e->vol_stage_bytes) {
-        if (e->vol_stage) CK(cudaFree(e->vol_stage));
-        e->vol_stage = nullptr;
-        e->vol_stage_bytes = 0;
-        if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
-            cudaGetLastError();
-            e->vol_stage = nullptr;
-            return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for the exported volumes and maps", fn, need);
-        }
-        e->vol_stage_bytes = need;
-    }
+    if ((rc = grow_stage(e, fn, need, "the exported volumes and maps"))) return rc;
     VolOuts dev;
     dev.n = n_vols;
     size_t off = 0;
@@ -863,6 +871,48 @@ int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, 
     *r = AdcRectGeom{{e->rect_map, e->rect_map + N}, e->rect_src_w, e->rect_src_h};
     e->rect_format = g->format;
     return ADC_OK;
+}
+
+// Reprojection outputs by kind (ADC_REPROJ_*), nullptr = not requested.
+struct ReprojOuts {
+    void* dst[3] = {nullptr, nullptr, nullptr};
+};
+size_t reproj_elem_bytes(int kind) { return kind == ADC_REPROJ_POINTS ? 3 * sizeof(float) : kind == ADC_REPROJ_DEPTH ? sizeof(float) : sizeof(int16_t); }
+
+// The rules of the reprojection entries, none of which needs the engine (device: the alignment rules too).
+int check_reproject_args(const char* fn, int n, const float* disp, const double* Q, const adc_reproject_out* outs,
+                         int n_outs, bool device, ReprojOuts* by_kind) {
+    if (n_outs < 1 || n_outs > 3) return fail(ADC_ERR_ARG, "%s: n_outs %d outside 1..3", fn, n_outs);
+    if (!outs) return fail(ADC_ERR_ARG, "%s: outs is NULL", fn);
+    for (int i = 0; i < n_outs; i++) {
+        const adc_reproject_out& o = outs[i];
+        if (o.kind < ADC_REPROJ_POINTS || o.kind > ADC_REPROJ_DISP_S16) return fail(ADC_ERR_ARG, "%s: outs[%d].kind %d unknown", fn, i, o.kind);
+        for (int j = 0; j < i; j++)
+            if (outs[j].kind == o.kind) return fail(ADC_ERR_ARG, "%s: outs[%d].kind %d requested twice", fn, i, o.kind);
+        if (!o.dst) return fail(ADC_ERR_ARG, "%s: outs[%d].dst is NULL", fn, i);
+        if (o.reserved != 0) return fail(ADC_ERR_ARG, "%s: outs[%d].reserved must be zero", fn, i);
+        const uintptr_t align = o.kind == ADC_REPROJ_DISP_S16 ? 2 : 4;
+        if (device && (uintptr_t)o.dst % align)
+            return fail(ADC_ERR_ARG, "%s: outs[%d].dst is not %d-byte aligned", fn, i, (int)align);
+        by_kind->dst[o.kind] = o.dst;
+    }
+    if (!disp) return fail(ADC_ERR_ARG, "%s: disp is NULL", fn);
+    if (!Q) return fail(ADC_ERR_ARG, "%s: Q is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (device && (uintptr_t)disp % 4) return fail(ADC_ERR_ARG, "%s: disp is not 4-byte aligned", fn);
+    return ADC_OK;
+}
+
+// The DISP_S16 value of a +inf pixel: (min_disparity - 1) * 16 saturated to int16.
+int16_t reproj_s16_invalid(const adc_engine* e) {
+    const long long v = ((long long)e->opt.min_disparity - 1) * 16;
+    return (int16_t)std::min(32767ll, std::max(-32768ll, v));
+}
+
+AdcReprojQ reproj_q(const double* Q) {
+    AdcReprojQ q;
+    memcpy(q.q, Q, sizeof(q.q));
+    return q;
 }
 
 }  // namespace
@@ -1299,6 +1349,55 @@ int adc_match_rectified(adc_engine* e, const uint8_t* left, const uint8_t* right
     AdcRectGeom r;
     if ((rc = resolve_rectified(e, fn, img, &g, &r))) return rc;
     return match_outputs_host(e, fn, left, right, cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps, &g, &r);
+}
+
+int adc_reproject_batch_device(adc_engine* e, int32_t n, const float* d_disp, const double Q[16],
+                               const adc_reproject_out* outs, int32_t n_outs, void* stream) {
+    const char* fn = "adc_reproject_batch_device";
+    ReprojOuts o;
+    int rc = check_reproject_args(fn, n, d_disp, Q, outs, n_outs, true, &o);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if (n == 0) return ADC_OK;
+    CK(cudaSetDevice(e->cfg.device));
+    adc_launch_reproject(e->P.dm, n, d_disp, reproj_q(Q), static_cast<float*>(o.dst[ADC_REPROJ_POINTS]),
+                         static_cast<float*>(o.dst[ADC_REPROJ_DEPTH]), static_cast<int16_t*>(o.dst[ADC_REPROJ_DISP_S16]),
+                         reproj_s16_invalid(e), (cudaStream_t)stream, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const adc_reproject_out* outs, int32_t n_outs) {
+    const char* fn = "adc_reproject";
+    ReprojOuts o;
+    int rc = check_reproject_args(fn, 1, disp, Q, outs, n_outs, false, &o);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    Lane& ln = e->lanes[0];
+    if ((rc = drain_lane(e, ln))) return rc;
+    CK(cudaStreamSynchronize(ln.st));
+    // staging: the map, then each requested output, 256-byte aligned
+    const size_t N = (size_t)e->P.dm.N;
+    size_t off[3] = {0, 0, 0}, need = align_up(N * sizeof(float), 256);
+    for (int k = 0; k < 3; k++)
+        if (o.dst[k]) {
+            off[k] = need;
+            need += align_up(N * reproj_elem_bytes(k), 256);
+        }
+    if ((rc = grow_stage(e, fn, need, "the disparity map and its reprojection"))) return rc;
+    char* stage = static_cast<char*>(e->vol_stage);
+    CK(cudaMemcpyAsync(stage, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
+    adc_launch_reproject(e->P.dm, 1, reinterpret_cast<const float*>(stage), reproj_q(Q),
+                         o.dst[ADC_REPROJ_POINTS] ? reinterpret_cast<float*>(stage + off[ADC_REPROJ_POINTS]) : nullptr,
+                         o.dst[ADC_REPROJ_DEPTH] ? reinterpret_cast<float*>(stage + off[ADC_REPROJ_DEPTH]) : nullptr,
+                         o.dst[ADC_REPROJ_DISP_S16] ? reinterpret_cast<int16_t*>(stage + off[ADC_REPROJ_DISP_S16]) : nullptr,
+                         reproj_s16_invalid(e), ln.st, &e->launches);
+    for (int k = 0; k < 3; k++)
+        if (o.dst[k]) CK(cudaMemcpyAsync(o.dst[k], stage + off[k], N * reproj_elem_bytes(k), cudaMemcpyDeviceToHost, ln.st));
+    CK(cudaStreamSynchronize(ln.st));
+    CK(cudaGetLastError());
+    return ADC_OK;
 }
 
 void* adc_host_alloc(size_t bytes) {

@@ -190,6 +190,28 @@ def _remap(maps, H: int, W: int):
     raise ValueError(f"maps must be float32 [H][W] x2 or int16 [H][W][2] + uint16 [H][W], got {t1} and {t2}")
 
 
+# reprojection to 3-D (adc_reproject*): which output a request names, and its element type
+REPROJ_POINTS, REPROJ_DEPTH, REPROJ_DISP_S16 = 0, 1, 2
+REPROJ_KINDS = {"points": REPROJ_POINTS, "depth": REPROJ_DEPTH, "disp_s16": REPROJ_DISP_S16}
+_REPROJ_NP = {REPROJ_POINTS: np.float32, REPROJ_DEPTH: np.float32, REPROJ_DISP_S16: np.int16}
+
+
+class ReprojectOut(ctypes.Structure):
+    """adc_reproject_out: one requested reprojection output (destination, ADC_REPROJ_* kind)."""
+    _fields_ = [("dst", ctypes.c_void_p), ("kind", ctypes.c_int32), ("reserved", ctypes.c_int32)]
+
+
+assert ctypes.sizeof(ReprojectOut) == 16
+
+
+def _q_matrix(Q):
+    """ctypes double[16] of a 4x4 array-like, converted to float64 as cv::Mat::convertTo(CV_64F) does."""
+    q = np.asarray(Q)
+    if q.shape != (4, 4):
+        raise ValueError(f"Q must be a 4x4 matrix, got shape {q.shape}")
+    return (ctypes.c_double * 16)(*q.astype(np.float64).reshape(-1).tolist())
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -258,6 +280,9 @@ def load_library() -> ctypes.CDLL:
                                       ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32]
     L.adc_match_rectified_batch_device.argtypes = [vp, i32, u8p, u8p, ctypes.POINTER(ImageDesc), vp, i32, i32, f32p,
                                                    ctypes.POINTER(VolumeOut), i32, ctypes.POINTER(MapOut), i32, vp]
+    L.adc_reproject.argtypes = [vp, f32p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ReprojectOut), i32]
+    L.adc_reproject_batch_device.argtypes = [vp, i32, f32p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ReprojectOut),
+                                             i32, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -299,6 +324,14 @@ def _map_outs(maps):
     arr = (MapOut * max(1, len(maps)))()
     for i, (ptr, kind) in enumerate(maps):
         arr[i] = MapOut(ptr, _code(MAP_KINDS, kind, "map kind"), 0)
+    return arr
+
+
+def _reproject_outs(outs):
+    """ctypes array of adc_reproject_out from (ptr, kind) tuples (names or ADC_REPROJ_* codes)."""
+    arr = (ReprojectOut * max(1, len(outs)))()
+    for i, (ptr, kind) in enumerate(outs):
+        arr[i] = ReprojectOut(ptr, _code(REPROJ_KINDS, kind, "reprojection kind"), 0)
     return arr
 
 
@@ -547,6 +580,33 @@ class Engine:
                                                         _code(COST_LAYOUTS, cost_layout, "layout"),
                                                         _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
                                                         len(volumes), marr, len(maps), stream))
+
+    # ---- reprojection to 3-D (adc_reproject*) ---------------------------------------------------------
+    def reproject(self, disp, Q, outputs=("points",)):
+        """{name: array} of one disparity map (float32 [H][W], +inf = invalid) and the 4x4 matrix Q of
+        cv2.stereoRectify: "points" float32 [H][W][3] (cv2.reprojectImageTo3D(disp, Q) bit for bit), "depth" float32
+        [H][W] (its Z), "disp_s16" int16 [H][W] (the StereoSGBM "disparity * 16" encoding, invalid pixels
+        (min_disparity - 1) * 16)."""
+        H, W = self.height, self.width
+        disp = np.ascontiguousarray(disp, np.float32)
+        if disp.shape != (H, W):
+            raise ValueError(f"expected a disparity map of shape {(H, W)}, got {disp.shape}")
+        outputs = [outputs] if isinstance(outputs, (str, int)) else list(outputs)
+        shape = {REPROJ_POINTS: (H, W, 3), REPROJ_DEPTH: (H, W), REPROJ_DISP_S16: (H, W)}
+        out = {}
+        for name in outputs:
+            k = _code(REPROJ_KINDS, name, "reprojection kind")
+            out[name] = np.empty(shape.get(k, (H, W)), _REPROJ_NP.get(k, np.float32))
+        arr = _reproject_outs([(out[name].ctypes.data, name) for name in outputs])
+        _check(self._L.adc_reproject(self._h, disp.ctypes.data, _q_matrix(Q), arr, len(outputs)))
+        return out
+
+    def reproject_batch_device(self, n: int, d_disp: int, Q, outs, stream: int = 0):
+        """Device pointers (ints): n maps of H*W float32 at d_disp; `outs` a list of (ptr, kind), each ptr n outputs of
+        H*W pixels (points: 3 float32, depth: float32, disp_s16: int16).  One launch enqueued on `stream` without
+        synchronising; in pipelined mode the maps must be joined on `stream` first."""
+        arr = _reproject_outs(outs)
+        _check(self._L.adc_reproject_batch_device(self._h, n, d_disp, _q_matrix(Q), arr, len(outs), stream))
 
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""

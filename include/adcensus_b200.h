@@ -373,6 +373,47 @@ int adc_match_rectified(adc_engine* e, const uint8_t* left, const uint8_t* right
                         const void* cost, int32_t cost_layout, int32_t cost_dtype, float* disp,
                         const adc_volume_out* vols, int32_t n_vols, const adc_map_out* maps, int32_t n_maps);
 
+/* ---- reprojection to 3-D ------------------------------------------------------------------------------
+ * The entry points below turn f32 [H][W] disparity maps of the engine's size (the engine's final maps, +inf = invalid,
+ * or any other) into up to three outputs in one pass, with the 4x4 row-major double matrix Q that cv::stereoRectify
+ * returns next to the rectification maps:
+ *   ADC_REPROJ_POINTS    f32 [H][W][3]  cv::reprojectImageTo3D(disp, Q, handleMissingValues = false), bit for bit (CV_32FC3)
+ *   ADC_REPROJ_DEPTH     f32 [H][W]     the third coordinate of ADC_REPROJ_POINTS, bit for bit (a third of the bytes)
+ *   ADC_REPROJ_DISP_S16  int16 [H][W]   the StereoBM / StereoSGBM encoding "disparity * 16" that cv::filterSpeckles,
+ *                                       cv::validateDisparity and ximgproc's WLS filter take
+ * Semantics of pixel (x, y) with value d; every operation is one IEEE double operation, round to nearest, no fused
+ * multiply-add:
+ *   h_i = (((+0.0 + Q[i][0]*x) + Q[i][1]*y) + Q[i][2]*d) + Q[i][3]      i = 0..3; x, y, d as double
+ *   P_c = (float)((double)(float)h_c * (1.0 / h_3))                     c = 0, 1, 2
+ * which is OpenCV's: each coordinate is rounded to float twice (Vec3f /= double multiplies by the reciprocal), and the
+ * +0.0 start turns a -0 first product into +0.  With a stereoRectify Q, column 2 of rows 0..2 is zero, so an invalid
+ * (+inf) pixel gives 0 * inf = NaN in all three coordinates, exactly as OpenCV does; that is also the NaN-as-missing
+ * convention of organised point clouds (PCL, Open3D).  NaN payloads are not specified.
+ * DISP_S16: d = +inf gives (min_disparity - 1) * 16 saturated to int16 (the StereoMatcher invalid value, with the
+ * engine's min_disparity); any other d gives cv::saturate_cast<short>(d * 16) as on x86: t = d * 16 rounded half to
+ * even, saturated to [-32768, 32767] when it fits in int32, and -32768 otherwise, for NaN and for -inf.
+ * Fails with ADC_ERR_ARG naming the field, every rule before the engine is checked: n_outs outside 1..3; outs NULL; a
+ * kind unknown or requested twice; a NULL dst; a non-zero reserved; a NULL map or Q; a negative n; on the device entry
+ * also a map or a POINTS / DEPTH dst not 4-byte aligned, or a DISP_S16 dst not 2-byte aligned. */
+enum { ADC_REPROJ_POINTS = 0, ADC_REPROJ_DEPTH = 1, ADC_REPROJ_DISP_S16 = 2 };
+typedef struct adc_reproject_out {
+    void*   dst;      /* n outputs of H*W pixels of the kind, map i at pixel i*H*W */
+    int32_t kind;     /* ADC_REPROJ_* */
+    int32_t reserved; /* must be zero */
+} adc_reproject_out;  /* 16 bytes */
+
+/* n maps in device memory (map i at element i*H*W) to the requested outputs in device memory, one kernel launch
+ * enqueued on `stream` (a cudaStream_t, NULL = legacy default stream), not synchronised.  Q is passed to the kernel by
+ * value: the caller may free it on return.  No engine buffer is touched, so the call may run next to the engine's batch
+ * calls.  The maps must be complete in `stream`'s order: in pipelined mode, after adc_join on that stream.  A second
+ * stream that waits with adc_join keeps the next batch call from waiting for the reprojection (INTEGRATION.md). */
+int adc_reproject_batch_device(adc_engine* e, int32_t n, const float* d_disp, const double Q[16],
+                               const adc_reproject_out* outs, int32_t n_outs, void* stream);
+/* One map, host pointers, synchronous.  The map and the outputs pass through the device staging of adc_match_volumes
+ * (allocated on first use, grown when needed; ADC_ERR_NOMEM before any work if that fails).  Like adc_render_disparity,
+ * not concurrently with another call on the same engine. */
+int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const adc_reproject_out* outs, int32_t n_outs);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);

@@ -169,4 +169,36 @@ for k, fmt in enumerate(IT.FORMATS):
         cudart.cudaFree(p)
     print("rectified ok", fmt, flush=True)
 eng.close()
+
+# reprojection: n maps and every output, each in its own cudaMalloc allocation that ends exactly with its last element,
+# the S16 output at a 2-byte offset, one kind at a time and all three together
+import reproject_testlib as RP
+w, h, n = 71, 47, 3
+N = w * h
+eng = A.Engine(w, h, A.ADCensusOption(min_disparity=-2, max_disparity=21), wave_pairs=2, lanes=2)
+maps = np.stack([eng.match(*T.synthetic_pair(w, h, 23, 60 + i)) for i in range(n)])
+Q = np.array([[1, 0, 0, -35.2], [0, 1, 0, -23.9], [0, 0, 0, 60.0], [0, 0, 8.3, -0.0]])
+sizes = {"points": 12 * n * N, "depth": 4 * n * N, "disp_s16": 2 * n * N + 2}
+for kinds in (["points"], ["depth"], ["disp_s16"], ["points", "depth", "disp_s16"]):
+    p = ctypes.c_void_p()
+    assert cudart.cudaMalloc(ctypes.byref(p), maps.nbytes) == 0
+    assert cudart.cudaMemcpy(p, maps.ctypes.data, maps.nbytes, 1) == 0
+    ptrs = {"disp": p.value}
+    for k in kinds:
+        q = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(q), sizes[k]) == 0
+        ptrs[k] = q.value + (2 if k == "disp_s16" else 0)
+    eng.reproject_batch_device(n, ptrs["disp"], Q, [(ptrs[k], k) for k in kinds], torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    for k in kinds:
+        got = np.empty(sizes[k] - (2 if k == "disp_s16" else 0), np.uint8)
+        assert cudart.cudaMemcpy(got.ctypes.data, ptrs[k], got.nbytes, 2) == 0
+        for i in range(n):
+            want = eng.reproject(maps[i], Q, [k])[k]
+            assert got.reshape(n, -1)[i].tobytes() == want.tobytes(), (kinds, k, i)
+        cudart.cudaFree(ptrs[k] - (2 if k == "disp_s16" else 0))
+    cudart.cudaFree(ptrs["disp"])
+    assert RP.same_nan(eng.reproject(maps[0], Q)["points"], RP.points(maps[0], Q))
+    print("reprojection ok", kinds, flush=True)
+eng.close()
 print("all ok")
