@@ -12,7 +12,8 @@ from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TA
                      VOL_COST, VOL_AGGR, VOL_OPT, MAP_WTA_LEFT, MAP_WTA_RIGHT, MAP_OUTLIERS, MAP_MIN_COST,
                      MAP_PEAK_RATIO, IMG_BGR, IMG_RGB, IMG_BGRA, IMG_RGBA, IMG_GRAY, IMG_RGB_PLANAR, ImageDesc,
                      image_desc, REMAP_F32, REMAP_FIXED, Remap, Rectification, REPROJ_POINTS, REPROJ_DEPTH,
-                     REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut)
+                     REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut, SPECKLE_S16,
+                     SPECKLE_F32, SPECKLE_TYPES, SpeckleParams)
 from .build import build_library  # noqa: F401
 
 __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "TAP", "lib_path",
@@ -20,4 +21,5 @@ __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "T
            "COST_MAX", "VOL_COST", "VOL_AGGR", "VOL_OPT", "MAP_WTA_LEFT", "MAP_WTA_RIGHT", "MAP_OUTLIERS", "MAP_MIN_COST",
            "MAP_PEAK_RATIO", "IMG_BGR", "IMG_RGB", "IMG_BGRA", "IMG_RGBA", "IMG_GRAY", "IMG_RGB_PLANAR", "ImageDesc",
            "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
-           "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut"]
+           "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut", "SPECKLE_S16", "SPECKLE_F32", "SPECKLE_TYPES",
+           "SpeckleParams"]

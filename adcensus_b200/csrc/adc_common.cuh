@@ -175,6 +175,18 @@ void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8
 struct AdcReprojQ { double q[16]; };
 void adc_launch_reproject(const AdcDims& dm, long long n, const float* disp, const AdcReprojQ& Q, float* points,
                           float* depth, int16_t* s16, int16_t s16_invalid, cudaStream_t st, unsigned long long* launches);
+// speckle removal (k_speckle.cu): the rules resolved on the host.  S16: missing = (int)v == nv_i, connected =
+// |a - b| <= md_i in int, written (int16)nv_i.  F32: missing = v == nv_f, connected = fabsf(a - b) <= md_f (the largest
+// float not above max_diff), written nv_f.  A component of at most max_size pixels is removed.
+struct AdcSpeckle {
+    int nv_i, md_i;
+    float nv_f, md_f;
+    int max_size;
+};
+// n maps of dm.N pixels at maps (int16, or float when f32), filtered in place; work = n*N int32 parents, then n*N
+// uint32 sizes.  Four launches.
+void adc_launch_speckles(const AdcDims& dm, long long n, bool f32, void* maps, void* work, const AdcSpeckle& p,
+                         cudaStream_t st, unsigned long long* launches);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

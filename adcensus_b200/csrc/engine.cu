@@ -9,6 +9,7 @@
 // if the CUDA library cannot run, the call fails.
 #include <cuda_runtime.h>
 
+#include <float.h>
 #include <math.h>
 #include <stdarg.h>
 #include <stddef.h>
@@ -36,6 +37,9 @@ static_assert(sizeof(adc_remap) == 32 && offsetof(adc_remap, map2) == 8 && offse
 static_assert(sizeof(adc_rectification) == 80 && offsetof(adc_rectification, src_height) == 4 &&
               offsetof(adc_rectification, map_type) == 8 && offsetof(adc_rectification, reserved) == 12 &&
               offsetof(adc_rectification, view) == 16, "adc_rectification layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_speckle_params) == 32 && offsetof(adc_speckle_params, max_size) == 4 &&
+              offsetof(adc_speckle_params, new_val) == 8 && offsetof(adc_speckle_params, max_diff) == 16 &&
+              offsetof(adc_speckle_params, reserved) == 24, "adc_speckle_params layout (include/adcensus_b200.h)");
 static_assert(sizeof(adc_reproject_out) == 16 && offsetof(adc_reproject_out, kind) == 8 &&
               offsetof(adc_reproject_out, reserved) == 12, "adc_reproject_out layout (include/adcensus_b200.h)");
 
@@ -915,6 +919,53 @@ AdcReprojQ reproj_q(const double* Q) {
     return q;
 }
 
+// cvRound on x86 (cvtsd2si): round half to even, INT_MIN for NaN and for anything outside int32.
+int cv_round(double v) {
+    const double r = nearbyint(v);
+    return r >= -2147483648.0 && r <= 2147483647.0 ? (int)r : INT32_MIN;
+}
+
+// The largest float not above v (v not NaN): (double)f <= v  <=>  f <= this, for every float f.
+float float_at_most(double v) {
+    if (v >= (double)FLT_MAX) return v == INFINITY ? INFINITY : FLT_MAX;
+    if (v < -(double)FLT_MAX) return -INFINITY;
+    const float f = (float)v;
+    return (double)f > v ? nextafterf(f, -INFINITY) : f;
+}
+
+size_t speckle_elem_bytes(int type) { return type == ADC_SPECKLE_S16 ? sizeof(int16_t) : sizeof(float); }
+
+// The rules of the speckle entries that need no engine (device: the alignment rules too).
+int check_speckle_args(const char* fn, int n, const void* maps, const adc_speckle_params* p, const void* work,
+                       bool device) {
+    if (!p) return fail(ADC_ERR_ARG, "%s: params is NULL", fn);
+    if (p->type != ADC_SPECKLE_S16 && p->type != ADC_SPECKLE_F32)
+        return fail(ADC_ERR_ARG, "%s: params.type %d unknown", fn, p->type);
+    if (p->reserved != 0) return fail(ADC_ERR_ARG, "%s: params.reserved must be zero", fn);
+    if (p->type == ADC_SPECKLE_F32 && std::isnan(p->max_diff))
+        return fail(ADC_ERR_ARG, "%s: params.max_diff is NaN (F32 maps take a number)", fn);
+    if (!maps) return fail(ADC_ERR_ARG, "%s: map is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (device) {
+        const int a = (int)speckle_elem_bytes(p->type);
+        if ((uintptr_t)maps % a) return fail(ADC_ERR_ARG, "%s: maps are not %d-byte aligned", fn, a);
+        if ((uintptr_t)work % 4) return fail(ADC_ERR_ARG, "%s: work is not 4-byte aligned", fn);
+    }
+    return ADC_OK;
+}
+
+AdcSpeckle speckle_rules(const adc_speckle_params& p) {
+    AdcSpeckle s;
+    s.nv_i = cv_round(p.new_val);
+    s.md_i = cv_round(p.max_diff);
+    s.nv_f = (float)p.new_val;
+    s.md_f = p.type == ADC_SPECKLE_F32 ? float_at_most(p.max_diff) : 0.0f;
+    s.max_size = p.max_size;
+    return s;
+}
+
+size_t speckle_work_bytes(const adc_engine* e, long long n) { return 8 * (size_t)n * (size_t)e->P.dm.N; }
+
 }  // namespace
 
 // =============================================================================================
@@ -1395,6 +1446,54 @@ int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const ad
                          reproj_s16_invalid(e), ln.st, &e->launches);
     for (int k = 0; k < 3; k++)
         if (o.dst[k]) CK(cudaMemcpyAsync(o.dst[k], stage + off[k], N * reproj_elem_bytes(k), cudaMemcpyDeviceToHost, ln.st));
+    CK(cudaStreamSynchronize(ln.st));
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_speckle_workspace_bytes(const adc_engine* e, int32_t n, size_t* out) {
+    const char* fn = "adc_speckle_workspace_bytes";
+    if (!out) return fail(ADC_ERR_ARG, "%s: out is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    *out = speckle_work_bytes(e, n);
+    return ADC_OK;
+}
+
+int adc_filter_speckles_batch_device(adc_engine* e, int32_t n, void* d_maps, const adc_speckle_params* params,
+                                     void* d_work, size_t work_bytes, void* stream) {
+    const char* fn = "adc_filter_speckles_batch_device";
+    int rc = check_speckle_args(fn, n, d_maps, params, d_work, true);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    const size_t need = speckle_work_bytes(e, n);
+    if (work_bytes < need) return fail(ADC_ERR_ARG, "%s: work_bytes %zu below the %zu bytes of %d maps", fn, work_bytes, need, n);
+    if (n == 0) return ADC_OK;
+    if (!d_work) return fail(ADC_ERR_ARG, "%s: work is NULL", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    adc_launch_speckles(e->P.dm, n, params->type == ADC_SPECKLE_F32, d_maps, d_work, speckle_rules(*params),
+                        (cudaStream_t)stream, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* params) {
+    const char* fn = "adc_filter_speckles";
+    int rc = check_speckle_args(fn, 1, map, params, nullptr, false);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    Lane& ln = e->lanes[0];
+    if ((rc = drain_lane(e, ln))) return rc;
+    CK(cudaStreamSynchronize(ln.st));
+    // staging: the workspace, then the map
+    const size_t bytes = (size_t)e->P.dm.N * speckle_elem_bytes(params->type), off = align_up(speckle_work_bytes(e, 1), 256);
+    if ((rc = grow_stage(e, fn, off + bytes, "the map and its speckle workspace"))) return rc;
+    char* stage = static_cast<char*>(e->vol_stage);
+    CK(cudaMemcpyAsync(stage + off, map, bytes, cudaMemcpyHostToDevice, ln.st));
+    adc_launch_speckles(e->P.dm, 1, params->type == ADC_SPECKLE_F32, stage + off, stage, speckle_rules(*params), ln.st,
+                        &e->launches);
+    CK(cudaMemcpyAsync(map, stage + off, bytes, cudaMemcpyDeviceToHost, ln.st));
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
     return ADC_OK;

@@ -212,6 +212,20 @@ def _q_matrix(Q):
     return (ctypes.c_double * 16)(*q.astype(np.float64).reshape(-1).tolist())
 
 
+# speckle removal (adc_filter_speckles*): the map type, and the params struct
+SPECKLE_S16, SPECKLE_F32 = 0, 1
+SPECKLE_TYPES = {"s16": SPECKLE_S16, "f32": SPECKLE_F32}
+
+
+class SpeckleParams(ctypes.Structure):
+    """adc_speckle_params: map type (ADC_SPECKLE_*), max_size, new_val, max_diff, reserved (zero)."""
+    _fields_ = [("type", ctypes.c_int32), ("max_size", ctypes.c_int32), ("new_val", ctypes.c_double),
+                ("max_diff", ctypes.c_double), ("reserved", ctypes.c_int64)]
+
+
+assert ctypes.sizeof(SpeckleParams) == 32
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -283,6 +297,9 @@ def load_library() -> ctypes.CDLL:
     L.adc_reproject.argtypes = [vp, f32p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ReprojectOut), i32]
     L.adc_reproject_batch_device.argtypes = [vp, i32, f32p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ReprojectOut),
                                              i32, vp]
+    L.adc_speckle_workspace_bytes.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_size_t)]
+    L.adc_filter_speckles.argtypes = [vp, vp, ctypes.POINTER(SpeckleParams)]
+    L.adc_filter_speckles_batch_device.argtypes = [vp, i32, vp, ctypes.POINTER(SpeckleParams), vp, ctypes.c_size_t, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -607,6 +624,45 @@ class Engine:
         synchronising; in pipelined mode the maps must be joined on `stream` first."""
         arr = _reproject_outs(outs)
         _check(self._L.adc_reproject_batch_device(self._h, n, d_disp, _q_matrix(Q), arr, len(outs), stream))
+
+    # ---- speckle removal (adc_filter_speckles*) -------------------------------------------------------
+    def speckle_invalid(self, map_type):
+        """The engine's invalid value of a map type: +inf for f32, (min_disparity - 1) * 16 for s16 (StereoSGBM's)."""
+        return float("inf") if _code(SPECKLE_TYPES, map_type, "speckle map type") == SPECKLE_F32 else \
+            float((self.option.min_disparity - 1) * 16)
+
+    def speckle_workspace_bytes(self, n: int) -> int:
+        """Bytes of device workspace that filter_speckles_batch_device needs for n maps (8 per pixel)."""
+        out = ctypes.c_size_t()
+        _check(self._L.adc_speckle_workspace_bytes(self._h, n, ctypes.byref(out)))
+        return int(out.value)
+
+    def filter_speckles(self, map, max_size: int, max_diff: float, new_val=None) -> np.ndarray:
+        """cv2.filterSpeckles(map, new_val, max_size, max_diff) of one [H][W] map on the GPU, returned as a filtered copy.
+        int16 maps follow OpenCV's plain path (new_val and max_diff through cvRound), float32 maps the f32 rules of the
+        header.  new_val None = speckle_invalid(type): +inf for float32, (min_disparity - 1) * 16 for int16."""
+        a = np.asarray(map)
+        if a.dtype not in (np.int16, np.float32):
+            raise ValueError(f"speckle maps are int16 or float32, got {a.dtype}")
+        if a.shape != (self.height, self.width):
+            raise ValueError(f"expected a map of shape {(self.height, self.width)}, got {a.shape}")
+        t = SPECKLE_S16 if a.dtype == np.int16 else SPECKLE_F32
+        out = np.array(a, order="C", copy=True)
+        nv = self.speckle_invalid(t) if new_val is None else new_val
+        p = SpeckleParams(t, int(max_size), float(nv), float(max_diff), 0)
+        _check(self._L.adc_filter_speckles(self._h, out.ctypes.data, ctypes.byref(p)))
+        return out
+
+    def filter_speckles_batch_device(self, n: int, d_maps: int, map_type, max_size: int, max_diff: float, new_val,
+                                     d_work: int, work_bytes: int, stream: int = 0):
+        """Device pointers (ints): n maps of H*W elements (map_type "s16" = int16, "f32" = float32) at d_maps filtered in
+        place, with work_bytes >= speckle_workspace_bytes(n) of workspace at d_work.  Four launches enqueued on `stream`
+        without synchronising; in pipelined mode the maps must be joined on `stream` first.  new_val None =
+        speckle_invalid(map_type)."""
+        t = _code(SPECKLE_TYPES, map_type, "speckle map type")
+        nv = self.speckle_invalid(t) if new_val is None else new_val
+        p = SpeckleParams(t, int(max_size), float(nv), float(max_diff), 0)
+        _check(self._L.adc_filter_speckles_batch_device(self._h, n, d_maps, ctypes.byref(p), d_work, work_bytes, stream))
 
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""

@@ -414,6 +414,53 @@ int adc_reproject_batch_device(adc_engine* e, int32_t n, const float* d_disp, co
  * not concurrently with another call on the same engine. */
 int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const adc_reproject_out* outs, int32_t n_outs);
 
+/* ---- speckle removal ----------------------------------------------------------------------------------
+ * cv::filterSpeckles(img, new_val, max_size, max_diff) on [H][W] maps of the engine's size, in place, for two map types:
+ *   ADC_SPECKLE_S16  int16 maps (CV_16SC1: the ADC_REPROJ_DISP_S16 output, StereoSGBM's maps), OpenCV's plain C++ path
+ *   ADC_SPECKLE_F32  f32 maps (the engine's own final maps, +inf = invalid); OpenCV has no f32 counterpart
+ * A pixel is missing if its value equals new_val.  Two 4-neighbours are connected if neither is missing and their
+ * difference is at most max_diff.  Every connected component of at most max_size pixels has all its pixels set to
+ * new_val; missing pixels are left as they are.  Components do not depend on a scan order, so the result is exact.
+ * S16: new_val and max_diff are turned into ints with cvRound (round half to even as x86's cvtsd2si does, INT_MIN for
+ *   NaN and for anything outside int32); the missing test compares the pixel promoted to int with that int, the
+ *   differences are taken in int, and the value written is (int16)new_val, which wraps (new_val = 40000 marks nothing
+ *   as missing and writes -25536).  max_diff < 0 connects nothing; max_size <= 0 removes nothing.
+ *   OpenCV's IPP path (on in the pip wheel) differs in one corner: it wraps cvRound(max_diff) and cvRound(new_val) to
+ *   int16 first, so when either lies outside [-32768, 32767] the two paths may give different maps (max_diff 32768 ..
+ *   2^31-1 connect nothing under IPP, 65536 connects only equal values, 70000 differences up to 4464, 1e10 and NaN
+ *   round to INT_MIN, which IPP wraps to 0; new_val = 40000 makes the pixels equal to -25536 missing under IPP).  The
+ *   engine follows the plain path, which every build without IPP computes; with both inside int16, as in every
+ *   realistic call, the two agree.
+ * F32: nv = (float)new_val rounded to nearest; a pixel is missing if v == nv (IEEE); two pixels are connected if
+ *   neither is missing and (double)fabsf(a - b) <= max_diff, with a - b one float subtraction rounded to nearest.  A
+ *   NaN pixel never connects (it is removed when max_size >= 1), -inf next to -inf gives NaN and does not connect;
+ *   new_val = +inf makes the engine's invalid pixels the missing ones.  max_diff must not be NaN.
+ * Fails with ADC_ERR_ARG naming the field: params NULL, params.type unknown, params.reserved not zero, a NaN max_diff
+ * on F32, a NULL map, a negative n; on the device entry also maps not 2-byte (S16) or 4-byte (F32) aligned, or the
+ * workspace not 4-byte aligned -- all of them before the engine is checked; then (device entry) a workspace smaller
+ * than adc_speckle_workspace_bytes for n maps, or NULL while n > 0. */
+enum { ADC_SPECKLE_S16 = 0, ADC_SPECKLE_F32 = 1 };
+typedef struct adc_speckle_params {
+    int32_t type;      /* ADC_SPECKLE_* */
+    int32_t max_size;  /* OpenCV's maxSpeckleSize: components of at most this many pixels are removed */
+    double  new_val;   /* the missing value, and the value written */
+    double  max_diff;  /* the largest difference between connected neighbours */
+    int64_t reserved;  /* must be zero */
+} adc_speckle_params;  /* 32 bytes */
+
+/* *out = the device workspace n maps need: 8 bytes per pixel (n * H * W * 8). */
+int adc_speckle_workspace_bytes(const adc_engine* e, int32_t n, size_t* out);
+/* n maps in device memory (map i at element i*H*W) filtered in place, using only the caller's workspace d_work of
+ * work_bytes bytes: four kernel launches enqueued on `stream` (a cudaStream_t, NULL = legacy default stream) whatever the
+ * content, not synchronised, no host round trip.  No engine buffer is touched, so the call may run next to the engine's
+ * batch calls; the maps must be complete in `stream`'s order (in pipelined mode, after adc_join on that stream). */
+int adc_filter_speckles_batch_device(adc_engine* e, int32_t n, void* d_maps, const adc_speckle_params* params,
+                                     void* d_work, size_t work_bytes, void* stream);
+/* One map, host pointer, filtered in place, synchronous.  The map and the workspace pass through the device staging of
+ * adc_match_volumes (allocated on first use, grown when needed; ADC_ERR_NOMEM before any work if that fails).  Not
+ * concurrently with another call on the same engine. */
+int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* params);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);

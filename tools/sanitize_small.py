@@ -201,4 +201,33 @@ for kinds in (["points"], ["depth"], ["disp_s16"], ["points", "depth", "disp_s16
     assert RP.same_nan(eng.reproject(maps[0], Q)["points"], RP.points(maps[0], Q))
     print("reprojection ok", kinds, flush=True)
 eng.close()
+
+# speckle removal: n maps of each type and the workspace, each in its own cudaMalloc allocation that ends exactly with
+# its last element (the S16 maps start 2 bytes in), serpentine and noise content
+import speckle_testlib as SP
+w, h, n = 131, 67, 3
+N = w * h
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=8), wave_pairs=2, lanes=2)
+rng = np.random.default_rng(5)
+s16 = rng.integers(-3, 4, (n, h, w)).astype(np.int16)
+s16[0, 0::2] = 1
+s16[0, 1::2] = 0
+for t, maps, lead in (("s16", s16, 2), ("f32", (s16 / 4.0).astype(np.float32), 0)):
+    p, q = ctypes.c_void_p(), ctypes.c_void_p()
+    assert cudart.cudaMalloc(ctypes.byref(p), maps.nbytes + lead) == 0
+    wb = eng.speckle_workspace_bytes(n)
+    assert cudart.cudaMalloc(ctypes.byref(q), wb) == 0
+    assert cudart.cudaMemcpy(p.value + lead, maps.ctypes.data, maps.nbytes, 1) == 0
+    md = 1 if t == "s16" else 0.25
+    eng.filter_speckles_batch_device(n, p.value + lead, t, 5, md, 0.0, q.value, wb, torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    got = np.empty_like(maps)
+    assert cudart.cudaMemcpy(got.ctypes.data, p.value + lead, maps.nbytes, 2) == 0
+    for i in range(n):
+        assert got[i].tobytes() == SP.filter_any(maps[i], 0.0, 5, md).tobytes(), (t, i)
+        assert got[i].tobytes() == eng.filter_speckles(maps[i], 5, md, 0.0).tobytes(), (t, i)
+    cudart.cudaFree(p)
+    cudart.cudaFree(q)
+    print("speckles ok", t, flush=True)
+eng.close()
 print("all ok")
