@@ -344,6 +344,11 @@ def _map_outs(maps):
     return arr
 
 
+def _device_cost(d_cost, layout, dtype):
+    """(pointer or None, layout code, dtype code): the cost arguments of a device batch entry."""
+    return d_cost or None, _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
+
+
 def _reproject_outs(outs):
     """ctypes array of adc_reproject_out from (ptr, kind) tuples (names or ADC_REPROJ_* codes)."""
     arr = (ReprojectOut * max(1, len(outs)))()
@@ -401,20 +406,38 @@ class Engine:
         a bf16 volume is passed as its uint16 bit patterns with dtype="bf16"."""
         lay = _code(COST_LAYOUTS, layout, "layout")
         cost = np.ascontiguousarray(cost)
-        want_np = {COST_F32: np.float32, COST_F16: np.float16, COST_BF16: np.uint16}
         if dtype is None:
             dt = {np.dtype(np.float32): COST_F32, np.dtype(np.float16): COST_F16}.get(cost.dtype)
             if dt is None:
                 raise ValueError(f"cost volume must be float32 or float16 (or uint16 bits with dtype='bf16'), got {cost.dtype}")
         else:
             dt = _code(COST_DTYPES, dtype, "dtype")
-            if cost.dtype != want_np.get(dt):
-                raise ValueError(f"dtype {dtype!r} expects a numpy {np.dtype(want_np.get(dt, np.float32)).name} array, got {cost.dtype}")
+            if cost.dtype != _VOL_NP.get(dt):
+                raise ValueError(f"dtype {dtype!r} expects a numpy {np.dtype(_VOL_NP.get(dt, np.float32)).name} array, got {cost.dtype}")
         H, W, D = self.height, self.width, self.D
         want = (H, W, D) if lay == COST_HWD else (D, H, W)
         if cost.shape != want:
             raise ValueError(f"expected a cost volume of shape {want} for layout {layout!r}, got {cost.shape}")
         return cost, lay, dt
+
+    def _outputs(self, maps, volumes, layout, dtype, cost, cost_layout, cost_dtype, disparity):
+        """The arrays a host entry with outputs fills, and its C arguments after the views: (disp or None, {name: array}
+        of the requested volumes and maps, (cost, cost_layout, cost_dtype, disp, vols, n_vols, maps, n_maps)).  The
+        arguments hold the cost volume and the arrays until the call."""
+        maps = [maps] if isinstance(maps, (str, int)) else list(maps)
+        volumes = [volumes] if isinstance(volumes, (str, int)) else list(volumes)
+        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
+        H, W, D = self.height, self.width, self.D
+        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
+        out = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in volumes}
+        vouts = _volume_outs([(out[s].ctypes.data, s, lay, dt) for s in volumes])
+        for m in maps:
+            out[m] = np.empty((H, W), _MAP_NP.get(_code(MAP_KINDS, m, "map kind"), np.float32))
+        mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
+        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
+        disp = np.empty((H, W), np.float32) if disparity else None
+        return disp, out, (None if c is None else c.ctypes, clay, cdt, None if disp is None else disp.ctypes, vouts,
+                           len(volumes), mouts, len(maps))
 
     def match_cost(self, left, right, cost, layout="hwd", dtype=None) -> np.ndarray:
         """Match with the given matching cost instead of the AD-census cost: `cost` is one pair's volume, float32 or
@@ -430,8 +453,8 @@ class Engine:
                                 layout="dhw", dtype="f32", stream: int = 0):
         """Device pointers (ints): n pairs of images, n cost volumes of H*W*D elements each (layout "hwd" / "dhw", dtype
         "f32" / "f16" / "bf16"), n maps out; enqueued on `stream` without synchronising, like match_batch_device."""
-        _check(self._L.adc_match_cost_batch_device(self._h, n, d_left, d_right, d_cost, _code(COST_LAYOUTS, layout, "layout"),
-                                                   _code(COST_DTYPES, dtype, "dtype"), d_disp, stream))
+        _check(self._L.adc_match_cost_batch_device(self._h, n, d_left, d_right, *_device_cost(d_cost, layout, dtype), d_disp,
+                                                   stream))
 
     # ---- exporting the cost volumes (adc_match_volumes*) --------------------------------------
     def match_volumes(self, left, right, stages, layout="hwd", dtype="f32", cost=None, cost_layout="hwd", cost_dtype=None,
@@ -443,17 +466,9 @@ class Engine:
         the latest requested volume."""
         left = _img(left, (self.height, self.width, 3))
         right = _img(right, (self.height, self.width, 3))
-        if isinstance(stages, (str, int)):
-            stages = [stages]
-        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
-        H, W, D = self.height, self.width, self.D
-        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
-        vols = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in stages}
-        outs = _volume_outs([(v.ctypes.data, s, lay, dt) for s, v in vols.items()])
-        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
-        disp = np.empty((H, W), np.float32) if disparity else None
-        _check(self._L.adc_match_volumes(self._h, left.ctypes.data, right.ctypes.data, None if c is None else c.ctypes.data,
-                                         clay, cdt, None if disp is None else disp.ctypes.data, outs, len(vols)))
+        stages = dict.fromkeys([stages] if isinstance(stages, (str, int)) else stages)   # a stage named twice: one volume
+        disp, vols, args = self._outputs((), stages, layout, dtype, cost, cost_layout, cost_dtype, disparity)
+        _check(self._L.adc_match_volumes(self._h, left.ctypes.data, right.ctypes.data, *args[:6]))
         return disp, vols
 
     def match_volumes_batch_device(self, n: int, d_left: int, d_right: int, outs, d_disp: int = 0, d_cost: int = 0,
@@ -461,11 +476,9 @@ class Engine:
         """Device pointers (ints): n pairs of images, optional n cost volumes, optional n maps (d_disp 0 = volumes only);
         `outs` a list of (ptr, stage, layout, dtype), each ptr n volumes of H*W*D elements.  Enqueued on `stream` without
         synchronising, like match_batch_device."""
-        arr = _volume_outs(outs)
-        _check(self._L.adc_match_volumes_batch_device(self._h, n, d_left, d_right, d_cost or None,
-                                                      _code(COST_LAYOUTS, cost_layout, "layout"),
-                                                      _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, arr,
-                                                      len(outs), stream))
+        _check(self._L.adc_match_volumes_batch_device(self._h, n, d_left, d_right,
+                                                      *_device_cost(d_cost, cost_layout, cost_dtype), d_disp or None,
+                                                      _volume_outs(outs), len(outs), stream))
 
     # ---- per-pixel side maps, with or without volumes (adc_match_outputs*) -----------------------
     def match_outputs(self, left, right, maps=(), volumes=(), layout="hwd", dtype="f32", cost=None, cost_layout="hwd",
@@ -477,21 +490,8 @@ class Engine:
         cost, as for match_cost.  disparity=False stops the pipeline after the latest requested output."""
         left = _img(left, (self.height, self.width, 3))
         right = _img(right, (self.height, self.width, 3))
-        maps = [maps] if isinstance(maps, (str, int)) else list(maps)
-        volumes = [volumes] if isinstance(volumes, (str, int)) else list(volumes)
-        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
-        H, W, D = self.height, self.width, self.D
-        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
-        out = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in volumes}
-        vouts = _volume_outs([(out[s].ctypes.data, s, lay, dt) for s in volumes])
-        for m in maps:
-            out[m] = np.empty((H, W), _MAP_NP.get(_code(MAP_KINDS, m, "map kind"), np.float32))
-        mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
-        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
-        disp = np.empty((H, W), np.float32) if disparity else None
-        _check(self._L.adc_match_outputs(self._h, left.ctypes.data, right.ctypes.data, None if c is None else c.ctypes.data,
-                                         clay, cdt, None if disp is None else disp.ctypes.data, vouts, len(volumes),
-                                         mouts, len(maps)))
+        disp, out, args = self._outputs(maps, volumes, layout, dtype, cost, cost_layout, cost_dtype, disparity)
+        _check(self._L.adc_match_outputs(self._h, left.ctypes.data, right.ctypes.data, *args))
         return disp, out
 
     def match_outputs_batch_device(self, n: int, d_left: int, d_right: int, maps=(), volumes=(), d_disp: int = 0,
@@ -500,11 +500,10 @@ class Engine:
         `maps` a list of (ptr, kind), each ptr n maps of H*W elements (float32, uint8 for "outliers"); `volumes` a list
         of (ptr, stage, layout, dtype) as for match_volumes_batch_device.  Enqueued on `stream` without synchronising,
         like match_batch_device."""
-        varr, marr = _volume_outs(volumes), _map_outs(maps)
-        _check(self._L.adc_match_outputs_batch_device(self._h, n, d_left, d_right, d_cost or None,
-                                                      _code(COST_LAYOUTS, cost_layout, "layout"),
-                                                      _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
-                                                      len(volumes), marr, len(maps), stream))
+        _check(self._L.adc_match_outputs_batch_device(self._h, n, d_left, d_right,
+                                                      *_device_cost(d_cost, cost_layout, cost_dtype), d_disp or None,
+                                                      _volume_outs(volumes), len(volumes), _map_outs(maps), len(maps),
+                                                      stream))
 
     # ---- image input formats (adc_match_images*) -----------------------------------------------
     def match_images(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
@@ -521,24 +520,12 @@ class Engine:
         """The host entries that take views in an IMG_* format: adc_match_images (views of H x W) and
         adc_match_rectified (raw frames of vh x vw)."""
         fmt = _img_format(format)
-        H, W, D = self.height, self.width, self.D
         desc = _image_view_desc(left, fmt, vh, vw)
         if _image_view_desc(right, fmt, vh, vw).row_pitch != desc.row_pitch or \
                 (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
             raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
-        maps = [maps] if isinstance(maps, (str, int)) else list(maps)
-        volumes = [volumes] if isinstance(volumes, (str, int)) else list(volumes)
-        lay, dt = _code(COST_LAYOUTS, layout, "layout"), _code(COST_DTYPES, dtype, "dtype")
-        shape = (H, W, D) if lay == COST_HWD else (D, H, W)
-        out = {s: np.empty(shape, _VOL_NP.get(dt, np.float32)) for s in volumes}
-        vouts = _volume_outs([(out[s].ctypes.data, s, lay, dt) for s in volumes])
-        for m in maps:
-            out[m] = np.empty((H, W), _MAP_NP.get(_code(MAP_KINDS, m, "map kind"), np.float32))
-        mouts = _map_outs([(out[m].ctypes.data, m) for m in maps])
-        c, clay, cdt = (None, 0, 0) if cost is None else self._cost(cost, cost_layout, cost_dtype)
-        disp = np.empty((H, W), np.float32) if disparity else None
-        _check(call(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc), None if c is None else c.ctypes.data,
-                    clay, cdt, None if disp is None else disp.ctypes.data, vouts, len(volumes), mouts, len(maps)))
+        disp, out, args = self._outputs(maps, volumes, layout, dtype, cost, cost_layout, cost_dtype, disparity)
+        _check(call(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc), *args))
         return disp, out
 
     def match_images_batch_device(self, n: int, d_left: int, d_right: int, image=None, maps=(), volumes=(),
@@ -546,12 +533,11 @@ class Engine:
         """match_outputs_batch_device for images described by `image` (an ImageDesc, e.g. from image_desc(); None = tight
         packed BGR): device pointers (ints) to the first pair's left and right view, pair i at i * image_stride bytes.
         Enqueued on `stream` without synchronising, like match_batch_device."""
-        varr, marr = _volume_outs(volumes), _map_outs(maps)
         _check(self._L.adc_match_images_batch_device(self._h, n, d_left, d_right,
-                                                     None if image is None else ctypes.byref(image), d_cost or None,
-                                                     _code(COST_LAYOUTS, cost_layout, "layout"),
-                                                     _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
-                                                     len(volumes), marr, len(maps), stream))
+                                                     None if image is None else ctypes.byref(image),
+                                                     *_device_cost(d_cost, cost_layout, cost_dtype), d_disp or None,
+                                                     _volume_outs(volumes), len(volumes), _map_outs(maps), len(maps),
+                                                     stream))
 
     # ---- rectification on the way in (adc_set_rectification, adc_match_rectified*) --------------------
     def set_rectification(self, left_maps, right_maps=None, src_size=None):
@@ -591,12 +577,11 @@ class Engine:
         """match_images_batch_device for raw frames: `image` (an ImageDesc, None = tight packed BGR) describes the raw
         views of the src_size given to set_rectification; pair i at i * image_stride bytes.  Enqueued on `stream`
         without synchronising, like match_batch_device."""
-        varr, marr = _volume_outs(volumes), _map_outs(maps)
         _check(self._L.adc_match_rectified_batch_device(self._h, n, d_left, d_right,
-                                                        None if image is None else ctypes.byref(image), d_cost or None,
-                                                        _code(COST_LAYOUTS, cost_layout, "layout"),
-                                                        _code(COST_DTYPES, cost_dtype, "dtype"), d_disp or None, varr,
-                                                        len(volumes), marr, len(maps), stream))
+                                                        None if image is None else ctypes.byref(image),
+                                                        *_device_cost(d_cost, cost_layout, cost_dtype), d_disp or None,
+                                                        _volume_outs(volumes), len(volumes), _map_outs(maps), len(maps),
+                                                        stream))
 
     # ---- reprojection to 3-D (adc_reproject*) ---------------------------------------------------------
     def reproject(self, disp, Q, outputs=("points",)):
