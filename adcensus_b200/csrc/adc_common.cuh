@@ -118,19 +118,16 @@ struct AdcWave {            // device pointers of one wave (S pairs)
     unsigned* so_bitrows;   // [S][4][H][row words] mirrored per-row bit vectors of the right image (scanline optimiser)
     unsigned* so_rec;       // [S][4][N][rec words] per-pixel penalty records of the four pass directions
     const AdcSoTmaps* so_tm;     // host memory, owned by the lane: tensor maps of the scanline passes
-    int* tile_stamp;        // [S][tiles] region voting: epoch of the last change near a 16x16 tile
-    int* last_eval;         // [S][N]     region voting: epoch of a pixel's (or tile's) last evaluation
     unsigned long long* wta_key;  // [S][N] right-view WTA keys (ordered cost << 32 | disparity index)
-    int2* vote_dirty;       // [S][N]     region voting: work list of the current round
+    int* vote_work;         // [S][N]     region voting: slots whose histogram changed, to derive this round
+    int2* vote_chg;         // [S][N]     region voting: change records of the current round / fills of a commit
     uchar2* vote_alr;       // [S][N]     region voting: horizontal arms only (left, right)
-    uint8_t* vote_dq;       // [S][2][N]  region voting: rounded disparity index per pixel, NEW and OLD state
     uchar2* vote_atbT;      // [S][W][H]  region voting: vertical arms (top, bottom), transposed (a column is contiguous)
     int* vote_pslotT;       // [S][W][H]  region voting: histogram slot of a pending pixel, -1 otherwise (transposed)
-    uint8_t* vote_val;      // [S][N]     region voting: current vote per slot (255 = none)
+    uint16_t* vote_val;     // [S][N]     region voting: current vote per slot (one byte used unless D > 254 or L1 > 127)
     uint8_t* vote_dirtyb;   // [S][N]     region voting: slot's histogram changed since its last derive
     int* vote_state;        // [S][N]     region voting: disparity index of a valid pixel, -1 invalid, -(slot+2) pending
-    int* vote_deg;          // [S][N]     region voting: adjacency list lengths / fill cursors per slot
-    int* vote_off;          // [S][N+1]   region voting: adjacency list offsets (CSR by target slot)
+    int* vote_off;          // [S][N+1]   region voting: adjacency list lengths -> offsets -> fill cursors (CSR by target slot)
     unsigned* vote_hist;    // [S][vol_stride] region voting: histograms + forward lists + adjacency (= volB, idle after the last scanline pass)
     const float* lut_ad;    // [766]  (1 - exp(-(s/3)/lambda_ad)) + 1, host libm expf
     const float* lut_cen;   // [64]   exp(-h/lambda_census)
@@ -222,10 +219,10 @@ void adc_launch_confidence(const AdcParams& P, const AdcWave& w, const float* vo
                            cudaStream_t st, unsigned long long* launches);
 void adc_launch_outlier(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_build_lists(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
+// the voting lists (w.vlist, counters 10/11): the listed pixels whose cross region can ever pass the vote
+void adc_launch_active_lists(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
+// region voting (k_vote.cu): fills pixels of disp_l / disp_t, then rebuilds the outlier lists; uses w.volB as storage
 void adc_launch_voting(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
-// incremental-histogram voting (k_vote.cu); expects the active lists (w.vlist, counters 10/11) and the byte state
-// (w.vote_dq, w.vote_alr); uses w.volB as histogram storage.  false = not applicable, nothing launched
-bool adc_launch_vote_push(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // k = 0: mismatch list, k = 1: occlusion list; reads disp_l, writes disp_t
 void adc_launch_interp_list(const AdcParams& P, const AdcWave& w, int k, cudaStream_t st, unsigned long long* launches);
 void adc_launch_discontinuity(const AdcParams& P, const AdcWave& w, const float* vol, cudaStream_t st, unsigned long long* launches);

@@ -161,22 +161,19 @@ size_t carve_lane(void* base, const AdcDims& dm, int L1, int S, AdcWave* w) {
     t.pend = c.take<int>((size_t)S * 2 * N);
     t.vlist = c.take<int>((size_t)S * 2 * N);
     t.counters = c.take<int>((size_t)S * ADC_CNT);
-    t.vote_dq = c.take<uint8_t>((size_t)S * 2 * N);
     t.vote_alr = c.take<uchar2>((size_t)S * N);
-    t.vote_dirty = c.take<int2>((size_t)S * N);
+    t.vote_chg = c.take<int2>((size_t)S * N);
     t.vote_atbT = c.take<uchar2>((size_t)S * N);
     t.vote_pslotT = c.take<int>((size_t)S * N);
-    t.vote_val = c.take<uint8_t>((size_t)S * N);
+    t.vote_val = c.take<uint16_t>((size_t)S * N);
     t.vote_dirtyb = c.take<uint8_t>((size_t)S * N);
     t.vote_state = c.take<int>((size_t)S * N);
-    t.vote_deg = c.take<int>((size_t)S * N);
     t.vote_off = c.take<int>((size_t)S * (N + 1));
     t.wta_key = c.take<unsigned long long>((size_t)S * N);
     t.rowcnt = c.take<int>((size_t)S * 2 * dm.H);
     t.so_bitrows = c.take<unsigned>((size_t)S * adc_so_bitrow_bytes(dm) / 4);
     t.so_rec = c.take<unsigned>((size_t)S * adc_so_rec_bytes(dm) / 4);
-    t.tile_stamp = c.take<int>((size_t)S * ((dm.W + 15) / 16) * ((dm.H + 15) / 16));
-    t.last_eval = c.take<int>((size_t)S * N);
+    t.vote_work = c.take<int>((size_t)S * N);
     t.vote_hist = reinterpret_cast<unsigned*>(t.volB);   // idle after the last scanline pass
     if (w) *w = t;
     return c.off;
@@ -1550,7 +1547,7 @@ int adc_render_disparity(adc_engine* e, const float* disp, uint8_t* gray8, uint8
     Lane& ln = e->lanes[0];
     const size_t N = (size_t)e->P.dm.N;
     // lane 0's buffers are idle between calls: disp_t holds the map, flag the 8-bit image, bgr the colour image,
-    // the first words of tile_stamp the min/max keys and (as floats) the values handed back
+    // the first words of rowcnt the min/max keys and (as floats) the values handed back
     float* d_disp = ln.w.disp_t;
     unsigned* d_mm = reinterpret_cast<unsigned*>(ln.w.rowcnt);
     float* d_mm_out = reinterpret_cast<float*>(ln.w.rowcnt) + 2;

@@ -10,12 +10,6 @@
 #include <stdlib.h>
 #include <algorithm>
 
-// barrier over all threads of the thread-block cluster, with release/acquire ordering of memory
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-
 // =============================================================================================
 // 1. Outlier detection.  The raster scan reads disp_left[col_rl] of the same row while already
 //    having invalidated pixels to the left of x.  Whether a pixel gets invalidated depends only on
@@ -80,36 +74,15 @@ void adc_launch_outlier(const AdcParams& P, const AdcWave& w, cudaStream_t st, u
 }
 
 // =============================================================================================
-// 2. Iterative region voting -- the PULL form.  The default path is the incremental-histogram (push) form in
-//    k_vote.cu; the kernels below remain as the fallback for configurations that path does not take (more than
-//    254 disparities, arms longer than 127) and as the A/B reference (ADC_VOTE_MODE=1 / 2 / 3).
-//    Reference: 5 iterations x {mismatch list, occlusion list}; within a
-//    sweep pixels are visited in list (= raster) order and a filled pixel is immediately visible to
-//    later ones (Gauss-Seidel).  Exact parallel form ("raster-aware fixed point"): keep OLD (state at
-//    sweep start) and NEW.  Repeatedly recompute pending pixels p of the list in parallel, reading
-//    neighbour q from NEW if q precedes p in raster order and from OLD otherwise, until a full round
-//    changes nothing.  The sequential result is the unique fixed point of that map (induction over
-//    raster order: the first pending pixel only depends on OLD, pixel p only on OLD and on earlier
-//    pixels), so ANY asynchronous evaluation order converges to it, and a round without changes
-//    certifies it.
-//    Work filter (does not change the fixed point): a pixel's vote is a pure function of the
-//    disparities inside its cross region, which lies within +-L1 of it.  Every value change stamps
-//    the 16x16 tiles within that reach with the current epoch; a pending pixel is re-evaluated only
-//    if its tile carries a stamp >= the epoch of its own last evaluation.  Otherwise its inputs are
-//    bit-for-bit what they were and so is its vote -- this also carries over from sweep to sweep.
-//    One CTA per stereo pair (so plain L1-cached accesses are coherent); the batch and the other
-//    lanes keep the rest of the chip busy.
+// 2. Pixel lists.  Iterative region voting (:153-227) itself is in k_vote.cu; it works on the active lists built
+//    here and leaves the outlier lists, rebuilt here, to the interpolation.
 // =============================================================================================
-#define RV_THREADS 1024
-#define RV_WARPS (RV_THREADS / 32)
-#define RV_MAXD 256
-#define RV_TILE 16
 
 // ---- ordered (raster) pixel lists of the two outlier classes: row counts -> scan -> scatter ----
 __global__ void __launch_bounds__(128)
 k_list_row_counts(AdcDims dm, const uint8_t* __restrict__ label, const uint16_t* __restrict__ region_size, int min_size,
                   int* __restrict__ rowcnt) {
-    // region_size != NULL: only pixels whose cross region holds more than min_size pixels (see adc_launch_voting)
+    // region_size != NULL: only pixels whose cross region holds more than min_size pixels (see adc_launch_active_lists)
     const int pair = blockIdx.y, y = blockIdx.x;
     const uint8_t* lab = label + (size_t)pair * dm.N + (size_t)y * dm.W;
     const uint16_t* rs = region_size ? region_size + (size_t)pair * dm.N + (size_t)y * dm.W : nullptr;
@@ -194,451 +167,13 @@ void adc_launch_build_lists(const AdcParams& P, const AdcWave& w, cudaStream_t s
 // cross_aggregator.cpp:271-325 already counted.  A pixel whose whole region is not larger than irv_ts can
 // never pass, in any sweep, whatever its neighbours become: it is left out of the voting lists (about 40 %
 // of the listed pixels on Cone) and simply stays in the outlier lists for the interpolation step.
-static void launch_active_lists(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
+void adc_launch_active_lists(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
     const bool exact = P.L1 <= 127;   // beyond that the reference's uint16 counts may wrap
     dim3 grid(P.dm.H, w.S);
     k_list_row_counts<<<grid, 128, 0, st>>>(P.dm, w.label, exact ? w.sup_h : nullptr, P.irv_ts, w.rowcnt);
     k_list_row_scan<<<w.S, 64, 0, st>>>(P.dm, w.rowcnt, w.counters, 10);
     k_list_row_scatter<<<grid, 128, 0, st>>>(P.dm, w.label, exact ? w.sup_h : nullptr, P.irv_ts, w.rowcnt, w.vlist);
     *launches += 3;
-}
-
-// in-place ordered compaction of list[0..n) keeping the pixels that are still invalid (one CTA)
-__device__ int rv_compact_invalid(int n, int* list, const float* d_old, int* s_warp_tot) {
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    int base = 0;
-    for (int start = 0; start < n; start += RV_THREADS) {
-        const int i = start + tid;
-        int p = 0;
-        bool keep = false;
-        if (i < n) { p = __ldcg(list + i); keep = __ldcg(d_old + p) == ADC_INVALID_F; }
-        const unsigned b = __ballot_sync(0xffffffffu, keep);
-        if (lane == 0) s_warp_tot[wid] = __popc(b);
-        __syncthreads();  // also orders this chunk's reads before its writes
-        int off = base, tot = 0;
-        for (int w2 = 0; w2 < RV_WARPS; w2++) {
-            const int c = s_warp_tot[w2];
-            if (w2 < wid) off += c;
-            tot += c;
-        }
-        if (keep) __stcg(list + off + __popc(b & ((1u << lane) - 1u)), p);
-        base += tot;
-        __syncthreads();
-    }
-    return base;
-}
-
-// `reach_up`: how far above (x,y) dependants can sit.  At commit time that is `reach` (everybody around sees
-// the new OLD value); during the rounds of a sweep it is 0: a changed NEW value is only read by pixels that
-// come LATER in raster order, and every pixel of a tile row above (x,y)'s own comes earlier.
-__device__ __forceinline__ void rv_stamp_tiles(int* tiles, int tw, int th, int x, int y, int reach, int epoch, int lane,
-                                               int reach_up) {
-    const int tx0 = max(0, (x - reach) / RV_TILE), tx1 = min(tw - 1, (x + reach) / RV_TILE);
-    const int ty0 = max(0, (y - reach_up) / RV_TILE), ty1 = min(th - 1, (y + reach) / RV_TILE);
-    const int nx = tx1 - tx0 + 1, nt = nx * (ty1 - ty0 + 1);
-    for (int i = lane; i < nt; i += 32) __stcg(tiles + (ty0 + i / nx) * tw + tx0 + i % nx, epoch);
-}
-
-// A thread-block cluster of RV_CLUSTER CTAs works on one stereo pair: the pending pixels of a
-// round are dealt round-robin to its RV_CLUSTER*32 warps, the rounds are separated by cluster
-// barriers, and all mutable state lives in global memory and is accessed at L2 (ld.cg / st.cg)
-// because the CTAs sit on different SMs.
-#define RV_CLUSTER 8
-
-// USE_L1: read through L1 (plain loads).  The cluster barrier between rounds carries an acquire at
-// cluster scope, for which ptxas emits an L1 invalidate, so a round never sees lines cached before
-// the previous barrier; lines going stale *within* a round are harmless (asynchronous fixed point,
-// and the certifying round has no writes at all).
-template <bool USE_L1> __device__ __forceinline__ float rv_ld(const float* p) { return USE_L1 ? __ldca(p) : __ldcg(p); }
-template <bool USE_L1> __device__ __forceinline__ int rv_ld(const int* p) { return USE_L1 ? __ldca(p) : __ldcg(p); }
-
-template <bool USE_L1>
-__global__ void __cluster_dims__(RV_CLUSTER, 1, 1) __launch_bounds__(RV_THREADS)
-k_region_voting_global(AdcParams P, const uchar4* __restrict__ arms, float* disp_old, float* disp_new,
-                       uint8_t* label, int* pend, int* counters, int* tile_stamp, int* last_eval) {
-    __shared__ int s_hist[RV_WARPS][RV_MAXD];
-    __shared__ int s_tot[RV_WARPS];
-    const AdcDims& dm = P.dm;
-    const int pair = blockIdx.x / RV_CLUSTER;
-    const int crank = blockIdx.x % RV_CLUSTER;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int gwarp = crank * RV_WARPS + wid, n_gwarps = RV_CLUSTER * RV_WARPS;
-    const int gtid = crank * RV_THREADS + tid, n_gthreads = RV_CLUSTER * RV_THREADS;
-    const int W = dm.W, D = dm.D;
-    const int tw = (W + RV_TILE - 1) / RV_TILE, th = (dm.H + RV_TILE - 1) / RV_TILE;
-    const int reach = max(P.L1, 0);
-    const uchar4* A = arms + (size_t)pair * dm.N;
-    float* d_old = disp_old + (size_t)pair * dm.N;
-    float* d_new = disp_new + (size_t)pair * dm.N;
-    uint8_t* lab = label + (size_t)pair * dm.N;
-    int* tiles = tile_stamp + (size_t)pair * tw * th;
-    int* evalep = last_eval + (size_t)pair * dm.N;
-    int* cnt = counters + pair * ADC_CNT;   // 0,1: list sizes   2: rounds   3: evaluations   4..6: change flags (mod 3)
-    int n_list[2] = {__ldcg(cnt + 0), __ldcg(cnt + 1)};
-    int rounds_total = 0, evals = 0;
-    int* hist = s_hist[wid];
-
-    // nothing stamped, nothing evaluated: stamp(0) >= last_eval(0) makes the first round evaluate everyone
-    for (int i = gtid; i < tw * th; i += n_gthreads) __stcg(tiles + i, 0);
-    for (int k = 0; k < 2; k++) {
-        const int* list = pend + ((size_t)pair * 2 + k) * dm.N;
-        for (int i = gtid; i < n_list[k]; i += n_gthreads) __stcg(evalep + list[i], 0);
-    }
-    if (gtid < 3) __stcg(cnt + 4 + gtid, 0);
-    int epoch = 1, rnd = 0;   // rnd indexes the three rotating change flags
-    cluster_sync_all();
-
-    for (int it = 0; it < 5; it++) {
-        for (int k = 0; k < 2; k++) {
-            int* list = pend + ((size_t)pair * 2 + k) * dm.N;
-            const int n = n_list[k];
-            if (n == 0) continue;  // uniform across the cluster
-            bool any_fill = false;
-            while (true) {
-                if (gtid == 0) __stcg(cnt + 4 + (rnd + 1) % 3, 0);  // flag of the NEXT round; nobody reads it now
-                bool warp_changed = false;
-                for (int idx = gwarp; idx < n; idx += n_gwarps) {
-                    const int p = rv_ld<USE_L1>(list + idx);
-                    const int y = p / W, x = p - y * W;
-                    if (rv_ld<USE_L1>(tiles + (y / RV_TILE) * tw + x / RV_TILE) < rv_ld<USE_L1>(evalep + p)) continue;  // inputs untouched since
-                    evals++;
-                    for (int b = lane; b < D; b += 32) hist[b] = 0;
-                    __syncwarp();
-                    const uchar4 a = __ldg(A + p);
-                    // one region row per lane: the arm loads of all rows go out together, then every lane
-                    // streams its own row segment (independent loads, several in flight)
-                    for (int t = -(int)a.z + lane; t <= (int)a.w; t += 32) {
-                        const int rowi = (y + t) * W + x;
-                        const uchar4 a2 = __ldg(A + rowi);
-                        const int s_lo = -(int)a2.x, s_hi = (int)a2.y;
-                        const int s_mid = t < 0 ? s_hi + 1 : (t == 0 ? 0 : s_lo);   // first s that reads OLD
-#pragma unroll 4
-                        for (int s = s_lo; s <= s_hi; s++) {
-                            const float d = s < s_mid ? rv_ld<USE_L1>(d_new + rowi + s) : rv_ld<USE_L1>(d_old + rowi + s);
-                            if (d != ADC_INVALID_F) {
-                                const int di = (int)roundf(d) - dm.dmin;  // lround: half away from zero
-                                if (di >= 0 && di < D) atomicAdd(&hist[di], 1);
-                            }
-                        }
-                    }
-                    __syncwarp();
-                    int peak = 0, best = 0x7fffffff, total = 0;
-                    for (int b = lane; b < D; b += 32) {
-                        const int h = hist[b];
-                        if (peak < h) { peak = h; best = b; }
-                        total += h;
-                    }
-                    const int gpeak = __reduce_max_sync(0xffffffffu, peak);
-                    const int gbest = __reduce_min_sync(0xffffffffu, peak == gpeak ? best : 0x7fffffff);
-                    total = __reduce_add_sync(0xffffffffu, total);
-                    float r = ADC_INVALID_F;
-                    if (gpeak > 0 && total > P.irv_ts &&
-                        __fdiv_rn(__fmul_rn((float)gpeak, 1.0f), (float)total) > P.irv_th)
-                        r = (float)(gbest + dm.dmin);
-                    const bool changed = __float_as_uint(r) != __float_as_uint(__ldcg(d_new + p));
-                    __syncwarp();
-                    if (lane == 0) {
-                        __stcg(evalep + p, epoch);
-                        if (changed) __stcg(d_new + p, r);
-                    }
-                    if (changed) { rv_stamp_tiles(tiles, tw, th, x, y, reach, epoch, lane, 0); warp_changed = true; }
-                }
-                if (warp_changed && lane == 0) __stcg(cnt + 4 + rnd % 3, 1);
-                cluster_sync_all();
-                const int ch = __ldcg(cnt + 4 + rnd % 3);
-                rounds_total++;
-                epoch++;
-                rnd++;
-                if (!ch) break;
-                any_fill = true;
-            }
-            if (!any_fill) continue;  // nothing was filled in this sweep: list and maps unchanged
-            // ---- commit the sweep (OLD <- NEW for filled pixels; they become visible to everyone, so
-            //      their neighbourhoods are stamped again), then erase them from the list
-            for (int idx = gwarp; idx < n; idx += n_gwarps) {
-                const int p = __ldcg(list + idx);
-                const float v = __ldcg(d_new + p);
-                if (v != ADC_INVALID_F) {
-                    if (lane == 0) { __stcg(d_old + p, v); lab[p] = 0; }
-                    const int y = p / W;
-                    rv_stamp_tiles(tiles, tw, th, p - y * W, y, reach, epoch, lane, reach);
-                }
-            }
-            epoch++;
-            cluster_sync_all();
-            if (crank == 0) {
-                const int kept = rv_compact_invalid(n, list, d_old, s_tot);
-                if (tid == 0) __stcg(cnt + k, kept);
-            }
-            cluster_sync_all();
-            n_list[k] = __ldcg(cnt + k);
-        }
-    }
-    evals = __reduce_add_sync(0xffffffffu, lane == 0 ? evals : 0);
-    if (lane == 0) atomicAdd(cnt + 3, evals);
-    if (gtid == 0) __stcg(cnt + 2, rounds_total);
-}
-
-// ---------------------------------------------------------------------------------------------
-// Byte state for the fast voting kernel: only the rounded disparity index matters for a vote, so the
-// state is one byte per pixel (0..253 = index, 254 = valid but outside [0,D), 255 = invalid).
-// ---------------------------------------------------------------------------------------------
-__global__ void k_vote_encode(AdcDims dm, const float* __restrict__ disp, const uchar4* __restrict__ arms,
-                              uint8_t* __restrict__ dq, uchar2* __restrict__ alr, int* __restrict__ vstate) {   // dq: [2i] = NEW, [2i+1] = OLD
-    const int pair = blockIdx.y;
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= dm.N) return;
-    const float d = disp[(size_t)pair * dm.N + i];
-    uint8_t v = 255;
-    if (d != ADC_INVALID_F) {
-        const int di = (int)roundf(d) - dm.dmin;
-        v = (di >= 0 && di < dm.D && di < 254) ? (uint8_t)di : (uint8_t)254;
-    }
-    reinterpret_cast<uchar2*>(dq + (size_t)pair * 2 * dm.N)[i] = make_uchar2(v, v);
-    if (vstate) vstate[(size_t)pair * dm.N + i] = v == 255 ? -1 : (int)v;   // k_vote.cu: index of a valid pixel, -1 = invalid
-    const uchar4 a = arms[(size_t)pair * dm.N + i];
-    alr[(size_t)pair * dm.N + i] = make_uchar2(a.x, a.y);   // horizontal arms, 2 bytes per pixel
-}
-
-// ---------------------------------------------------------------------------------------------
-// Byte-state version of the balanced cluster kernel (default).  Same algorithm as
-// k_region_voting_global with two changes that matter for speed: (1) the per-round "does this pending
-// pixel need another look?" test is done 32 list entries at a time, one per lane, instead of one
-// dependent L2 round trip after the other per warp (that serial test loop, not the votes, dominated
-// the first versions); (2) the state is one byte per pixel and the horizontal arms two, so a vote
-// moves 4x fewer bytes.  Mutable state is read at L2 (ld.cg) -- the CTAs of the cluster sit on
-// different SMs -- the constant arms through the read-only path.
-// ---------------------------------------------------------------------------------------------
-// (capping this kernel at 32 registers so that other lanes' kernels fit beside it was measured: slower overall)
-__global__ void __cluster_dims__(RV_CLUSTER, 1, 1) __launch_bounds__(RV_THREADS)
-k_region_voting_bytes(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restrict__ alr_all,
-                      float* disp_old, float* disp_new, uint8_t* dq, uint8_t* label, int* pend, int* counters,
-                      int* tile_stamp, int* last_eval) {
-    __shared__ int s_hist[RV_WARPS][RV_MAXD];
-    __shared__ int s_tot[RV_WARPS];
-    const AdcDims& dm = P.dm;
-    const int pair = blockIdx.x / RV_CLUSTER;
-    const int crank = blockIdx.x % RV_CLUSTER;
-    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int gwarp = crank * RV_WARPS + wid, n_gwarps = RV_CLUSTER * RV_WARPS;
-    const int gtid = crank * RV_THREADS + tid, n_gthreads = RV_CLUSTER * RV_THREADS;
-    const int W = dm.W, D = dm.D;
-    const int tw = (W + RV_TILE - 1) / RV_TILE, th = (dm.H + RV_TILE - 1) / RV_TILE;
-    const int reach = max(P.L1, 0);
-    const uchar4* A = arms + (size_t)pair * dm.N;
-    const uchar2* ALR = alr_all + (size_t)pair * dm.N;
-    float* d_old = disp_old + (size_t)pair * dm.N;
-    float* d_new = disp_new + (size_t)pair * dm.N;
-    uint8_t* q2 = dq + (size_t)pair * 2 * dm.N;        // per pixel two bytes: [2p] = NEW state, [2p+1] = OLD state
-    const unsigned short* q2w = reinterpret_cast<const unsigned short*>(q2);
-    uint8_t* lab = label + (size_t)pair * dm.N;
-    int* tiles = tile_stamp + (size_t)pair * tw * th;
-    int* evalep = last_eval + (size_t)pair * dm.N;
-    int* cnt = counters + pair * ADC_CNT;
-    int n_list[2] = {__ldcg(cnt + 10), __ldcg(cnt + 11)};   // active (fillable) lists, see launch_active_lists
-    int rounds_total = 0, evals = 0;
-    int* hist = s_hist[wid];
-    unsigned long long t_work = 0, t_bar = 0, t_commit = 0, t_compact = 0, t0 = 0;
-    auto now = []() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; };
-
-    for (int i = gtid; i < tw * th; i += n_gthreads) __stcg(tiles + i, 0);
-    for (int k = 0; k < 2; k++) {
-        const int* list = pend + ((size_t)pair * 2 + k) * dm.N;
-        for (int i = gtid; i < n_list[k]; i += n_gthreads) __stcg(evalep + list[i], 0);
-    }
-    if (gtid < 3) __stcg(cnt + 4 + gtid, 0);
-    int epoch = 1, rnd = 0;
-    cluster_sync_all();
-
-    for (int it = 0; it < 5; it++) {
-        for (int k = 0; k < 2; k++) {
-            int* list = pend + ((size_t)pair * 2 + k) * dm.N;
-            const int n = n_list[k];
-            if (n == 0) continue;  // uniform across the cluster
-            bool any_fill = false;
-            while (true) {
-                if (gtid == 0) __stcg(cnt + 4 + (rnd + 1) % 3, 0);
-                bool warp_changed = false;
-                t0 = now();
-                // 32 list entries per warp trip: every lane checks one pending pixel (is its tile stamped since
-                // its last evaluation?), then the warp evaluates the dirty ones one after the other
-                // (entries are dealt so that neighbouring list entries -- neighbouring pixels, which tend to be
-                //  dirty together -- go to different warps: entry = trip*32*n_gwarps + lane*n_gwarps + gwarp)
-                for (int base = 0; base < n; base += n_gwarps * 32) {
-                    const int my = base + lane * n_gwarps + gwarp;
-                    int p_l = 0;
-                    unsigned tb_l = 0;
-                    bool dirty_l = false;
-                    if (my < n) {
-                        p_l = __ldcg(list + my);
-                        const int yy = p_l / W, xx = p_l - yy * W;
-                        const uchar4 a_l = __ldg(A + p_l);
-                        tb_l = (unsigned)a_l.z | ((unsigned)a_l.w << 8);
-                        dirty_l = __ldcg(tiles + (yy / RV_TILE) * tw + xx / RV_TILE) >= __ldcg(evalep + p_l);
-                    }
-                    unsigned todo = __ballot_sync(0xffffffffu, dirty_l);
-                    while (todo) {
-                        const int src = __ffs(todo) - 1;
-                        todo &= todo - 1;
-                        const int p = __shfl_sync(0xffffffffu, p_l, src);
-                        const unsigned tb = __shfl_sync(0xffffffffu, tb_l, src);
-                        const int y = p / W, x = p - y * W;
-                        evals++;
-                        for (int b = lane; b < D; b += 32) hist[b] = 0;
-                        __syncwarp();
-                        // Region scan.  The horizontal arms of all (<= 69) region rows are fetched in ONE round of loads
-                        // (three per lane at most) and handed out by shuffle; then the region is visited in trips of
-                        // 4 rows x 16 columns, software-pipelined (the loads of trip j+1 are in flight while trip j is
-                        // added to the histogram).  Trip count = ceil(rows/4) x ceil(longest row/16): small regions cost
-                        // few instructions.  One 16-bit load brings a pixel's NEW and OLD state; it goes through L1
-                        // (ld.ca): neighbouring pixels are evaluated on the same SM and share their regions, and every
-                        // cluster barrier ends in CCTL.IVALL (see the SASS), so no line outlives a round.  A line going
-                        // stale inside a round is harmless (asynchronous fixed point; the certifying round writes nothing).
-                        const int top = (int)(tb & 255u), rows = top + (int)(tb >> 8) + 1;
-                        const int rbase = (y - top) * W + x;
-                        unsigned ar0, ar1 = 0, ar2 = 0;
-                        {
-                            const uchar2 v = lane < rows ? __ldg(ALR + rbase + lane * W) : make_uchar2(0, 0);
-                            ar0 = (unsigned)v.x | ((unsigned)v.y << 8);
-                        }
-                        if (rows > 32) {
-                            const uchar2 v1 = lane + 32 < rows ? __ldg(ALR + rbase + (lane + 32) * W) : make_uchar2(0, 0);
-                            const uchar2 v2 = lane + 64 < rows ? __ldg(ALR + rbase + (lane + 64) * W) : make_uchar2(0, 0);
-                            ar1 = (unsigned)v1.x | ((unsigned)v1.y << 8);
-                            ar2 = (unsigned)v2.x | ((unsigned)v2.y << 8);
-                        }
-                        const int span_l = (int)(ar0 & 255u) + (int)(ar0 >> 8);
-                        const int span_m = max(span_l, max((int)(ar1 & 255u) + (int)(ar1 >> 8), (int)(ar2 & 255u) + (int)(ar2 >> 8)));
-                        const int ncp = (__reduce_max_sync(0xffffffffu, span_m) >> 4) + 1;   // 16-column chunks per row
-                        const int grp = lane >> 3, sub = lane & 7;
-                        const int n_trips = ((rows + 3) >> 2) * ncp;
-                        int ti = 0, tc = 0;                        // row group / column chunk of the trip being FETCHED
-                        auto fetch_trip = [&](int& o0, int& o1) {
-                            const int ri = 4 * ti + grp;
-                            unsigned a2 = __shfl_sync(0xffffffffu, ar0, ri & 31);
-                            if (rows > 32) {
-                                const unsigned a2b = __shfl_sync(0xffffffffu, ar1, ri & 31);
-                                const unsigned a2c = __shfl_sync(0xffffffffu, ar2, ri & 31);
-                                a2 = ri < 32 ? a2 : (ri < 64 ? a2b : a2c);
-                            }
-                            const int s_hi = ri < rows ? (int)(a2 >> 8) : -0x10000;       // dead rows: empty segment
-                            const int s0 = -(int)(a2 & 255u) + sub + 16 * tc, s1 = s0 + 8;
-                            const int t = ri - top;
-                            const int mid = t < 0 ? 0x10000 : (t == 0 ? 0 : -0x10000);   // columns below `mid` read NEW
-                            const unsigned short* rp = q2w + rbase + ri * W;
-                            o0 = o1 = 255;
-                            if (s0 <= s_hi) { const unsigned w2 = __ldca(rp + s0); o0 = s0 < mid ? (int)(w2 & 255u) : (int)(w2 >> 8); }
-                            if (s1 <= s_hi) { const unsigned w2 = __ldca(rp + s1); o1 = s1 < mid ? (int)(w2 & 255u) : (int)(w2 >> 8); }
-                            if (++tc == ncp) { tc = 0; ti++; }
-                        };
-                        int d0, d1;
-                        fetch_trip(d0, d1);
-                        for (int j = 0; j < n_trips; j++) {
-                            int n0 = 255, n1 = 255;
-                            if (j + 1 < n_trips) fetch_trip(n0, n1);
-                            if (d0 < 254) atomicAdd(&hist[d0], 1);
-                            if (d1 < 254) atomicAdd(&hist[d1], 1);
-                            d0 = n0; d1 = n1;
-                        }
-                        __syncwarp();
-                        int peak = 0, best = 0x7fffffff, total = 0;
-                        for (int b = lane; b < D; b += 32) {
-                            const int h = hist[b];
-                            if (peak < h) { peak = h; best = b; }
-                            total += h;
-                        }
-                        const int gpeak = __reduce_max_sync(0xffffffffu, peak);
-                        const int gbest = __reduce_min_sync(0xffffffffu, peak == gpeak ? best : 0x7fffffff);
-                        total = __reduce_add_sync(0xffffffffu, total);
-                        int r = 255;
-                        if (gpeak > 0 && total > P.irv_ts &&
-                            __fdiv_rn(__fmul_rn((float)gpeak, 1.0f), (float)total) > P.irv_th)
-                            r = gbest;
-                        const bool changed = r != (int)__ldcg(q2 + 2 * p);
-                        __syncwarp();
-                        if (lane == 0) {
-                            __stcg(evalep + p, epoch);
-                            if (changed) __stcg(q2 + 2 * p, (uint8_t)r);
-                        }
-                        if (changed) { rv_stamp_tiles(tiles, tw, th, x, y, reach, epoch, lane, 0); warp_changed = true; }
-                    }
-                }
-                if (warp_changed && lane == 0) __stcg(cnt + 4 + rnd % 3, 1);
-                { const unsigned long long t1 = now(); t_work += t1 - t0; t0 = t1; }
-                cluster_sync_all();
-                { const unsigned long long t1 = now(); t_bar += t1 - t0; t0 = t1; }
-                const int ch = __ldcg(cnt + 4 + rnd % 3);
-                rounds_total++;
-                epoch++;
-                rnd++;
-                if (!ch) break;
-                any_fill = true;
-            }
-            if (!any_fill) continue;
-            t0 = now();
-            for (int base = gwarp * 32; base < n; base += n_gwarps * 32) {   // one list entry per lane
-                const int my = base + lane;
-                int p_l = 0, v_l = 255;
-                if (my < n) { p_l = __ldcg(list + my); v_l = __ldcg(q2 + 2 * p_l); }
-                if (v_l != 255) {
-                    const float f = (float)(v_l + dm.dmin);
-                    __stcg(q2 + 2 * p_l + 1, (uint8_t)v_l);
-                    __stcg(d_old + p_l, f);
-                    __stcg(d_new + p_l, f);
-                    __stcg(lab + p_l, (uint8_t)0);
-                }
-                unsigned filled = __ballot_sync(0xffffffffu, v_l != 255);
-                while (filled) {
-                    const int src = __ffs(filled) - 1;
-                    filled &= filled - 1;
-                    const int p = __shfl_sync(0xffffffffu, p_l, src);
-                    const int y = p / W;
-                    rv_stamp_tiles(tiles, tw, th, p - y * W, y, reach, epoch, lane, reach);
-                }
-            }
-            epoch++;
-            cluster_sync_all();
-            { const unsigned long long t1 = now(); t_commit += t1 - t0; t0 = t1; }
-            if (crank == 0) {
-                const int kept = rv_compact_invalid(n, list, d_old, s_tot);
-                if (tid == 0) __stcg(cnt + 10 + k, kept);
-            }
-            cluster_sync_all();
-            { const unsigned long long t1 = now(); t_compact += t1 - t0; t0 = t1; }
-            n_list[k] = __ldcg(cnt + 10 + k);
-        }
-    }
-    evals = __reduce_add_sync(0xffffffffu, lane == 0 ? evals : 0);
-    if (lane == 0) atomicAdd(cnt + 3, evals);
-    if (gtid == 0) {
-        __stcg(cnt + 2, rounds_total);
-        __stcg(cnt + 12, (int)(t_work / 1000)); __stcg(cnt + 13, (int)(t_bar / 1000));     // warp 0's view, microseconds
-        __stcg(cnt + 14, (int)(t_commit / 1000)); __stcg(cnt + 15, (int)(t_compact / 1000));
-    }
-}
-
-// Three kernels, chosen by the parameters alone (each has its parity cases in tests/test_gpu_parity.py):
-//   D <= 254 and L1 <= 127   incremental histograms, k_vote.cu (every BASELINE configuration)
-//   D <= 254, L1 > 127       byte-state pull kernel (a cross region may hold more than 65535 pixels)
-//   D = 255, 256             float-state pull kernel (the byte state codes a disparity index in one byte)
-void adc_launch_voting(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
-    // disp_l = committed state (OLD), disp_t = working copy (NEW); both hold the post-outlier map here
-    dim3 egrid((P.dm.N + 255) / 256, w.S);
-    if (P.dm.D <= 254) {
-        launch_active_lists(P, w, st, launches);
-        k_vote_encode<<<egrid, 256, 0, st>>>(P.dm, w.disp_l, w.arms, w.vote_dq, w.vote_alr, w.vote_state);
-        ++*launches;
-        if (!adc_launch_vote_push(P, w, st, launches)) {
-            k_region_voting_bytes<<<w.S * RV_CLUSTER, RV_THREADS, 0, st>>>(P, w.arms, w.vote_alr, w.disp_l, w.disp_t, w.vote_dq,
-                                                                          w.label, w.vlist, w.counters, w.tile_stamp, w.last_eval);
-            ++*launches;
-        }
-        adc_launch_build_lists(P, w, st, launches);   // outlier lists = every listed pixel that is still invalid
-    } else {
-        k_region_voting_global<false><<<w.S * RV_CLUSTER, RV_THREADS, 0, st>>>(P, w.arms, w.disp_l, w.disp_t, w.label, w.pend,
-                                                                               w.counters, w.tile_stamp, w.last_eval);
-        ++*launches;
-    }
 }
 
 // =============================================================================================
@@ -813,7 +348,7 @@ void adc_launch_interp_list(const AdcParams& P, const AdcWave& w, int k, cudaStr
     const int L = P.max_search, B = L - 1;
     const size_t map_bytes = (size_t)(P.dm.W + 2 * B) * (P.dm.H + 2 * B);
     if (w.ray_off && L >= 2 && map_bytes <= (size_t)P.dm.N * 8 && (size_t)16 * L * sizeof(int) <= 48 * 1024) {
-        uint8_t* imap = reinterpret_cast<uint8_t*>(w.vote_dirty);   // [S][N] int2 scratch of the voting step, idle by now
+        uint8_t* imap = reinterpret_cast<uint8_t*>(w.vote_chg);   // voting's change list, 8 bytes per pixel, idle by now
         dim3 mgrid((unsigned)((map_bytes + 255) / 256), w.S);
         k_interp_map<<<mgrid, 256, 0, st>>>(P.dm, B, w.disp_l, imap);
         k_interpolate_fast<<<grid, 256, (size_t)16 * L * sizeof(int), st>>>(P, k, w.bgrx, w.disp_l, w.disp_t, w.pend, w.counters,

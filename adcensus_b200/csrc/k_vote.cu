@@ -32,14 +32,41 @@
 // If the adjacency lists do not fit the idle cost volume they live in (pathological inputs: huge regions
 // that are almost entirely invalid), the pair falls back to enumerating the inverse region of every change
 // on the fly from transposed arm tables (push_enum below).
+//
+// Two instantiations of the scan and push kernels, WIDE = D > 254 || L1 > 127.  The narrow one keeps a slot's vote in
+// one byte (255 = none) and the histogram counts in 16 bits, two per word (a region of L1 <= 127 holds < 65536 pixels).
+// WIDE keeps the vote in 16 bits (0xffff = none) and one 32-bit count per word, which covers every D <= 256 and
+// L1 <= 255.  For L1 > 127 the uint16 support counts the forward lists are reserved from may wrap, so those pairs
+// always enumerate.
 #include "adc_common.cuh"
+#include <type_traits>
 
 #define VP_THREADS 1024
 #define VP_WARPS (VP_THREADS / 32)
 #define VI_WARPS 8
 #define VP_MAXD 256
-// counters (ADC_CNT ints per pair): 10/11 = active list sizes, 12 = changes, 13 = 1 when the adjacency lists are
-// in use, 14 = total adjacency entries
+#define VOTE_OUTSIDE 256   // vstate of a valid pixel whose rounded disparity lies outside [0,D): no histogram counts it
+// counters (ADC_CNT ints per pair): 2 = fixed-point rounds, 3 = derives, 4..8 = microseconds spent in the phases of
+// k_vote_push, 9 = forward-list cursor, 10/11 = active list sizes, 12 = changes, 13 = 1 when the adjacency lists are in
+// use, 14 = total adjacency entries, 15 = forward-list room
+
+// ---- state maps: vstate[p] = rounded disparity index of a valid pixel, VOTE_OUTSIDE, or -1 = invalid; alr = the
+// horizontal arms alone (2 bytes per pixel), which is all the region scans read of a row ----
+__global__ void k_vote_encode(AdcDims dm, const float* __restrict__ disp, const uchar4* __restrict__ arms,
+                              uchar2* __restrict__ alr, int* __restrict__ vstate) {
+    const int pair = blockIdx.y;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= dm.N) return;
+    const float d = disp[(size_t)pair * dm.N + i];
+    int v = -1;
+    if (d != ADC_INVALID_F) {
+        const int di = (int)roundf(d) - dm.dmin;   // lround: half away from zero
+        v = di >= 0 && di < dm.D ? di : VOTE_OUTSIDE;
+    }
+    vstate[(size_t)pair * dm.N + i] = v;
+    const uchar4 a = arms[(size_t)pair * dm.N + i];
+    alr[(size_t)pair * dm.N + i] = make_uchar2(a.x, a.y);
+}
 
 // ---- transposed per-pixel tables for the fallback: vertical arms (top,bottom) as [x][y] ----
 __global__ void __launch_bounds__(256)
@@ -62,7 +89,7 @@ k_vote_transpose(AdcDims dm, const uchar4* __restrict__ arms, uchar2* __restrict
 }
 
 // ---- slots.  slot = position in the active list (+ n0 for the occlusion list).  vstate[p]: rounded disparity
-// index of a valid pixel (254 = outside [0,D)), -1 = invalid, -(slot+2) = invalid and pending in slot. ----
+// index of a valid pixel (VOTE_OUTSIDE = outside [0,D)), -1 = invalid, -(slot+2) = invalid and pending in slot. ----
 __global__ void __launch_bounds__(256)
 k_vote_slots(AdcDims dm, const int* __restrict__ vlist, int* __restrict__ counters, int* __restrict__ vstate,
              int* __restrict__ pslotT, const uint16_t* __restrict__ sup) {
@@ -144,11 +171,13 @@ __device__ __forceinline__ void vote_scan_region(int p, int W, const uchar4* __r
     }
 }
 
-// ---- batch-wide scan: histogram of every slot (D counters packed two per 32-bit word; a region holds < 65536 pixels) and,
-// when there is room, its forward list: an entry (t, s) for every pending pixel t of the region of slot s, written compacted
-// at a base taken from the pair's cursor (counters[9]).  A slot reserves as many entries as its region has pixels and marks
-// the ones it does not use (-1): the lists of a pair are ONE dense array of `room` entries that k_vote_push streams through.
+// ---- batch-wide scan: histogram of every slot (D counters packed two per 32-bit word, a region holding < 65536 pixels;
+// WIDE: one per word) and, when there is room, its forward list: an entry (t, s) for every pending pixel t of the region
+// of slot s, written compacted at a base taken from the pair's cursor (counters[9]).  A slot reserves as many entries as
+// its region has pixels and marks the ones it does not use (-1): the lists of a pair are ONE dense array of `room`
+// entries that k_vote_push streams through.
 __host__ __device__ inline long long vote_fwd_offset(long long ns, int HW) { return (ns * HW + 1) & ~1ll; }   // in 32-bit words, 8-byte aligned
+template <bool WIDE>
 __global__ void __launch_bounds__(VI_WARPS * 32)
 k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restrict__ alr_all, const int* __restrict__ vstate_all,
             const uint16_t* __restrict__ sup_all, const int* __restrict__ vlist, int* counters, unsigned* __restrict__ hist_all,
@@ -157,7 +186,7 @@ k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restri
     const AdcDims& dm = P.dm;
     const int pair = blockIdx.y;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int W = dm.W, D = dm.D, HW = (D + 1) >> 1;
+    const int W = dm.W, D = dm.D, HW = WIDE ? D : (D + 1) >> 1;
     int* cnt = counters + pair * ADC_CNT;
     const int n0 = cnt[10], n1 = cnt[11], ns = n0 + n1;
     const long long room = (unsigned)cnt[15];
@@ -190,8 +219,12 @@ k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restri
         });
         __syncwarp();
         for (int w2 = lane; w2 < HW; w2 += 32) {
-            const unsigned c0 = (unsigned)hs[2 * w2], c1 = (2 * w2 + 1 < D) ? (unsigned)hs[2 * w2 + 1] : 0u;
-            hist[(size_t)s * HW + w2] = c0 | (c1 << 16);
+            if constexpr (WIDE) {
+                hist[(size_t)s * HW + w2] = (unsigned)hs[w2];
+            } else {
+                const unsigned c0 = (unsigned)hs[2 * w2], c1 = (2 * w2 + 1 < D) ? (unsigned)hs[2 * w2 + 1] : 0u;
+                hist[(size_t)s * HW + w2] = c0 | (c1 << 16);
+            }
         }
         if (use_fwd)
             for (int k2 = fn + lane; k2 < reserved; k2 += 32) fwd[fb + k2] = make_int2(-1, -1);
@@ -207,17 +240,24 @@ k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restri
 #define VP_FLAG_DIRTY 1
 #define VP_FLAG_DEAD 2
 
+template <bool WIDE> using VoteVal = typename std::conditional<WIDE, uint16_t, uint8_t>::type;   // a slot's vote
+
+template <bool WIDE>
 __global__ void __launch_bounds__(VP_THREADS)
 k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
-            const uchar2* __restrict__ atbT_all, const int* __restrict__ pslotT_all, unsigned* hist_all, long long hist_stride, int* cur_all, uint8_t* val_all, uint8_t* flag_all,
+            const uchar2* __restrict__ atbT_all, const int* __restrict__ pslotT_all, unsigned* hist_all, long long hist_stride, int* cur_all, VoteVal<WIDE>* val_all, uint8_t* flag_all,
             const int* __restrict__ vlist, int* counters, int* work_all, int2* chg_all,
             float* disp_old, float* disp_new, uint8_t* label, int cols_cap, int slot_cap, int force_enum) {
+    using VT = VoteVal<WIDE>;
+    constexpr int NONE = WIDE ? 0xffff : 255;   // "no vote"; a change record packs old and new vote in VB-bit fields
+    constexpr int VB = WIDE ? 16 : 8;
+    constexpr int NHW = WIDE ? 8 : 4;           // histogram words per lane, at most
     extern __shared__ __align__(16) unsigned char vp_smem[];
     __shared__ int s_nwork, s_nchg, s_warp[32], s_base, s_fits;
     const AdcDims& dm = P.dm;
     const int pair = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int W = dm.W, H = dm.H, D = dm.D, HW = (D + 1) >> 1;
+    const int W = dm.W, H = dm.H, D = dm.D, HW = WIDE ? D : (D + 1) >> 1;
     const int L1 = max(P.L1, 0), R = 2 * L1 + 1;
     const uchar2* ALR = alr_all + (size_t)pair * dm.N;
     const uchar2* ATB = atbT_all + (size_t)pair * dm.N;
@@ -236,20 +276,20 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     // shared memory: [fallback column lists][val][flg][cur]
     unsigned short* cols = reinterpret_cast<unsigned short*>(vp_smem) + (size_t)wid * cols_cap;
     unsigned char* after_hist = vp_smem + (size_t)VP_WARPS * cols_cap * 2;
-    uint8_t* val;    // [slot] current vote, 255 = none
+    VT* val;         // [slot] current vote, NONE = none
     uint8_t* flg;    // [slot] VP_FLAG_*
     int* cur;        // [slot + 1] list lengths -> list starts -> fill cursors (= list ends once filled)
     const bool state_smem = ns <= slot_cap;
     if (state_smem) {
-        val = after_hist;
-        flg = val + slot_cap;
+        val = reinterpret_cast<VT*>(after_hist);
+        flg = reinterpret_cast<uint8_t*>(val + slot_cap);
         cur = reinterpret_cast<int*>(flg + slot_cap);
     } else {
         val = val_all + (size_t)pair * dm.N;
         flg = flag_all + (size_t)pair * dm.N;
         cur = cur_all + (size_t)pair * (dm.N + 1);
     }
-    for (int i = tid; i < ns; i += VP_THREADS) { val[i] = 255; flg[i] = VP_FLAG_DIRTY; }
+    for (int i = tid; i < ns; i += VP_THREADS) { val[i] = NONE; flg[i] = VP_FLAG_DIRTY; }
     for (int i = tid; i <= ns; i += VP_THREADS) cur[i] = 0;
     __syncthreads();
     int rounds_total = 0, derives = 0, changes = 0;
@@ -319,21 +359,26 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
         __stcg(cnt + 13, use_adj ? 1 : 0); __stcg(cnt + 14, n_adj); __stcg(cnt + 4, (int)((t1 - t_start) / 1000));   // us spent building the lists
     }
 
-    // value change of the pixel in slot t (a -> b, 255 = invalid) -> histograms of the pending pixels whose region
+    // value change of the pixel in slot t (a -> b, NONE = invalid) -> histograms of the pending pixels whose region
     // holds it.
     //   phase 0 (inside the sweep of list k): pixels of list k that come after it in raster order
-    //   phase 1 (commit, a == 255):           pixels of list k before it, and every pixel of the other list
+    //   phase 1 (commit, a == NONE):          pixels of list k before it, and every pixel of the other list
     auto touch = [&](int s, bool after, int a, int b, int k, int phase) {
         const int f = flg[s];
         if (f & VP_FLAG_DEAD) return;
         const int kk = s >= n0 ? 1 : 0;
         bool go;
         if (phase == 0) go = kk == k && after;
-        else            go = (kk != k || !after) && val[s] == 255;   // (pixels filled by this very sweep are leaving)
+        else            go = (kk != k || !after) && val[s] == NONE;   // (pixels filled by this very sweep are leaving)
         if (!go) return;
         unsigned* h = hist + (size_t)s * HW;
-        if (a < D) atomicSub(h + (a >> 1), 1u << ((a & 1) * 16));
-        if (b < D) atomicAdd(h + (b >> 1), 1u << ((b & 1) * 16));
+        if constexpr (WIDE) {
+            if (a < D) atomicSub(h + a, 1u);
+            if (b < D) atomicAdd(h + b, 1u);
+        } else {
+            if (a < D) atomicSub(h + (a >> 1), 1u << ((a & 1) * 16));
+            if (b < D) atomicAdd(h + (b >> 1), 1u << ((b & 1) * 16));
+        }
         // (racecheck flags this byte: concurrent pushes may read and set the same slot's flag -- every writer stores the same
         //  value into its own byte and a reader that still sees 0 merely stores it again; the flags are consumed after a barrier)
         if (!(f & VP_FLAG_DIRTY)) flg[s] = (uint8_t)VP_FLAG_DIRTY;
@@ -411,18 +456,24 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
         int peak = 0, best = 0x7fffffff, total = 0;
         for (int i = 0; i < nw; i++) {
             const int w2 = lane + 32 * i;
-            const int c0 = (int)(hv[i] & 0xffffu), c1 = (int)(hv[i] >> 16);
-            if (peak < c0) { peak = c0; best = 2 * w2; }       // strict '<': the lowest disparity wins ties
-            if (peak < c1) { peak = c1; best = 2 * w2 + 1; }
-            total += c0 + c1;
+            if constexpr (WIDE) {
+                const int c = (int)hv[i];
+                if (peak < c) { peak = c; best = w2; }         // strict '<': the lowest disparity wins ties
+                total += c;
+            } else {
+                const int c0 = (int)(hv[i] & 0xffffu), c1 = (int)(hv[i] >> 16);
+                if (peak < c0) { peak = c0; best = 2 * w2; }       // strict '<': the lowest disparity wins ties
+                if (peak < c1) { peak = c1; best = 2 * w2 + 1; }
+                total += c0 + c1;
+            }
         }
         const int gpeak = __reduce_max_sync(0xffffffffu, peak);
         const int gbest = __reduce_min_sync(0xffffffffu, peak == gpeak ? best : 0x7fffffff);
         total = __reduce_add_sync(0xffffffffu, total);
         if (gpeak > 0 && total > P.irv_ts && __fdiv_rn(__fmul_rn((float)gpeak, 1.0f), (float)total) > P.irv_th) return gbest;
-        return 255;
+        return NONE;
     };
-    const int nhw = (HW + 31) / 32;   // histogram words per lane (<= 4 for D <= 254)
+    const int nhw = (HW + 31) / 32;   // histogram words per lane (<= NHW)
     // phase clock of thread 0 (diagnostics, adc_debug_counters): ns spent collecting / deriving / pushing
     // (kept in shared memory: only thread 0 touches them, and registers are short here)
     __shared__ unsigned long long s_clk[4];   // mark, collect, derive, push
@@ -469,13 +520,13 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
                 // ---- derive: vote of every such pixel from its histogram, four pixels per trip (their loads in flight together)
                 for (int t = 4 * wid; t < nwork; t += 4 * VP_WARPS) {
                     int sl[4];
-                    unsigned hv[4][4];
+                    unsigned hv[4][NHW];
 #pragma unroll
                     for (int u = 0; u < 4; u++) sl[u] = work[min(t + u, nwork - 1)];
 #pragma unroll
                     for (int u = 0; u < 4; u++) {
 #pragma unroll
-                        for (int j = 0; j < 4; j++) {
+                        for (int j = 0; j < NHW; j++) {
                             const int w2 = lane + 32 * j;
                             hv[u][j] = (j < nhw && w2 < HW) ? __ldcg(hist + (size_t)sl[u] * HW + w2) : 0u;
                         }
@@ -490,8 +541,8 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
                             derives++;
                             const int a = val[sl[u]];
                             if (r[u] != a) {
-                                val[sl[u]] = (uint8_t)r[u];
-                                chg[atomicAdd(&s_nchg, 1)] = make_int2(sl[u], a | (r[u] << 8));
+                                val[sl[u]] = (VT)r[u];
+                                chg[atomicAdd(&s_nchg, 1)] = make_int2(sl[u], a | (r[u] << VB));
                             }
                         }
                     }
@@ -505,8 +556,8 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
                 // ---- push the changes into the histograms of the later pixels of this list
                 for (int t = wid; t < nchg; t += VP_WARPS) {
                     const int2 c = chg[t];
-                    if (use_adj) push_adj(c.x, c.y & 255, (c.y >> 8) & 255, k, 0);
-                    else         push_enum(pix(c.x), c.y & 255, (c.y >> 8) & 255, k, 0);
+                    if (use_adj) push_adj(c.x, c.y & NONE, (c.y >> VB) & NONE, k, 0);
+                    else         push_enum(pix(c.x), c.y & NONE, (c.y >> VB) & NONE, k, 0);
                 }
                 __syncthreads();
                 lap(ns_push);
@@ -519,8 +570,8 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
             for (int i0 = 0; i0 < n; i0 += VP_THREADS) {
                 const int i = i0 + tid;
                 bool f = false;
-                int v = 255;
-                if (i < n && !(flg[base + i] & VP_FLAG_DEAD)) { v = val[base + i]; f = v != 255; }
+                int v = NONE;
+                if (i < n && !(flg[base + i] & VP_FLAG_DEAD)) { v = val[base + i]; f = v != NONE; }
                 const unsigned m = __ballot_sync(0xffffffffu, f);
                 int o = 0;
                 if (lane == 0 && m) o = atomicAdd(&s_nchg, __popc(m));
@@ -539,8 +590,8 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
             changes += ncommit;
             for (int t = wid; t < ncommit; t += VP_WARPS) {
                 const int2 c = chg[t];
-                if (use_adj) push_adj(c.x, 255, (int)val[c.x], k, 1);
-                else         push_enum(c.y, 255, (int)val[c.x], k, 1);
+                if (use_adj) push_adj(c.x, NONE, (int)val[c.x], k, 1);
+                else         push_enum(c.y, NONE, (int)val[c.x], k, 1);
             }
             __syncthreads();
             for (int t = tid; t < ncommit; t += VP_THREADS) flg[chg[t].x] = (uint8_t)VP_FLAG_DEAD;
@@ -558,40 +609,53 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     }
 }
 
-// Expects the active lists (w.vlist, counters 10/11), w.vote_alr and w.vote_state (valid / invalid part, from
-// k_vote_encode).  Returns false when the fast path does not apply (caller falls back to the pull kernels).
-bool adc_launch_vote_push(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
+// The histograms (ns * HW <= N * D words), forward lists and adjacency lists live in w.vote_hist, the idle cost volume.
+template <bool WIDE>
+static void launch_scan_push(const AdcParams& P, const AdcWave& w, int L1, int force_enum, cudaStream_t st) {
+    const AdcDims& dm = P.dm;
+    unsigned* hist = w.vote_hist;
+    int gx = (adc_sm_count() * 8 + w.S - 1) / w.S;
+    if (gx < 1) gx = 1;
+    dim3 igrid(gx, w.S);
+    k_vote_scan<WIDE><<<igrid, VI_WARPS * 32, 0, st>>>(P, w.arms, w.vote_alr, w.vote_state, w.sup_h, w.vlist, w.counters,
+                                                       hist, dm.vol_stride, force_enum);
+    const int cols_cap = (2 * L1 + 1 + 7) / 8 * 8;
+    // shared memory: column lists (fallback), then val / flg / cur for as many slots as fit
+    const size_t fixed = (size_t)VP_WARPS * cols_cap * 2;
+    const size_t slot_bytes = sizeof(VoteVal<WIDE>) + 1 + 4;
+    int slot_cap = (int)((220 * 1024 - fixed - 16) / slot_bytes) & ~15;
+    if (slot_cap > VP_SMEM_SLOTS) slot_cap = VP_SMEM_SLOTS;
+    if ((P.dbg & 4) && slot_cap > 256) slot_cap = 256;   // ADC_DBG_VOTE_GLOBAL_STATE: global-memory copy of the per-slot state (tests)
+    const size_t smem = fixed + (slot_bytes - 4) * (size_t)slot_cap + ((size_t)slot_cap + 1) * 4;
+    static AdcOnce attr_once;
+    if (adc_once_needed(attr_once)) {
+        cudaFuncSetAttribute(k_vote_push<WIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 222 * 1024);   // (+ static < 227 KB)
+        adc_once_done(attr_once);
+    }
+    k_vote_push<WIDE><<<w.S, VP_THREADS, smem, st>>>(P, w.vote_alr, w.vote_atbT, w.vote_pslotT, hist, dm.vol_stride, w.vote_off,
+                                                     reinterpret_cast<VoteVal<WIDE>*>(w.vote_val), w.vote_dirtyb, w.vlist,
+                                                     w.counters, w.vote_work, w.vote_chg, w.disp_l, w.disp_t, w.label,
+                                                     cols_cap, slot_cap, force_enum);
+}
+
+// Region voting for every D and L1: the active lists, the state maps, the incremental histograms, then the outlier lists
+// rebuilt from the labels (every listed pixel that is still invalid).  disp_l = committed state, disp_t = working copy;
+// both hold the post-outlier map here.
+void adc_launch_voting(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
     const AdcDims& dm = P.dm;
     const int L1 = P.L1 > 0 ? P.L1 : 0;
-    if (dm.D > 254 || (2 * L1 + 1) * (2 * L1 + 1) > 65535) return false;
-    if ((long long)dm.N * ((dm.D + 1) / 2) > dm.vol_stride) return false;   // histograms live in the idle cost volume
-    const int force_enum = (P.dbg & 2) ? 1 : 0;   // ADC_DBG_VOTE_ENUM: exercise the enumeration fallback (tests)
+    adc_launch_active_lists(P, w, st, launches);
+    dim3 egrid((dm.N + 255) / 256, w.S);
+    k_vote_encode<<<egrid, 256, 0, st>>>(dm, w.disp_l, w.arms, w.vote_alr, w.vote_state);
     cudaMemsetAsync(w.vote_pslotT, 0xff, (size_t)w.S * dm.N * sizeof(int), st);
     dim3 tgrid((dm.W + 31) / 32, (dm.H + 31) / 32, w.S);
     k_vote_transpose<<<tgrid, 256, 0, st>>>(dm, w.arms, w.vote_atbT);
     dim3 sgrid(64, w.S);
     k_vote_slots<<<sgrid, 256, 0, st>>>(dm, w.vlist, w.counters, w.vote_state, w.vote_pslotT, w.sup_h);
-    unsigned* hist = w.vote_hist;
-    int gx = (adc_sm_count() * 8 + w.S - 1) / w.S;
-    if (gx < 1) gx = 1;
-    dim3 igrid(gx, w.S);
-    k_vote_scan<<<igrid, VI_WARPS * 32, 0, st>>>(P, w.arms, w.vote_alr, w.vote_state, w.sup_h, w.vlist, w.counters, hist,
-                                                 dm.vol_stride, force_enum);
-    const int cols_cap = (2 * L1 + 1 + 7) / 8 * 8;
-    // shared memory: column lists (fallback), then val / flg / cur for as many slots as fit
-    const size_t fixed = (size_t)VP_WARPS * cols_cap * 2;
-    int slot_cap = (int)((220 * 1024 - fixed - 16) / 6) & ~15;
-    if (slot_cap > VP_SMEM_SLOTS) slot_cap = VP_SMEM_SLOTS;
-    if ((P.dbg & 4) && slot_cap > 256) slot_cap = 256;   // ADC_DBG_VOTE_GLOBAL_STATE: global-memory copy of the per-slot state (tests)
-    const size_t smem = fixed + 2 * (size_t)slot_cap + ((size_t)slot_cap + 1) * 4;
-    static AdcOnce attr_once;
-    if (adc_once_needed(attr_once)) {
-        cudaFuncSetAttribute(k_vote_push, cudaFuncAttributeMaxDynamicSharedMemorySize, 222 * 1024);   // (+ static < 227 KB)
-        adc_once_done(attr_once);
-    }
-    k_vote_push<<<w.S, VP_THREADS, smem, st>>>(P, w.vote_alr, w.vote_atbT, w.vote_pslotT, hist, dm.vol_stride,
-                                              w.vote_off, w.vote_val, w.vote_dirtyb, w.vlist, w.counters, w.last_eval,
-                                              w.vote_dirty, w.disp_l, w.disp_t, w.label, cols_cap, slot_cap, force_enum);
-    *launches += 4;
-    return true;
+    // ADC_DBG_VOTE_ENUM forces the enumeration fallback (tests); L1 > 127 takes it always (the support counts may wrap)
+    const int force_enum = (P.dbg & 2) || L1 > 127 ? 1 : 0;
+    if (dm.D > 254 || L1 > 127) launch_scan_push<true>(P, w, L1, force_enum, st);
+    else                        launch_scan_push<false>(P, w, L1, force_enum, st);
+    *launches += 5;
+    adc_launch_build_lists(P, w, st, launches);
 }

@@ -539,8 +539,10 @@ int adc_debug_run(adc_engine* e, const uint8_t* img_left, const uint8_t* img_rig
 int adc_debug_run_cost(adc_engine* e, const uint8_t* img_left, const uint8_t* img_right,
                        const void* cost, int32_t layout, int32_t dtype, int32_t last_stage);
 /* region-voting statistics of pair 0 of the last run: out[0],out[1] = remaining mismatch / occlusion
- * list sizes, out[2] = fixed-point rounds, out[3] = vote evaluations, out[12..15] = microseconds one warp spent
- * evaluating / waiting at round barriers / committing / compacting lists */
+ * list sizes, out[2] = fixed-point rounds, out[3] = vote evaluations, out[4..8] = microseconds spent building the
+ * adjacency lists / in the whole voting kernel / deriving / pushing / collecting, out[9] = forward-list entries
+ * reserved, out[10],out[11] = voting list sizes, out[12] = vote changes, out[13] = 1 when the adjacency lists were
+ * used (0: the inverse regions were enumerated), out[14] = adjacency entries, out[15] = forward-list room */
 int adc_debug_counters(adc_engine* e, int32_t out[16]);
 /* returns the tap's size in bytes (also when dst is NULL or cap is too small), 0 on error */
 size_t adc_debug_get(adc_engine* e, int32_t tap, void* dst, size_t cap);

@@ -54,12 +54,13 @@ CASES = [
     (80, 60, 32, {"min_disparity": 2, "max_disparity": 34}, 31),     # dmin > 0
     (80, 60, 32, {"min_disparity": -4, "max_disparity": 28}, 32),    # negative dmin
     (200, 40, 200, {}, 13),         # a whole warp per line
-    (300, 24, 256, {}, 14),         # the largest range: 8 WTA chunks, voting with int state (D > 254: k_region_voting_global)
-    (64, 40, 255, {}, 15),          # D = 255 (padded to 256), same voting path
+    (300, 24, 256, {}, 14),         # the largest range: 8 WTA chunks, WIDE voting (16-bit votes, one count per word)
+    (64, 40, 255, {}, 15),          # D = 255 (padded to 256), WIDE voting
     (90, 200, 16, {"cross_L1": 70, "cross_L2": 30, "cross_t1": 300, "cross_t2": 300}, 16),   # arms never stop on colour: cross
     #                                 regions of up to 141 rows (the voting scan works in 96-row chunks), 141-tap windows
-    (60, 300, 16, {"cross_L1": 130, "cross_L2": 17, "cross_t1": 300, "cross_t2": 300}, 17),  # L1 > 127: byte-state pull voting
-    #                                 (k_region_voting_bytes), fused aggregation with a larger shared-memory budget
+    (60, 300, 16, {"cross_L1": 130, "cross_L2": 17, "cross_t1": 300, "cross_t2": 300}, 17),  # L1 > 127: WIDE voting that
+    #                                 enumerates (regions of more than 65535 pixels), fused aggregation with a larger
+    #                                 shared-memory budget
     (700, 20, 12, {}, 18),          # a long row: the horizontal double pass of the aggregation cut into segments
     (33, 21, 5, {}, 19),            # D < 8: a single padded quad pair per pixel
 ]
@@ -207,11 +208,12 @@ def test_alternate_code_paths(flag, cone):
     DBG_VOTE_GLOBAL_STATE  its per-slot state in global instead of shared memory (more than 32768 pending pixels);
     DBG_NO_RAY_TABLE       interpolation rays evaluated in double per step (image sizes for which the integer ray table is
                            not exact);
-    DBG_UNFUSED_AGG        the eight single aggregation passes through the whole pipeline (arms too long for the fused plan)."""
+    DBG_UNFUSED_AGG        the eight single aggregation passes through the whole pipeline (arms too long for the fused plan).
+    The 64x40 pair with D = 255 (2439 pending pixels) takes the voting kernel's WIDE instantiation."""
     import adcensus_b200 as A
     fl = getattr(A.engine, flag)
     cases = [cone + (64,)]
-    for (w, h, D, seed) in ((120, 90, 48, 3), (97, 61, 24, 5)):
+    for (w, h, D, seed) in ((120, 90, 48, 3), (97, 61, 24, 5), (64, 40, 255, 15)):
         l, r = T.synthetic_pair(w, h, D, seed)
         cases.append((l, r, D))
     for left, right, D in cases:

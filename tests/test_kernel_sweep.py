@@ -1,7 +1,8 @@
 """Parity sweep over the kernel instantiations and launch-plan branches that the disparity range and the shape select.
 
 The scanline, fused-cost and fused-aggregation kernels are templates whose instantiation follows from the disparity
-range, and their launch plans (adcensus_b200/csrc/so_plan.h, ca_plan.h) cut rows and columns differently per shape.
+range (the voting kernels' also from the arm length), and their launch plans (adcensus_b200/csrc/so_plan.h, ca_plan.h)
+cut rows and columns differently per shape.
 
 CPU: the instantiations compiled into the library (cuobjdump -symbols), the instantiations every GPU case of this file
 reaches by the launch rules, and the assertion that together they reach every one; the plan branch each plan-branch case
@@ -138,12 +139,14 @@ def so_lanes_per_line(Dp):
 
 
 def reached(c, plans):
-    """The instantiations of the five templates one batched run of case c launches, by the launch rules of
-    k_aggregate.cu, k_cost.cu and k_scanline.cu (a run that matches, so every stage runs, with the fused aggregation):
+    """The instantiations of the seven templates one batched run of case c launches, by the launch rules of
+    k_aggregate.cu, k_cost.cu, k_scanline.cu and k_vote.cu (a run that matches, so every stage runs, with the fused
+    aggregation):
       cost:      k_cost_arm_sum_h<D == Dp, ca_plan.qc> where ca_plan is ok, else k_cost_volume<D == Dp>;
       axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok (the tensor maps are encoded for both) and,
                  on rows, the row is one segment; else k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC);
-      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp)."""
+      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp);
+      voting:    k_vote_scan<WIDE> and k_vote_push<WIDE>, WIDE iff D > 254 or L1 > 127."""
     out = set()
     exact = c.D == c.Dp
     ca = plans.ca(c)
@@ -159,6 +162,9 @@ def reached(c, plans):
     lps = so_lanes_per_line(c.Dp)
     K = -(-c.Dp // lps)
     out.add(("k_scanline", K, lps, c.D == K * lps))
+    wide = c.D > 254 or min(c.L1, 255) > 127
+    out.add(("k_vote_scan", wide))
+    out.add(("k_vote_push", wide))
     return out
 
 
@@ -169,11 +175,13 @@ _SYMBOLS = {
     "k_cost_arm_sum_h": re.compile(r"_Z16k_cost_arm_sum_hILb([01])ELi(\d+)EE"),
     "k_arm_sum2t": re.compile(r"_Z11k_arm_sum2tILb([01])ELi(\d+)EE"),
     "k_arm_sum2": re.compile(r"_Z10k_arm_sum2ILb([01])ELi(\d+)EE"),
+    "k_vote_scan": re.compile(r"_Z11k_vote_scanILb([01])EE"),
+    "k_vote_push": re.compile(r"_Z11k_vote_pushILb([01])EE"),
 }
 
 
 def library_instantiations():
-    """{(template, args...)} of the five templates, read from the built library's device symbols."""
+    """{(template, args...)} of the seven templates, read from the built library's device symbols."""
     from adcensus_b200.build import build_library
     cuobjdump = Path(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")).parent / "cuobjdump"
     if not cuobjdump.exists():
@@ -192,8 +200,8 @@ def library_instantiations():
 
 
 def test_every_instantiation_is_reached(plans):
-    """Every instantiation of k_scanline, k_cost_volume, k_cost_arm_sum_h, k_arm_sum2t and k_arm_sum2 in the library is
-    launched by at least one GPU case of this file; one that no case reaches fails here."""
+    """Every instantiation of k_scanline, k_cost_volume, k_cost_arm_sum_h, k_arm_sum2t, k_arm_sum2, k_vote_scan and
+    k_vote_push in the library is launched by at least one GPU case of this file; one that no case reaches fails here."""
     lib = library_instantiations()
     assert sum(1 for i in lib if i[0] == "k_scanline") == 32, sorted(lib)
     assert {i[0] for i in lib} == set(_SYMBOLS), sorted(lib)

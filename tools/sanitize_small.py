@@ -12,7 +12,9 @@ cases = [(97, 61, 24, 2, {}), (130, 70, 37, 3, {}), (80, 60, 32, 10, {"do_discon
          (80, 60, 32, 31, {"min_disparity": 2, "max_disparity": 34}),
          (70, 44, 64, 4, {}),        # D = 64: eight quads per CTA (compile-time strides), 8 lanes per scanline
          (150, 40, 130, 12, {}),     # 16 lanes per scanline, padded disparity stride
-         (600, 16, 12, 18, {})]      # a row cut into segments by the fused horizontal double pass
+         (600, 16, 12, 18, {}),      # a row cut into segments by the fused horizontal double pass
+         (64, 40, 255, 15, {}),      # D = 255: the WIDE voting kernels (16-bit votes, one count per histogram word)
+         (60, 300, 16, 17, {"cross_L1": 130, "cross_L2": 17, "cross_t1": 300, "cross_t2": 300})]   # L1 > 127: WIDE, enumerating
 for (w, h, D, seed, over) in cases:
     left, right = T.synthetic_pair(w, h, D, seed)
     kw = dict(max_disparity=D); kw.update(over)
