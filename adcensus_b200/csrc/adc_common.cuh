@@ -85,8 +85,9 @@ inline int adc_sm_count() {
     return n > 0 ? n : 1;
 }
 
-// TMA descriptors (CUtensorMap, 128 bytes each) of a lane's two cost volumes for the two axes of the fused aggregation kernel
-struct alignas(64) AdcArmTmaps { unsigned char map[2][2][128]; int ok; };
+// TMA descriptors (CUtensorMap, 128 bytes each) of a lane's two cost volumes for the axes of the double passes that take
+// the TMA form (arm_sum2_form, ca_plan.h); the other axis's are zero and never read
+struct alignas(64) AdcArmTmaps { unsigned char map[2][2][128]; };
 // TMA descriptors of the scanline passes, per axis (0: +-x, 1: +-y): the two volumes and the penalty records, with the boxes
 // of that axis's launch plan (T steps per ring slot, NS slots per warp, dynamic shared memory per CTA; so_plan.h)
 struct alignas(64) AdcSoTmaps { unsigned char cost[2][2][128]; unsigned char rec[2][128]; int T[2], NS[2]; unsigned smem[2]; };
@@ -105,7 +106,7 @@ struct AdcWave {            // device pointers of one wave (S pairs)
     unsigned long long* census; // [S][2][N]
     float* volA; float* volB;
     uchar4* arms;
-    const AdcArmTmaps* arm_tm;   // host memory, owned by the lane (NULL: the fused kernel loads its source with LDG)
+    const AdcArmTmaps* arm_tm;   // host memory, owned by the lane: tensor maps of the aggregation double passes
     unsigned* arm_rec;      // [S][window records of both axes] which of a group's four outputs takes which tap (k_aggregate.cu)
     uint16_t* sup_h; uint16_t* sup_v;
     uint8_t* dmap;          // [S][4][N]: 0 = left-horizontal, 1 = left-vertical, 2 = right-horizontal, 3 = right-vertical
@@ -191,9 +192,9 @@ void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsi
 void adc_launch_arm_sum(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int dir,
                         const uint16_t* sup, cudaStream_t st, unsigned long long* launches);
 // two consecutive passes along the same axis (second pass of an iteration, divided by `sup_mid`, then the first pass of the
-// next iteration) with the intermediate kept in shared memory; false = not applicable for these parameters, nothing launched
-bool adc_arm_sum2_available(const AdcParams& P);
-bool adc_launch_arm_sum2(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int dir,
+// next iteration) with the intermediate kept in shared memory, in the form arm_sum2_form picks (ca_plan.h); src = w.volA
+// or w.volB
+void adc_launch_arm_sum2(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int dir,
                          const uint16_t* sup_mid, cudaStream_t st, unsigned long long* launches);
 // the AD-census cost computed in place of the cost volume and summed as the first horizontal pass (no division) into
 // `dst`; cost_out (nullable) also receives the cost volume, padding disparities included, as adc_launch_cost writes it.
@@ -202,7 +203,8 @@ bool adc_cost_arm_sum_h_available(const AdcParams& P);
 bool adc_launch_cost_arm_sum_h(const AdcParams& P, const AdcWave& w, float* dst, float* cost_out, cudaStream_t st,
                                unsigned long long* launches);
 size_t adc_arm_rec_bytes(const AdcDims& dm, int L1);   // window records of one pair
-bool adc_arm_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, AdcArmTmaps* out);   // false: TMA path not available
+// tensor maps of the double passes' TMA-form axes over a lane of capacity S (false: they cannot be encoded)
+bool adc_arm_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, AdcArmTmaps* out);
 size_t adc_arm_overread_floats(const AdcDims& dm);     // padding the arena keeps behind the two volumes
 void adc_launch_so_bitrows(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 size_t adc_so_rec_bytes(const AdcDims& dm);

@@ -70,7 +70,7 @@ struct Lane {
     cudaEvent_t ev_in_free = nullptr;  // the H2D of the latest wave has consumed the staging-in buffer
     void* arena = nullptr;
     AdcWave w{};                       // device pointers, capacity S pairs
-    AdcArmTmaps arm_tm{};              // TMA descriptors of this lane's volumes (fused aggregation kernel)
+    AdcArmTmaps arm_tm{};              // TMA descriptors of this lane's volumes (aggregation double passes)
     AdcSoTmaps so_tm{};                // TMA descriptors of this lane's volumes and penalty records (scanline passes)
     uint8_t* pin_in = nullptr;         // [S][2][N*3] pinned staging (pageable callers only)
     float* pin_out = nullptr;          // [S][N]
@@ -97,7 +97,7 @@ struct adc_engine {
     double* d_rays = nullptr;  // [32]: sin[16], cos[16]
     short2* d_ray_off = nullptr;  // [16][max_search] integer ray offsets, when verified exact for this image size
     bool pipelined = false;            // adc_set_pipelined: batch calls do not join the caller's stream themselves
-    bool agg_fused = false;            // same-axis aggregation passes of neighbouring iterations run as one kernel (k_arm_sum2)
+    bool agg_fused = false;            // same-axis aggregation passes of neighbouring iterations run as one kernel (k_arm_sum2t / k_arm_sum2)
     unsigned long long launches = 0;
     float stage_ms[6] = {0, 0, 0, 0, 0, 0};
     cudaEvent_t ev_stage[8] = {};
@@ -418,10 +418,9 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
         } else {
             adc_launch_arm_sum(P, w, B, A, 0, nullptr, st, L);                   // it 0: H
         }
-        if (!adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L) ||               // it 0: V /   + it 1: V
-            !adc_launch_arm_sum2(P, w, B, A, 0, w.sup_v, st, L) ||               // it 1: H /   + it 2: H
-            !adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L))                 // it 2: V /   + it 3: V
-            return fail(ADC_ERR_UNSUPPORTED, "fused aggregation pass not applicable");
+        adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L);                      // it 0: V /   + it 1: V
+        adc_launch_arm_sum2(P, w, B, A, 0, w.sup_v, st, L);                      // it 1: H /   + it 2: H
+        adc_launch_arm_sum2(P, w, A, B, 1, w.sup_h, st, L);                      // it 2: V /   + it 3: V
         adc_launch_arm_sum(P, w, B, A, 0, w.sup_v, st, L);                       // it 3: H /
         export_vol(ADC_VOL_AGGR, A);
         e->dbg_aggr = A;
@@ -1093,7 +1092,7 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
     }
     e->S = S;
     e->cfg.wave_pairs = S; e->cfg.lanes = nl;
-    e->agg_fused = adc_arm_sum2_available(e->P) && !(e->cfg.debug_flags & ADC_DBG_UNFUSED_AGG);
+    e->agg_fused = !(e->cfg.debug_flags & ADC_DBG_UNFUSED_AGG);
 
     int rc = upload_tables(e);
     if (rc) return bail(rc);
@@ -1109,7 +1108,9 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
         const size_t bytes = carve_lane(nullptr, e->P.dm, e->P.L1, S, nullptr);
         if (cudaMalloc(&ln.arena, bytes) != cudaSuccess) { cudaGetLastError(); return bail(fail(ADC_ERR_NOMEM, "device arena of %zu bytes", bytes)); }
         carve_lane(ln.arena, e->P.dm, e->P.L1, S, &ln.w);
-        if (adc_arm_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, &ln.arm_tm)) ln.w.arm_tm = &ln.arm_tm;
+        if (!adc_arm_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, &ln.arm_tm))
+            return bail(fail(ADC_ERR_CUDA, "adc_create: the aggregation passes' tensor maps could not be encoded (cuTensorMapEncodeTiled)"));
+        ln.w.arm_tm = &ln.arm_tm;
         if (!adc_so_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, ln.w.so_rec, &ln.so_tm))
             return bail(fail(ADC_ERR_CUDA, "adc_create: the scanline passes' tensor maps could not be encoded (cuTensorMapEncodeTiled)"));
         ln.w.so_tm = &ln.so_tm;
@@ -1609,8 +1610,8 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
             case 3: if (adc_launch_scanline(P, w, w.volA, w.volB, 1, 0, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "scanline"); bytes = 2 * V + 6 * N; break;
             case 4: if (adc_launch_scanline(P, w, w.volA, w.volB, 0, 1, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "scanline"); bytes = 2 * V + 6 * N; break;
             case 5: if (adc_launch_wta(P, w, w.volA, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "wta"); bytes = V + 8 * N; break;
-            case 6: if (!adc_launch_arm_sum2(P, w, w.volA, w.volB, 1, w.sup_h, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "fused vertical arm sums not applicable"); bytes = 2 * V + 6 * N; break;
-            case 7: if (!adc_launch_arm_sum2(P, w, w.volA, w.volB, 0, w.sup_v, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "fused horizontal arm sums not applicable"); bytes = 2 * V + 6 * N; break;
+            case 6: adc_launch_arm_sum2(P, w, w.volA, w.volB, 1, w.sup_h, ln.st, &e->launches); bytes = 2 * V + 6 * N; break;
+            case 7: adc_launch_arm_sum2(P, w, w.volA, w.volB, 0, w.sup_v, ln.st, &e->launches); bytes = 2 * V + 6 * N; break;
             case 8: adc_launch_arm_sum(P, w, w.volA, w.volB, 0, w.sup_v, ln.st, &e->launches); bytes = 2 * V + 6 * N; break;
             case 9: adc_launch_arm_sum(P, w, w.volA, w.volB, 1, nullptr, ln.st, &e->launches); bytes = 2 * V + 4 * N; break;
             case 10:    // source: volA's bytes taken as the wave's raw volumes (the kernel's traffic does not depend on the values)
@@ -1652,7 +1653,7 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
             case 15:    // the cost computed from the wave's images and census words, summed as iteration 0's H pass into volA
                 if (!adc_launch_cost_arm_sum_h(P, w, w.volA, nullptr, ln.st, &e->launches))
                     return fail(ADC_ERR_UNSUPPORTED, "fused cost and horizontal arm sums not applicable");
-                bytes = V + 24 * N + (double)P.dm.H * ((P.dm.W + 3) / 4) * arm_rec_words(P.L1) * 4.0;   // + horizontal records
+                bytes = V + 24 * N + (double)arm_line_rec(P.dm.W, P.dm.H, 1, 0) * arm_rec_words(P.L1) * 4.0;   // + horizontal records (all before the vertical axis's first)
                 break;
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);
         }

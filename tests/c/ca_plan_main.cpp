@@ -2,8 +2,10 @@
 // Usage: ca_plan_main W Dp L1   ->   the fused cost + first horizontal arm sum:
 //                                    "qc Ls nseg nchunks gm lpc threads smem ok budget" then one "s0 s1 m0 m1" line per segment
 //        ca_plan_main arm W H Dp L1   ->   the double passes, one line per axis (dir 0 = rows, then dir 1 = columns):
-//                                    "dir t_ok t_qc t_Ls t_nseg t_nchunks t_lpc t_threads t_smem  ldg_ok ldg_qc_log2 ldg_Ls ldg_nseg ldg_smem"
-//                                    (t_*: k_arm_sum2t's plan, ldg_*: k_arm_sum2's)
+//                                    "dir t_ok t_qc t_Ls t_nseg t_nchunks t_lpc t_threads t_smem  ldg_qc_log2 ldg_Ls ldg_nseg ldg_smem
+//                                     form smem_attr"
+//                                    (t_*: k_arm_sum2t's plan, ldg_*: k_arm_sum2's, form: the kernel arm_sum2_form picks,
+//                                     A2_TMA or A2_LDG, smem_attr: the dynamic shared memory both are launched under)
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -16,8 +18,8 @@ int main(int argc, char** argv) {
         for (int dir = 0; dir < 2; dir++) {
             const ArmSum2tPlan t = plan_arm_sum2t(W, H, Dp, L1, dir);
             const ArmSum2Plan g = plan_arm_sum2(W, H, Dp, L1, dir);
-            printf("%d %d %d %d %d %d %d %d %zu %d %d %d %d %zu\n", dir, (int)t.ok, t.qc, t.Ls, t.nseg, t.nchunks, t.lpc,
-                   t.threads, t.smem, (int)g.ok, g.qc_log2, g.Ls, g.nseg, g.smem);
+            printf("%d %d %d %d %d %d %d %d %zu %d %d %d %zu %d %d\n", dir, (int)t.ok, t.qc, t.Ls, t.nseg, t.nchunks, t.lpc,
+                   t.threads, t.smem, g.qc_log2, g.Ls, g.nseg, g.smem, arm_sum2_form(W, H, Dp, L1, dir), A2_SMEM_ATTR);
         }
         return 0;
     }

@@ -126,7 +126,7 @@ class Plans:
         for line in self._run("ca_plan_main", "arm", c.W, c.H, c.Dp, c.L1).strip().split("\n"):
             v = list(map(int, line.split()))
             out.append(dict(zip(("dir", "t_ok", "t_qc", "t_Ls", "t_nseg", "t_nchunks", "t_lpc", "t_threads", "t_smem",
-                                 "ldg_ok", "ldg_qc_log2", "ldg_Ls", "ldg_nseg", "ldg_smem"), v)))
+                                 "ldg_qc_log2", "ldg_Ls", "ldg_nseg", "ldg_smem", "form", "smem_attr"), v)))
         return out
 
     def so(self, c, axis):
@@ -138,13 +138,17 @@ def so_lanes_per_line(Dp):
     return 8 if Dp <= 64 else (16 if Dp <= 128 else 32)
 
 
+A2_TMA, A2_LDG = 1, 0     # the forms arm_sum2_form (ca_plan.h) picks
+
+
 def reached(c, plans):
     """The instantiations of the seven templates one batched run of case c launches, by the launch rules of
     k_aggregate.cu, k_cost.cu, k_scanline.cu and k_vote.cu (a run that matches, so every stage runs, with the fused
     aggregation):
       cost:      k_cost_arm_sum_h<D == Dp, ca_plan.qc> where ca_plan is ok, else k_cost_volume<D == Dp>;
-      axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok (the tensor maps are encoded for both) and,
-                 on rows, the row is one segment; else k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC);
+      axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok and, on rows, the row is one segment; else
+                 k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC).  This restates arm_sum2_form, and the form the plan
+                 executable prints for the axis must agree with it;
       scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp);
       voting:    k_vote_scan<WIDE> and k_vote_push<WIDE>, WIDE iff D > 254 or L1 > 127."""
     out = set()
@@ -152,10 +156,13 @@ def reached(c, plans):
     ca = plans.ca(c)
     out.add(("k_cost_arm_sum_h", exact, ca["qc"]) if ca["ok"] else ("k_cost_volume", exact))
     arm = plans.arm(c)
-    assert arm[0]["ldg_ok"] and arm[1]["ldg_ok"], (c.name, arm)       # the fused aggregation runs on every shape
     tmaps = bool(arm[0]["t_ok"] and arm[1]["t_ok"])
     for a in arm:
-        if tmaps and not (a["dir"] == 0 and a["t_nseg"] > 1):
+        # the fused aggregation runs on every shape: both plans fit the shared memory the passes are launched under
+        assert a["t_smem"] <= a["smem_attr"] and a["ldg_smem"] <= a["smem_attr"], (c.name, a)
+        tma = tmaps and not (a["dir"] == 0 and a["t_nseg"] > 1)
+        assert a["form"] == (A2_TMA if tma else A2_LDG), (c.name, a)
+        if tma:
             out.add(("k_arm_sum2t", a["dir"] == 1, a["t_qc"]))
         else:
             out.add(("k_arm_sum2", a["dir"] == 1, 8 if a["ldg_qc_log2"] == 3 else 0))
