@@ -719,7 +719,9 @@ MatchReq output_req(const void* cost, int cost_layout, int cost_dtype, const flo
 // The rules of an image descriptor that need no image size (adc_match_images*, checked before the engine).
 int check_image_desc(const char* fn, const adc_image_desc* img) {
     if (!img) return ADC_OK;
-    if (img->format < ADC_IMG_BGR || img->format > ADC_IMG_RGB_PLANAR) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
+    const bool known = (img->format >= ADC_IMG_BGR && img->format <= ADC_IMG_RGB_PLANAR) ||
+                       (img->format >= ADC_IMG_BAYER_RGGB && img->format <= ADC_IMG_BAYER_GBRG);
+    if (!known) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
     if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
     if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
     if (img->plane_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is negative", fn, (long long)img->plane_pitch);

@@ -9,29 +9,12 @@
 // for planar images); neighbouring lanes take neighbouring groups, so a warp's loads cover one contiguous stretch of a
 // row (of each plane): coalesced along x.  Every pixel is loaded by exactly one thread, alpha bytes are never loaded, and
 // nothing past the last pixel of the last row is touched.  All source offsets are 64-bit.
+// The kernel template (k_image_ingest) is in k_image.cuh; this file instantiates it for the six formats above, and
+// k_bayer.cu for the Bayer mosaics.
 #include <algorithm>
 
 #include "adc_common.cuh"
 #include "k_image.cuh"
-
-template <int F>
-__global__ void __launch_bounds__(II_THREADS)
-k_image_ingest(int W, int N, const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, long long row_pitch,
-               long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
-    const int view = blockIdx.y, pair = blockIdx.z;
-    const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
-    uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
-    store_view_bgr(o, N, W, blockIdx.x,
-                   [&](int, int y, int x) { return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch); });
-}
-
-template <int F>
-static void launch_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                         uint8_t* bgr, cudaStream_t st) {
-    const int groups = dm.N / 4;
-    dim3 grid(std::max(1, (groups + II_GROUPS - 1) / II_GROUPS), 2, S);
-    k_image_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.N, left, right, g.row_pitch, g.plane_pitch, g.image_stride, bgr);
-}
 
 void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
                              const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches) {
@@ -41,6 +24,9 @@ void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t
         case ADC_IMG_BGRA: launch_image<ADC_IMG_BGRA>(P.dm, w.S, left, right, g, w.bgr, st); break;
         case ADC_IMG_RGBA: launch_image<ADC_IMG_RGBA>(P.dm, w.S, left, right, g, w.bgr, st); break;
         case ADC_IMG_GRAY: launch_image<ADC_IMG_GRAY>(P.dm, w.S, left, right, g, w.bgr, st); break;
+        case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
+            adc_launch_bayer_image(P.dm, w.S, left, right, g, w.bgr, st);
+            break;
         default: launch_image<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, w.bgr, st); break;
     }
     ++*launches;
@@ -50,6 +36,6 @@ int adc_image_bytes_per_pixel(int format) {
     switch (format) {
         case ADC_IMG_BGR: case ADC_IMG_RGB: return 3;
         case ADC_IMG_BGRA: case ADC_IMG_RGBA: return 4;
-        default: return 1;   // gray, and each plane of a planar image
+        default: return 1;   // gray, Bayer, and each plane of a planar image
     }
 }

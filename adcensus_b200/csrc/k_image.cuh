@@ -1,6 +1,6 @@
 // k_image.cuh -- the pieces the two image ingestion kernels share (k_image.cu: images in any format / pitch,
-// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers and the store scheme that
-// writes one view's packed BGR.
+// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the Bayer demosaic and the
+// store scheme that writes one view's packed BGR.
 //
 // The output of one view is a contiguous run of 3*N bytes.  A thread takes four consecutive pixels of it at a time:
 // 12 bytes, stored as three 32-bit words.  The view's run starts at an arbitrary byte phase (3*N*(2*pair + view) mod
@@ -10,7 +10,10 @@
 
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "../../include/adcensus_b200.h"
+#include "adc_common.cuh"
 
 // One pixel of a format as B | G << 8 | R << 16.  `row` points at the pixel row (of the first plane).  Alpha bytes are
 // never loaded.  The loads are single bytes because the caller's bases and pitches may have any alignment.
@@ -48,6 +51,57 @@ template <> struct ImgIn<ADC_IMG_RGB_PLANAR> {
         return __ldg(p + 2 * plane) | (unsigned)__ldg(p + plane) << 8 | (unsigned)__ldg(p) << 16;
     }
 };
+
+// Bayer mosaics (ADC_IMG_BAYER_*): the demosaiced pixel (x, y) of a w x h mosaic at src as B | G << 8 | R << 16,
+// equal to cv::cvtColor(mosaic, COLOR_Bayer*2BGR) (the rule is in include/adcensus_b200.h).  Frames narrower or lower
+// than 3 pixels are all zero.  The position is clamped to [1, w - 2] x [1, h - 2] first, which is the border rule and
+// also keeps all nine loads of the 3x3 neighbourhood inside the frame, so none of them needs a predicate.  The colour of
+// a site comes from the parities of x and y against the R site of the pattern (bit 0: its column, bit 1: its row).
+__host__ __device__ constexpr bool is_bayer(int F) { return F >= ADC_IMG_BAYER_RGGB && F <= ADC_IMG_BAYER_GBRG; }
+__host__ __device__ constexpr int bayer_r_site(int F) {
+    return F == ADC_IMG_BAYER_RGGB ? 0 : F == ADC_IMG_BAYER_GRBG ? 1 : F == ADC_IMG_BAYER_GBRG ? 2 : 3;
+}
+
+// The interior rule at (x, y) from the raw value c there and its eight neighbours.
+template <int F>
+static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n, int s, int wv, int e, int nw, int ne,
+                                                      int sw, int se) {
+    const int cross = (n + s + wv + e + 2) >> 2, diag = (nw + ne + sw + se + 2) >> 2;
+    const int hor = (wv + e + 1) >> 1, ver = (n + s + 1) >> 1;
+    const int dx = (x ^ bayer_r_site(F)) & 1, dy = (y ^ bayer_r_site(F) >> 1) & 1;
+    int r, g, b;
+    if (dx == dy) {   // an R (dy = 0) or B (dy = 1) site
+        g = cross;
+        r = dy ? diag : c;
+        b = dy ? c : diag;
+    } else {          // a G site in an R row (dy = 0: R left and right, B above and below) or in a B row
+        g = c;
+        r = dy ? ver : hor;
+        b = dy ? hor : ver;
+    }
+    return (unsigned)b | (unsigned)g << 8 | (unsigned)r << 16;
+}
+
+template <int F>
+static __device__ __forceinline__ unsigned bayer_px(const uint8_t* src, long long row_pitch, int w, int h, int x, int y) {
+    if (w < 3 || h < 3) return 0u;
+    x = min(max(x, 1), w - 2);
+    y = min(max(y, 1), h - 2);
+    const uint8_t* m = src + (long long)y * row_pitch + x;
+    const uint8_t* u = m - row_pitch;
+    const uint8_t* d = m + row_pitch;
+    return bayer_rule<F>(x, y, __ldg(m), __ldg(u), __ldg(d), __ldg(m - 1), __ldg(m + 1), __ldg(u - 1), __ldg(u + 1),
+                         __ldg(d - 1), __ldg(d + 1));
+}
+
+// Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the one-pixel readers above, or the
+// demosaic of a Bayer mosaic.
+template <int F>
+static __device__ __forceinline__ unsigned view_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int w,
+                                                   int h, int x, int y) {
+    if constexpr (is_bayer(F)) return bayer_px<F>(src, row_pitch, w, h, x, y);
+    else return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch);
+}
 
 #define II_THREADS 256
 #define II_GROUPS 1024   // four-pixel groups per CTA
@@ -87,3 +141,110 @@ __device__ __forceinline__ void store_view_bgr(uint8_t* __restrict__ o, int N, i
         }
     }
 }
+
+// ---- the kernels (instantiated per format in k_image.cu and k_rectify.cu, the Bayer formats in k_bayer.cu) ----
+
+// k_image.cu: pixel (x, y) of the view, read in place.
+template <int F>
+__global__ void __launch_bounds__(II_THREADS)
+k_image_ingest(int W, int H, int N, const uint8_t* __restrict__ left, const uint8_t* __restrict__ right,
+               long long row_pitch, long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
+    const int view = blockIdx.y, pair = blockIdx.z;
+    const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
+    uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
+    store_view_bgr(o, N, W, blockIdx.x,
+                   [&](int, int y, int x) { return view_px<F>(src, row_pitch, plane_pitch, W, H, x, y); });
+}
+
+template <int F>
+static void launch_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                         uint8_t* bgr, cudaStream_t st) {
+    const int groups = dm.N / 4;
+    dim3 grid(std::max(1, (groups + II_GROUPS - 1) / II_GROUPS), 2, S);
+    k_image_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.H, dm.N, left, right, g.row_pitch, g.plane_pitch, g.image_stride, bgr);
+}
+
+// One output pixel: the bilinear blend of the raw view `src` at map entry m, as B | G << 8 | R << 16.
+template <int F>
+static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* src, int sw, int sh, long long row_pitch,
+                                                        long long plane_pitch) {
+    const int x0 = (short)(m.x & 0xffffu), y0 = (short)(m.x >> 16);
+    const int ax = m.y & 31, ay = m.y >> 5;
+    unsigned s[4];   // (x0, y0), (x0 + 1, y0), (x0, y0 + 1), (x0 + 1, y0 + 1)
+    if constexpr (is_bayer(F)) {
+        // each neighbour inside the frame is demosaiced from its clamped 3x3 neighbourhood.  When no clamp applies
+        // (1 <= x0, x0 + 1 <= sw - 2, likewise y0), the four neighbourhoods are one 4x4 window, loaded once.
+        if (x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
+            int v[4][4];
+            const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch + (x0 - 1);
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) v[i][j] = __ldg(r0 + i * row_pitch + j);
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int dx = k & 1, dy = k >> 1;
+                s[k] = bayer_rule<F>(x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
+                                     v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int x = x0 + (k & 1), y = y0 + (k >> 1);
+                s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? bayer_px<F>(src, row_pitch, sw, sh, x, y)
+                                                                                : 0u;
+            }
+        }
+    } else if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
+        const uint8_t* r0 = src + y0 * row_pitch;
+        s[0] = ImgIn<F>::px(r0, x0, plane_pitch);
+        s[1] = ImgIn<F>::px(r0, x0 + 1, plane_pitch);
+        s[2] = ImgIn<F>::px(r0 + row_pitch, x0, plane_pitch);
+        s[3] = ImgIn<F>::px(r0 + row_pitch, x0 + 1, plane_pitch);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int x = x0 + (k & 1), y = y0 + (k >> 1);
+            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? ImgIn<F>::px(src + y * row_pitch, x, plane_pitch) : 0u;
+        }
+    }
+    const int w[4] = {(32 - ax) * (32 - ay), ax * (32 - ay), (32 - ax) * ay, ax * ay};
+    unsigned out = 0;
+#pragma unroll
+    for (int c = 0; c < 24; c += 8) {
+        int v = 512;
+#pragma unroll
+        for (int k = 0; k < 4; k++) v += w[k] * (int)(s[k] >> c & 255u);
+        out |= (unsigned)(v >> 10) << c;
+    }
+    return out;
+}
+
+template <int F>
+__global__ void __launch_bounds__(II_THREADS)
+k_rectify_ingest(int W, int N, int S, int sw, int sh, const uint2* __restrict__ map_l, const uint2* __restrict__ map_r,
+                 const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, long long row_pitch,
+                 long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
+    const int pair = blockIdx.x % S, tile = blockIdx.x / S, view = blockIdx.y;
+    const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
+    const uint2* map = view ? map_r : map_l;
+    uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
+    store_view_bgr(o, N, W, tile, [&](int p, int, int) {
+        return rectified_px<F>(__ldg(map + p), src, sw, sh, row_pitch, plane_pitch);
+    });
+}
+
+template <int F>
+static void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                           const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
+    const int tiles = std::max(1, (dm.N / 4 + II_GROUPS - 1) / II_GROUPS);
+    dim3 grid((unsigned)(tiles * S), 2);
+    k_rectify_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.N, S, r.src_w, r.src_h, r.map[0], r.map[1], left, right,
+                                                     g.row_pitch, g.plane_pitch, g.image_stride, bgr);
+}
+
+// The Bayer instantiations of both kernels (k_bayer.cu), for g.format one of ADC_IMG_BAYER_*.
+void adc_launch_bayer_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                            uint8_t* bgr, cudaStream_t st);
+void adc_launch_bayer_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                              const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);

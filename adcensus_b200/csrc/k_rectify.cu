@@ -11,7 +11,8 @@
 //     [-2^20, 2^20] has x0 = +-32767 / -32768 after the int16 saturation, and since src_width, src_height <= 32767
 //     both neighbours x0 and x0 + 1 lie outside the frame: the border value 0 whichever way X saturated.
 //
-// Per wave: k_rectify_ingest<F> makes one launch over the wave's pairs x 2 views.  For each output pixel it gathers
+// Per wave: k_rectify_ingest<F> (k_image.cuh; instantiated here for the six formats of k_image.cu, in k_bayer.cu for
+// the Bayer mosaics) makes one launch over the wave's pairs x 2 views.  For each output pixel it gathers
 // the four neighbours of (x0, y0) from the raw view through the format readers of k_image.cuh, weights them
 // (32 - ax | ax) * (32 - ay | ay), and writes (sum + 512) >> 10 per channel with the store scheme of k_image.cuh.  When
 // all four neighbours lie inside the frame (0 <= x0 < src_width - 1, 0 <= y0 < src_height - 1; never for a frame one
@@ -66,61 +67,6 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
     else k_remap_convert_fixed<<<grid, RC_THREADS, 0, st>>>(dm.W, dm.N, m1, pitch1, m2, pitch2, out);
 }
 
-// One output pixel: the bilinear blend of the raw view `src` at map entry m, as B | G << 8 | R << 16.
-template <int F>
-static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* src, int sw, int sh, long long row_pitch,
-                                                        long long plane_pitch) {
-    const int x0 = (short)(m.x & 0xffffu), y0 = (short)(m.x >> 16);
-    const int ax = m.y & 31, ay = m.y >> 5;
-    unsigned s[4];   // (x0, y0), (x0 + 1, y0), (x0, y0 + 1), (x0 + 1, y0 + 1)
-    if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
-        const uint8_t* r0 = src + y0 * row_pitch;
-        s[0] = ImgIn<F>::px(r0, x0, plane_pitch);
-        s[1] = ImgIn<F>::px(r0, x0 + 1, plane_pitch);
-        s[2] = ImgIn<F>::px(r0 + row_pitch, x0, plane_pitch);
-        s[3] = ImgIn<F>::px(r0 + row_pitch, x0 + 1, plane_pitch);
-    } else {
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const int x = x0 + (k & 1), y = y0 + (k >> 1);
-            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? ImgIn<F>::px(src + y * row_pitch, x, plane_pitch) : 0u;
-        }
-    }
-    const int w[4] = {(32 - ax) * (32 - ay), ax * (32 - ay), (32 - ax) * ay, ax * ay};
-    unsigned out = 0;
-#pragma unroll
-    for (int c = 0; c < 24; c += 8) {
-        int v = 512;
-#pragma unroll
-        for (int k = 0; k < 4; k++) v += w[k] * (int)(s[k] >> c & 255u);
-        out |= (unsigned)(v >> 10) << c;
-    }
-    return out;
-}
-
-template <int F>
-__global__ void __launch_bounds__(II_THREADS)
-k_rectify_ingest(int W, int N, int S, int sw, int sh, const uint2* __restrict__ map_l, const uint2* __restrict__ map_r,
-                 const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, long long row_pitch,
-                 long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
-    const int pair = blockIdx.x % S, tile = blockIdx.x / S, view = blockIdx.y;
-    const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
-    const uint2* map = view ? map_r : map_l;
-    uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
-    store_view_bgr(o, N, W, tile, [&](int p, int, int) {
-        return rectified_px<F>(__ldg(map + p), src, sw, sh, row_pitch, plane_pitch);
-    });
-}
-
-template <int F>
-static void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                           const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
-    const int tiles = std::max(1, (dm.N / 4 + II_GROUPS - 1) / II_GROUPS);
-    dim3 grid((unsigned)(tiles * S), 2);
-    k_rectify_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.N, S, r.src_w, r.src_h, r.map[0], r.map[1], left, right,
-                                                     g.row_pitch, g.plane_pitch, g.image_stride, bgr);
-}
-
 void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
                                const AdcImageGeom& g, const AdcRectGeom& r, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
@@ -129,6 +75,9 @@ void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8
         case ADC_IMG_BGRA: launch_rectify<ADC_IMG_BGRA>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
         case ADC_IMG_RGBA: launch_rectify<ADC_IMG_RGBA>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
         case ADC_IMG_GRAY: launch_rectify<ADC_IMG_GRAY>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
+        case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
+            adc_launch_bayer_rectify(P.dm, w.S, left, right, g, r, w.bgr, st);
+            break;
         default: launch_rectify<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
     }
     ++*launches;

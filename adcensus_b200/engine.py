@@ -90,6 +90,11 @@ IMG_BGR, IMG_RGB, IMG_BGRA, IMG_RGBA, IMG_GRAY, IMG_RGB_PLANAR = 0, 1, 2, 3, 4, 
 IMG_FORMATS = {"bgr": IMG_BGR, "rgb": IMG_RGB, "bgra": IMG_BGRA, "rgba": IMG_RGBA, "gray": IMG_GRAY,
                "rgb_planar": IMG_RGB_PLANAR}
 IMG_CHANNELS = {IMG_BGR: 3, IMG_RGB: 3, IMG_BGRA: 4, IMG_RGBA: 4, IMG_GRAY: 1, IMG_RGB_PLANAR: 1}   # bytes per pixel (plane)
+# Bayer mosaics, 1 byte per pixel, demosaiced as cv2.cvtColor does; the name is the view's own top-left 2x2 block
+# (GenICam BayerRG8 = "bayer_rggb" = OpenCV's legacy COLOR_BayerBG2BGR)
+IMG_BAYER_RGGB, IMG_BAYER_GRBG, IMG_BAYER_BGGR, IMG_BAYER_GBRG = 16, 17, 18, 19
+BAYER_FORMATS = {"bayer_rggb": IMG_BAYER_RGGB, "bayer_grbg": IMG_BAYER_GRBG, "bayer_bggr": IMG_BAYER_BGGR,
+                 "bayer_gbrg": IMG_BAYER_GBRG}
 
 
 class ImageDesc(ctypes.Structure):
@@ -108,22 +113,23 @@ def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> Imag
 
 def _img_format(v) -> int:
     if isinstance(v, str):
-        if v not in IMG_FORMATS:
-            raise ValueError(f"unknown image format {v!r} (one of {sorted(IMG_FORMATS)})")
-        return IMG_FORMATS[v]
+        names = {**IMG_FORMATS, **BAYER_FORMATS}
+        if v not in names:
+            raise ValueError(f"unknown image format {v!r} (one of {sorted(names)})")
+        return names[v]
     return int(v)
 
 
 def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
-    """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray) or [3][H][W] (planar R, G, B)
-    with the pixels / channels of a row contiguous; the pitches come from the view's strides, so slices of a larger
-    frame (crops, side-by-side halves) need no copy."""
+    """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray, Bayer) or [3][H][W] (planar R,
+    G, B) with the pixels / channels of a row contiguous; the pitches come from the view's strides, so slices of a
+    larger frame (crops, side-by-side halves) need no copy."""
     if a.dtype != np.uint8:
         raise ValueError(f"images must be uint8, got {a.dtype}")
-    C = IMG_CHANNELS[fmt]
+    C = IMG_CHANNELS.get(fmt, 1)
     if fmt == IMG_RGB_PLANAR:
         shape, inner, pitches = (3, H, W), (1,), (0, a.strides[1], a.strides[0])
-    elif fmt == IMG_GRAY:
+    elif fmt == IMG_GRAY or fmt in BAYER_FORMATS.values():
         shape, inner, pitches = (H, W), (1,), (0, a.strides[0], 0)
     else:
         shape, inner, pitches = (H, W, C), (C, 1), (0, a.strides[0], 0)
@@ -509,9 +515,10 @@ class Engine:
     def match_images(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
                      cost_layout="hwd", cost_dtype=None, disparity=True):
         """match_outputs for images in any IMG_* format, read in place: `left` / `right` are uint8 numpy views of shape
-        [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray) or [3][H][W] (rgb_planar) whose rows may be pitched, e.g.
-        frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.  The result is
-        what match_outputs gives for the same pixels packed as BGR."""
+        [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray, bayer_*) or [3][H][W] (rgb_planar) whose rows may be
+        pitched, e.g. frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.
+        The result is what match_outputs gives for the same pixels packed as BGR (for a Bayer mosaic: for
+        cv2.cvtColor(view, COLOR_Bayer*2BGR), the pattern being the view's own top-left 2x2 block)."""
         return self._match_views(self._L.adc_match_images, self.height, self.width, left, right, format, maps, volumes,
                                  layout, dtype, cost, cost_layout, cost_dtype, disparity)
 

@@ -283,12 +283,34 @@ int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, 
  * Rule violations fail with ADC_ERR_ARG naming the field: the rules that need no image size before the engine is
  * checked, the size-dependent ones before any device work.
  * Cost: tight packed BGR takes the packed-BGR entry points' copies; every other format or geometry runs one ingestion
- * kernel per wave that writes the wave's packed BGR in one pass. */
+ * kernel per wave that writes the wave's packed BGR in one pass.  The Bayer formats (below) are formats of this list. */
 enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC_IMG_GRAY = 4, ADC_IMG_RGB_PLANAR = 5 };
+/* Bayer mosaics: raw 8-bit colour-filter frames, 1 byte per pixel in one plane (geometry and rules as for ADC_IMG_GRAY),
+ * demosaiced on the way in.  The name gives the colours of the view's OWN top-left 2x2 block, row 0 then row 1, as
+ * GenICam's pixel formats do; a crop that starts at an odd x or y has a different pattern, and both views share one.
+ *   ADC_IMG_BAYER_RGGB  R G / G B   GenICam BayerRG8   OpenCV COLOR_BayerRGGB2BGR = legacy COLOR_BayerBG2BGR (46)
+ *   ADC_IMG_BAYER_GRBG  G R / B G   GenICam BayerGR8   OpenCV COLOR_BayerGRBG2BGR = legacy COLOR_BayerGB2BGR (47)
+ *   ADC_IMG_BAYER_BGGR  B G / G R   GenICam BayerBG8   OpenCV COLOR_BayerBGGR2BGR = legacy COLOR_BayerRG2BGR (48)
+ *   ADC_IMG_BAYER_GBRG  G B / R G   GenICam BayerGB8   OpenCV COLOR_BayerGBRG2BGR = legacy COLOR_BayerGR2BGR (49)
+ * Beware OpenCV's legacy names: they name the second row's second and third pixels, so COLOR_BayerBG2BGR is the RGGB
+ * sensor, not BGGR.
+ * Semantics: a Bayer view is matched exactly as if the caller had run cv::cvtColor(view, <the code above>) (bilinear;
+ * OpenCV's result is the same with and without IPP) and passed the result as packed BGR; through the rectified entries,
+ * cvtColor on the raw frame, then cv::remap as described there.  The demosaic of a W x H view:
+ *   if W < 3 or H < 3, every pixel is (0, 0, 0);
+ *   otherwise pixel (x, y) is the interior rule at (clamp(x, 1, W - 2), clamp(y, 1, H - 2)) -- the border rows and
+ *   columns, corners included, repeat their inner neighbours.  Interior rule, the site's colour from the pattern at
+ *   (y mod 2, x mod 2), N / S / W / E / NW / ... the raw neighbours:
+ *     the site's own colour is its raw value;
+ *     at an R or B site: G = (N + S + W + E + 2) >> 2, the other of R / B = (NW + NE + SW + SE + 2) >> 2;
+ *     at a G site: the colour of its left and right neighbours = (W + E + 1) >> 1, that of the ones above and below
+ *     = (N + S + 1) >> 1.
+ * Only the view's own pixels are read. */
+enum { ADC_IMG_BAYER_RGGB = 16, ADC_IMG_BAYER_GRBG = 17, ADC_IMG_BAYER_BGGR = 18, ADC_IMG_BAYER_GBRG = 19 };
 typedef struct adc_image_desc {
-    int32_t format;        /* ADC_IMG_* */
+    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_*) */
     int32_t reserved;      /* must be zero */
-    int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / planar) */
+    int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / Bayer / planar) */
     int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; other formats: must be 0 */
     int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch) */
 } adc_image_desc;          /* 32 bytes */
@@ -319,7 +341,9 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
  *   cv::remap(view, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) on each view, then the same call through
  *   adc_match_outputs* with the rectified images packed as BGR.
  * Channels are resampled independently; formats are resolved as for adc_match_images (gray v -> (v, v, v)), which
- * commutes with the resampling.  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
+ * commutes with the resampling.  A Bayer mosaic is demosaiced over the whole src_width x src_height frame first (the
+ * rule under ADC_IMG_BAYER_*, with its clamp at the frame's edges; frames narrower or lower than 3 pixels give all-zero
+ * views), and that BGR frame is resampled.  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
  * the 5-bit fractions:
  *   ADC_REMAP_F32 (map1 = float x [H][W], map2 = float y [H][W], CV_32FC1 each):
  *     X = round_half_even(x * 32) saturated to int32, where NaN and values outside int32 give INT_MIN;

@@ -232,4 +232,65 @@ for t, maps, lead in (("s16", s16, 2), ("f32", (s16 / 4.0).astype(np.float32), 0
     cudart.cudaFree(q)
     print("speckles ok", t, flush=True)
 eng.close()
+
+# Bayer mosaics: raw odd-x crops, the right view of each ending exactly at the end of its own cudaMalloc allocation,
+# plain (every pattern) and rectified (maps sampling the last row and column and beyond, and a 2-row frame)
+import bayer_testlib as BT
+
+
+def bayer_views(raws, n, vw, vh, x0):
+    rp = vw + x0
+    stride = vh * rp
+    ptrs = []
+    for img in raws:
+        host = np.zeros(n * stride, np.uint8)
+        for i in range(n):
+            host[i * stride:(i + 1) * stride].reshape(vh, rp)[:, x0:] = img
+        size = n * stride
+        p = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(p), size) == 0
+        assert cudart.cudaMemcpy(p, host.ctypes.data, size, 1) == 0
+        ptrs.append(p.value)
+    return ptrs, rp, stride
+
+
+w, h, D, n, x0 = 71, 47, 23, 3, 3
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+rng = np.random.default_rng(9)
+for pat in BT.NAMES:
+    raws = [rng.integers(0, 256, (h, w), dtype=np.uint8) for _ in range(2)]
+    ptrs, rp, stride = bayer_views(raws, n, w, h, x0)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_images_batch_device(n, ptrs[0] + x0, ptrs[1] + x0, image=A.image_desc(pat, rp, 0, stride),
+                                  d_disp=d_o.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(BT.demosaic(raws[0], pat), BT.demosaic(raws[1], pat))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), pat
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("bayer ok", pat, flush=True)
+for k, (sw, sh) in enumerate(((83, 53), (40, 2))):
+    pat = BT.NAMES[k + 1]
+    edge = np.array([sw - 1, sw - 1.5, sw - 0.5, sw - 1 / 64, sw, sw + 0.5, -0.5, -1 / 64], np.float32)
+    maps = []
+    for v in range(2):
+        mx, my = R.warp_maps(w, h, sw, sh, 80 + v, specials=False)
+        mx[:, -8:] = edge
+        my[-8:, :] = (edge * sh / sw).astype(np.float32)[:, None]
+        my[-1, :] = sh - 1
+        mx[-1, ::2] = sw - 1
+        maps.append(R.convert_maps(mx, my) if k % 2 else (mx, my))
+    eng.set_rectification(maps[0], maps[1], (sw, sh))
+    raws = [rng.integers(0, 256, (sh, sw), dtype=np.uint8) for _ in range(2)]
+    ptrs, rp, stride = bayer_views(raws, n, sw, sh, x0)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_rectified_batch_device(n, ptrs[0] + x0, ptrs[1] + x0, image=A.image_desc(pat, rp, 0, stride),
+                                     d_disp=d_o.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(*(R.remap(BT.demosaic(raws[v], pat), *maps[v]) for v in range(2)))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), (sw, sh)
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("bayer rectified ok", sw, sh, flush=True)
+eng.close()
 print("all ok")
