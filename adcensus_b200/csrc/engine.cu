@@ -1054,11 +1054,26 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
     *out = nullptr;
     if (!opt) return fail(ADC_ERR_ARG, "adc_create: option is NULL");
     if (width <= 0 || height <= 0) return fail(ADC_ERR_ARG, "adc_create: non-positive image size %dx%d", width, height);
-    if (opt->max_disparity - opt->min_disparity <= 0)
+    const long long dmin = opt->min_disparity, dmax = opt->max_disparity;
+    if (dmax - dmin <= 0)
         return fail(ADC_ERR_ARG, "adc_create: empty disparity range [%d,%d)", opt->min_disparity, opt->max_disparity);
+    // The option domain (include/adcensus_b200.h, adc_option): values for which the reference's arithmetic is undefined
+    // or leaves its cost volume non-finite.  All in 64 bits, before any device work.
+    if (dmax - dmin > INT32_MAX || dmin == INT32_MIN || dmax == INT32_MIN)
+        return fail(ADC_ERR_ARG, "adc_create: min_disparity %d / max_disparity %d: max - min or abs() overflows int32",
+                    opt->min_disparity, opt->max_disparity);
+    if ((width - 1) - dmin > INT32_MAX || (width - 1) + (dmax - 1) > INT32_MAX)
+        return fail(ADC_ERR_ARG, "adc_create: min_disparity %d / max_disparity %d: a candidate column x - d or x + d "
+                    "overflows int32 at width %d", opt->min_disparity, opt->max_disparity, width);
+    if (opt->lambda_ad < 1) return fail(ADC_ERR_ARG, "adc_create: lambda_ad %d < 1", opt->lambda_ad);
+    if (opt->lambda_census < 1) return fail(ADC_ERR_ARG, "adc_create: lambda_census %d < 1", opt->lambda_census);
+    if (!std::isfinite(opt->so_p1) || opt->so_p1 < 0)
+        return fail(ADC_ERR_ARG, "adc_create: so_p1 %g is negative or not finite", (double)opt->so_p1);
+    if (!std::isfinite(opt->so_p2) || opt->so_p2 < 0)
+        return fail(ADC_ERR_ARG, "adc_create: so_p2 %g is negative or not finite", (double)opt->so_p2);
     // Limits of the kernels (the reference has none; INTEGRATION.md lists them).  They are checked HERE, so that a caller
     // never sees Initialize() succeed and Match() fail for a size: whatever adc_create accepts, adc_match runs.
-    const int drange = opt->max_disparity - opt->min_disparity;
+    const int drange = (int)(dmax - dmin);
     if ((long long)width * height > (1ll << 28)) return fail(ADC_ERR_UNSUPPORTED, "adc_create: image too large (more than 2^28 pixels)");
     if (drange > ADC_MAX_DISPARITY_RANGE)
         return fail(ADC_ERR_UNSUPPORTED, "adc_create: disparity range %d > %d is not supported (scanline kernel: 8 disparities per lane)", drange, ADC_MAX_DISPARITY_RANGE);
