@@ -105,3 +105,13 @@ def warp_maps(W, H, src_w, src_h, seed, fixed=False, specials=True):
     if specials:
         m2 = m2 | (rng.integers(0, 64, (H, W)).astype(np.uint16) << 10)
     return m1, m2
+
+
+def cone_rig(cv2, sw, sh, W, H, t, baseline):
+    """initUndistortRectifyMap maps (map type t) of one view of a made-up rig: a camera of sw x sh with some
+    distortion, rotated a little (baseline +1 / -1 picks the view), rectified into W x H."""
+    K = np.array([[0.9 * sw, 0, sw / 2 - 3.3], [0, 0.9 * sw, sh / 2 + 2.1], [0, 0, 1]], np.float64)
+    dist = np.array([-0.12, 0.05, 0.0008, -0.0006, -0.004])
+    R1, _ = cv2.Rodrigues(np.array([0.004, -0.011 * baseline, 0.002]))
+    P = np.array([[0.95 * W, 0, W / 2, 0], [0, 0.95 * W, H / 2, 0], [0, 0, 1, 0]], np.float64)
+    return cv2.initUndistortRectifyMap(K, dist, R1, P, (W, H), t)

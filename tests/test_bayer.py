@@ -10,20 +10,17 @@ and not) against adc_match_outputs_batch_device on the restated images, every ou
 raw frames through both map types, larger and smaller than the engine, 1 x 1 and 2 x N; launch counts.
 """
 import ctypes
-import os
 import re
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
 import bayer_testlib as B
+import engine_testlib as E
 import rectify_testlib as R
-from test_volume_export import _engine, _same
 
-ROOT = Path(__file__).resolve().parent.parent
+ROOT = T.REPO
 MAPS = ["wta_left", "wta_right", "outliers", "min_cost", "peak_ratio"]
 VOLS = ["cost", "aggr", "opt"]
 GOLDEN = T.GOLDEN_DIR / "golden_bayer_cases.npz"
@@ -145,66 +142,24 @@ def test_bayer_constants():
         A.engine._image_view_desc(np.zeros((8, 27, 3), np.uint8), A.IMG_BAYER_RGGB, 8, 27)
 
 
-def test_bayer_kernels_use_no_local_memory(tmp_path):
-    """-Xptxas -v on k_bayer.cu: the four plain and four rectified Bayer instantiations have no stack frame and no
+def test_bayer_kernels_use_no_local_memory():
+    """ptxas -v on k_bayer.cu: the four plain and four rectified Bayer instantiations have no stack frame and no
     spills."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip("nvcc not available")
-    src = ROOT / "adcensus_b200" / "csrc" / "k_bayer.cu"
     assert "k_bayer.cu" in (ROOT / "adcensus_b200" / "csrc" / "Makefile").read_text()
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(src), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 8 and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
+    report = E.ptxas_report(ROOT / "adcensus_b200" / "csrc" / "k_bayer.cu")
+    assert len(report) == 8 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                                    for f in report.values()), report
     for k in ("k_image_ingest", "k_rectify_ingest"):
-        codes = re.findall(rf"Compiling entry function '\w*{k}ILi(\d+)E", r.stderr)
-        assert sorted(int(c) for c in codes) == [16, 17, 18, 19], (k, r.stderr)
+        codes = [re.search(rf"{k}ILi(\d+)E", name) for name, f in report.items() if f["regs"] is not None]
+        assert sorted(int(c.group(1)) for c in codes if c) == [16, 17, 18, 19], (k, sorted(report))
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _torch():
-    import torch
-    return torch, torch.device("cuda", 0)
-
-
-def _run(eng, n, d_left, d_right, image, stride, pipelined, rectified=False):
-    """Every output of one call (two in pipelined mode): the final map, all three volumes (f32 HWD) and all five side
-    maps, on the host.  image None: adc_match_outputs_batch_device on tight packed BGR."""
-    torch, dev = _torch()
-    h, w, D = eng.height, eng.width, eng.D
-    out = {"disp": torch.full((n, h, w), -1.0, dtype=torch.float32, device=dev)}
-    for v in VOLS:
-        out[v] = torch.empty((n, h, w, D), dtype=torch.float32, device=dev)
-    for m in MAPS:
-        out[m] = torch.empty((n, h, w), dtype=torch.uint8 if m == "outliers" else torch.float32, device=dev)
-    st = torch.cuda.current_stream()
-    eng.set_pipelined(pipelined)
-    half = n // 2 if pipelined else n
-    for first, cnt in ((0, half), (half, n - half)):
-        if cnt == 0:
-            continue
-        kw = dict(maps=[(out[m][first:].data_ptr(), m) for m in MAPS],
-                  volumes=[(out[v][first:].data_ptr(), v, "hwd", "f32") for v in VOLS],
-                  d_disp=out["disp"][first:].data_ptr(), stream=st.cuda_stream)
-        if image is None:
-            eng.match_outputs_batch_device(cnt, d_left + first * stride, d_right + first * stride, **kw)
-        else:
-            call = eng.match_rectified_batch_device if rectified else eng.match_images_batch_device
-            call(cnt, d_left + first * stride, d_right + first * stride, image=image, **kw)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.set_pipelined(False)
-    return {k: v.cpu().numpy() for k, v in out.items()}
-
-
 def _mosaic_batch(n, vw, vh, rng, x0, y0, extra_row, extra_stride):
     """n pairs of random mosaics laid out as crops at (x0, y0) of frames with row pitch vw + x0 + extra_row and image
     stride footprint + extra_stride, random surroundings, one device buffer per view with guard bytes after the last
     view.  (views, offset of the first pixel, row pitch, image stride, left mosaics, right mosaics)."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     rp = vw + x0 + extra_row
     stride = (vh + y0) * rp + extra_stride
     off = y0 * rp + x0
@@ -229,10 +184,10 @@ def test_bayer_cone_against_oracle(cone):
     """Cone mosaiced with each pattern through adc_match_images_batch_device: the final map equals the CPU oracle run on
     the restated demosaic of the same mosaic, bit for bit."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option())
+    eng = E.engine(w, h, T.default_option())
     oracle = T.Oracle(w, h, T.default_option())
     st = torch.cuda.current_stream()
     for pat in B.NAMES:
@@ -244,8 +199,8 @@ def test_bayer_cone_against_oracle(cone):
         torch.cuda.synchronize()
         want = oracle.match(B.demosaic(ml, pat), B.demosaic(mr, pat))
         got = d_o.cpu().numpy()
-        _same(f"cone {pat} pair 0", got[0], want)
-        _same(f"cone {pat} pair 1", got[1], want)
+        E.same(f"cone {pat} pair 0", got[0], want)
+        E.same(f"cone {pat} pair 1", got[1], want)
     eng.close()
 
 
@@ -256,9 +211,9 @@ def test_bayer_batched(pipelined):
     crop at even and odd offsets with row pitch > W and image stride > footprint: every output equals
     adc_match_outputs_batch_device on the restated BGR images, and the source buffers are unchanged."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, D = 71, 47, 23
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     rng = np.random.default_rng(8)
     for k, pat in enumerate(B.NAMES):
@@ -267,9 +222,11 @@ def test_bayer_batched(pipelined):
         before = [t.clone() for t in views]
         packed_l = torch.from_numpy(np.stack([B.demosaic(x, pat) for x in L])).to(dev)
         packed_r = torch.from_numpy(np.stack([B.demosaic(x, pat) for x in Rr])).to(dev)
-        want = _run(eng, n, packed_l.data_ptr(), packed_r.data_ptr(), None, 3 * w * h, pipelined)
-        got = _run(eng, n, views[0].data_ptr() + off, views[1].data_ptr() + off, A.image_desc(pat, rp, 0, stride),
-                   stride, pipelined)
+        outputs = dict(volumes=[(v, "hwd", "f32") for v in VOLS], maps=MAPS, pipelined=pipelined)
+        want = E.batch_outputs(eng, eng.match_outputs_batch_device, n, packed_l.data_ptr(), packed_r.data_ptr(),
+                               3 * w * h, **outputs)
+        got = E.batch_outputs(eng, eng.match_images_batch_device, n, views[0].data_ptr() + off,
+                              views[1].data_ptr() + off, stride, image=A.image_desc(pat, rp, 0, stride), **outputs)
         _equal_all(got, want, f"{pat} crop ({x0}, {y0})")
         assert all(torch.equal(t, c) for t, c in zip(views, before)), f"{pat}: source buffer changed"
     eng.close()
@@ -280,16 +237,16 @@ def test_bayer_host_entry():
     """The single-pair host entry match_images on pitched numpy crops gives what match_outputs gives on the restated
     images: final map, all three volumes, all five side maps; also for a tight mosaic of an even-sized frame."""
     w, h, D = 61, 45, 20
-    eng = _engine(w, h, T.default_option(max_disparity=D))
+    eng = E.engine(w, h, T.default_option(max_disparity=D))
     rng = np.random.default_rng(21)
     for pat in B.NAMES:
         frame = [rng.integers(0, 256, (h + 3, w + 8), dtype=np.uint8) for _ in range(2)]
         views = [f[1:1 + h, 3:3 + w] for f in frame]
         want_disp, want = eng.match_outputs(*(B.demosaic(v, pat) for v in views), maps=MAPS, volumes=VOLS)
         disp, got = eng.match_images(views[0], views[1], format=pat, maps=MAPS, volumes=VOLS)
-        _same(f"{pat} host disp", disp, want_disp)
+        E.same(f"{pat} host disp", disp, want_disp)
         for k in want:
-            _same(f"{pat} host {k}", got[k], want[k])
+            E.same(f"{pat} host {k}", got[k], want[k])
     eng.close()
 
 
@@ -300,9 +257,9 @@ def test_bayer_rectified(pipelined):
     engine, and 1 x 1 and 2 x N frames (all-zero views), as odd-offset crops with row pitch > W: every output equals
     adc_match_outputs_batch_device on remap(demosaic(raw)); the host entry match_rectified agrees."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, D = 71, 47, 23
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
     n = 2 * eng.wave_pairs + 1
     rng = np.random.default_rng(12)
     for k, (sw, sh) in enumerate(((83, 53), (64, 40), (1, 1), (57, 2), (3, 3))):
@@ -315,15 +272,17 @@ def test_bayer_rectified(pipelined):
         packed_r = torch.from_numpy(np.stack([R.remap(B.demosaic(x, pat), *maps[1]) for x in Rr])).to(dev)
         if min(sw, sh) < 3:
             assert not packed_l.any() and not packed_r.any()
-        want = _run(eng, n, packed_l.data_ptr(), packed_r.data_ptr(), None, 3 * w * h, pipelined)
-        got = _run(eng, n, views[0].data_ptr() + off, views[1].data_ptr() + off, A.image_desc(pat, rp, 0, stride),
-                   stride, pipelined, rectified=True)
+        outputs = dict(volumes=[(v, "hwd", "f32") for v in VOLS], maps=MAPS, pipelined=pipelined)
+        want = E.batch_outputs(eng, eng.match_outputs_batch_device, n, packed_l.data_ptr(), packed_r.data_ptr(),
+                               3 * w * h, **outputs)
+        got = E.batch_outputs(eng, eng.match_rectified_batch_device, n, views[0].data_ptr() + off,
+                              views[1].data_ptr() + off, stride, image=A.image_desc(pat, rp, 0, stride), **outputs)
         _equal_all(got, want, f"{sw}x{sh} {pat} fixed={fixed}")
         if not pipelined:
             disp, one = eng.match_rectified(L[1], Rr[1], format=pat, maps=MAPS)
-            _same(f"{sw}x{sh} {pat} host disp", disp, want["disp"][1])
+            E.same(f"{sw}x{sh} {pat} host disp", disp, want["disp"][1])
             for m in MAPS:
-                _same(f"{sw}x{sh} {pat} host {m}", one[m], want[m][1])
+                E.same(f"{sw}x{sh} {pat} host {m}", one[m], want[m][1])
     eng.close()
 
 
@@ -333,17 +292,16 @@ def test_bayer_cone_rig(cone):
     equals the packed-BGR call on cv2.remap(cv2.cvtColor(raw)), computed by OpenCV itself."""
     cv2 = pytest.importorskip("cv2")
     import adcensus_b200 as A
-    from test_rectify import _cone_rig
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
     sw, sh = 640, 480
     raw = [B.mosaic(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_AREA), "bayer_rggb") for img in (left, right)]
-    eng = _engine(w, h, T.default_option())
+    eng = E.engine(w, h, T.default_option())
     st = torch.cuda.current_stream()
     d = [torch.from_numpy(r).to(dev) for r in raw]
     for t in (cv2.CV_32FC1, cv2.CV_16SC2):
-        maps = [_cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
+        maps = [R.cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
         eng.set_rectification(maps[0], maps[1], (sw, sh))
         rect = [cv2.remap(B.cv_demosaic(cv2, raw[v], "bayer_rggb"), *maps[v], cv2.INTER_LINEAR,
                           borderMode=cv2.BORDER_CONSTANT, borderValue=0) for v in range(2)]
@@ -352,7 +310,7 @@ def test_bayer_cone_rig(cone):
         eng.match_rectified_batch_device(1, d[0].data_ptr(), d[1].data_ptr(), image=A.image_desc("bayer_rggb"),
                                          d_disp=d_o.data_ptr(), stream=st.cuda_stream)
         torch.cuda.synchronize()
-        _same(f"rig {t}", d_o[0].cpu().numpy(), want)
+        E.same(f"rig {t}", d_o[0].cpu().numpy(), want)
     eng.close()
 
 
@@ -362,9 +320,9 @@ def test_bayer_launch_counts():
     both the image and the rectified entry (where a packed-BGR call also takes one ingestion launch per wave); the
     ingestion profile ids replay the Bayer kernels after a Bayer call."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, D = 71, 47, 23
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=2)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=2)
     n = 3 * eng.wave_pairs + 1
     waves = -(-n // eng.wave_pairs)
     rng = np.random.default_rng(2)

@@ -1,33 +1,23 @@
 """The AD-census cost computed inside the first horizontal aggregation pass (k_cost_arm_sum_h, k_aggregate.cu): its
 launch plan (adcensus_b200/csrc/ca_plan.h) on the CPU, its compiled resources, and on the GPU the volumes it produces
 against the separate cost kernel and the unfused aggregation."""
-import os
-import re
 import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E
 
-ROOT = Path(__file__).resolve().parent.parent
-CSRC = ROOT / "adcensus_b200" / "csrc"
+CSRC = T.REPO / "adcensus_b200" / "csrc"
 
 # H100: 228 KB of shared memory per SM, 1 KB reserved per CTA; the kernel is planned for two CTAs per SM
 SMEM_PER_SM, SMEM_RESERVED = 228 * 1024, 1024
 
 
-@pytest.fixture(scope="module")
-def plan_exe(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("ca_plan") / "ca_plan_main"
-    subprocess.run(["g++", "-O2", "-std=c++17", "-o", str(exe), str(ROOT / "tests" / "c" / "ca_plan_main.cpp")], check=True)
-    return exe
-
-
-def _plan(exe, W, D, L1):
+def _plan(W, D, L1):
     Dp = (D + 3) // 4 * 4
-    r = subprocess.run([str(exe), str(W), str(Dp), str(L1)], capture_output=True, text=True)
+    r = subprocess.run([str(E.c_tool("ca_plan_main")), str(W), str(Dp), str(L1)], capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     lines = r.stdout.split("\n")
     qc, Ls, nseg, nchunks, gm, lpc, threads, smem, ok, budget = map(int, lines[0].split())
@@ -45,9 +35,9 @@ PLAN_SHAPES = {
 
 
 @pytest.mark.parametrize("name", sorted(PLAN_SHAPES))
-def test_cost_fused_plan(plan_exe, name):
+def test_cost_fused_plan(name):
     W, D, L1 = PLAN_SHAPES[name]
-    p, segs = _plan(plan_exe, W, D, L1)
+    p, segs = _plan(W, D, L1)
     assert p["ok"], p
     L1c = min(max(L1, 0), 255)
     # shared memory within the budget, and two CTAs per SM
@@ -70,53 +60,29 @@ def test_cost_fused_plan(plan_exe, name):
         assert p["nseg"] == 1, p                      # Cone and smaller rows are one segment
 
 
-def test_cost_fused_plan_cone_choice(plan_exe):
-    p, _ = _plan(plan_exe, 450, 64, 34)
+def test_cost_fused_plan_cone_choice():
+    p, _ = _plan(450, 64, 34)
     assert (p["qc"], p["nseg"], p["nchunks"], p["threads"]) == (8, 1, 2, 256), p
 
 
-def _ptxas(src):
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip(f"nvcc not found at {nvcc}")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        "-Xcompiler", "-ffp-contract=off", str(CSRC / src), "-o", os.devnull],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    out = {}
-    for m in re.finditer(r"Compiling entry function '(\w+)'.*?\n(.*?)Used (\d+) registers", r.stderr, re.S):
-        out[m.group(1)] = (m.group(2), int(m.group(3)))
-    return out
-
-
 def test_cost_fused_kernel_resources():
-    """-Xptxas -v: no stack frame, no spills in any instantiation of k_cost_arm_sum_h, and at most 128 registers, which
+    """ptxas -v: no stack frame, no spills in any instantiation of k_cost_arm_sum_h, and at most 128 registers, which
     two CTAs of 256 threads per SM need; k_cost_volume keeps its 64 registers."""
-    fused = {k: v for k, v in _ptxas("k_aggregate.cu").items() if "k_cost_arm_sum_h" in k}
+    flags = ("-Xcompiler", "-ffp-contract=off")
+    fused = {k: v for k, v in E.ptxas_report(CSRC / "k_aggregate.cu", flags).items()
+             if "k_cost_arm_sum_h" in k and v["regs"] is not None}
     assert len(fused) == 4, sorted(fused)
-    for name, (props, regs) in fused.items():
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in props, (name, props)
-        assert regs <= 128, (name, regs)
-    cost = {k: v for k, v in _ptxas("k_cost.cu").items() if "k_cost_volume" in k}
+    for name, f in fused.items():
+        assert (f["stack"], f["spill_stores"], f["spill_loads"]) == (0, 0, 0), (name, f)
+        assert f["regs"] <= 128, (name, f)
+    cost = {k: v for k, v in E.ptxas_report(CSRC / "k_cost.cu", flags).items()
+            if "k_cost_volume" in k and v["regs"] is not None}
     assert len(cost) == 2, sorted(cost)
-    for name, (props, regs) in cost.items():
-        assert "0 bytes spill stores" in props and regs == 64, (name, props, regs)
+    for name, f in cost.items():
+        assert f["spill_stores"] == 0 and f["regs"] == 64, (name, f)
 
 
 # ---------------------------------------------------------------------------------------------------- GPU
-def _engine(w, h, opt, **kw):
-    import adcensus_b200 as A
-    o = A.ADCensusOption()
-    for name, _ in T.Option._fields_:
-        if not name.startswith("_"):
-            setattr(o, name, getattr(opt, name))
-    return A.Engine(w, h, o, **kw)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a).view(np.uint32)
-
-
 @pytest.mark.gpu
 def test_fused_cost_launch_count():
     """The fused path replaces k_cost_volume + the first horizontal pass by one launch: AGG4 takes 4 launches more than
@@ -124,7 +90,7 @@ def test_fused_cost_launch_count():
     w, h, D = 97, 61, 24
     opt = T.default_option(max_disparity=D)
     left, right = T.synthetic_pair(w, h, D, 2)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     c0 = eng.launch_count
     eng.debug_run(left, right, "ARMS")
     arms = eng.launch_count - c0
@@ -136,8 +102,7 @@ def test_fused_cost_launch_count():
 
 
 def _fused_cases():
-    from test_gpu_parity import CASES
-    cases = [(w, h, D, over, seed) for (w, h, D, over, seed) in CASES]
+    cases = [(w, h, D, over, seed) for (w, h, D, over, seed) in E.PARITY_CASES]
     cases.append(("cone", None, 64, {}, None))
     cases.append((1920, 1080, 192, {}, 41))          # rows cut into segments
     return cases
@@ -158,14 +123,14 @@ def test_fused_cost_export_and_aggregation(case, cone):
         opt = T.default_option(**{"max_disparity": D, **over})
         left, right = T.synthetic_pair(w, h, D, seed)
     kw = dict(wave_pairs=1, lanes=1)
-    eng = _engine(w, h, opt, **kw)
+    eng = E.engine(w, h, opt, **kw)
     eng.debug_run(left, right, "COST")
     want_cost = eng.tap("VOL_INIT").copy()
     disp, vols = eng.match_volumes(left, right, ["cost", "aggr"])
     eng.close()
-    assert np.array_equal(_bits(vols["cost"]), _bits(want_cost)), f"{w}x{h}x{D}: COST export differs from k_cost_volume"
-    ref = _engine(w, h, opt, debug_flags=A.engine.DBG_UNFUSED_AGG, **kw)
+    assert np.array_equal(E.bits(vols["cost"]), E.bits(want_cost)), f"{w}x{h}x{D}: COST export differs from k_cost_volume"
+    ref = E.engine(w, h, opt, debug_flags=A.engine.DBG_UNFUSED_AGG, **kw)
     rdisp, rvols = ref.match_volumes(left, right, ["aggr"])
     ref.close()
-    assert np.array_equal(_bits(vols["aggr"]), _bits(rvols["aggr"])), f"{w}x{h}x{D}: AGGR differs from the unfused passes"
-    assert np.array_equal(_bits(disp), _bits(rdisp)), f"{w}x{h}x{D}: final map differs from the unfused pipeline"
+    assert np.array_equal(E.bits(vols["aggr"]), E.bits(rvols["aggr"])), f"{w}x{h}x{D}: AGGR differs from the unfused passes"
+    assert np.array_equal(E.bits(disp), E.bits(rdisp)), f"{w}x{h}x{D}: final map differs from the unfused pipeline"

@@ -5,27 +5,17 @@ golden_cost_cases.json, tools/make_golden_cost.py), argument errors, the volume 
 GPU: round trips of the engine's own AD-census volume, stage parity of every layout x element type, the value domain,
 the batched device entry point.
 """
-import ctypes
-import json
-import sys
-from pathlib import Path
-
 import numpy as np
 import pytest
 
 import adc_testlib as T
 import cost_testlib as CT
-
-sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
-import make_golden as G  # noqa: E402
-import make_golden_cost as GC  # noqa: E402
+import engine_testlib as E  # puts tools/ on sys.path
+import make_golden as G
+import make_golden_cost as GC
 
 LAYOUTS = ["hwd", "dhw"]
 DTYPES = ["f32", "f16", "bf16"]
-
-
-def _golden_cost():
-    return json.loads((T.GOLDEN_DIR / "golden_cost_cases.json").read_text())
 
 
 def _as_input(vol_hwd, layout, dtype):
@@ -44,7 +34,7 @@ def _as_input(vol_hwd, layout, dtype):
 @pytest.mark.parametrize("case", GC.COST_CASES, ids=[GC.cost_case_id(c) for c in GC.COST_CASES])
 def test_cost_oracle_vs_reference_golden(case):
     """Every tap after every stage of the restatement with an injected volume: sha256 equal to the reference's."""
-    want = _golden_cost()[GC.cost_case_id(case)]
+    want = E.golden("golden_cost_cases.json")[GC.cost_case_id(case)]
     left, right, opt, cost = GC.cost_case_inputs(case)
     h, w, _ = left.shape
     orc = CT.CostOracle(w, h, opt)
@@ -108,21 +98,6 @@ def test_cost_argument_errors_need_no_gpu():
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _engine(w, h, opt, **kw):
-    import adcensus_b200 as A
-    o = A.ADCensusOption()
-    for name, _ in T.Option._fields_:
-        if not name.startswith("_"):
-            setattr(o, name, getattr(opt, name))
-    return A.Engine(w, h, o, **kw)
-
-
-def _same(name, got, want):
-    assert got.shape == want.shape, f"{name}: shape {got.shape} vs {want.shape}"
-    eq = got.view(np.uint32) == want.view(np.uint32) if got.dtype.kind == "f" else got == want
-    assert eq.all(), f"{name}: {int((~eq).sum())} of {eq.size} values differ"
-
-
 ROUND_TRIP = [(97, 61, 24, {}, 2), (130, 70, 37, {}, 3), (80, 60, 32, {"min_disparity": -4, "max_disparity": 28}, 32)]
 
 
@@ -138,7 +113,7 @@ def test_own_volume_round_trip(case, cone):
         opt = T.default_option(**{"max_disparity": D, **over})
         left, right = T.synthetic_pair(w, h, opt.max_disparity - opt.min_disparity, seed)
     h, w, _ = left.shape
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     eng.debug_run(left, right, "COST")
     vol = eng.tap("VOL_INIT").copy()
     want = eng.match(left, right)
@@ -148,8 +123,8 @@ def test_own_volume_round_trip(case, cone):
     for layout in LAYOUTS:
         v = vol if layout == "hwd" else np.ascontiguousarray(vol.transpose(2, 0, 1))
         got = eng.match_cost(left, right, v, layout)
-        _same(f"{layout} map", got, want)
-        _same(f"{layout} right map", eng.right_disparity(), want_r)
+        E.same(f"{layout} map", got, want)
+        E.same(f"{layout} right map", eng.right_disparity(), want_r)
         if case == "cone":
             assert T.sha(got).startswith("77d70a58d1aa5c71")
     eng.close()
@@ -159,17 +134,17 @@ def test_own_volume_round_trip(case, cone):
 @pytest.mark.parametrize("case", GC.COST_CASES, ids=[GC.cost_case_id(c) for c in GC.COST_CASES])
 def test_cost_stage_parity_vs_reference(case):
     """Every golden cost case, every layout x element type, every stage: the reference's hashes; VOL_INIT = the volume."""
-    want = _golden_cost()[GC.cost_case_id(case)]
+    want = E.golden("golden_cost_cases.json")[GC.cost_case_id(case)]
     left, right, opt, cost = GC.cost_case_inputs(case)
     h, w, _ = left.shape
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     for layout in LAYOUTS:
         for dtype in DTYPES:
             v, dt = _as_input(cost, layout, dtype)
             for st in T.STAGES:
                 eng.debug_run_cost(left, right, v, layout, st, dtype=dt)
                 if st == "COST":
-                    _same(f"{layout}/{dtype} VOL_INIT", eng.tap("VOL_INIT"), cost)
+                    E.same(f"{layout}/{dtype} VOL_INIT", eng.tap("VOL_INIT"), cost)
                 for tap in GC.COST_STAGE_TAPS[st]:
                     assert T.sha(G.ref_case_tap(opt, tap, eng.tap(tap))) == want[f"{st}/{tap}"], f"{layout}/{dtype} {st}/{tap}"
             got = eng.match_cost(left, right, v, layout, dtype=dt)
@@ -191,20 +166,19 @@ def test_cost_value_domain():
     cost[mask] = specials[rng.integers(0, len(specials), int(mask.sum()))]
     clamped = CT.cost_domain(cost)
     want = CT.CostOracle(w, h, opt).match_cost(left, right, clamped)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     for layout in LAYOUTS:
         v = cost if layout == "hwd" else np.ascontiguousarray(cost.transpose(2, 0, 1))
         eng.debug_run_cost(left, right, v, layout, "COST")
-        _same(f"{layout} VOL_INIT", eng.tap("VOL_INIT"), clamped)
-        _same(f"{layout} map", eng.match_cost(left, right, v, layout), want)
+        E.same(f"{layout} VOL_INIT", eng.tap("VOL_INIT"), clamped)
+        E.same(f"{layout} map", eng.match_cost(left, right, v, layout), want)
     eng.close()
 
 
 def _device_batch_check(eng, pairs, n, layout, dtype):
     """n pairs (pair i = pairs[i % len(pairs)]) through match_cost_batch_device; every map equals the single-pair
     match_cost of its own pair."""
-    import torch
-    dev = torch.device("cuda", 0)
+    torch, dev = E.cuda()
     singles = [eng.match_cost(l, r, v, layout, dtype=dt) for (l, r, v, dt) in pairs]
     k = len(pairs)
     d_l = torch.from_numpy(np.stack([pairs[i % k][0] for i in range(n)])).to(dev)
@@ -212,17 +186,13 @@ def _device_batch_check(eng, pairs, n, layout, dtype):
     d_c = torch.from_numpy(np.stack([pairs[i % k][2] for i in range(n)])).to(dev)
     d_out = torch.full((n, eng.height, eng.width), -1.0, dtype=torch.float32, device=dev)
     st = torch.cuda.current_stream()
-    eng.set_pipelined(True)
-    half = n // 2          # two calls that flow into each other, joined once
-    eng.match_cost_batch_device(half, d_l.data_ptr(), d_r.data_ptr(), d_c.data_ptr(), d_out.data_ptr(), layout, dtype,
-                                st.cuda_stream)
-    eng.match_cost_batch_device(n - half, d_l[half:].data_ptr(), d_r[half:].data_ptr(), d_c[half:].data_ptr(),
-                                d_out[half:].data_ptr(), layout, dtype, st.cuda_stream)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
+    # two calls that flow into each other, joined once
+    E.split_calls(eng, n, True, lambda first, count: eng.match_cost_batch_device(
+        count, d_l[first:].data_ptr(), d_r[first:].data_ptr(), d_c[first:].data_ptr(), d_out[first:].data_ptr(), layout,
+        dtype, st.cuda_stream))
     out = d_out.cpu().numpy()
     for i in range(n):
-        _same(f"pair {i}", out[i], singles[i % k])
+        E.same(f"pair {i}", out[i], singles[i % k])
 
 
 @pytest.mark.gpu
@@ -230,7 +200,7 @@ def test_cost_batch_device_order_and_stride():
     """n = 3 * wave_pairs + 2 distinct pairs with wave_pairs = 4, lanes = 3, pipelined."""
     w, h, D = 72, 48, 24
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     pairs = []
     for s in range(n):
@@ -245,7 +215,7 @@ def test_cost_batch_device_loaded_waves_bf16():
     """Default configuration with several waves per lane in flight, DHW bf16: every map equals its single-pair result."""
     w, h, D = 160, 120, 64
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     n = 2 * eng.wave_pairs * eng.lanes + 5
     pairs = []
     for s in range(7):    # 7 distinct pairs cycled: coprime with the wave size, so every wave slot sees different pairs

@@ -11,6 +11,8 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import engine_testlib as E
+
 ROOT = Path(__file__).resolve().parent.parent
 
 
@@ -86,15 +88,11 @@ def test_product_never_touches_the_oracle():
             assert "adc_oracle" not in txt and "adc_testlib" not in txt and "libadcensus_ref" not in txt, f
 
 
-def test_reference_style_cpp_caller_compiles_and_links(tmp_path):
+def test_reference_style_cpp_caller_compiles_and_links():
     """A C++ program written against the reference's class interface builds against include/ and
     the shared library, and sees the reference's error truth table."""
-    A, L = _lib()
-    exe = tmp_path / "dropin"
-    r = subprocess.run(["g++", "-std=c++17", str(ROOT / "tests" / "cpp" / "dropin_main.cpp"), f"-I{ROOT / 'include'}",
-                        f"-L{A.lib_path().parent}", "-ladcensus_b200", f"-Wl,-rpath,{A.lib_path().parent}", "-o", str(exe)],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-2000:]
+    _lib()
+    exe = E.c_tool("dropin_main")
     run = subprocess.run([str(exe)], capture_output=True, text=True, env=dict(os.environ, ADC_B200_QUIET="1"))
     assert run.returncode == 0, (run.returncode, run.stdout, run.stderr)
     assert "DROPIN_OK" in run.stdout or "DROPIN_NO_GPU" in run.stdout
@@ -109,10 +107,9 @@ def test_shard_bounds():
 
 
 _WORKER = r'''
-import os, sys
+import os
 import numpy as np
 import torch.distributed as dist
-sys.path.insert(0, os.environ["ADC_ROOT"])
 from adcensus_b200.parallel import run_sharded
 dist.init_process_group("gloo", init_method="tcp://127.0.0.1:%s" % os.environ["ADC_PORT"],
                         rank=int(os.environ["RANK"]), world_size=int(os.environ["WORLD_SIZE"]))
@@ -141,7 +138,8 @@ def test_two_rank_scatter_gather_gloo(tmp_path):
         port = str(sk.getsockname()[1])
     procs = []
     for r in range(2):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE="2", ADC_ROOT=str(ROOT), ADC_PORT=port)
+        path = os.pathsep.join(p for p in (str(ROOT), os.environ.get("PYTHONPATH")) if p)
+        env = dict(os.environ, RANK=str(r), WORLD_SIZE="2", ADC_PORT=port, PYTHONPATH=path)
         procs.append(subprocess.Popen([sys.executable, str(script)], env=env, stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True))
     outs = [p.communicate(timeout=180) for p in procs]
     for p, (so, se) in zip(procs, outs):

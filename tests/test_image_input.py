@@ -9,23 +9,15 @@ the gray golden cases; side-by-side, stacked, cropped and gray batches through t
 lane; image strides past 2^31 bytes; the unchanged default path; the size-dependent argument rules.
 """
 import ctypes
-import json
-import os
-import re
-import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E  # puts tools/ on sys.path
 import images_testlib as IT
-from test_volume_export import _engine, _same
-
-sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
-import make_golden as G  # noqa: E402
-import make_golden_gray as GG  # noqa: E402
+import make_golden as G
+import make_golden_gray as GG
 
 MAPS = ["wta_left", "wta_right", "outliers", "min_cost", "peak_ratio"]
 COLOUR = ["bgr", "rgb", "bgra", "rgba", "rgb_planar"]
@@ -142,7 +134,7 @@ def test_to_bgr_helper_hand_built():
 def test_gray_golden_restatement():
     """The C restatement reproduces every tap the unmodified reference recorded for the gray golden cases, and the
     replicated input's GRAY tap is not the input: gray(128, 128, 128) = 127."""
-    golden = json.loads((T.GOLDEN_DIR / "golden_gray_cases.json").read_text())
+    golden = E.golden("golden_gray_cases.json")
     assert set(golden) == set(GG.GRAY_CASES)
     for name, g in golden.items():
         gl, gr, opt = GG.gray_case_inputs(name)
@@ -162,26 +154,14 @@ def test_gray_golden_restatement():
     assert golden["synth_gray_odd"]["width"] % 2 == 1
 
 
-def test_image_kernel_uses_no_local_memory(tmp_path):
-    """-Xptxas -v on k_image.cu: no stack frame and no spills in any of the six instantiations."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip("nvcc not available")
-    src = Path(__file__).resolve().parent.parent / "adcensus_b200" / "csrc" / "k_image.cu"
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(src), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 6 and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
+def test_image_kernel_uses_no_local_memory():
+    """ptxas -v on k_image.cu: no stack frame and no spills in any of the six instantiations."""
+    report = E.ptxas_report(T.REPO / "adcensus_b200" / "csrc" / "k_image.cu")
+    assert len(report) == 6 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                                    for f in report.values()), report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _torch():
-    import torch
-    return torch, torch.device("cuda", 0)
-
-
 def _padded(img, fmt, extra_row, extra_plane=0, extra_stride=0, lead=0):
     """(flat buffer, row_pitch, plane_pitch, offset) of a tight image laid out with padded pitches and `lead` bytes
     before it; every padding byte is 0xEE."""
@@ -203,10 +183,10 @@ def test_colour_formats_cone(fmt, cone):
     the final map is the reference's and the f32 ADC_VOL_COST export -- the earliest output that depends on every
     converted byte of both views -- is bit-identical to the packed-BGR call's."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option())
+    eng = E.engine(w, h, T.default_option())
     want_disp, want = eng.match_outputs(left, right, volumes=["cost"])
     assert T.sha(want_disp).startswith(CONE_SHA)
     st = torch.cuda.current_stream()
@@ -224,7 +204,7 @@ def test_colour_formats_cone(fmt, cone):
             mk = lambda b, o: np.lib.stride_tricks.as_strided(b[o:], (h, w, C), (rp, C, 1))
         disp, got = eng.match_images(mk(*views[0]), mk(*views[1]), format=fmt, volumes=["cost"])
         assert T.sha(disp).startswith(CONE_SHA), name
-        _same(f"{name} host cost volume", got["cost"], want["cost"])
+        E.same(f"{name} host cost volume", got["cost"], want["cost"])
         # batched device entry: two pairs per call, image stride = footprint + 3 (odd), the right view in its own buffer
         n = 2
         stride = views[0][0].size + 3
@@ -241,12 +221,8 @@ def test_colour_formats_cone(fmt, cone):
         torch.cuda.synchronize()
         for i in range(n):
             assert T.sha(d_disp[i].cpu().numpy()).startswith(CONE_SHA), f"{name} pair {i}"
-            _same(f"{name} device cost volume pair {i}", d_cost[i].cpu().numpy(), want["cost"])
+            E.same(f"{name} device cost volume pair {i}", d_cost[i].cpu().numpy(), want["cost"])
     eng.close()
-
-
-def _gray_golden():
-    return json.loads((T.GOLDEN_DIR / "golden_gray_cases.json").read_text())
 
 
 def _check_gray(name, g, opt, disp, got):
@@ -267,13 +243,13 @@ def _check_gray(name, g, opt, disp, got):
 def test_gray_golden(name):
     """The gray golden cases through both entry points: every exported volume (f32 [H][W][D]), the WTA maps, the
     outlier lists and the final map hash to what the unmodified reference gives for the replicated images."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
-    g = _gray_golden()[name]
+    g = E.golden("golden_gray_cases.json")[name]
     gl, gr, opt = GG.gray_case_inputs(name)
     assert [T.sha(gl), T.sha(gr)] == g["input_sha"]
     h, w = gl.shape
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     disp, got = eng.match_images(gl, gr, format="gray", maps=MAPS, volumes=["cost", "aggr", "opt"])
     _check_gray(f"{name} host", g, opt, disp, got)
     n, D = 3, eng.D
@@ -307,7 +283,7 @@ def _geometry(kind, fmt, n, h, w, D, rng):
     [n][H][2W][4], right view at +4W bytes), "stacked" (planar pairs [n][2][3][H][W] in one buffer), "crop" (odd-x crops
     of larger frames with random surroundings, any format), "gray" ([n][H][W])."""
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     pairs = [T.synthetic_pair(w, h, D, 900 + s) for s in range(n)]
     if fmt == "gray":
         pairs = [(IT.gray_to_bgr(l[:, :, 1]), IT.gray_to_bgr(r[:, :, 1])) for l, r in pairs]
@@ -346,33 +322,6 @@ def _resolved(desc, fmt, h, w):
     return rp, pp, desc.image_stride or IT.footprint(fmt, h, rp, pp)
 
 
-def _run_all_outputs(eng, n, d_left, d_right, image, d_cost, pipelined, fmt="bgr"):
-    """One call (two in pipelined mode: the batch split in halves) with the cost volume, the optimised volume as DHW bf16,
-    all five side maps and the final map; returns every output on the host."""
-    torch, dev = _torch()
-    h, w, D = eng.height, eng.width, eng.D
-    stride = _resolved(image, fmt, h, w)[2] if image is not None else 3 * h * w
-    out = {"disp": torch.full((n, h, w), -1.0, dtype=torch.float32, device=dev),
-           "opt": torch.empty((n, D, h, w), dtype=torch.bfloat16, device=dev)}
-    for m in MAPS:
-        out[m] = torch.empty((n, h, w), dtype=torch.uint8 if m == "outliers" else torch.float32, device=dev)
-    st = torch.cuda.current_stream()
-    eng.set_pipelined(pipelined)
-    half = n // 2 if pipelined else n
-    for first, cnt in ((0, half), (half, n - half)):
-        if cnt == 0:
-            continue
-        eng.match_images_batch_device(cnt, d_left + first * stride, d_right + first * stride, image=image,
-                                      maps=[(out[m][first:].data_ptr(), m) for m in MAPS],
-                                      volumes=[(out["opt"][first:].data_ptr(), "opt", "dhw", "bf16")],
-                                      d_disp=out["disp"][first:].data_ptr(), d_cost=d_cost[first:].data_ptr(),
-                                      cost_layout="dhw", cost_dtype="f32", stream=st.cuda_stream)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.set_pipelined(False)
-    return {k: (v.view(torch.int16) if v.dtype == torch.bfloat16 else v).cpu().numpy() for k, v in out.items()}
-
-
 GEOMETRIES = [("sbs", "bgra"), ("stacked", "rgb_planar"), ("gray", "gray")] + [("crop", f) for f in IT.FORMATS]
 
 
@@ -383,10 +332,10 @@ def test_geometry_batched(pipelined):
     (the right view's base is not word-aligned), stacked planar pairs, odd-x crops of larger frames in every format, and
     gray.  Every output of a call with a cost volume, an exported volume and all five side maps equals the same call's on
     the packed BGR images (to_bgr of the same bytes), and the source buffers are unchanged."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, D = 71, 47, 23
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     rng = np.random.default_rng(3)
     d_cost = torch.from_numpy(rng.random((n, D, h, w), dtype=np.float32) * np.float32(40)).to(dev)
@@ -401,8 +350,11 @@ def test_geometry_batched(pipelined):
                 assert np.array_equal(IT.to_bgr(raw, fmt, h, w, rp, pp, off + i * stride), imgs[i]), (kind, fmt, i)
         packed_l = torch.from_numpy(np.stack(b.bgr_l)).to(dev)
         packed_r = torch.from_numpy(np.stack(b.bgr_r)).to(dev)
-        want = _run_all_outputs(eng, n, packed_l.data_ptr(), packed_r.data_ptr(), None, d_cost, pipelined)
-        got = _run_all_outputs(eng, n, b.bases[0], b.bases[1], b.desc, d_cost, pipelined, fmt)
+        outputs = dict(volumes=[("opt", "dhw", "bf16")], maps=MAPS, d_cost=d_cost, cost_layout="dhw", cost_dtype="f32",
+                       pipelined=pipelined)
+        entry = eng.match_images_batch_device
+        want = E.batch_outputs(eng, entry, n, packed_l.data_ptr(), packed_r.data_ptr(), 3 * h * w, **outputs)
+        got = E.batch_outputs(eng, entry, n, b.bases[0], b.bases[1], stride, image=b.desc, **outputs)
         for k in want:
             assert np.array_equal(got[k].view(np.uint8), want[k].view(np.uint8)), f"{kind} {fmt}: {k}"
         assert all(torch.equal(t, c) for (t, _), c in zip(b.views, before)), f"{kind} {fmt}: source buffer changed"
@@ -412,7 +364,7 @@ def test_geometry_batched(pipelined):
 @pytest.mark.gpu
 def test_image_stride_past_2_31():
     """n = 2 gray pairs with an image stride above 2^31 bytes: the second pair's views are read from past 2^31."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     w, h, D = 97, 61, 24
     opt = T.default_option(max_disparity=D)
@@ -424,14 +376,14 @@ def test_image_stride_past_2_31():
     for i, (gl, gr) in enumerate(grays):
         buf[i * stride:i * stride + N] = torch.from_numpy(gl.reshape(-1)).to(dev)
         buf[i * stride + N + 1:i * stride + 2 * N + 1] = torch.from_numpy(gr.reshape(-1)).to(dev)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     d_disp = torch.empty((2, h, w), dtype=torch.float32, device=dev)
     eng.match_images_batch_device(2, buf.data_ptr(), buf.data_ptr() + N + 1, image=A.image_desc("gray", 0, 0, stride),
                                   d_disp=d_disp.data_ptr(), stream=torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
     for i, (gl, gr) in enumerate(grays):
         want = eng.match(IT.gray_to_bgr(gl), IT.gray_to_bgr(gr))
-        _same(f"pair {i}", d_disp[i].cpu().numpy(), want)
+        E.same(f"pair {i}", d_disp[i].cpu().numpy(), want)
     del buf
     eng.close()
 
@@ -440,11 +392,11 @@ def test_image_stride_past_2_31():
 def test_default_path_unchanged(cone):
     """A NULL descriptor and a tight packed-BGR descriptor issue exactly the launches of adc_match_outputs_batch_device
     and give identical maps; any other format adds one launch per wave."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
     n = 9
     waves = -(-n // eng.wave_pairs)
     d_l = torch.from_numpy(np.repeat(left[None], n, 0)).to(dev)
@@ -469,17 +421,17 @@ def test_default_path_unchanged(cone):
         m1, s1, l1 = run(lambda d: eng.match_images_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), image=image, maps=maps,
                                                                  d_disp=d.data_ptr(), stream=st.cuda_stream))
         assert l1 == l0
-        _same("map", m1, m0)
+        E.same("map", m1, m0)
         for m in side:
-            _same(m, s1[m], s0[m])
+            E.same(m, s1[m], s0[m])
     m2, s2, l2 = run(lambda d: eng.match_images_batch_device(n, rgb_l.data_ptr(), rgb_r.data_ptr(), image=A.image_desc("rgb"),
                                                              maps=maps, d_disp=d.data_ptr(), stream=st.cuda_stream))
     assert l2 == l0 + waves
-    _same("rgb map", m2, m0)
+    E.same("rgb map", m2, m0)
     m3, _, l3 = run(lambda d: eng.match_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), d.data_ptr(), st.cuda_stream))
-    hashes = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
+    hashes = E.golden_hashes("cone_full")
     assert all(T.sha(m2[i]) == hashes["MEDIAN/DISP_L"] for i in range(n))
-    _same("plain batch", m3, m0)
+    E.same("plain batch", m3, m0)
     # the host entry: NULL descriptor = adc_match_outputs, launch for launch; gray / planar add one launch
     c0 = eng.launch_count
     d_a, _ = eng.match_outputs(left, right)
@@ -487,11 +439,11 @@ def test_default_path_unchanged(cone):
     c0 = eng.launch_count
     d_b, _ = eng.match_images(left, right, format="bgr")
     assert eng.launch_count - c0 == la
-    _same("host bgr", d_b, d_a)
+    E.same("host bgr", d_b, d_a)
     c0 = eng.launch_count
     d_c, _ = eng.match_images(IT.from_bgr(left, "rgb_planar"), IT.from_bgr(right, "rgb_planar"), format="rgb_planar")
     assert eng.launch_count - c0 == la + 1
-    _same("host planar", d_c, d_a)
+    E.same("host planar", d_c, d_a)
     eng.close()
 
 
@@ -499,10 +451,10 @@ def test_default_path_unchanged(cone):
 def test_size_dependent_image_rules():
     """Rules that need the image size fail after the engine check, with ADC_ERR_ARG naming the field, before any device
     work (no launch)."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     w, h, D = 33, 20, 16
-    eng = _engine(w, h, T.default_option(max_disparity=D))
+    eng = E.engine(w, h, T.default_option(max_disparity=D))
     L = A.load_library()
     buf = torch.zeros(1 << 16, dtype=torch.uint8, device=dev)
     out = torch.zeros((1, h, w), dtype=torch.float32, device=dev)

@@ -11,40 +11,21 @@ GPU: for every disparity range 1..256 and every plan-branch case, one batched ca
 of two, the last partial; a flat and a white-noise pair between textured ones) that exports every volume and side map,
 each pair compared bit for bit with its own oracle run.
 """
-import json
 import os
 import re
 import subprocess
-import sys
-from concurrent.futures import ThreadPoolExecutor
 from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
-import maps_testlib as MT
-from test_gpu_parity import _engine, _same
-
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT / "tools"))
-import make_golden_sweep as GS  # noqa: E402  (case definitions shared with the fixture generator)
-
-SMEM_RESERVED_PER_CTA = 1024     # shared memory the driver reserves per CTA on sm_90
+import engine_testlib as E  # puts tools/ on sys.path
+import make_golden_sweep as GS  # case definitions shared with the fixture generator
+from sweep_testlib import Case, check_case, plans, reached, so_lanes_per_line  # noqa: F401  (plans: the fixture)
 
 
 # ---- cases ----------------------------------------------------------------------------------------------------------
-class Case:
-    """One batched GPU run: W x H x D with `opt`, n pairs in waves of `wave_pairs` over `lanes` lanes."""
-
-    def __init__(self, name, W, H, opt, seed, wave_pairs=2, lanes=2, n=5):
-        self.name, self.W, self.H, self.opt, self.seed = name, W, H, opt, seed
-        self.D = opt.max_disparity - opt.min_disparity
-        self.Dp = (self.D + 3) // 4 * 4
-        self.L1 = opt.cross_L1
-        self.wave_pairs, self.lanes, self.n = wave_pairs, lanes, n
-
-
 def _sweep_case(D):
     W, H, opt, seed = GS.sweep_case(D)
     return Case(f"D{D}", W, H, opt, seed)
@@ -87,92 +68,6 @@ SWEEP_DS = list(range(1, 257))
 
 def _all_cases():
     return [_sweep_case(D) for D in SWEEP_DS] + [c for c, _ in PLAN_CASES.values()]
-
-
-# ---- plans (tests/c/*_plan_main.cpp print the plans of the headers the kernels are launched with) ---------------------
-@pytest.fixture(scope="module")
-def plans(tmp_path_factory):
-    d = tmp_path_factory.mktemp("plans")
-    for name in ("ca_plan_main", "so_plan_main"):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-o", str(d / name), str(ROOT / "tests" / "c" / f"{name}.cpp")], check=True)
-    return Plans(d)
-
-
-def _device_figures():
-    """(SM count, shared memory per SM, reserved per CTA) of device 0, or an H100 SXM's where there is no GPU."""
-    import torch
-    if torch.cuda.is_available():
-        p = torch.cuda.get_device_properties(0)
-        return p.multi_processor_count, p.shared_memory_per_multiprocessor, SMEM_RESERVED_PER_CTA
-    return 132, 228 * 1024, SMEM_RESERVED_PER_CTA
-
-
-class Plans:
-    def __init__(self, d):
-        self.d = d
-        self.dev = _device_figures()
-
-    def _run(self, exe, *args):
-        r = subprocess.run([str(self.d / exe), *map(str, args)], capture_output=True, text=True)
-        assert r.returncode == 0, (exe, args, r.stdout, r.stderr)
-        return r.stdout
-
-    def ca(self, c):
-        v = list(map(int, self._run("ca_plan_main", c.W, c.Dp, c.L1).split("\n")[0].split()))
-        return dict(zip(("qc", "Ls", "nseg", "nchunks", "gm", "lpc", "threads", "smem", "ok", "budget"), v))
-
-    def arm(self, c):
-        out = []
-        for line in self._run("ca_plan_main", "arm", c.W, c.H, c.Dp, c.L1).strip().split("\n"):
-            v = list(map(int, line.split()))
-            out.append(dict(zip(("dir", "t_ok", "t_qc", "t_Ls", "t_nseg", "t_nchunks", "t_lpc", "t_threads", "t_smem",
-                                 "ldg_qc_log2", "ldg_Ls", "ldg_nseg", "ldg_smem", "form", "smem_attr"), v)))
-        return out
-
-    def so(self, c, axis):
-        v = list(map(int, self._run("so_plan_main", c.W, c.H, c.Dp, c.wave_pairs, axis, *self.dev).split()))
-        return dict(zip(("T", "NS", "smem", "ctas", "ctas_per_sm", "waves"), v))
-
-
-def so_lanes_per_line(Dp):
-    return 8 if Dp <= 64 else (16 if Dp <= 128 else 32)
-
-
-A2_TMA, A2_LDG = 1, 0     # the forms arm_sum2_form (ca_plan.h) picks
-
-
-def reached(c, plans):
-    """The instantiations of the seven templates one batched run of case c launches, by the launch rules of
-    k_aggregate.cu, k_cost.cu, k_scanline.cu and k_vote.cu (a run that matches, so every stage runs, with the fused
-    aggregation):
-      cost:      k_cost_arm_sum_h<D == Dp, ca_plan.qc> where ca_plan is ok, else k_cost_volume<D == Dp>;
-      axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok and, on rows, the row is one segment; else
-                 k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC).  This restates arm_sum2_form, and the form the plan
-                 executable prints for the axis must agree with it;
-      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp);
-      voting:    k_vote_scan<WIDE> and k_vote_push<WIDE>, WIDE iff D > 254 or L1 > 127."""
-    out = set()
-    exact = c.D == c.Dp
-    ca = plans.ca(c)
-    out.add(("k_cost_arm_sum_h", exact, ca["qc"]) if ca["ok"] else ("k_cost_volume", exact))
-    arm = plans.arm(c)
-    tmaps = bool(arm[0]["t_ok"] and arm[1]["t_ok"])
-    for a in arm:
-        # the fused aggregation runs on every shape: both plans fit the shared memory the passes are launched under
-        assert a["t_smem"] <= a["smem_attr"] and a["ldg_smem"] <= a["smem_attr"], (c.name, a)
-        tma = tmaps and not (a["dir"] == 0 and a["t_nseg"] > 1)
-        assert a["form"] == (A2_TMA if tma else A2_LDG), (c.name, a)
-        if tma:
-            out.add(("k_arm_sum2t", a["dir"] == 1, a["t_qc"]))
-        else:
-            out.add(("k_arm_sum2", a["dir"] == 1, 8 if a["ldg_qc_log2"] == 3 else 0))
-    lps = so_lanes_per_line(c.Dp)
-    K = -(-c.Dp // lps)
-    out.add(("k_scanline", K, lps, c.D == K * lps))
-    wide = c.D > 254 or min(c.L1, 255) > 127
-    out.add(("k_vote_scan", wide))
-    out.add(("k_vote_push", wide))
-    return out
 
 
 # ---- CPU ------------------------------------------------------------------------------------------------------------
@@ -264,7 +159,7 @@ def test_sweep_case_shapes(plans):
 def test_sweep_oracle_vs_reference(D):
     """The oracle on the sweep cases the other fixtures do not reach (D = 1, 2, 96, 161, 253, ...): every tap after every
     stage of the first pair against the unmodified reference's sha256 (tools/make_golden_sweep.py)."""
-    want = json.loads((T.GOLDEN_DIR / "golden_sweep_ref.json").read_text())[str(D)]
+    want = E.golden("golden_sweep_ref.json")[str(D)]
     W, H, opt, seed = GS.sweep_case(D)
     left, right = GS.sweep_pairs(W, H, D, seed)[0]
     orc = T.Oracle(W, H, opt)
@@ -275,83 +170,20 @@ def test_sweep_oracle_vs_reference(D):
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------
-def _oracle_taps(W, H, opt, left, right):
-    """The taps the batched run's outputs are compared with, from one oracle run of one pair."""
-    want = {("COST", "VOL_INIT"): "cost", ("AGG4", "VOL_AGGR"): "aggr", ("SO4", "VOL_AGGR"): "opt",
-            ("WTA", "DISP_L"): "wta_left", ("WTA", "DISP_R"): "wta_right", ("OUTLIER", "MISMATCHES"): "mismatches",
-            ("OUTLIER", "OCCLUSIONS"): "occlusions", ("MEDIAN", "DISP_L"): "final"}
-    orc = T.Oracle(W, H, opt)
-    orc.begin(left, right)
-    out = {}
-    for st in T.STAGES:
-        orc.step()
-        for tap in T.STAGE_TAPS[st]:
-            if (st, tap) in want:
-                out[want[(st, tap)]] = orc.tap(tap).copy()
-    orc.close()
-    return out
-
-
-def _run_batched(c, pairs):
-    """One match_outputs_batch_device call over all pairs: the three volumes (f32, [H][W][D]), the WTA maps, the outlier
-    map and the final map of every pair, as numpy arrays."""
-    import torch
-    dev = torch.device("cuda", 0)
-    n, H, W, D = len(pairs), c.H, c.W, c.D
-    d_l = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev)
-    d_r = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev)
-    vols = {s: torch.full((n, H, W, D), float("nan"), dtype=torch.float32, device=dev) for s in ("cost", "aggr", "opt")}
-    maps = {"wta_left": torch.full((n, H, W), -7.0, device=dev), "wta_right": torch.full((n, H, W), -7.0, device=dev),
-            "outliers": torch.full((n, H, W), 0xee, dtype=torch.uint8, device=dev)}
-    d_disp = torch.full((n, H, W), -7.0, device=dev)
-    eng = _engine(W, H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes)
-    assert (eng.wave_pairs, eng.lanes) == (c.wave_pairs, c.lanes), (eng.wave_pairs, eng.lanes)
-    st = torch.cuda.current_stream()
-    eng.match_outputs_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), maps=[(t.data_ptr(), k) for k, t in maps.items()],
-                                   volumes=[(t.data_ptr(), s, "hwd", "f32") for s, t in vols.items()],
-                                   d_disp=d_disp.data_ptr(), stream=st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.close()
-    got = {k: t.cpu().numpy() for k, t in {**vols, **maps}.items()}
-    got["final"] = d_disp.cpu().numpy()
-    return got
-
-
-def _check_case(c):
-    # the oracle runs overlap in threads (ctypes releases the GIL during the call) while the GPU runs the batch
-    pairs = GS.sweep_pairs(c.W, c.H, c.D, c.seed)[:c.n]
-    with ThreadPoolExecutor(len(pairs)) as ex:
-        futs = [ex.submit(_oracle_taps, c.W, c.H, c.opt, l, r) for l, r in pairs]
-        got = _run_batched(c, pairs)
-        want = [f.result() for f in futs]
-    for i, w in enumerate(want):
-        tag = f"{c.name} ({c.W}x{c.H}x{c.D}, dmin {c.opt.min_disparity}) pair {i}"
-        _same(f"{tag} COST/VOL_INIT", got["cost"][i], w["cost"])
-        _same(f"{tag} AGG4/VOL_AGGR", got["aggr"][i], w["aggr"])
-        _same(f"{tag} SO4/VOL_AGGR", got["opt"][i], w["opt"])
-        _same(f"{tag} WTA/DISP_L", got["wta_left"][i], w["wta_left"])
-        _same(f"{tag} WTA/DISP_R", got["wta_right"][i], w["wta_right"])
-        mis, occ = MT.outlier_lists(got["outliers"][i])
-        _same(f"{tag} OUTLIER/MISMATCHES", mis, w["mismatches"].reshape(-1, 2))
-        _same(f"{tag} OUTLIER/OCCLUSIONS", occ, w["occlusions"].reshape(-1, 2))
-        _same(f"{tag} MEDIAN/DISP_L", got["final"][i], w["final"])
-    return got
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("D", SWEEP_DS)
 def test_disparity_sweep(D):
     """Disparity range D through one batched call (five distinct pairs, waves of two, the last partial) against the
     oracle, every exported volume and side map bit for bit; the ranges pinned to the reference also by the final map's
     sha256."""
-    got = _check_case(_sweep_case(D))
+    got = check_case(_sweep_case(D))
     if D in GS.GOLDEN_DS:
-        want = json.loads((T.GOLDEN_DIR / "golden_sweep_ref.json").read_text())[str(D)]
-        assert T.sha(got["final"][0]) == want["MEDIAN/DISP_L"], f"D={D}: final map differs from the reference's hash"
+        want = E.golden("golden_sweep_ref.json")[str(D)]
+        assert T.sha(got["disp"][0]) == want["MEDIAN/DISP_L"], f"D={D}: final map differs from the reference's hash"
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(PLAN_CASES))
 def test_plan_branch(name):
     """A shape that sends a kernel down a plan branch the sweep's small shapes do not take, checked as the sweep is."""
-    _check_case(PLAN_CASES[name][0])
+    check_case(PLAN_CASES[name][0])

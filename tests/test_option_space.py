@@ -18,22 +18,15 @@ side map bit for bit against each pair's oracle run, the pinned cases also by th
 through the staged debug run, tap by tap.
 """
 import ctypes
-import json
 import math
-import sys
-from pathlib import Path
 
-import numpy as np
 import pytest
 
 import adc_testlib as T
-from test_gpu_parity import _engine, _same
-from test_kernel_sweep import Case, _check_case, plans, reached  # noqa: F401  (plans: the module fixture)
-
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT / "tools"))
-import make_golden_options as GO  # noqa: E402  (case definitions shared with the fixture generator)
-import make_golden_sweep as GS  # noqa: E402
+import engine_testlib as E  # puts tools/ on sys.path
+import make_golden_options as GO  # case definitions shared with the fixture generator
+import make_golden_sweep as GS
+from sweep_testlib import Case, check_case, plans, reached  # noqa: F401  (plans: the fixture)
 
 CASES = GO.cases()
 ADC_DBG_VOTE_ENUM = 2
@@ -45,7 +38,7 @@ def _case(name):
 
 
 def _golden():
-    return json.loads((T.GOLDEN_DIR / "golden_options_ref.json").read_text())
+    return E.golden("golden_options_ref.json")
 
 
 def arm_rec_words(L1):
@@ -179,9 +172,9 @@ def test_adc_create_accepts_the_domain_edges(fields, vals):
 def test_option_case(name):
     """One option-space case through one batched call (five distinct pairs, waves of two, the last partial) against the
     oracle, every exported volume and side map bit for bit; the pinned cases also by the final map's sha256."""
-    got = _check_case(_case(name))
+    got = check_case(_case(name))
     if name in GO.PINNED:
-        assert T.sha(got["final"][0]) == _golden()[name]["MEDIAN/DISP_L"], f"{name}: final map differs from the reference's hash"
+        assert T.sha(got["disp"][0]) == _golden()[name]["MEDIAN/DISP_L"], f"{name}: final map differs from the reference's hash"
 
 
 # name -> debug_flags of the staged run (ADC_DBG_VOTE_ENUM: region voting enumerates on the narrow instantiation)
@@ -199,7 +192,7 @@ def test_option_case_staged(name):
     """Every pair of a few cases through the staged debug run, every tap after every stage against the oracle."""
     W, H, over, seed = CASES[name]
     opt = GO.option(over)
-    eng = _engine(W, H, opt, debug_flags=STAGED[name])
+    eng = E.engine(W, H, opt, debug_flags=STAGED[name])
     for i, (left, right) in enumerate(GS.sweep_pairs(W, H, opt.max_disparity - opt.min_disparity, seed)):
         orc = T.Oracle(W, H, opt)
         orc.begin(left, right)
@@ -207,6 +200,6 @@ def test_option_case_staged(name):
             orc.step()
             eng.debug_run(left, right, st)
             for tap in T.STAGE_TAPS[st]:
-                _same(f"{name} pair {i} {st}/{tap}", eng.tap(tap), orc.tap(tap))
+                E.same(f"{name} pair {i} {st}/{tap}", eng.tap(tap), orc.tap(tap))
         orc.close()
     eng.close()

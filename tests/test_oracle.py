@@ -1,16 +1,13 @@
 """CPU tests of the oracle (test infrastructure): pinned against the committed golden vectors produced by the
 real reference."""
 import json
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
-
-sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
-import make_golden as G  # noqa: E402  (case definitions shared with the fixture generator)
+import engine_testlib as E  # noqa: F401  (puts tools/ on sys.path)
+import make_golden as G  # case definitions shared with the fixture generator
 
 FAST_CASES = ["cone_crop", "synth_a", "synth_b", "synth_opts", "synth_disc"]
 

@@ -9,23 +9,15 @@ against the same call's optimised volume; the cost-input cases; batched device c
 map-only mode; the unchanged paths.
 """
 import ctypes
-import json
-import os
-import re
-import subprocess
-import sys
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E  # puts tools/ on sys.path
 import maps_testlib as MT
-from test_volume_export import _engine, _same
-
-sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
-import make_golden as G  # noqa: E402
-import make_golden_cost as GC  # noqa: E402
+import make_golden as G
+import make_golden_cost as GC
 
 MAPS = ["wta_left", "wta_right", "outliers", "min_cost", "peak_ratio"]
 
@@ -132,7 +124,7 @@ def test_confidence_helper_matches_loop():
             want = MT.confidence_loop(v)
             for name, g, w in zip(("min_cost", "peak_ratio"), got, want):
                 assert g.dtype == np.float32 and g.shape == (6, 7)
-                _same(f"D={D} {name}", g, w)
+                E.same(f"D={D} {name}", g, w)
             r = got[1]
             assert ((r >= 0) & (r <= 1)).all()
             if D <= 2:
@@ -155,55 +147,26 @@ def test_outlier_lists_helper():
     assert mis.dtype == np.int32 and MT.outlier_lists(np.zeros((2, 2), np.uint8))[0].shape == (0, 2)
 
 
-def test_confidence_kernel_uses_no_local_memory(tmp_path):
-    """-Xptxas -v on k_confidence.cu: no stack frame, no spills."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip("nvcc not available")
-    src = Path(__file__).resolve().parent.parent / "adcensus_b200" / "csrc" / "k_confidence.cu"
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(src), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert frames and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
+def test_confidence_kernel_uses_no_local_memory():
+    """ptxas -v on k_confidence.cu: no stack frame, no spills."""
+    report = E.ptxas_report(T.REPO / "adcensus_b200" / "csrc" / "k_confidence.cu")
+    assert report and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                          for f in report.values()), report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _oracle_maps(w, h, opt, left, right):
-    """The restatement's WTA maps, outlier lists, optimised volume and final map."""
-    orc = T.Oracle(w, h, opt)
-    orc.begin(left, right)
-    orc.run_to("SO4")
-    vol = orc.tap("VOL_AGGR").copy()
-    orc.run_to("WTA")
-    wl, wr = orc.tap("DISP_L").copy(), orc.tap("DISP_R").copy()
-    orc.run_to("OUTLIER")
-    mis, occ = orc.tap("MISMATCHES").copy(), orc.tap("OCCLUSIONS").copy()
-    while orc.step() >= 0:
-        pass
-    disp = orc.tap("DISP_L").copy()
-    orc.close()
-    return dict(wta_left=wl, wta_right=wr, lists=(mis, occ), vol=vol), disp
-
-
-def _check_maps(name, got, wl, wr, lists, vol):
-    _same(f"{name} wta_left", got["wta_left"], wl)
-    _same(f"{name} wta_right", got["wta_right"], wr)
+def _check_maps(name, got, want):
+    E.same(f"{name} wta_left", got["wta_left"], want["wta_left"])
+    E.same(f"{name} wta_right", got["wta_right"], want["wta_right"])
     gm, go = MT.outlier_lists(got["outliers"])
-    assert np.array_equal(gm, lists[0].reshape(-1, 2)), f"{name}: mismatch list"
-    assert np.array_equal(go, lists[1].reshape(-1, 2)), f"{name}: occlusion list"
-    c1, ratio = MT.confidence(vol)
-    _same(f"{name} min_cost", got["min_cost"], c1)
-    _same(f"{name} peak_ratio", got["peak_ratio"], ratio)
+    assert np.array_equal(gm, want["mismatches"].reshape(-1, 2)), f"{name}: mismatch list"
+    assert np.array_equal(go, want["occlusions"].reshape(-1, 2)), f"{name}: occlusion list"
+    c1, ratio = MT.confidence(want["opt"])
+    E.same(f"{name} min_cost", got["min_cost"], c1)
+    E.same(f"{name} peak_ratio", got["peak_ratio"], ratio)
 
 
-def _cases():
-    from test_gpu_parity import CASES
-    return CASES + [(40, 30, 3, {}, 20)]      # D = 3: pixels with d1 = 1 have no d with |d - d1| >= 2
-
-
-CASES = _cases()
+CASES = E.PARITY_CASES + [(40, 30, 3, {}, 20)]      # D = 3: pixels with d1 = 1 have no d with |d - d1| >= 2
 
 
 @pytest.mark.gpu
@@ -220,20 +183,16 @@ def test_maps_parity(case, cone):
         opt = T.default_option(**{"max_disparity": D, **over})
         left, right = T.synthetic_pair(w, h, D, seed)
     h, w, _ = left.shape
-    want, want_disp = _oracle_maps(w, h, opt, left, right)
-    eng = _engine(w, h, opt)
+    want = E.oracle_outputs(w, h, opt, left, right)
+    eng = E.engine(w, h, opt)
     disp, got = eng.match_outputs(left, right, maps=MAPS)
-    _same("final map", disp, want_disp)
-    _check_maps(case, got, want["wta_left"], want["wta_right"], want["lists"], want["vol"])
+    E.same("final map", disp, want["final"])
+    _check_maps(case, got, want)
     if not opt.do_lr_check:
         assert not got["outliers"].any()
     if case == "cone":
         assert T.sha(disp).startswith("77d70a58d1aa5c71")
     eng.close()
-
-
-def _big():
-    return json.loads((T.GOLDEN_DIR / "golden_big.json").read_text())
 
 
 def _check_hashes(name, got, g, opt):
@@ -252,7 +211,7 @@ def test_maps_large_shapes_vs_reference_goldens(name):
     hashes.  Cloth3 and 1242x375x128 also export the optimised volume (f32) in the same call: it must hash to the
     reference's SO4/VOL_AGGR and the confidence must equal the helper on it.  1080p goes through the batched device
     call with two pairs, so that the second pair's volume reads run past 2^31 bytes inside the arena."""
-    g = _big()[name]
+    g = E.golden("golden_big.json")[name]
     if name in ("cloth3", "wood2", "piano"):
         z = np.load(T.GOLDEN_DIR / "real_pairs.npz")
         left, right = z[f"{name}_left"], z[f"{name}_right"]
@@ -265,7 +224,7 @@ def test_maps_large_shapes_vs_reference_goldens(name):
     opt = T.default_option(max_disparity=D)
     hs = g["hashes"]
     if name != "p1080_s1":
-        eng = _engine(w, h, opt)
+        eng = E.engine(w, h, opt)
         vols = ["opt"] if name in ("cloth3", "kitti_s1") else []
         disp, got = eng.match_outputs(left, right, maps=MAPS, volumes=vols)
         assert T.sha(disp) == hs["MEDIAN/DISP_L"]
@@ -273,14 +232,14 @@ def test_maps_large_shapes_vs_reference_goldens(name):
         if vols:
             assert T.sha(got["opt"]) == hs["SO4/VOL_AGGR"]
             c1, ratio = MT.confidence(got["opt"])
-            _same(f"{name} min_cost", got["min_cost"], c1)
-            _same(f"{name} peak_ratio", got["peak_ratio"], ratio)
+            E.same(f"{name} min_cost", got["min_cost"], c1)
+            E.same(f"{name} peak_ratio", got["peak_ratio"], ratio)
         eng.close()
         return
     import torch
     dev = torch.device("cuda", 0)
     n = 2
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     assert eng.wave_pairs >= n
     assert n * h * w * ((D + 3) // 4 * 4) * 4 > 2 ** 31
     d_l = torch.from_numpy(np.stack([left] * n)).to(dev)
@@ -296,12 +255,8 @@ def test_maps_large_shapes_vs_reference_goldens(name):
         assert T.sha(d_disp[i].cpu().numpy()) == hs["MEDIAN/DISP_L"], f"pair {i} map"
         _check_hashes(f"pair {i}", got[i], hs, opt)
     for m in ("min_cost", "peak_ratio"):
-        _same(f"pair 1 {m}", got[1][m], got[0][m])
+        E.same(f"pair 1 {m}", got[1][m], got[0][m])
     eng.close()
-
-
-def _golden_cost():
-    return json.loads((T.GOLDEN_DIR / "golden_cost_cases.json").read_text())
 
 
 @pytest.mark.gpu
@@ -312,12 +267,12 @@ def test_maps_cost_input(case):
     hashes to the reference's SO4/VOL_AGGR."""
     import torch
     from cost_testlib import to_bf16_bits
-    want = _golden_cost()[GC.cost_case_id(case)]
+    want = E.golden("golden_cost_cases.json")[GC.cost_case_id(case)]
     left, right, opt, cost = GC.cost_case_inputs(case)
     h, w, _ = left.shape
     D = cost.shape[2]
     dev = torch.device("cuda", 0)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     n = 2
     d_l = torch.from_numpy(np.stack([left] * n)).to(dev)
     d_r = torch.from_numpy(np.stack([right] * n)).to(dev)
@@ -341,26 +296,17 @@ def test_maps_cost_input(case):
             assert T.sha(d_disp[i].cpu().numpy()) == want["MEDIAN/DISP_L"], name
             _check_hashes(name, got, want, opt)
             c1, ratio = MT.confidence(vol)
-            _same(f"{name} min_cost", got["min_cost"], c1)
-            _same(f"{name} peak_ratio", got["peak_ratio"], ratio)
+            E.same(f"{name} min_cost", got["min_cost"], c1)
+            E.same(f"{name} peak_ratio", got["peak_ratio"], ratio)
     eng.close()
-
-
-def _guarded(n, N, kind, dev, skew):
-    """A device buffer for n maps of N elements starting `skew` elements (u8: bytes) in, sentinel-filled."""
-    import torch
-    guard = 4096
-    whole = torch.empty(n * N + 2 * guard, dtype=torch.uint8 if kind == "outliers" else torch.float32, device=dev)
-    whole.view(torch.uint8).fill_(0xA5)
-    return whole, guard + skew
 
 
 def _maps_batch_check(eng, pairs, n, specs, with_disp, pipelined, vol=None):
     """n pairs (pair i = pairs[i % len(pairs)]) through match_outputs_batch_device with the map requests `specs`
-    [(kind, skew)] (and optionally one volume request (stage, layout, dtype)); every map equals the single-pair
-    match_outputs result at its offset, the final maps the single-pair maps, and no element outside the n maps changes."""
-    import torch
-    dev = torch.device("cuda", 0)
+    [(kind, skew)], each destination `skew` elements (u8: bytes) into a buffer with 4096 elements of 0xA5 bytes on either
+    side (and optionally one volume request (stage, layout, dtype)); every map equals the single-pair match_outputs
+    result at its offset, the final maps the single-pair maps, and no element outside the n maps changes."""
+    torch, dev = E.cuda()
     H, W, D = eng.height, eng.width, eng.D
     N = H * W
     k = len(pairs)
@@ -373,39 +319,29 @@ def _maps_batch_check(eng, pairs, n, specs, with_disp, pipelined, vol=None):
     d_l = torch.from_numpy(np.stack([pairs[i % k][0] for i in range(n)])).to(dev)
     d_r = torch.from_numpy(np.stack([pairs[i % k][1] for i in range(n)])).to(dev)
     d_out = torch.full((n, H, W), -1.0, dtype=torch.float32, device=dev) if with_disp else None
-    bufs = [_guarded(n, N, m, dev, skew) for m, skew in specs]
-    before = [whole.clone() for whole, _ in bufs]
+    es = {m: 1 if m == "outliers" else 4 for m in kinds}
+    bufs = [E.guarded(n * N * es[m], torch.uint8, (4096 + skew) * es[m], (4096 - skew) * es[m], 0xA5) for m, skew in specs]
     if vol:
         tdt = {"f32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16}[vol[2]]
         d_vol = torch.empty((n, H * W * D), dtype=tdt, device=dev)
-
-    def requests(first):
-        maps = [(whole.data_ptr() + (off + first * N) * whole.element_size(), m) for (whole, off), (m, _) in zip(bufs, specs)]
-        vols = [(d_vol[first:].data_ptr(), *vol)] if vol else []
-        return maps, vols
-
     st = torch.cuda.current_stream()
-    eng.set_pipelined(pipelined)
-    half = n // 2 if pipelined else n
-    for first, cnt in ((0, half), (half, n - half)):
-        if cnt == 0:
-            continue
-        maps, vols = requests(first)
-        eng.match_outputs_batch_device(cnt, d_l[first:].data_ptr(), d_r[first:].data_ptr(), maps=maps, volumes=vols,
+
+    def issue(first, count):
+        maps = [(data.data_ptr() + first * N * es[m], m) for (data, _), m in zip(bufs, kinds)]
+        vols = [(d_vol[first:].data_ptr(), *vol)] if vol else []
+        eng.match_outputs_batch_device(count, d_l[first:].data_ptr(), d_r[first:].data_ptr(), maps=maps, volumes=vols,
                                        d_disp=d_out[first:].data_ptr() if with_disp else 0, stream=st.cuda_stream)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.set_pipelined(False)
+
+    E.split_calls(eng, n, pipelined, issue)
     if with_disp:
         out = d_out.cpu().numpy()
         for i in range(n):
-            _same(f"pair {i} map", out[i], singles[i % k][0])
-    for (whole, off), (m, _), orig in zip(bufs, specs, before):
-        assert torch.equal(whole[:off], orig[:off]), f"{m}: bytes before the maps written"
-        assert torch.equal(whole[off + n * N:], orig[off + n * N:]), f"{m}: bytes after the maps written"
-        got = whole[off:off + n * N].cpu().numpy()
+            E.same(f"pair {i} map", out[i], singles[i % k][0])
+    for (data, intact), m in zip(bufs, kinds):
+        assert intact(), f"{m}: bytes outside the maps written"
+        got = data.cpu().numpy().view(np.uint8 if m == "outliers" else np.float32)
         for i in range(n):
-            _same(f"pair {i} {m}", got[i * N:(i + 1) * N].reshape(H, W), singles[i % k][1][m])
+            E.same(f"pair {i} {m}", got[i * N:(i + 1) * N].reshape(H, W), singles[i % k][1][m])
     if vol:
         raw = d_vol.view(torch.int32 if vol[2] == "f32" else torch.int16).cpu().numpy()
         for i in range(n):
@@ -424,7 +360,7 @@ def test_maps_batch_device_order_and_stride(pipelined):
     wave size); all five maps at odd offsets, with the final map, then with an exported volume in the same call."""
     w, h, D = 71, 47, 23
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     pairs = [T.synthetic_pair(w, h, D, 500 + s) for s in range(n)]
     _maps_batch_check(eng, pairs, n, BATCH_SPECS, True, pipelined)
@@ -438,7 +374,7 @@ def test_maps_batch_device_loaded_waves(pipelined):
     """Default configuration with several waves per lane in flight: confidence and outliers plus the final map."""
     w, h, D = 160, 120, 64
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     n = 2 * eng.wave_pairs * eng.lanes + 5
     pairs = [T.synthetic_pair(w, h, D, 600 + s) for s in range(7)]
     _maps_batch_check(eng, pairs, n, [("min_cost", 0), ("peak_ratio", 0), ("outliers", 0)], True, pipelined)
@@ -451,7 +387,7 @@ def test_maps_batch_device_map_only(pipelined):
     """No final map (d_disp NULL): the same side maps as a call with one."""
     w, h, D = 71, 47, 23
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     pairs = [T.synthetic_pair(w, h, D, 700 + s) for s in range(n)]
     _maps_batch_check(eng, pairs, n, BATCH_SPECS, False, pipelined)
@@ -466,7 +402,7 @@ def test_map_only_mode_skips_refinement():
     w, h, D = 97, 61, 23
     opt = T.default_option(max_disparity=D)
     left, right = T.synthetic_pair(w, h, D, 2)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     want_disp, want = eng.match_outputs(left, right, maps=MAPS)
     want_r = eng.right_disparity()
     counts = {}
@@ -483,15 +419,15 @@ def test_map_only_mode_skips_refinement():
         assert none is None
         assert eng.launch_count - c0 == counts[stop] + extra, maps
         for m in maps:
-            _same(f"{maps} {m}", got[m], want[m])
+            E.same(f"{maps} {m}", got[m], want[m])
     # with the final map: the full pipeline plus k_confidence, and the same final and right-view maps as match()
     c0 = eng.launch_count
     disp, _ = eng.match_outputs(left, right, maps=["peak_ratio"])
     assert eng.launch_count - c0 == counts["MEDIAN"] + 1
-    _same("final map", disp, want_disp)
-    _same("match()", eng.match(left, right), want_disp)
-    _same("right map", eng.right_disparity(), want_r)
-    _same("right map = wta_right", want["wta_right"], want_r)
+    E.same("final map", disp, want_disp)
+    E.same("match()", eng.match(left, right), want_disp)
+    E.same("right map", eng.right_disparity(), want_r)
+    E.same("right map = wta_right", want["wta_right"], want_r)
     eng.close()
 
 
@@ -502,7 +438,7 @@ def test_no_map_path_unchanged(cone):
     import torch
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
     n = 9
     dev = torch.device("cuda", 0)
     d_l = torch.from_numpy(np.repeat(left[None], n, 0)).to(dev)
@@ -520,16 +456,16 @@ def test_no_map_path_unchanged(cone):
     maps1, launches1 = run(lambda d: eng.match_outputs_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), d_disp=d.data_ptr(),
                                                                     stream=st.cuda_stream))
     assert launches1 == launches0
-    _same("no requests", maps1, maps0)
+    E.same("no requests", maps1, maps0)
     side = {m: torch.empty((n, h, w), dtype=torch.uint8 if m == "outliers" else torch.float32, device=dev) for m in MAPS}
     maps2, launches2 = run(lambda d: eng.match_outputs_batch_device(
         n, d_l.data_ptr(), d_r.data_ptr(), maps=[(b.data_ptr(), m) for m, b in side.items()], d_disp=d.data_ptr(),
         stream=st.cuda_stream))
     assert launches2 == launches0 + -(-n // eng.wave_pairs)     # one k_confidence per wave
-    _same("with side maps", maps2, maps0)
+    E.same("with side maps", maps2, maps0)
     maps3, launches3 = run(lambda d: eng.match_batch_device(n, d_l.data_ptr(), d_r.data_ptr(), d.data_ptr(), st.cuda_stream))
     assert launches3 == launches0
-    _same("after side maps", maps3, maps0)
-    hashes = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
+    E.same("after side maps", maps3, maps0)
+    hashes = E.golden_hashes("cone_full")
     assert all(T.sha(maps2[i]) == hashes["MEDIAN/DISP_L"] for i in range(n))
     eng.close()

@@ -12,18 +12,14 @@ host, pinned and device maps, re-setting between pipelined calls, clearing; one 
 entry's staging fallback; the rules that need an engine.
 """
 import ctypes
-import os
-import re
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E  # puts tools/ on sys.path
 import images_testlib as IT
 import rectify_testlib as R
-from test_volume_export import _engine, _same
 
 MAPS = ["wta_left", "wta_right", "outliers", "min_cost", "peak_ratio"]
 GOLDEN = T.GOLDEN_DIR / "golden_remap_cases.npz"
@@ -57,8 +53,6 @@ def test_restatement_against_opencv():
     initUndistortRectifyMap maps from 450x375, 640x480 and 1280x720 into 450x375 (both types), convertMaps of float maps,
     and 1 x 1, 1 x N, N x 1 sources."""
     cv2 = pytest.importorskip("cv2")
-    import sys
-    sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
     import make_golden_remap as MG
     rng = np.random.default_rng(11)
     for i in range(40):
@@ -167,7 +161,7 @@ def test_rectification_constants():
     assert [(n, getattr(A.Rectification, n).offset) for n, _ in A.Rectification._fields_] == [
         ("src_width", 0), ("src_height", 4), ("map_type", 8), ("reserved", 12), ("view", 16)]
     assert A.Engine.PROFILE_KERNELS["rectify"] == 14
-    h = (Path(__file__).resolve().parent.parent / "include" / "adcensus_b200.h").read_text()
+    h = (T.REPO / "include" / "adcensus_b200.h").read_text()
     assert "enum { ADC_REMAP_F32 = 0, ADC_REMAP_FIXED = 1 };" in h
 
 
@@ -189,28 +183,16 @@ def test_map_builders_python():
         _remap((mx[:, ::2], my[:, ::2]), 5, 4)
 
 
-def test_rectify_kernel_uses_no_local_memory(tmp_path):
-    """-Xptxas -v on k_rectify.cu: no stack frame and no spills in the six ingestion instantiations and the two map
+def test_rectify_kernel_uses_no_local_memory():
+    """ptxas -v on k_rectify.cu: no stack frame and no spills in the six ingestion instantiations and the two map
     conversions."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip("nvcc not available")
-    src = Path(__file__).resolve().parent.parent / "adcensus_b200" / "csrc" / "k_rectify.cu"
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(src), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 8 and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
-    assert len(re.findall(r"Compiling entry function '\w*k_rectify_ingest", r.stderr)) == 6, r.stderr
+    report = E.ptxas_report(T.REPO / "adcensus_b200" / "csrc" / "k_rectify.cu")
+    assert len(report) == 8 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                                    for f in report.values()), report
+    assert sum(f["regs"] is not None and "k_rectify_ingest" in name for name, f in report.items()) == 6, report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _torch():
-    import torch
-    return torch, torch.device("cuda", 0)
-
-
 def _frame_view(buf, fmt, h, w, rp, pp, off):
     """numpy view of one raw view in a flat buffer, as Engine.match_rectified takes it."""
     if fmt == "rgb_planar":
@@ -247,14 +229,6 @@ def _restated(bgr, fmt, maps):
     return R.remap(src, *maps)
 
 
-def _cone_rig(cv2, sw, sh, W, H, t, baseline):
-    K = np.array([[0.9 * sw, 0, sw / 2 - 3.3], [0, 0.9 * sw, sh / 2 + 2.1], [0, 0, 1]], np.float64)
-    dist = np.array([-0.12, 0.05, 0.0008, -0.0006, -0.004])
-    R1, _ = cv2.Rodrigues(np.array([0.004, -0.011 * baseline, 0.002]))
-    P = np.array([[0.95 * W, 0, W / 2, 0], [0, 0.95 * W, H / 2, 0], [0, 0, 1, 0]], np.float64)
-    return cv2.initUndistortRectifyMap(K, dist, R1, P, (W, H), t)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("src_size", [(400, 330), (450, 375), (640, 480)])
 def test_rectified_cone_rig(src_size, cone):
@@ -264,15 +238,15 @@ def test_rectified_cone_rig(src_size, cone):
     ones)."""
     cv2 = pytest.importorskip("cv2")
     import adcensus_b200 as A
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
     sw, sh = src_size
     raw = [cv2.resize(img, (sw, sh), interpolation=cv2.INTER_AREA) for img in (left, right)]
-    eng = _engine(w, h, T.default_option())
+    eng = E.engine(w, h, T.default_option())
     st = torch.cuda.current_stream()
     for t in (cv2.CV_32FC1, cv2.CV_16SC2):
-        maps = [_cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
+        maps = [R.cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
         eng.set_rectification(maps[0], maps[1], (sw, sh))
         for fmt in IT.FORMATS:
             rect = [_restated(raw[v], fmt, maps[v]) for v in range(2)]
@@ -282,9 +256,9 @@ def test_rectified_cone_rig(src_size, cone):
                 lay = [_layout(_raw(raw[v], fmt), fmt, extra, lead, 3 if extra else 0) for v in range(2)]
                 views = [_frame_view(b, fmt, sh, sw, rp, pp, off) for b, rp, pp, off in lay]
                 disp, got = eng.match_rectified(views[0], views[1], format=fmt, maps=MAPS, volumes=["cost"])
-                _same(f"{name} host disp", disp, want_disp)
+                E.same(f"{name} host disp", disp, want_disp)
                 for k in want:
-                    _same(f"{name} host {k}", got[k], want[k])
+                    E.same(f"{name} host {k}", got[k], want[k])
                 if extra == 0 and fmt not in ("bgra", "gray"):
                     continue
                 # device: both views in one buffer, the right one 1 byte after the left one's padding
@@ -301,10 +275,10 @@ def test_rectified_cone_rig(src_size, cone):
                                                  volumes=[(d_cost.data_ptr(), "cost", "hwd", "f32")],
                                                  d_disp=d_disp.data_ptr(), stream=st.cuda_stream)
                 torch.cuda.synchronize()
-                _same(f"{name} device disp", d_disp[0].cpu().numpy(), want_disp)
-                _same(f"{name} device cost", d_cost[0].cpu().numpy(), want["cost"])
+                E.same(f"{name} device disp", d_disp[0].cpu().numpy(), want_disp)
+                E.same(f"{name} device cost", d_cost[0].cpu().numpy(), want["cost"])
                 for m in MAPS:
-                    _same(f"{name} device {m}", out[m][0].cpu().numpy(), want[m])
+                    E.same(f"{name} device {m}", out[m][0].cpu().numpy(), want[m])
     eng.close()
 
 
@@ -314,7 +288,7 @@ def test_identity_maps_match_images(cone):
     format."""
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option())
+    eng = E.engine(w, h, T.default_option())
     for fixed in (False, True):
         m = R.identity_maps(w, h, fixed)
         eng.set_rectification(m, m, (w, h))
@@ -325,42 +299,15 @@ def test_identity_maps_match_images(cone):
                 l, r = IT.from_bgr(left, fmt), IT.from_bgr(right, fmt)
             want_disp, want = eng.match_images(l, r, format=fmt, volumes=["cost"])
             disp, got = eng.match_rectified(l, r, format=fmt, volumes=["cost"])
-            _same(f"identity {fixed} {fmt} disp", disp, want_disp)
-            _same(f"identity {fixed} {fmt} cost", got["cost"], want["cost"])
+            E.same(f"identity {fixed} {fmt} disp", disp, want_disp)
+            E.same(f"identity {fixed} {fmt} cost", got["cost"], want["cost"])
     eng.close()
-
-
-def _run_all(eng, n, d_left, d_right, image, stride, d_cost, pipelined, rectified=True):
-    """One call (two in pipelined mode) with a cost volume, the optimised volume as DHW bf16, all five side maps and
-    the final map; every output on the host."""
-    torch, dev = _torch()
-    h, w, D = eng.height, eng.width, eng.D
-    out = {"disp": torch.full((n, h, w), -1.0, dtype=torch.float32, device=dev),
-           "opt": torch.empty((n, D, h, w), dtype=torch.bfloat16, device=dev)}
-    for m in MAPS:
-        out[m] = torch.empty((n, h, w), dtype=torch.uint8 if m == "outliers" else torch.float32, device=dev)
-    st = torch.cuda.current_stream()
-    eng.set_pipelined(pipelined)
-    half = n // 2 if pipelined else n
-    call = eng.match_rectified_batch_device if rectified else eng.match_images_batch_device
-    for first, cnt in ((0, half), (half, n - half)):
-        if cnt == 0:
-            continue
-        call(cnt, d_left + first * stride, d_right + first * stride, image=image,
-             maps=[(out[m][first:].data_ptr(), m) for m in MAPS],
-             volumes=[(out["opt"][first:].data_ptr(), "opt", "dhw", "bf16")],
-             d_disp=out["disp"][first:].data_ptr(), d_cost=d_cost[first:].data_ptr(), cost_layout="dhw",
-             cost_dtype="f32", stream=st.cuda_stream)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.set_pipelined(False)
-    return {k: (v.view(torch.int16) if v.dtype == torch.bfloat16 else v).cpu().numpy() for k, v in out.items()}
 
 
 def _raw_batch(fmt, n, sw, sh, rng, x0=5, y0=1):
     """n pairs of random raw frames (packed BGR; gray: (g, g, g)), laid out as odd-x crops of larger frames with
     random surroundings on the device, every view in its own buffer with guard bytes after the last view."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     L = [rng.integers(0, 256, (sh, sw, 3), dtype=np.uint8) for _ in range(n)]
     Rr = [rng.integers(0, 256, (sh, sw, 3), dtype=np.uint8) for _ in range(n)]
@@ -388,9 +335,9 @@ def test_rectified_batched(pipelined):
     map types with specials (NaN, inf, huge, ties, junk high bits), every format as odd-x crops with guard bytes: every
     output of a call with a cost volume, an exported volume and all five side maps equals the packed-BGR call's on the
     restated images, and the source buffers are unchanged."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, D = 71, 47, 23
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     rng = np.random.default_rng(4)
     d_cost = torch.from_numpy(rng.random((n, D, h, w), dtype=np.float32) * np.float32(40)).to(dev)
@@ -403,8 +350,12 @@ def test_rectified_batched(pipelined):
         before = [t.clone() for t in views]
         packed_l = torch.from_numpy(np.stack([R.remap(x, *maps[0]) for x in L])).to(dev)
         packed_r = torch.from_numpy(np.stack([R.remap(x, *maps[1]) for x in Rr])).to(dev)
-        want = _run_all(eng, n, packed_l.data_ptr(), packed_r.data_ptr(), None, 3 * w * h, d_cost, pipelined, False)
-        got = _run_all(eng, n, views[0].data_ptr() + off, views[1].data_ptr() + off, desc, stride, d_cost, pipelined)
+        outputs = dict(volumes=[("opt", "dhw", "bf16")], maps=MAPS, d_cost=d_cost, cost_layout="dhw", cost_dtype="f32",
+                       pipelined=pipelined)
+        want = E.batch_outputs(eng, eng.match_images_batch_device, n, packed_l.data_ptr(), packed_r.data_ptr(), 3 * w * h,
+                               **outputs)
+        got = E.batch_outputs(eng, eng.match_rectified_batch_device, n, views[0].data_ptr() + off,
+                              views[1].data_ptr() + off, stride, image=desc, **outputs)
         for key in want:
             assert np.array_equal(got[key].view(np.uint8), want[key].view(np.uint8)), f"{fmt} fixed={fixed}: {key}"
         assert all(torch.equal(t, c) for t, c in zip(views, before)), f"{fmt}: source buffer changed"
@@ -414,7 +365,7 @@ def test_rectified_batched(pipelined):
 @pytest.mark.gpu
 def test_rectified_stride_past_2_31():
     """n = 2 gray raw pairs with an image stride above 2^31 bytes: the second pair is read from past 2^31."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     w, h, D = 97, 61, 24
     sw, sh = 120, 77
@@ -427,7 +378,7 @@ def test_rectified_stride_past_2_31():
     for i, (gl, gr) in enumerate(grays):
         buf[i * stride:i * stride + N] = torch.from_numpy(gl.reshape(-1)).to(dev)
         buf[i * stride + N + 1:i * stride + 2 * N + 1] = torch.from_numpy(gr.reshape(-1)).to(dev)
-    eng = _engine(w, h, T.default_option(max_disparity=D))
+    eng = E.engine(w, h, T.default_option(max_disparity=D))
     maps = [R.warp_maps(w, h, sw, sh, 60 + v) for v in range(2)]
     eng.set_rectification(maps[0], maps[1], (sw, sh))
     d_disp = torch.empty((2, h, w), dtype=torch.float32, device=dev)
@@ -436,7 +387,7 @@ def test_rectified_stride_past_2_31():
     torch.cuda.synchronize()
     for i, (gl, gr) in enumerate(grays):
         want = eng.match(R.remap(IT.gray_to_bgr(gl), *maps[0]), R.remap(IT.gray_to_bgr(gr), *maps[1]))
-        _same(f"pair {i}", d_disp[i].cpu().numpy(), want)
+        E.same(f"pair {i}", d_disp[i].cpu().numpy(), want)
     del buf
     eng.close()
 
@@ -447,11 +398,11 @@ def test_map_sources_and_updates():
     re-set between pipelined calls apply to the calls made after them only; clearing the maps makes the rectified
     entries fail with ADC_ERR_ARG; the rectified batch issues exactly one ingestion launch per wave more than the
     packed-BGR batch."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     w, h, D = 64, 40, 16
     sw, sh = 90, 58
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=3, lanes=2)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=3, lanes=2)
     rng = np.random.default_rng(12)
     n = 7
     waves = -(-n // eng.wave_pairs)
@@ -478,7 +429,7 @@ def test_map_sources_and_updates():
         ref = want(maps)
         # pageable host
         eng.set_rectification(maps[0], maps[1], (sw, sh))
-        _same(f"host maps {fixed}", run().cpu().numpy(), ref)
+        E.same(f"host maps {fixed}", run().cpu().numpy(), ref)
         # pinned host: the same bytes in adc_host_alloc memory
         pinned = []
         for mv in maps:
@@ -493,7 +444,7 @@ def test_map_sources_and_updates():
         for pair in pinned:
             for p, _ in pair:
                 eng._L.adc_host_free(p)   # the engine holds its own copy
-        _same(f"pinned maps {fixed}", run().cpu().numpy(), ref)
+        E.same(f"pinned maps {fixed}", run().cpu().numpy(), ref)
         # device, pitched: the maps sit in wider tensors
         dmaps = []
         for mv in maps:
@@ -507,7 +458,7 @@ def test_map_sources_and_updates():
         eng.set_rectification(dmaps[0], dmaps[1], (sw, sh))
         del dmaps
         torch.cuda.synchronize()
-        _same(f"device maps {fixed}", run().cpu().numpy(), ref)
+        E.same(f"device maps {fixed}", run().cpu().numpy(), ref)
     # re-setting between pipelined calls: each call uses the maps set when it was made
     m1 = [R.warp_maps(w, h, sw, sh, 90 + v) for v in range(2)]
     m2 = [R.warp_maps(w, h, sw, sh, 95 + v, True) for v in range(2)]
@@ -521,8 +472,8 @@ def test_map_sources_and_updates():
     eng.join(st.cuda_stream)
     torch.cuda.synchronize()
     eng.set_pipelined(False)
-    _same("pipelined call with the first maps", a.cpu().numpy(), w1)
-    _same("pipelined call with the second maps", b.cpu().numpy(), w2)
+    E.same("pipelined call with the first maps", a.cpu().numpy(), w1)
+    E.same("pipelined call with the second maps", b.cpu().numpy(), w2)
     # one ingestion launch per wave on top of the packed-BGR batch's launches
     pl = torch.from_numpy(np.stack(L)[:, :h, :w].copy()).to(dev)
     d = torch.empty((n, h, w), dtype=torch.float32, device=dev)
@@ -551,7 +502,7 @@ def test_host_entry_staging_fallback():
     """The host entry runs for raw frames that fit in the lane volume and for frames far larger than it (device
     staging), for every format, and equals the packed-BGR call on the restated images."""
     w, h, D = 24, 16, 4
-    eng = _engine(w, h, T.default_option(max_disparity=D), wave_pairs=1, lanes=1)
+    eng = E.engine(w, h, T.default_option(max_disparity=D), wave_pairs=1, lanes=1)
     vol_bytes = w * h * 4 * 4
     rng = np.random.default_rng(21)
     for sw, sh in ((20, 12), (300, 200)):
@@ -564,9 +515,9 @@ def test_host_entry_staging_fallback():
             rect = [_restated(raw[v], fmt, maps[v]) for v in range(2)]
             want_disp, want = eng.match_outputs(rect[0], rect[1], maps=["peak_ratio"], volumes=["cost"])
             disp, got = eng.match_rectified(frames[0], frames[1], format=fmt, maps=["peak_ratio"], volumes=["cost"])
-            _same(f"{sw}x{sh} {fmt} disp", disp, want_disp)
-            _same(f"{sw}x{sh} {fmt} cost", got["cost"], want["cost"])
-            _same(f"{sw}x{sh} {fmt} peak ratio", got["peak_ratio"], want["peak_ratio"])
+            E.same(f"{sw}x{sh} {fmt} disp", disp, want_disp)
+            E.same(f"{sw}x{sh} {fmt} cost", got["cost"], want["cost"])
+            E.same(f"{sw}x{sh} {fmt} peak ratio", got["peak_ratio"], want["peak_ratio"])
     eng.close()
 
 
@@ -574,11 +525,11 @@ def test_host_entry_staging_fallback():
 def test_rules_that_need_an_engine():
     """Map pitches shorter than a row, and image descriptors checked against the raw frame size (not W x H), fail with
     ADC_ERR_ARG naming the field, before any device work."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     import adcensus_b200 as A
     w, h, D = 33, 20, 16
     sw, sh = 50, 30
-    eng = _engine(w, h, T.default_option(max_disparity=D))
+    eng = E.engine(w, h, T.default_option(max_disparity=D))
     L = A.load_library()
     mx, my = R.identity_maps(w, h)
     m1, m2 = R.identity_maps(w, h, True)
@@ -610,5 +561,5 @@ def test_rules_that_need_an_engine():
     frame = np.random.default_rng(1).integers(0, 256, (sh, sw), dtype=np.uint8)
     disp, _ = eng.match_rectified(frame, frame, format="gray")
     want = eng.match(R.remap(IT.gray_to_bgr(frame), mx, my), R.remap(IT.gray_to_bgr(frame), mx, my))
-    _same("tight gray raw frame", disp, want)
+    E.same("tight gray raw frame", disp, want)
     eng.close()

@@ -14,16 +14,17 @@ import ctypes
 import os
 import re
 import subprocess
-import sys
 from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E  # puts tools/ on sys.path
+import rectify_testlib as R
 import reproject_testlib as RP
 
-ROOT = Path(__file__).resolve().parent.parent
+ROOT = T.REPO
 GOLDEN = T.GOLDEN_DIR / "golden_reproject_cases.npz"
 KINDS = ["points", "depth", "disp_s16"]
 SRC = ROOT / "adcensus_b200" / "csrc" / "k_reproject.cu"
@@ -67,7 +68,6 @@ def test_restatement_against_opencv():
     +-3e38.  The two plausible alternatives (one division h_c / h_3; a sum that starts at the first product) differ
     from OpenCV on these trials, so the trials can tell them apart."""
     cv2 = pytest.importorskip("cv2")
-    sys.path.insert(0, str(ROOT / "tools"))
     import make_golden_reproject as MG
     rng = np.random.default_rng(15)
     div_differs = start_differs = 0
@@ -175,16 +175,13 @@ def _nvcc():
     return nvcc
 
 
-def test_reproject_kernel_uses_no_local_memory(tmp_path):
-    """-Xptxas -v on k_reproject.cu: no stack frame and no spills in any of the seven instantiations (one per set of
+def test_reproject_kernel_uses_no_local_memory():
+    """ptxas -v on k_reproject.cu: no stack frame and no spills in any of the seven instantiations (one per set of
     requested outputs)."""
-    r = subprocess.run([_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(SRC), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 7 and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
-    assert len(re.findall(r"Compiling entry function '\w*k_reproject", r.stderr)) == 7, r.stderr
+    report = E.ptxas_report(SRC)
+    assert len(report) == 7 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                                    for f in report.values()), report
+    assert sum(f["regs"] is not None and "k_reproject" in name for name, f in report.items()) == 7, report
 
 
 def test_reproject_arithmetic_is_not_contracted(tmp_path):
@@ -223,21 +220,6 @@ def test_reproject_arithmetic_is_not_contracted(tmp_path):
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _torch():
-    import torch
-    return torch, torch.device("cuda", 0)
-
-
-def _engine(w, h, **kw):
-    import adcensus_b200 as A
-    return A.Engine(w, h, A.ADCensusOption(**kw))
-
-
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view({4: np.uint32, 2: np.uint16}[a.dtype.itemsize])
-
-
 def _host_all(eng, disp, Q):
     return eng.reproject(disp, Q, KINDS)
 
@@ -247,18 +229,18 @@ def _check_restated(name, got, disp, Q, dmin):
     assert RP.same_nan(got["depth"], RP.depth(disp, Q)), f"{name}: depth"
     assert np.array_equal(got["disp_s16"], RP.disp_s16(disp, dmin)), f"{name}: disp_s16"
     # depth is the points' Z bit for bit, NaN payload included: both come from the same kernel
-    assert np.array_equal(_bits(got["depth"]), _bits(np.ascontiguousarray(got["points"][:, :, 2]))), name
+    assert np.array_equal(E.bits(got["depth"]), E.bits(np.ascontiguousarray(got["points"][:, :, 2]))), name
 
 
 @pytest.mark.gpu
 def test_fixture_through_both_entries():
     """Every fixture map, on an engine of its size and min_disparity, through the host entry (all three kinds) and the
     device entry (all three kinds in one call, then each alone): equal to OpenCV's recorded output, NaN as NaN."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     st = torch.cuda.current_stream().cuda_stream
     for name, disp, Q, dmin, pts, s16 in _fixture():
         H, W = disp.shape
-        eng = _engine(W, H, min_disparity=dmin, max_disparity=dmin + 4)
+        eng = E.engine(W, H, T.default_option(min_disparity=dmin, max_disparity=dmin + 4))
         got = _host_all(eng, disp, Q)
         assert RP.same_nan(got["points"], pts), f"{name} host points"
         assert RP.same_nan(got["depth"], np.ascontiguousarray(pts[:, :, 2])), f"{name} host depth"
@@ -273,32 +255,26 @@ def test_fixture_through_both_entries():
             eng.reproject_batch_device(1, d.data_ptr(), Q, [(out[k].data_ptr(), k) for k in kinds], st)
             torch.cuda.synchronize()
             for k in kinds:
-                assert np.array_equal(_bits(out[k].cpu().numpy()), _bits(got[k])), f"{name} device {kinds}: {k}"
+                assert np.array_equal(E.bits(out[k].cpu().numpy()), E.bits(got[k])), f"{name} device {kinds}: {k}"
         eng.close()
 
 
-def _parity_cases():
-    sys.path.insert(0, str(ROOT / "tests"))
-    import test_gpu_parity as GP
-    return GP.CASES
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["cone"] + list(range(len(_parity_cases()))))
+@pytest.mark.parametrize("case", ["cone"] + list(range(len(E.PARITY_CASES))))
 def test_engine_maps(case, cone):
     """The engine's final map of Cone and of every test_gpu_parity case (min_disparity < 0 and > 0 included),
     reprojected with stereoRectify Q (CALIB_ZERO_DISPARITY on and off) through both entries: all three kinds equal the
     restatement on the same map."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     if case == "cone":
         left, right = cone
         h, w, _ = left.shape
         opt = dict(max_disparity=64)
     else:
-        w, h, D, over, seed = _parity_cases()[case]
+        w, h, D, over, seed = E.PARITY_CASES[case]
         opt = {"max_disparity": D, **over}
         left, right = T.synthetic_pair(w, h, opt["max_disparity"] - opt.get("min_disparity", 0), seed)
-    eng = _engine(w, h, **opt)
+    eng = E.engine(w, h, T.default_option(**opt))
     disp = eng.match(left, right)
     dmin = eng.option.min_disparity
     d = torch.from_numpy(disp).to(dev)
@@ -313,7 +289,7 @@ def test_engine_maps(case, cone):
                                    torch.cuda.current_stream().cuda_stream)
         torch.cuda.synchronize()
         for k in KINDS:
-            assert np.array_equal(_bits(out[k].cpu().numpy()), _bits(got[k])), f"{case} {qname} device {k}"
+            assert np.array_equal(E.bits(out[k].cpu().numpy()), E.bits(got[k])), f"{case} {qname} device {k}"
     eng.close()
 
 
@@ -322,14 +298,13 @@ def test_camera_path(cone):
     """Raw 640x480 frames of test_rectify's rig through match_rectified, then the reprojection: equal to the
     restatement and to cv2.reprojectImageTo3D of the same map."""
     cv2 = pytest.importorskip("cv2")
-    from test_rectify import _cone_rig
     left, right = cone
     h, w, _ = left.shape
     sw, sh = 640, 480
     raw = [cv2.resize(img, (sw, sh), interpolation=cv2.INTER_AREA) for img in (left, right)]
-    eng = _engine(w, h, max_disparity=64)
+    eng = E.engine(w, h, T.default_option(max_disparity=64))
     for t in (cv2.CV_32FC1, cv2.CV_16SC2):
-        maps = [_cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
+        maps = [R.cone_rig(cv2, sw, sh, w, h, t, s) for s in (1, -1)]
         eng.set_rectification(maps[0], maps[1], (sw, sh))
         disp, _ = eng.match_rectified(raw[0], raw[1])
         assert np.isfinite(disp).mean() > 0.5
@@ -340,12 +315,6 @@ def test_camera_path(cone):
     eng.close()
 
 
-def _guarded(torch, dev, count, dtype, lead):
-    """(buffer with `lead` elements before and 7 after `count` elements, all set to a sentinel, the data view)."""
-    buf = torch.full((lead + count + 7,), -7, dtype=torch.int32 if dtype == torch.float32 else torch.int16, device=dev)
-    return buf, buf[lead:lead + count].view(dtype)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("pipelined", [False, True])
 def test_batched_device_calls(pipelined):
@@ -354,10 +323,10 @@ def test_batched_device_calls(pipelined):
     elements before and after untouched, each map equal to the host entry's result.  Pipelined: the maps come from a
     pipelined match batch, and a second stream waits with adc_join before it reprojects them.  Each device call is
     exactly one launch."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, dmin, D, n = 71, 47, -3, 20, 9
     N = w * h
-    eng = _engine(w, h, min_disparity=dmin, max_disparity=dmin + D)
+    eng = E.engine(w, h, T.default_option(min_disparity=dmin, max_disparity=dmin + D))
     rng = np.random.default_rng(3)
     pairs = [T.synthetic_pair(w, h, D, 40 + i) for i in range(n)]
     Q = _fixture_Q("rig_free_1")
@@ -380,11 +349,14 @@ def test_batched_device_calls(pipelined):
         d.copy_(torch.from_numpy(flat))
         stream = st
     for kinds in (["points"], ["depth"], ["disp_s16"], KINDS):
-        bufs, views = {}, {}
+        # destinations 1 (depth: 3) elements into buffers of -7 (int32 for f32 elements) with 7 more after them
+        intact, views = {}, {}
         for k, (count, dt) in {"points": (3 * n * N, torch.float32), "depth": (n * N, torch.float32),
                                "disp_s16": (n * N, torch.int16)}.items():
             if k in kinds:
-                bufs[k], views[k] = _guarded(torch, dev, count, dt, 1 if k != "depth" else 3)
+                data, intact[k] = E.guarded(count, torch.int32 if dt == torch.float32 else torch.int16,
+                                            1 if k != "depth" else 3, 7, -7)
+                views[k] = data.view(dt)
         c0 = eng.launch_count
         with torch.cuda.stream(stream):
             eng.reproject_batch_device(n, d.data_ptr(), Q, [(views[k].data_ptr(), k) for k in kinds],
@@ -396,15 +368,13 @@ def test_batched_device_calls(pipelined):
             want = _host_all(eng, host_maps[i], Q)
             for k in kinds:
                 got = views[k].cpu().numpy().reshape((n,) + want[k].shape)[i]
-                assert np.array_equal(_bits(got), _bits(want[k])), f"pipelined={pipelined} {kinds} map {i}: {k}"
-        for k, b in bufs.items():
-            lead = 1 if k != "depth" else 3
-            raw = b.cpu().numpy()
-            assert (raw[:lead] == -7).all() and (raw[-7:] == -7).all(), f"{kinds}: guard of {k} overwritten"
+                assert np.array_equal(E.bits(got), E.bits(want[k])), f"pipelined={pipelined} {kinds} map {i}: {k}"
+        for k, ok in intact.items():
+            assert ok(), f"{kinds}: guard of {k} overwritten"
     if pipelined:
         eng.set_pipelined(False)
         for i in range(n):
-            assert np.array_equal(_bits(host_maps[i]), _bits(eng.match(*pairs[i]))), f"pipelined map {i}"
+            assert np.array_equal(E.bits(host_maps[i]), E.bits(eng.match(*pairs[i]))), f"pipelined map {i}"
     eng.close()
 
 
@@ -412,12 +382,12 @@ def test_batched_device_calls(pipelined):
 def test_points_past_2_31():
     """n = 5500 maps of 256 x 128 (three distinct ones, repeated): the points destination spans 2.16e9 bytes, past
     2^31.  Every map's points equal the host entry's for its source map, and the element after the last is untouched."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, n = 256, 128, 5500
     N = w * h
     assert 12 * n * N > 2 ** 31
     rng = np.random.default_rng(8)
-    eng = _engine(w, h, max_disparity=64)
+    eng = E.engine(w, h, T.default_option(max_disparity=64))
     base = np.stack([(rng.integers(0, 256, (h, w)) / 4.0).astype(np.float32) for _ in range(3)])
     base[0, 5, 7] = np.inf
     base[2, -1, -1] = np.nan
@@ -427,7 +397,7 @@ def test_points_past_2_31():
     pts = torch.full((3 * n * N + 1,), -7, dtype=torch.int32, device=dev)
     eng.reproject_batch_device(n, d.data_ptr(), Q, [(pts.data_ptr(), "points")], torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
-    want = torch.from_numpy(np.stack([_bits(eng.reproject(base[r], Q)["points"]).view(np.int32).reshape(-1)
+    want = torch.from_numpy(np.stack([E.bits(eng.reproject(base[r], Q)["points"]).view(np.int32).reshape(-1)
                                       for r in range(3)])).to(dev)
     got = pts[:-1].view(n, 3 * N)
     for r in range(3):
@@ -441,10 +411,10 @@ def test_points_past_2_31():
 def test_launches_and_match_unchanged(cone):
     """Each device call adds exactly one launch, the host entry one; a match batch gives the same maps with the same
     number of launches before and after reprojection calls."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, max_disparity=64)
+    eng = E.engine(w, h, T.default_option(max_disparity=64))
     n = 3
     dl = torch.from_numpy(np.stack([left] * n)).to(dev)
     dr = torch.from_numpy(np.stack([right] * n)).to(dev)
@@ -474,5 +444,5 @@ def test_launches_and_match_unchanged(cone):
     torch.cuda.synchronize()
     d1, l1 = batch()
     assert l1 == l0 and torch.equal(d0.view(torch.int32), d1.view(torch.int32))
-    assert np.array_equal(_bits(host["depth"]), _bits(np.ascontiguousarray(pts[0, :, :, 2].cpu().numpy())))
+    assert np.array_equal(E.bits(host["depth"]), E.bits(np.ascontiguousarray(pts[0, :, :, 2].cpu().numpy())))
     eng.close()

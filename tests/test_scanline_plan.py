@@ -1,22 +1,15 @@
 """CPU test of the scanline passes' launch plan (adcensus_b200/csrc/so_plan.h): slot length T, ring depth NS and the
 residency that follows from them, for the three benchmark shapes on an H100 SXM (132 SMs, 228 KB shared memory per SM)."""
 import subprocess
-from pathlib import Path
 
 import pytest
 
-ROOT = Path(__file__).resolve().parent.parent
+import engine_testlib as E
 
 
-@pytest.fixture(scope="module")
-def plan_exe(tmp_path_factory):
-    exe = tmp_path_factory.mktemp("so_plan") / "so_plan_main"
-    subprocess.run(["g++", "-O2", "-std=c++17", "-o", str(exe), str(ROOT / "tests" / "c" / "so_plan_main.cpp")], check=True)
-    return exe
-
-
-def _plan(exe, W, H, Dp, S, axis):
-    r = subprocess.run([str(exe), str(W), str(H), str(Dp), str(S), str(axis)], capture_output=True, text=True)
+def _plan(W, H, Dp, S, axis):
+    r = subprocess.run([str(E.c_tool("so_plan_main")), str(W), str(H), str(Dp), str(S), str(axis)],
+                       capture_output=True, text=True)
     assert r.returncode == 0, r.stdout + r.stderr
     T, NS, smem, ctas, per_sm, waves = map(int, r.stdout.split())
     return dict(T=T, NS=NS, smem=smem, ctas=ctas, per_sm=per_sm, waves=waves)
@@ -34,16 +27,16 @@ CASES = {
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
-def test_scanline_plan_choices(plan_exe, name):
+def test_scanline_plan_choices(name):
     args, (T, NS, ctas, per_sm, waves) = CASES[name]
-    p = _plan(plan_exe, *args)
+    p = _plan(*args)
     assert (p["T"], p["NS"], p["ctas"], p["per_sm"], p["waves"]) == (T, NS, ctas, per_sm, waves), p
     assert p["T"] * p["NS"] >= 4                              # every warp keeps at least four steps in flight
     assert (p["smem"] + 1024) * p["per_sm"] <= 228 * 1024
 
 
-def test_scanline_plan_serves_every_disparity_range(plan_exe):
+def test_scanline_plan_serves_every_disparity_range():
     for Dp in range(4, 257, 4):
         for axis in (0, 1):
-            p = _plan(plan_exe, 450, 375, Dp, 32, axis)
+            p = _plan(450, 375, Dp, 32, axis)
             assert p["T"] >= 2 and p["per_sm"] >= 1, (Dp, axis, p)

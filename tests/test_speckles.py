@@ -13,19 +13,17 @@ maps and workspace, pipelined on a second stream after adc_join; a workspace pas
 and unchanged match calls around it.
 """
 import ctypes
-import os
 import re
-import subprocess
 from collections import deque
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
+import engine_testlib as E
 import speckle_testlib as S
 
-ROOT = Path(__file__).resolve().parent.parent
+ROOT = T.REPO
 GOLDEN = T.GOLDEN_DIR / "golden_speckle_cases.npz"
 SRC = ROOT / "adcensus_b200" / "csrc" / "k_speckle.cu"
 LAUNCHES = 4
@@ -222,39 +220,23 @@ def test_speckle_constants():
     assert "k_speckle.cu" in (ROOT / "adcensus_b200" / "csrc" / "Makefile").read_text()
 
 
-def test_speckle_kernel_uses_no_local_memory(tmp_path):
-    """-Xptxas -v on k_speckle.cu: no stack frame and no spills in any of the seven kernels (local labelling, border
+def test_speckle_kernel_uses_no_local_memory():
+    """ptxas -v on k_speckle.cu: no stack frame and no spills in any of the seven kernels (local labelling, border
     merge and apply for each map type, and the count)."""
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if not Path(nvcc).exists():
-        pytest.skip("nvcc not available")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xptxas", "-v", "-c",
-                        str(SRC), "-o", str(tmp_path / "k.o")], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", r.stderr)
-    assert len(frames) == 7 and all(f == ("0", "0", "0") for f in frames), r.stderr
-    assert re.search(r"[1-9]\d* bytes lmem", r.stderr) is None, r.stderr
-    assert len(re.findall(r"Compiling entry function '\w*k_speckle_", r.stderr)) == 7, r.stderr
+    report = E.ptxas_report(SRC)
+    assert len(report) == 7 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
+                                    for f in report.values()), report
+    assert sum(f["regs"] is not None and "k_speckle_" in name for name, f in report.items()) == 7, report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _torch():
-    import torch
-    return torch, torch.device("cuda", 0)
-
-
-def _engine(w, h, **kw):
-    import adcensus_b200 as A
-    return A.Engine(w, h, A.ADCensusOption(**kw))
-
-
 def _tname(a):
     return "s16" if a.dtype == np.int16 else "f32"
 
 
 def _device_filter(eng, maps, max_size, max_diff, new_val):
     """maps [n][H][W] through the device entry on the current stream: the filtered maps (host)."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     n = maps.shape[0]
     d = torch.from_numpy(np.ascontiguousarray(maps)).to(dev)
     wb = eng.speckle_workspace_bytes(n)
@@ -271,37 +253,32 @@ def test_fixture_through_both_entries():
     recorded output (the plain path)."""
     for name, img, nv, ms, md, want, _ in _fixture():
         H, W = img.shape
-        eng = _engine(W, H, max_disparity=4)
+        eng = E.engine(W, H, T.default_option(max_disparity=4))
         assert np.array_equal(eng.filter_speckles(img, ms, md, nv), want), f"{name} host"
         assert np.array_equal(_device_filter(eng, img[None], ms, md, nv)[0], want), f"{name} device"
         eng.close()
 
 
-def _parity_cases():
-    import test_gpu_parity as GP
-    return GP.CASES
-
-
-def _engine_map(case, cone):
+def _final_map(case, cone):
     if case == "cone":
         left, right = cone
         h, w, _ = left.shape
         opt = dict(max_disparity=64)
     else:
-        w, h, D, over, seed = _parity_cases()[case]
+        w, h, D, over, seed = E.PARITY_CASES[case]
         opt = {"max_disparity": D, **over}
         left, right = T.synthetic_pair(w, h, opt["max_disparity"] - opt.get("min_disparity", 0), seed)
-    eng = _engine(w, h, **opt)
+    eng = E.engine(w, h, T.default_option(**opt))
     return eng, eng.match(left, right)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("case", ["cone"] + list(range(len(_parity_cases()))))
+@pytest.mark.parametrize("case", ["cone"] + list(range(len(E.PARITY_CASES))))
 def test_engine_maps(case, cone):
     """The engine's final map of Cone and of every test_gpu_parity case: the F32 filter (+inf = missing) through both
     entries equals the restatement; its S16 reprojection through the S16 filter equals the restatement; and, on the
     map quantised to multiples of 1/16, F32 with max_diff k/16 equals S16 with max_diff k after reprojection."""
-    eng, disp = _engine_map(case, cone)
+    eng, disp = _final_map(case, cone)
     dmin = eng.option.min_disparity
     s16_invalid = float((dmin - 1) * 16)
     s16 = eng.reproject(disp, np.eye(4), ["disp_s16"])["disp_s16"]
@@ -379,7 +356,7 @@ def test_adversarial_maps(shape):
     size: equal to the restatement."""
     H, W = shape
     rng = np.random.default_rng(H + W)
-    eng = _engine(W, H, max_disparity=4)
+    eng = E.engine(W, H, T.default_option(max_disparity=4))
     for name, m, nv, md in _adversarial(H, W, rng):
         f = m.astype(np.float32)
         sizes = {"serpentine": int((m == 1).sum()), "constant": H * W, "checkerboard": 1, "noise": 3}
@@ -401,19 +378,13 @@ def test_components_straddling_tile_borders(s):
     H, W = 1080, 1920
     rng = np.random.default_rng(s)
     m = _straddling(H, W, s, rng)
-    eng = _engine(W, H, max_disparity=4)
+    eng = E.engine(W, H, T.default_option(max_disparity=4))
     want = S.filter_s16(m, 0.0, s, 0.0)
     assert (want != m).any() and (want != 0).any()
     assert np.array_equal(_device_filter(eng, m[None], s, 0.0, 0.0)[0], want)
     f = m.astype(np.float32)
     assert S.same_bits(_device_filter(eng, f[None], s, 0.0, 0.0)[0], S.filter_f32(f, 0.0, s, 0.0))
     eng.close()
-
-
-def _guarded(torch, dev, count, dtype, lead):
-    """(buffer with `lead` elements before and 7 after `count` elements, all a sentinel, the data view)."""
-    buf = torch.full((lead + count + 7,), -7, dtype=dtype, device=dev)
-    return buf, buf[lead:lead + count]
 
 
 @pytest.mark.gpu
@@ -424,13 +395,14 @@ def test_batched_device_calls(pipelined, map_type):
     offset: guard elements before and after both untouched, each map equal to the host entry's result and to the
     restatement, four launches.  Pipelined: the maps come from a pipelined match batch and a second stream waits with
     adc_join before it filters them (S16: after a reprojection on that stream)."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, dmin, D, n = 71, 47, -3, 20, 9
     N = w * h
-    eng = _engine(w, h, min_disparity=dmin, max_disparity=dmin + D)
+    eng = E.engine(w, h, T.default_option(min_disparity=dmin, max_disparity=dmin + D))
     pairs = [T.synthetic_pair(w, h, D, 40 + i) for i in range(n)]
     st = torch.cuda.current_stream()
-    fbuf, f = _guarded(torch, dev, n * N, torch.float32, 1)
+    # maps and workspace 1, 3 and 5 elements into buffers of -7 with 7 more after them
+    f, f_intact = E.guarded(n * N, torch.float32, 1, 7, -7)
     if pipelined:
         dl = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev)
         dr = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev)
@@ -442,14 +414,14 @@ def test_batched_device_calls(pipelined, map_type):
         f.copy_(torch.from_numpy(np.stack([eng.match(*p) for p in pairs]).reshape(-1)))
         stream = st
     if map_type == "s16":
-        mbuf, maps = _guarded(torch, dev, n * N, torch.int16, 3)
+        maps, maps_intact = E.guarded(n * N, torch.int16, 3, 7, -7)
         with torch.cuda.stream(stream):
             eng.reproject_batch_device(n, f.data_ptr(), np.eye(4), [(maps.data_ptr(), "disp_s16")], stream.cuda_stream)
     else:
-        mbuf, maps = fbuf, f
+        maps, maps_intact = f, f_intact
     wb = eng.speckle_workspace_bytes(n)
     assert wb == 8 * n * N
-    wbuf, work = _guarded(torch, dev, wb // 4, torch.int32, 5)
+    work, work_intact = E.guarded(wb // 4, torch.int32, 5, 7, -7)
     c0 = eng.launch_count
     with torch.cuda.stream(stream):
         src = maps.clone()
@@ -464,9 +436,7 @@ def test_batched_device_calls(pipelined, map_type):
         assert S.same_bits(got[i], eng.filter_speckles(srcs[i], 30, md)), (map_type, pipelined, i)
         nv = np.inf if map_type == "f32" else (dmin - 1) * 16
         assert S.same_bits(got[i], S.filter_any(srcs[i], nv, 30, md)), (map_type, pipelined, i)
-    for b, lead in ((mbuf, 1 if map_type == "f32" else 3), (wbuf, 5)):
-        raw = b.cpu().numpy()
-        assert (raw[:lead] == -7).all() and (raw[-7:] == -7).all(), "guard overwritten"
+    assert maps_intact() and work_intact(), "guard overwritten"
     # a workspace one byte short is refused, naming the field
     import adcensus_b200 as A
     with pytest.raises(A.AdcError, match="work_bytes"):
@@ -481,11 +451,11 @@ def test_batched_device_calls(pipelined, map_type):
 def test_workspace_past_2_31():
     """n = 8300 S16 maps of 256 x 128 (three distinct ones, repeated): the workspace spans 2.18e9 bytes, past 2^31.
     Every map equals the restatement of its source, and the element after the last map is untouched."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     w, h, n = 256, 128, 8300
     N = w * h
     rng = np.random.default_rng(9)
-    eng = _engine(w, h, max_disparity=4)
+    eng = E.engine(w, h, T.default_option(max_disparity=4))
     base = np.stack([rng.integers(-3, 4, (h, w)).astype(np.int16) * 16 for _ in range(3)])
     base[1] = 5
     wb = eng.speckle_workspace_bytes(n)
@@ -510,10 +480,10 @@ def test_workspace_past_2_31():
 def test_launches_and_match_unchanged(cone):
     """Each call makes exactly four launches whatever the content (n = 0: none); a match batch gives the same maps
     with the same number of launches before and after speckle calls."""
-    torch, dev = _torch()
+    torch, dev = E.cuda()
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, max_disparity=64)
+    eng = E.engine(w, h, T.default_option(max_disparity=64))
     n = 3
     dl = torch.from_numpy(np.stack([left] * n)).to(dev)
     dr = torch.from_numpy(np.stack([right] * n)).to(dev)

@@ -8,25 +8,20 @@ the cost-input round trip; volumes-only mode; the batched device entry point (of
 unchanged no-export path.
 """
 import ctypes
-import json
-import sys
 from fractions import Fraction
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import adc_testlib as T
 import cost_testlib as CT
+import engine_testlib as E  # puts tools/ on sys.path
 import export_testlib as XT
-
-sys.path.insert(0, str(Path(__file__).resolve().parent.parent / "tools"))
-import make_golden_cost as GC  # noqa: E402
+import make_golden_cost as GC
 
 STAGES = ["cost", "aggr", "opt"]
 LAYOUTS = ["hwd", "dhw"]
 DTYPES = ["f32", "f16", "bf16"]
-ORACLE_TAP = {"cost": ("COST", "VOL_INIT"), "aggr": ("AGG4", "VOL_AGGR"), "opt": ("SO4", "VOL_AGGR")}
 
 
 # ---- CPU ------------------------------------------------------------------------------------------
@@ -135,43 +130,7 @@ def test_bf16_rn_helper_exact():
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
-def _engine(w, h, opt, **kw):
-    import adcensus_b200 as A
-    o = A.ADCensusOption()
-    for name, _ in T.Option._fields_:
-        if not name.startswith("_"):
-            setattr(o, name, getattr(opt, name))
-    return A.Engine(w, h, o, **kw)
-
-
-def _bits(a):
-    a = np.ascontiguousarray(a)
-    return a.view({4: np.uint32, 2: np.uint16}[a.dtype.itemsize]) if a.dtype.kind == "f" else a
-
-
-def _same(name, got, want):
-    assert got.shape == want.shape, f"{name}: shape {got.shape} vs {want.shape}"
-    eq = _bits(got) == _bits(want)
-    assert eq.all(), f"{name}: {int((~eq).sum())} of {eq.size} values differ"
-
-
-def _oracle_volumes(w, h, opt, left, right):
-    orc = T.Oracle(w, h, opt)
-    orc.begin(left, right)
-    out = {}
-    for name in STAGES:
-        st, tap = ORACLE_TAP[name]
-        orc.run_to(st)
-        out[name] = orc.tap(tap).copy()
-    while orc.step() >= 0:
-        pass
-    disp = orc.tap("DISP_L").copy()
-    orc.close()
-    return out, disp
-
-
 def _parity_cases():
-    from test_gpu_parity import CASES
     pick = {"130x70x37": lambda c: c[:3] == (130, 70, 37),             # D % 4 != 0
             "33x21x5": lambda c: c[2] == 5,
             "300x24x256": lambda c: c[2] == 256,
@@ -181,7 +140,7 @@ def _parity_cases():
             "97x61x24-unfused": lambda c: c[:3] == (97, 61, 24)}     # COST in volA instead of volB
     out = []
     for k, f in pick.items():
-        (case,) = [c for c in CASES if f(c)]
+        (case,) = [c for c in E.PARITY_CASES if f(c)]
         out.append((k, case, "DBG_UNFUSED_AGG" if k.endswith("unfused") else 0))
     return out
 
@@ -206,21 +165,17 @@ def test_export_stage_parity(case, cone):
         left, right = T.synthetic_pair(w, h, D, seed)
         flags = getattr(A.engine, flag) if flag else 0
     h, w, _ = left.shape
-    want, want_disp = _oracle_volumes(w, h, opt, left, right)
-    eng = _engine(w, h, opt, debug_flags=flags)
+    want = E.oracle_outputs(w, h, opt, left, right)
+    eng = E.engine(w, h, opt, debug_flags=flags)
     for layout in LAYOUTS:
         for dtype in DTYPES:
             disp, vols = eng.match_volumes(left, right, STAGES, layout, dtype)
-            _same(f"{layout}/{dtype} map", disp, want_disp)
+            E.same(f"{layout}/{dtype} map", disp, want["final"])
             for name in STAGES:
-                _same(f"{layout}/{dtype} {name}", vols[name], XT.export_of(want[name], layout, dtype))
+                E.same(f"{layout}/{dtype} {name}", vols[name], XT.export_of(want[name], layout, dtype))
             if case == "cone":
                 assert T.sha(disp).startswith("77d70a58d1aa5c71")
     eng.close()
-
-
-def _big():
-    return json.loads((T.GOLDEN_DIR / "golden_big.json").read_text())
 
 
 @pytest.mark.gpu
@@ -230,7 +185,7 @@ def test_export_large_shapes_vs_reference_goldens(name):
     SO4/VOL_AGGR hashes.  1080p goes through the batched device call with two pairs, so that the second pair's
     volumes (1.6 GB each) lie beyond 2^31 bytes of the destinations; its OPT volume is exported as DHW and transposed back
     on the host."""
-    g = _big()[name]
+    g = E.golden("golden_big.json")[name]
     if name == "cloth3":
         z = np.load(T.GOLDEN_DIR / "real_pairs.npz")
         left, right = z["cloth3_left"], z["cloth3_right"]
@@ -242,7 +197,7 @@ def test_export_large_shapes_vs_reference_goldens(name):
     h, w, _ = left.shape
     opt = T.default_option(max_disparity=D)
     if name != "p1080_s1":
-        eng = _engine(w, h, opt)
+        eng = E.engine(w, h, opt)
         disp, vols = eng.match_volumes(left, right, ["aggr", "opt"], "hwd", "f32")
         assert T.sha(vols["aggr"]) == g["hashes"]["AGG4/VOL_AGGR"]
         assert T.sha(vols["opt"]) == g["hashes"]["SO4/VOL_AGGR"]
@@ -254,7 +209,7 @@ def test_export_large_shapes_vs_reference_goldens(name):
     n, ND = 2, h * w * D
     d_opt = torch.empty((n, D, h, w), dtype=torch.float32, device=dev)     # before the engine: its sizing sees them
     d_agg = torch.empty((n, h, w, D), dtype=torch.float32, device=dev)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     d_l = torch.from_numpy(np.stack([left] * n)).to(dev)
     d_r = torch.from_numpy(np.stack([right] * n)).to(dev)
     d_disp = torch.empty((n, h, w), dtype=torch.float32, device=dev)
@@ -273,28 +228,24 @@ def test_export_large_shapes_vs_reference_goldens(name):
     eng.close()
 
 
-def _golden_cost():
-    return json.loads((T.GOLDEN_DIR / "golden_cost_cases.json").read_text())
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", GC.COST_CASES, ids=[GC.cost_case_id(c) for c in GC.COST_CASES])
 def test_export_cost_input_round_trip(case):
     """A caller's cost in, the engine's volumes out: AGGR / OPT hash to the reference's AGG4 / SO4 volumes for that
     cost, COST is the cost itself, the map the reference's."""
-    want = _golden_cost()[GC.cost_case_id(case)]
+    want = E.golden("golden_cost_cases.json")[GC.cost_case_id(case)]
     left, right, opt, cost = GC.cost_case_inputs(case)
     h, w, _ = left.shape
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     for cl in LAYOUTS:
         c = cost if cl == "hwd" else np.ascontiguousarray(cost.transpose(2, 0, 1))
         disp, vols = eng.match_volumes(left, right, STAGES, "hwd", "f32", cost=c, cost_layout=cl)
-        _same(f"{cl} cost", vols["cost"], CT.cost_domain(cost))
+        E.same(f"{cl} cost", vols["cost"], CT.cost_domain(cost))
         assert T.sha(vols["aggr"]) == want["AGG4/VOL_AGGR"], cl
         assert T.sha(vols["opt"]) == want["SO4/VOL_AGGR"], cl
         assert T.sha(disp) == want["MEDIAN/DISP_L"], cl
         _, vo = eng.match_volumes(left, right, "opt", "dhw", "bf16", cost=c, cost_layout=cl, disparity=False)
-        _same(f"{cl} opt dhw bf16", vo["opt"], XT.export_of(vols["opt"], "dhw", "bf16"))
+        E.same(f"{cl} opt dhw bf16", vo["opt"], XT.export_of(vols["opt"], "dhw", "bf16"))
     eng.close()
 
 
@@ -310,13 +261,13 @@ def test_export_cost_value_domain():
     mask = rng.random(cost.shape) < 0.08
     cost[mask] = specials[rng.integers(0, len(specials), int(mask.sum()))]
     clamped = CT.cost_domain(cost)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     want_disp = eng.match_cost(left, right, cost, "hwd")
     for layout in LAYOUTS:
         for dtype in DTYPES:
             disp, vols = eng.match_volumes(left, right, ["cost"], layout, dtype, cost=cost)
-            _same(f"{layout}/{dtype} cost", vols["cost"], XT.export_of(clamped, layout, dtype))
-            _same(f"{layout}/{dtype} map", disp, want_disp)
+            E.same(f"{layout}/{dtype} cost", vols["cost"], XT.export_of(clamped, layout, dtype))
+            E.same(f"{layout}/{dtype} map", disp, want_disp)
     eng.close()
 
 
@@ -327,7 +278,7 @@ def test_volumes_only_mode():
     w, h, D = 97, 61, 23
     opt = T.default_option(max_disparity=D)
     left, right = T.synthetic_pair(w, h, D, 2)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     want = eng.match(left, right)
     want_r = eng.right_disparity()
     c0 = eng.launch_count
@@ -338,34 +289,23 @@ def test_volumes_only_mode():
         disp, full = eng.match_volumes(left, right, stages, "dhw", "bf16")
         with_map = eng.launch_count - c0
         assert with_map == per_match + len(stages), stages
-        _same(f"{stages} map", disp, want)
-        _same(f"{stages} right map", eng.right_disparity(), want_r)
+        E.same(f"{stages} map", disp, want)
+        E.same(f"{stages} right map", eng.right_disparity(), want_r)
         c0 = eng.launch_count
         none, only = eng.match_volumes(left, right, stages, "dhw", "bf16", disparity=False)
         assert none is None
         assert eng.launch_count - c0 < with_map, stages
         for s in stages:
-            _same(f"{stages} {s}", only[s], full[s])
+            E.same(f"{stages} {s}", only[s], full[s])
     eng.close()
-
-
-def _guarded(n, ND, dtype, dev, skew):
-    """A device buffer with n*ND elements of `dtype` starting `skew` elements in, sentinel-filled, plus the whole
-    allocation (for the guard check)."""
-    import torch
-    tdt = {"f32": torch.float32, "f16": torch.float16, "bf16": torch.bfloat16}[dtype]
-    guard = 4096
-    whole = torch.empty(n * ND + 2 * guard, dtype=tdt, device=dev)
-    whole.view(torch.uint8).fill_(0xA5)
-    return whole, guard + skew
 
 
 def _export_batch_check(eng, pairs, n, specs, with_disp, pipelined):
     """n pairs (pair i = pairs[i % len(pairs)]) through match_volumes_batch_device with the volume requests `specs`
-    [(stage, layout, dtype, skew)]; every volume and map equals the single-pair match_volumes result at its offset, and
-    no element outside the n volumes changes."""
-    import torch
-    dev = torch.device("cuda", 0)
+    [(stage, layout, dtype, skew)], each destination `skew` elements into a buffer with 4096 elements of 0xA5 bytes on
+    either side; every volume and map equals the single-pair match_volumes result at its offset, and no element outside
+    the n volumes changes."""
+    torch, dev = E.cuda()
     H, W, D = eng.height, eng.width, eng.D
     ND = H * W * D
     k = len(pairs)
@@ -380,39 +320,30 @@ def _export_batch_check(eng, pairs, n, specs, with_disp, pipelined):
     d_l = torch.from_numpy(np.stack([pairs[i % k][0] for i in range(n)])).to(dev)
     d_r = torch.from_numpy(np.stack([pairs[i % k][1] for i in range(n)])).to(dev)
     d_out = torch.full((n, H, W), -1.0, dtype=torch.float32, device=dev) if with_disp else None
-    bufs = [_guarded(n, ND, dtype, dev, skew) for (_, _, dtype, skew) in specs]
-    before = [whole.clone() for whole, _ in bufs]
     es = {"f32": 4, "f16": 2, "bf16": 2}
-
-    def outs(first):
-        return [(whole.data_ptr() + (off + first * ND) * es[dtype], stage, layout, dtype)
-                for (whole, off), (stage, layout, dtype, _) in zip(bufs, specs)]
-
+    bufs = [E.guarded(n * ND * es[dtype], torch.uint8, (4096 + skew) * es[dtype], (4096 - skew) * es[dtype], 0xA5)
+            for (_, _, dtype, skew) in specs]
     st = torch.cuda.current_stream()
-    eng.set_pipelined(pipelined)
-    half = n // 2 if pipelined else n
-    for first, cnt in ((0, half), (half, n - half)):
-        if cnt == 0:
-            continue
-        eng.match_volumes_batch_device(cnt, d_l[first:].data_ptr(), d_r[first:].data_ptr(), outs(first),
+
+    def issue(first, count):
+        outs = [(data.data_ptr() + first * ND * es[dtype], stage, layout, dtype)
+                for (data, _), (stage, layout, dtype, _) in zip(bufs, specs)]
+        eng.match_volumes_batch_device(count, d_l[first:].data_ptr(), d_r[first:].data_ptr(), outs,
                                        d_disp=d_out[first:].data_ptr() if with_disp else 0, stream=st.cuda_stream)
-    eng.join(st.cuda_stream)
-    torch.cuda.synchronize()
-    eng.set_pipelined(False)
+
+    E.split_calls(eng, n, pipelined, issue)
     if with_disp:
         out = d_out.cpu().numpy()
         for i in range(n):
-            _same(f"pair {i} map", out[i], singles[i % k][0])
-    for (whole, off), (stage, layout, dtype, _), orig in zip(bufs, specs, before):
-        raw = whole.view(torch.int32 if es[dtype] == 4 else torch.int16)
-        rawo = orig.view(raw.dtype)
-        assert torch.equal(raw[:off], rawo[:off]), f"{stage}: bytes before the volumes written"
-        assert torch.equal(raw[off + n * ND:], rawo[off + n * ND:]), f"{stage}: bytes after the volumes written"
-        got = raw[off:off + n * ND].cpu().numpy()
+            E.same(f"pair {i} map", out[i], singles[i % k][0])
+    for (data, intact), (stage, layout, dtype, _) in zip(bufs, specs):
+        assert intact(), f"{stage}: bytes outside the volumes written"
+        got = data.cpu().numpy()
         shape = (H, W, D) if layout == "hwd" else (D, H, W)
         for i in range(n):
             want = singles[i % k][1][stage]
-            _same(f"pair {i} {stage} {layout}/{dtype}", got[i * ND:(i + 1) * ND].reshape(shape).view(want.dtype), want)
+            raw = got[i * ND * es[dtype]:(i + 1) * ND * es[dtype]]
+            E.same(f"pair {i} {stage} {layout}/{dtype}", raw.view(want.dtype).reshape(shape), want)
 
 
 # N = 71*47 and D = 23 are odd: pair i starts at an odd element, so every path of the kernels' alignment handling runs
@@ -427,7 +358,7 @@ def test_export_batch_device_order_and_stride(pipelined):
     volume sizes and odd destination offsets."""
     w, h, D = 71, 47, 23
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     pairs = [T.synthetic_pair(w, h, D, 100 + s) for s in range(n)]
     _export_batch_check(eng, pairs, n, BATCH_SPECS, True, pipelined)
@@ -441,7 +372,7 @@ def test_export_batch_device_loaded_waves(pipelined):
     """Case B: default configuration with several waves per lane in flight, DHW bf16 OPT export plus the map."""
     w, h, D = 160, 120, 64
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt)
+    eng = E.engine(w, h, opt)
     n = 2 * eng.wave_pairs * eng.lanes + 5
     pairs = [T.synthetic_pair(w, h, D, 200 + s) for s in range(7)]
     _export_batch_check(eng, pairs, n, [("opt", "dhw", "bf16", 0)], True, pipelined)
@@ -454,7 +385,7 @@ def test_export_batch_device_volumes_only(pipelined):
     """Case C: no map output; the pipeline stops after the optimised volume."""
     w, h, D = 71, 47, 23
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=3)
     n = 3 * eng.wave_pairs + 2
     pairs = [T.synthetic_pair(w, h, D, 300 + s) for s in range(n)]
     _export_batch_check(eng, pairs, n, [("opt", "dhw", "bf16", 1), ("cost", "hwd", "f32", 0)], False, pipelined)
@@ -468,7 +399,7 @@ def test_export_batch_device_cost_input():
     dev = torch.device("cuda", 0)
     w, h, D = 72, 48, 24
     opt = T.default_option(max_disparity=D)
-    eng = _engine(w, h, opt, wave_pairs=4, lanes=2)
+    eng = E.engine(w, h, opt, wave_pairs=4, lanes=2)
     n = 11
     ins = [T.synthetic_pair(w, h, D, 400 + s) for s in range(n)]
     costs = [np.ascontiguousarray(CT.synthetic_cost(w, h, D, 400 + s).transpose(2, 0, 1)) for s in range(n)]
@@ -487,9 +418,9 @@ def test_export_batch_device_cost_input():
         for i in range(n):
             disp, v = eng.match_volumes(ins[i][0], ins[i][1], "opt", "dhw", "bf16", cost=CT.to_bf16_bits(costs[i]),
                                         cost_layout="dhw", cost_dtype="bf16")
-            _same(f"pair {i} opt", got[i], v["opt"])
+            E.same(f"pair {i} opt", got[i], v["opt"])
             if with_disp:
-                _same(f"pair {i} map", d_disp[i].cpu().numpy(), disp)
+                E.same(f"pair {i} map", d_disp[i].cpu().numpy(), disp)
     eng.close()
 
 
@@ -499,7 +430,7 @@ def test_no_export_path_unchanged(cone):
     import torch
     left, right = cone
     h, w, _ = left.shape
-    eng = _engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
+    eng = E.engine(w, h, T.default_option(), wave_pairs=4, lanes=3)
     n = 9
     dev = torch.device("cuda", 0)
     d_l = torch.from_numpy(np.repeat(left[None], n, 0)).to(dev)
@@ -520,8 +451,8 @@ def test_no_export_path_unchanged(cone):
     eng.match_volumes(left, right, STAGES, "hwd", "f16")
     torch.cuda.synchronize()
     maps1, launches1 = batch()
-    _same("maps", maps1, maps0)
+    E.same("maps", maps1, maps0)
     assert launches1 == launches0
-    hashes = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
+    hashes = E.golden_hashes("cone_full")
     assert all(T.sha(maps1[i]) == hashes["MEDIAN/DISP_L"] for i in range(n))
     eng.close()
