@@ -11,7 +11,9 @@ from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TA
                      load_library, Invalid_Float, COST_HWD, COST_DHW, COST_F32, COST_F16, COST_BF16, COST_MAX,
                      VOL_COST, VOL_AGGR, VOL_OPT, MAP_WTA_LEFT, MAP_WTA_RIGHT, MAP_OUTLIERS, MAP_MIN_COST,
                      MAP_PEAK_RATIO, IMG_BGR, IMG_RGB, IMG_BGRA, IMG_RGBA, IMG_GRAY, IMG_RGB_PLANAR, ImageDesc,
-                     IMG_BAYER_RGGB, IMG_BAYER_GRBG, IMG_BAYER_BGGR, IMG_BAYER_GBRG, BAYER_FORMATS, image_desc, REMAP_F32, REMAP_FIXED, Remap, Rectification, REPROJ_POINTS, REPROJ_DEPTH,
+                     IMG_BAYER_RGGB, IMG_BAYER_GRBG, IMG_BAYER_BGGR, IMG_BAYER_GBRG, BAYER_FORMATS, IMG_NV12, IMG_NV21,
+                     IMG_YUYV, IMG_UYVY, IMG_YVYU, YUV_FORMATS, image_desc, REMAP_F32, REMAP_FIXED, Remap,
+                     Rectification, REPROJ_POINTS, REPROJ_DEPTH,
                      REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut, SPECKLE_S16,
                      SPECKLE_F32, SPECKLE_TYPES, SpeckleParams)
 from .build import build_library  # noqa: F401
@@ -21,6 +23,7 @@ __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "T
            "COST_MAX", "VOL_COST", "VOL_AGGR", "VOL_OPT", "MAP_WTA_LEFT", "MAP_WTA_RIGHT", "MAP_OUTLIERS", "MAP_MIN_COST",
            "MAP_PEAK_RATIO", "IMG_BGR", "IMG_RGB", "IMG_BGRA", "IMG_RGBA", "IMG_GRAY", "IMG_RGB_PLANAR", "ImageDesc",
            "IMG_BAYER_RGGB", "IMG_BAYER_GRBG", "IMG_BAYER_BGGR", "IMG_BAYER_GBRG", "BAYER_FORMATS",
+           "IMG_NV12", "IMG_NV21", "IMG_YUYV", "IMG_UYVY", "IMG_YVYU", "YUV_FORMATS",
            "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
            "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut", "SPECKLE_S16", "SPECKLE_F32", "SPECKLE_TYPES",
            "SpeckleParams"]

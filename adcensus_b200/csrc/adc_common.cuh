@@ -155,7 +155,12 @@ struct AdcImageGeom {
 };
 void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
                              const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches);
-int adc_image_bytes_per_pixel(int format);   // per plane for ADC_IMG_RGB_PLANAR
+// The tight layout of a w x h view in `format`: row pitch, plane pitch (ADC_IMG_RGB_PLANAR: from one channel plane to
+// the next; NV12 / NV21: from the luma plane to the chroma plane; else 0) and footprint (in image_stride).
+AdcImageGeom adc_image_tight(int format, long long w, long long h);
+// The bytes of a w x h view the ingestion kernels read (the tight footprint without the padding byte of odd-width
+// 4:2:0 luma rows).
+long long adc_image_read_bytes(int format, long long w, long long h);
 // rectified ingestion (k_rectify.cu).  The engine's internal form of a view's remap table: one uint2 per output pixel,
 // .x = (u16)x0 | (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
 struct AdcRectGeom {

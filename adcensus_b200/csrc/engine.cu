@@ -720,14 +720,17 @@ MatchReq output_req(const void* cost, int cost_layout, int cost_dtype, const flo
 int check_image_desc(const char* fn, const adc_image_desc* img) {
     if (!img) return ADC_OK;
     const bool known = (img->format >= ADC_IMG_BGR && img->format <= ADC_IMG_RGB_PLANAR) ||
-                       (img->format >= ADC_IMG_BAYER_RGGB && img->format <= ADC_IMG_BAYER_GBRG);
+                       (img->format >= ADC_IMG_BAYER_RGGB && img->format <= ADC_IMG_BAYER_GBRG) ||
+                       (img->format >= ADC_IMG_NV12 && img->format <= ADC_IMG_YVYU);
     if (!known) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
     if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
     if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
     if (img->plane_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is negative", fn, (long long)img->plane_pitch);
     if (img->image_stride < 0) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld is negative", fn, (long long)img->image_stride);
-    if (img->format != ADC_IMG_RGB_PLANAR && img->plane_pitch != 0)
-        return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format that is not ADC_IMG_RGB_PLANAR", fn);
+    const bool planes = img->format == ADC_IMG_RGB_PLANAR || img->format == ADC_IMG_NV12 || img->format == ADC_IMG_NV21;
+    if (!planes && img->plane_pitch != 0)
+        return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format other than ADC_IMG_RGB_PLANAR, ADC_IMG_NV12 "
+                    "and ADC_IMG_NV21", fn);
     return ADC_OK;
 }
 
@@ -736,20 +739,25 @@ int check_image_desc(const char* fn, const adc_image_desc* img) {
 // replaced.
 int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, int n, AdcImageGeom* g) {
     const adc_image_desc d = img ? *img : adc_image_desc{};
-    const long long W = w, H = h, bpp = adc_image_bytes_per_pixel(d.format);
+    const long long H = h, min_row = adc_image_tight(d.format, w, h).row_pitch;
+    const bool yuv420 = d.format == ADC_IMG_NV12 || d.format == ADC_IMG_NV21;
+    const char* min_row_rule = yuv420 ? "2 * ceil(W / 2)" : d.format >= ADC_IMG_YUYV ? "4 * ceil(W / 2)" : "W * bytes per pixel";
     g->format = d.format;
-    g->row_pitch = d.row_pitch ? (long long)d.row_pitch : W * bpp;
-    if (g->row_pitch < W * bpp)
-        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is less than W * bytes per pixel (%lld)", fn, g->row_pitch, W * bpp);
+    g->row_pitch = d.row_pitch ? (long long)d.row_pitch : min_row;
+    if (g->row_pitch < min_row)
+        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is less than %s (%lld)", fn, g->row_pitch, min_row_rule, min_row);
     long long foot = 0;
     if (__builtin_mul_overflow(H, g->row_pitch, &foot)) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is too large", fn, g->row_pitch);
     g->plane_pitch = 0;
-    if (d.format == ADC_IMG_RGB_PLANAR) {
+    if (d.format == ADC_IMG_RGB_PLANAR || yuv420) {
         g->plane_pitch = d.plane_pitch ? (long long)d.plane_pitch : foot;
         if (g->plane_pitch < foot)
             return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is less than H * row_pitch (%lld)", fn, g->plane_pitch, foot);
-        if (__builtin_mul_overflow(3ll, g->plane_pitch, &foot))
-            return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is too large", fn, g->plane_pitch);
+        long long chroma = 0;   // NV12 / NV21: ceil(H/2) chroma rows after the plane pitch
+        const bool over = yuv420 ? __builtin_mul_overflow((H + 1) / 2, g->row_pitch, &chroma) ||
+                                       __builtin_add_overflow(g->plane_pitch, chroma, &foot)
+                                 : __builtin_mul_overflow(3ll, g->plane_pitch, &foot);
+        if (over) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is too large", fn, g->plane_pitch);
     }
     g->image_stride = d.image_stride ? (long long)d.image_stride : foot;
     if (g->image_stride < foot)
@@ -803,8 +811,7 @@ int view_h(const adc_engine* e, const MatchReq& q) { return q.rect ? q.rect->src
 
 // Bytes of one pair's views of an ingesting request, uploaded tightly (upload_pair).
 size_t staged_bytes(const adc_engine* e, const MatchReq& q) {
-    const size_t N = (size_t)view_w(e, q) * view_h(e, q);
-    return 2 * N * (q.img->format == ADC_IMG_RGB_PLANAR ? 3 : adc_image_bytes_per_pixel(q.img->format));
+    return 2 * (size_t)adc_image_tight(q.img->format, view_w(e, q), view_h(e, q)).image_stride;
 }
 
 // One pair's host inputs of request q -> lane ln, for a run that stops after `last`.  Packed BGR rows (raw ==
@@ -828,14 +835,18 @@ int upload_pair(adc_engine* e, Lane& ln, const MatchReq& q, const uint8_t* left,
         CK(cudaMemcpyAsync(ln.w.bgr, ln.pin_in, 2 * IMG, cudaMemcpyHostToDevice, ln.st));
     } else {
         const AdcImageGeom& g = *q.img;
-        const size_t sw = view_w(e, q), sh = view_h(e, q), bpp = (size_t)adc_image_bytes_per_pixel(g.format);
-        const bool planar = g.format == ADC_IMG_RGB_PLANAR;
-        const size_t foot = staged_bytes(e, q) / 2;
+        const size_t sh = view_h(e, q);
+        const AdcImageGeom tight = adc_image_tight(g.format, view_w(e, q), sh);
+        const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
+        // one block of tight rows per plane: the three planes of a planar image; the H luma rows and ceil(H/2) chroma
+        // rows of NV12 / NV21; the H rows of every other format
+        const bool yuv420 = g.format == ADC_IMG_NV12 || g.format == ADC_IMG_NV21;
+        const int planes = g.format == ADC_IMG_RGB_PLANAR ? 3 : yuv420 ? 2 : 1;
         for (int v = 0; v < 2; v++)
-            for (int c = 0; c < (planar ? 3 : 1); c++)
-                CK(cudaMemcpy2DAsync(raw + v * foot + c * sw * sh, bpp * sw, (v ? right : left) + c * g.plane_pitch,
-                                     (size_t)g.row_pitch, bpp * sw, sh, cudaMemcpyHostToDevice, ln.st));
-        const AdcImageGeom tight{g.format, (long long)(bpp * sw), planar ? (long long)(sw * sh) : 0, (long long)foot};
+            for (int c = 0; c < planes; c++)
+                CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
+                                     (size_t)g.row_pitch, tp, yuv420 && c ? (sh + 1) / 2 : sh, cudaMemcpyHostToDevice,
+                                     ln.st));
         if (q.rect)
             adc_launch_rectify_ingest(e->P, wave_view(e, ln, 1), raw, raw + foot, tight, *q.rect, ln.st, &e->launches);
         else
@@ -1644,27 +1655,25 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 bytes = N * P.dm.Dp * 4.0 + 2 * 4.0 * N;
                 break;
             case 13: {  // volA's bytes taken as the wave's tight images (at most 2*4*N bytes a pair: they fit in its N*Dp floats)
-                const int bpp = adc_image_bytes_per_pixel(e->img_format);
-                const bool planar = e->img_format == ADC_IMG_RGB_PLANAR;
-                const long long foot = (long long)P.dm.N * (planar ? 3 : bpp);
-                const AdcImageGeom g{e->img_format, (long long)P.dm.W * bpp, planar ? (long long)P.dm.N : 0, 2 * foot};
+                AdcImageGeom g = adc_image_tight(e->img_format, P.dm.W, P.dm.H);
+                const long long foot = g.image_stride;
+                g.image_stride = 2 * foot;
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
                 adc_launch_image_ingest(P, w, src, src + foot, g, ln.st, &e->launches);
-                bytes = 2.0 * foot + 2 * 3.0 * N;
+                bytes = 2.0 * adc_image_read_bytes(e->img_format, P.dm.W, P.dm.H) + 2 * 3.0 * N;
                 break;
             }
             case 14: {  // volA's bytes taken as the wave's tight raw frames, resampled through the engine's maps
                 if (!e->rect_map) return fail(ADC_ERR_ARG, "adc_profile_kernel: no rectification is set (adc_set_rectification)");
-                const int bpp = adc_image_bytes_per_pixel(e->rect_format);
-                const bool planar = e->rect_format == ADC_IMG_RGB_PLANAR;
-                const long long sN = (long long)e->rect_src_w * e->rect_src_h, foot = sN * (planar ? 3 : bpp);
+                AdcImageGeom g = adc_image_tight(e->rect_format, e->rect_src_w, e->rect_src_h);
+                const long long foot = g.image_stride;
                 if (2 * foot > P.dm.vol_stride * 4)
                     return fail(ADC_ERR_UNSUPPORTED, "adc_profile_kernel: a pair's raw frames (%lld bytes) exceed its share of a lane volume", 2 * foot);
-                const AdcImageGeom g{e->rect_format, (long long)e->rect_src_w * bpp, planar ? sN : 0, 2 * foot};
+                g.image_stride = 2 * foot;
                 const AdcRectGeom rg{{e->rect_map, e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h};
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
                 adc_launch_rectify_ingest(P, w, src, src + foot, g, rg, ln.st, &e->launches);
-                bytes = 2.0 * foot + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
+                bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
                 break;
             }
             case 15:    // the cost computed from the wave's images and census words, summed as iteration 0's H pass into volA

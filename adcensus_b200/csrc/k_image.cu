@@ -10,7 +10,7 @@
 // row (of each plane): coalesced along x.  Every pixel is loaded by exactly one thread, alpha bytes are never loaded, and
 // nothing past the last pixel of the last row is touched.  All source offsets are 64-bit.
 // The kernel template (k_image_ingest) is in k_image.cuh; this file instantiates it for the six formats above, and
-// k_bayer.cu for the Bayer mosaics.
+// k_bayer.cu for the Bayer mosaics, k_yuv.cu for the YUV formats.
 #include <algorithm>
 
 #include "adc_common.cuh"
@@ -27,15 +27,30 @@ void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t
         case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
             adc_launch_bayer_image(P.dm, w.S, left, right, g, w.bgr, st);
             break;
+        case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
+            adc_launch_yuv_image(P.dm, w.S, left, right, g, w.bgr, st);
+            break;
         default: launch_image<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, w.bgr, st); break;
     }
     ++*launches;
 }
 
-int adc_image_bytes_per_pixel(int format) {
+AdcImageGeom adc_image_tight(int format, long long w, long long h) {
+    long long rp = w;   // gray, Bayer, and each plane of a planar image
     switch (format) {
-        case ADC_IMG_BGR: case ADC_IMG_RGB: return 3;
-        case ADC_IMG_BGRA: case ADC_IMG_RGBA: return 4;
-        default: return 1;   // gray, Bayer, and each plane of a planar image
+        case ADC_IMG_BGR: case ADC_IMG_RGB: rp = 3 * w; break;
+        case ADC_IMG_BGRA: case ADC_IMG_RGBA: rp = 4 * w; break;
+        case ADC_IMG_NV12: case ADC_IMG_NV21: rp = 2 * ((w + 1) / 2); break;
+        case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU: rp = 4 * ((w + 1) / 2); break;
+        default: break;
     }
+    const long long plane = h * rp;
+    if (format == ADC_IMG_RGB_PLANAR) return AdcImageGeom{format, rp, plane, 3 * plane};
+    if (format == ADC_IMG_NV12 || format == ADC_IMG_NV21) return AdcImageGeom{format, rp, plane, plane + (h + 1) / 2 * rp};
+    return AdcImageGeom{format, rp, 0, plane};
+}
+
+long long adc_image_read_bytes(int format, long long w, long long h) {
+    if (format == ADC_IMG_NV12 || format == ADC_IMG_NV21) return w * h + 2 * ((w + 1) / 2) * ((h + 1) / 2);
+    return adc_image_tight(format, w, h).image_stride;   // 4:2:2: 4 * ceil(W/2) * H
 }

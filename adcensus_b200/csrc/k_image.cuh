@@ -1,6 +1,6 @@
 // k_image.cuh -- the pieces the two image ingestion kernels share (k_image.cu: images in any format / pitch,
-// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the Bayer demosaic and the
-// store scheme that writes one view's packed BGR.
+// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the Bayer demosaic, the YUV
+// conversion and the store scheme that writes one view's packed BGR.
 //
 // The output of one view is a contiguous run of 3*N bytes.  A thread takes four consecutive pixels of it at a time:
 // 12 bytes, stored as three 32-bit words.  The view's run starts at an arbitrary byte phase (3*N*(2*pair + view) mod
@@ -94,12 +94,45 @@ static __device__ __forceinline__ unsigned bayer_px(const uint8_t* src, long lon
                          __ldg(d - 1), __ldg(d + 1));
 }
 
-// Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the one-pixel readers above, or the
-// demosaic of a Bayer mosaic.
+// YUV frames (ADC_IMG_NV12 ... ADC_IMG_YVYU): pixel (x, y) of the frame at src as B | G << 8 | R << 16, equal to
+// cv::cvtColor(frame, COLOR_YUV2BGR_*) (BT.601 limited range, the rule and geometry are in include/adcensus_b200.h).
+// One luma and two chroma byte loads; neighbouring pixels share their chroma, so L1 serves that reuse.
+__host__ __device__ constexpr bool is_yuv(int F) { return F >= ADC_IMG_NV12 && F <= ADC_IMG_YVYU; }
+__host__ __device__ constexpr bool is_yuv420(int F) { return F == ADC_IMG_NV12 || F == ADC_IMG_NV21; }
+
+static __device__ __forceinline__ unsigned yuv_rule(int Y, int U, int V) {
+    const int y = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
+    const int r = min(max((y + 1673527 * v) >> 20, 0), 255);
+    const int g = min(max((y - 852492 * v - 409993 * u) >> 20, 0), 255);
+    const int b = min(max((y + 2116026 * u) >> 20, 0), 255);
+    return (unsigned)b | (unsigned)g << 8 | (unsigned)r << 16;
+}
+
+template <int F>
+static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int x,
+                                                  int y) {
+    if constexpr (is_yuv420(F)) {
+        const uint8_t* c = src + plane_pitch + (long long)(y >> 1) * row_pitch + (x & ~1);
+        const int c0 = __ldg(c), c1 = __ldg(c + 1);
+        return yuv_rule(__ldg(src + (long long)y * row_pitch + x), F == ADC_IMG_NV12 ? c0 : c1,
+                        F == ADC_IMG_NV12 ? c1 : c0);
+    } else {
+        // byte offsets of Y0, U and V in the 4-byte macropixel; Y1 is Y0 + 2
+        constexpr int oy = F == ADC_IMG_UYVY ? 1 : 0;
+        constexpr int ou = F == ADC_IMG_YUYV ? 1 : F == ADC_IMG_UYVY ? 0 : 3;
+        constexpr int ov = F == ADC_IMG_YUYV ? 3 : F == ADC_IMG_UYVY ? 2 : 1;
+        const uint8_t* m = src + (long long)y * row_pitch + 2ll * (x & ~1);
+        return yuv_rule(__ldg(m + oy + 2 * (x & 1)), __ldg(m + ou), __ldg(m + ov));
+    }
+}
+
+// Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the one-pixel readers above, the demosaic
+// of a Bayer mosaic, or the conversion of a YUV frame.
 template <int F>
 static __device__ __forceinline__ unsigned view_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int w,
                                                    int h, int x, int y) {
     if constexpr (is_bayer(F)) return bayer_px<F>(src, row_pitch, w, h, x, y);
+    else if constexpr (is_yuv(F)) return yuv_px<F>(src, row_pitch, plane_pitch, x, y);
     else return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch);
 }
 
@@ -142,7 +175,8 @@ __device__ __forceinline__ void store_view_bgr(uint8_t* __restrict__ o, int N, i
     }
 }
 
-// ---- the kernels (instantiated per format in k_image.cu and k_rectify.cu, the Bayer formats in k_bayer.cu) ----
+// ---- the kernels (instantiated per format in k_image.cu and k_rectify.cu, the Bayer formats in k_bayer.cu, the YUV
+// formats in k_yuv.cu) ----
 
 // k_image.cu: pixel (x, y) of the view, read in place.
 template <int F>
@@ -194,6 +228,15 @@ static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* 
                 s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? bayer_px<F>(src, row_pitch, sw, sh, x, y)
                                                                                 : 0u;
             }
+        }
+    } else if constexpr (is_yuv(F)) {
+        // each neighbour inside the frame is converted from its own luma and chroma (nearest chroma, no chroma
+        // interpolation); one outside the frame is BGR 0, not the conversion of zero samples
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const int x = x0 + (k & 1), y = y0 + (k >> 1);
+            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? yuv_px<F>(src, row_pitch, plane_pitch, x, y)
+                                                                            : 0u;
         }
     } else if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
         const uint8_t* r0 = src + y0 * row_pitch;
@@ -248,3 +291,8 @@ void adc_launch_bayer_image(const AdcDims& dm, int S, const uint8_t* left, const
                             uint8_t* bgr, cudaStream_t st);
 void adc_launch_bayer_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                               const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);
+// The YUV instantiations of both kernels (k_yuv.cu), for g.format one of ADC_IMG_NV12 ... ADC_IMG_YVYU.
+void adc_launch_yuv_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                          uint8_t* bgr, cudaStream_t st);
+void adc_launch_yuv_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                            const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);

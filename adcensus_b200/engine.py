@@ -95,6 +95,10 @@ IMG_CHANNELS = {IMG_BGR: 3, IMG_RGB: 3, IMG_BGRA: 4, IMG_RGBA: 4, IMG_GRAY: 1, I
 IMG_BAYER_RGGB, IMG_BAYER_GRBG, IMG_BAYER_BGGR, IMG_BAYER_GBRG = 16, 17, 18, 19
 BAYER_FORMATS = {"bayer_rggb": IMG_BAYER_RGGB, "bayer_grbg": IMG_BAYER_GRBG, "bayer_bggr": IMG_BAYER_BGGR,
                  "bayer_gbrg": IMG_BAYER_GBRG}
+# YUV frames, converted as cv2.cvtColor(frame, COLOR_YUV2BGR_<name>) does (BT.601 limited range): NV12 / NV21 are a Y
+# plane and an interleaved chroma plane at plane_pitch (video decoders), the others packed 4:2:2 (UVC cameras)
+IMG_NV12, IMG_NV21, IMG_YUYV, IMG_UYVY, IMG_YVYU = 32, 33, 34, 35, 36
+YUV_FORMATS = {"nv12": IMG_NV12, "nv21": IMG_NV21, "yuyv": IMG_YUYV, "uyvy": IMG_UYVY, "yvyu": IMG_YVYU}
 
 
 class ImageDesc(ctypes.Structure):
@@ -113,7 +117,7 @@ def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> Imag
 
 def _img_format(v) -> int:
     if isinstance(v, str):
-        names = {**IMG_FORMATS, **BAYER_FORMATS}
+        names = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS}
         if v not in names:
             raise ValueError(f"unknown image format {v!r} (one of {sorted(names)})")
         return names[v]
@@ -121,9 +125,10 @@ def _img_format(v) -> int:
 
 
 def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
-    """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray, Bayer) or [3][H][W] (planar R,
-    G, B) with the pixels / channels of a row contiguous; the pitches come from the view's strides, so slices of a
-    larger frame (crops, side-by-side halves) need no copy."""
+    """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray, Bayer), [3][H][W] (planar R,
+    G, B), [H + ceil(H/2)][2*ceil(W/2)] (NV12 / NV21: the luma rows, then the chroma rows; OpenCV's (H*3/2, W) Mat for
+    even sizes) or [H][2*ceil(W/2)][2] (4:2:2, OpenCV's CV_8UC2) with the pixels / channels of a row contiguous; the
+    pitches come from the view's strides, so slices of a larger frame (crops, side-by-side halves) need no copy."""
     if a.dtype != np.uint8:
         raise ValueError(f"images must be uint8, got {a.dtype}")
     C = IMG_CHANNELS.get(fmt, 1)
@@ -131,6 +136,10 @@ def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
         shape, inner, pitches = (3, H, W), (1,), (0, a.strides[1], a.strides[0])
     elif fmt == IMG_GRAY or fmt in BAYER_FORMATS.values():
         shape, inner, pitches = (H, W), (1,), (0, a.strides[0], 0)
+    elif fmt in (IMG_NV12, IMG_NV21):
+        shape, inner, pitches = (H + (H + 1) // 2, 2 * ((W + 1) // 2)), (1,), (0, a.strides[0], H * a.strides[0])
+    elif fmt in YUV_FORMATS.values():
+        shape, inner, pitches = (H, 2 * ((W + 1) // 2), 2), (2, 1), (0, a.strides[0], 0)
     else:
         shape, inner, pitches = (H, W, C), (C, 1), (0, a.strides[0], 0)
     if a.shape != shape:
@@ -515,10 +524,12 @@ class Engine:
     def match_images(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
                      cost_layout="hwd", cost_dtype=None, disparity=True):
         """match_outputs for images in any IMG_* format, read in place: `left` / `right` are uint8 numpy views of shape
-        [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray, bayer_*) or [3][H][W] (rgb_planar) whose rows may be
-        pitched, e.g. frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.
+        [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray, bayer_*), [3][H][W] (rgb_planar),
+        [H + ceil(H/2)][2*ceil(W/2)] (nv12, nv21) or [H][2*ceil(W/2)][2] (yuyv, uyvy, yvyu) whose rows may be pitched,
+        e.g. frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.
         The result is what match_outputs gives for the same pixels packed as BGR (for a Bayer mosaic: for
-        cv2.cvtColor(view, COLOR_Bayer*2BGR), the pattern being the view's own top-left 2x2 block)."""
+        cv2.cvtColor(view, COLOR_Bayer*2BGR), the pattern being the view's own top-left 2x2 block; for a YUV frame: for
+        cv2.cvtColor(frame, COLOR_YUV2BGR_*) cropped to W x H)."""
         return self._match_views(self._L.adc_match_images, self.height, self.width, left, right, format, maps, volumes,
                                  layout, dtype, cost, cost_layout, cost_dtype, disparity)
 

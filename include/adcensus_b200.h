@@ -296,7 +296,8 @@ int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, 
  * Rule violations fail with ADC_ERR_ARG naming the field: the rules that need no image size before the engine is
  * checked, the size-dependent ones before any device work.
  * Cost: tight packed BGR takes the packed-BGR entry points' copies; every other format or geometry runs one ingestion
- * kernel per wave that writes the wave's packed BGR in one pass.  The Bayer formats (below) are formats of this list. */
+ * kernel per wave that writes the wave's packed BGR in one pass.  The Bayer and YUV formats (below) are formats of this
+ * list, with the geometry rules stated there. */
 enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC_IMG_GRAY = 4, ADC_IMG_RGB_PLANAR = 5 };
 /* Bayer mosaics: raw 8-bit colour-filter frames, 1 byte per pixel in one plane (geometry and rules as for ADC_IMG_GRAY),
  * demosaiced on the way in.  The name gives the colours of the view's OWN top-left 2x2 block, row 0 then row 1, as
@@ -320,12 +321,50 @@ enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC
  *     = (N + S + 1) >> 1.
  * Only the view's own pixels are read. */
 enum { ADC_IMG_BAYER_RGGB = 16, ADC_IMG_BAYER_GRBG = 17, ADC_IMG_BAYER_BGGR = 18, ADC_IMG_BAYER_GBRG = 19 };
+/* YUV video and camera frames, 8-bit, converted on the way in:
+ *   ADC_IMG_NV12  Y plane, then one plane of interleaved U V   OpenCV COLOR_YUV2BGR_NV12 (91)   (NVDEC, V4L2, Jetson)
+ *   ADC_IMG_NV21  Y plane, then one plane of interleaved V U   OpenCV COLOR_YUV2BGR_NV21 (93)   (Android)
+ *   ADC_IMG_YUYV  packed 4:2:2, macropixel Y0 U Y1 V           OpenCV COLOR_YUV2BGR_YUYV (116) = _YUY2   (UVC, ZED)
+ *   ADC_IMG_UYVY  packed 4:2:2, macropixel U Y0 V Y1           OpenCV COLOR_YUV2BGR_UYVY (108) = _Y422
+ *   ADC_IMG_YVYU  packed 4:2:2, macropixel Y0 V Y1 U           OpenCV COLOR_YUV2BGR_YVYU (118)
+ * Conversion: OpenCV's ITU-R BT.601 limited-range fixed-point rule (20-bit shift, arithmetic shifts), per pixel from
+ * its own Y and the U, V of its chroma sample:
+ *   y' = max(0, Y - 16) * 1220542,  u = U - 128,  v = V - 128,  h = 1 << 19
+ *   R = sat_u8((y' + h + 1673527*v) >> 20)
+ *   G = sat_u8((y' + h - 852492*v - 409993*u) >> 20)
+ *   B = sat_u8((y' + h + 2116026*u) >> 20)
+ * Every intermediate fits in int32.  Limited range means Y = 16..235 is expanded to 0..255: Y = U = V = 128 gives
+ * (130, 130, 130), and Y = U = V = 0 gives (0, 154, 0).
+ * Geometry (offsets in bytes, 64-bit; each view has its own base; image_stride as for every format):
+ *   NV12 / NV21: luma of pixel (x, y) at base + i*image_stride + y*row_pitch + x; its chroma pair at
+ *     base + i*image_stride + plane_pitch + (y >> 1)*row_pitch + 2*(x >> 1), U first for NV12, V first for NV21.
+ *     row_pitch: 0 = 2*ceil(W/2) (W rounded up to even), and at least that -- a chroma row of an odd-width view is one
+ *     byte wider than its luma row.  plane_pitch: 0 = H * row_pitch, and at least that (an NVDEC surface of height
+ *     Hs has plane_pitch = pitch * Hs).  Footprint: plane_pitch + ceil(H/2)*row_pitch.  plane_pitch is measured from the
+ *     view's own base, so the right half of a side-by-side NV12 frame of even W is simply base + W; a top-bottom NV12
+ *     pair cannot be expressed with one shared plane_pitch.
+ *   YUYV / UYVY / YVYU: pixel (x, y) is the Y0 (x even) or Y1 (x odd) of the macropixel at
+ *     base + i*image_stride + y*row_pitch + 4*(x >> 1), with that macropixel's U and V.  row_pitch: 0 = 4*ceil(W/2),
+ *     and at least that.  plane_pitch must be 0.  Footprint: H * row_pitch.
+ * Semantics: a W x H view is matched exactly as if the caller had taken any even-sized frame holding the view at its
+ * top-left, run cv::cvtColor(frame, COLOR_YUV2BGR_<F>) on it, cropped the result to W x H and passed that as packed BGR
+ * (for even sizes: cvtColor on the view itself).  Chroma is sited at even positions relative to the view's own (0, 0),
+ * so a crop of a larger frame must start at an even x (and, for NV12 / NV21, an even y): that is the caller's
+ * responsibility, as the pattern is for the Bayer formats.  Through the rectified entries the whole src_width x
+ * src_height frame is converted first and that BGR frame is resampled; a neighbour outside the frame is BGR (0, 0, 0),
+ * not the conversion of YUV (0, 0, 0).  Only the view's own samples are read: nothing past the last chroma byte of an
+ * NV12 / NV21 view, nothing past 4*ceil(W/2) bytes of a packed 4:2:2 row.
+ * Out of scope: three-plane 4:2:0 (I420 / YV12), BT.709, full range, 10-bit (P010). */
+enum { ADC_IMG_NV12 = 32, ADC_IMG_NV21 = 33, ADC_IMG_YUYV = 34, ADC_IMG_UYVY = 35, ADC_IMG_YVYU = 36 };
 typedef struct adc_image_desc {
-    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_*) */
+    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_* and the YUV formats) */
     int32_t reserved;      /* must be zero */
-    int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / Bayer / planar) */
-    int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; other formats: must be 0 */
-    int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch) */
+    int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / Bayer / planar;
+                              2*ceil(W/2) for NV12 / NV21; 4*ceil(W/2) for YUYV / UYVY / YVYU) */
+    int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; NV12 / NV21: bytes
+                              from the luma plane to the chroma plane, 0 = H * row_pitch; other formats: must be 0 */
+    int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch;
+                              plane_pitch + ceil(H/2) * row_pitch for NV12 / NV21) */
 } adc_image_desc;          /* 32 bytes */
 
 /* adc_match_outputs_batch_device with the images described by `img` (NULL = tight packed BGR, the same call as
@@ -356,7 +395,8 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
  * Channels are resampled independently; formats are resolved as for adc_match_images (gray v -> (v, v, v)), which
  * commutes with the resampling.  A Bayer mosaic is demosaiced over the whole src_width x src_height frame first (the
  * rule under ADC_IMG_BAYER_*, with its clamp at the frame's edges; frames narrower or lower than 3 pixels give all-zero
- * views), and that BGR frame is resampled.  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
+ * views), and that BGR frame is resampled; so is a YUV frame (each neighbour converted from its own luma and chroma,
+ * a neighbour outside the frame BGR 0).  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
  * the 5-bit fractions:
  *   ADC_REMAP_F32 (map1 = float x [H][W], map2 = float y [H][W], CV_32FC1 each):
  *     X = round_half_even(x * 32) saturated to int32, where NaN and values outside int32 give INT_MIN;

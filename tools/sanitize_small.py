@@ -293,4 +293,68 @@ for k, (sw, sh) in enumerate(((83, 53), (40, 2))):
         cudart.cudaFree(p)
     print("bayer rectified ok", sw, sh, flush=True)
 eng.close()
+
+# YUV frames: odd-size views at even-x offsets with row and plane pitch above their minimums, the right view of each
+# ending with its last read byte (the last chroma byte of NV12 / NV21, byte 4*ceil(W/2) of the last 4:2:2 row) at the
+# end of its own cudaMalloc allocation; plain (every format) and rectified (maps sampling the last row and column and
+# beyond, a 1-row frame)
+import yuv_testlib as YT
+
+
+def yuv_views(frames, fmt, n, vw, vh, lead):
+    rp = YT.tight_row(fmt, vw) + lead + 4
+    pp = vh * rp + 6 if YT.is420(fmt) else 0
+    stride = YT.footprint(fmt, vh, rp, pp)
+    last = pp + (YT.half(vh) - 1) * rp if YT.is420(fmt) else (vh - 1) * rp
+    size = lead + (n - 1) * stride + last + YT.tight_row(fmt, vw)
+    ptrs = []
+    for f in frames:
+        host = np.zeros(size, np.uint8)
+        for i in range(n):
+            YT.write_view(host, f, fmt, vw, vh, rp, pp, lead + i * stride)
+        p = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(p), size) == 0
+        assert cudart.cudaMemcpy(p, host.ctypes.data, size, 1) == 0
+        ptrs.append(p.value)
+    return ptrs, A.image_desc(fmt, rp, pp, stride)
+
+
+w, h, D, n = 71, 47, 23, 3
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+rng = np.random.default_rng(10)
+for fmt in YT.NAMES:
+    frames = [YT.random_frame(rng, fmt, w, h) for _ in range(2)]
+    ptrs, desc = yuv_views(frames, fmt, n, w, h, 4)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_images_batch_device(n, ptrs[0] + 4, ptrs[1] + 4, image=desc, d_disp=d_o.data_ptr(),
+                                  stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(YT.decode(frames[0], fmt, w, h), YT.decode(frames[1], fmt, w, h))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), fmt
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("yuv ok", fmt, flush=True)
+for k, (sw, sh, fmt) in enumerate(((83, 53, "nv12"), (40, 1, "nv21"), (57, 9, "uyvy"))):
+    edge = np.array([sw - 1, sw - 1.5, sw - 0.5, sw - 1 / 64, sw, sw + 0.5, -0.5, -1 / 64], np.float32)
+    maps = []
+    for v in range(2):
+        mx, my = R.warp_maps(w, h, sw, sh, 90 + v, specials=False)
+        mx[:, -8:] = edge
+        my[-8:, :] = (edge * sh / sw).astype(np.float32)[:, None]
+        my[-1, :] = sh - 1
+        mx[-1, ::2] = sw - 1
+        maps.append(R.convert_maps(mx, my) if k % 2 else (mx, my))
+    eng.set_rectification(maps[0], maps[1], (sw, sh))
+    frames = [YT.random_frame(rng, fmt, sw, sh) for _ in range(2)]
+    ptrs, desc = yuv_views(frames, fmt, n, sw, sh, 2)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_rectified_batch_device(n, ptrs[0] + 2, ptrs[1] + 2, image=desc, d_disp=d_o.data_ptr(),
+                                     stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(*(R.remap(YT.decode(frames[v], fmt, sw, sh), *maps[v]) for v in range(2)))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), (sw, sh, fmt)
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("yuv rectified ok", fmt, sw, sh, flush=True)
+eng.close()
 print("all ok")
