@@ -16,6 +16,12 @@ from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TA
                      Rectification, REPROJ_POINTS, REPROJ_DEPTH,
                      REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut, SPECKLE_S16,
                      SPECKLE_F32, SPECKLE_TYPES, SpeckleParams)
+from .engine import (IMG_MONO10, IMG_BAYER_RG10, IMG_BAYER_GR10, IMG_BAYER_BG10, IMG_BAYER_GB10, IMG_MONO12,
+                     IMG_BAYER_RG12, IMG_BAYER_GR12, IMG_BAYER_BG12, IMG_BAYER_GB12, IMG_MONO16,
+                     IMG_BAYER_RG16, IMG_BAYER_GR16, IMG_BAYER_BG16, IMG_BAYER_GB16,
+                     IMG_MONO10P, IMG_BAYER_RG10P, IMG_BAYER_GR10P, IMG_BAYER_BG10P,
+                     IMG_BAYER_GB10P, IMG_MONO12P, IMG_BAYER_RG12P, IMG_BAYER_GR12P,
+                     IMG_BAYER_BG12P, IMG_BAYER_GB12P, RAW_DEPTH_FORMATS)  # noqa: F401
 from .build import build_library  # noqa: F401
 
 __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "TAP", "lib_path",
@@ -24,6 +30,11 @@ __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "T
            "MAP_PEAK_RATIO", "IMG_BGR", "IMG_RGB", "IMG_BGRA", "IMG_RGBA", "IMG_GRAY", "IMG_RGB_PLANAR", "ImageDesc",
            "IMG_BAYER_RGGB", "IMG_BAYER_GRBG", "IMG_BAYER_BGGR", "IMG_BAYER_GBRG", "BAYER_FORMATS",
            "IMG_NV12", "IMG_NV21", "IMG_YUYV", "IMG_UYVY", "IMG_YVYU", "YUV_FORMATS",
+           "IMG_MONO10", "IMG_BAYER_RG10", "IMG_BAYER_GR10", "IMG_BAYER_BG10", "IMG_BAYER_GB10", "IMG_MONO12",
+           "IMG_BAYER_RG12", "IMG_BAYER_GR12", "IMG_BAYER_BG12", "IMG_BAYER_GB12", "IMG_MONO16",
+           "IMG_BAYER_RG16", "IMG_BAYER_GR16", "IMG_BAYER_BG16", "IMG_BAYER_GB16", "IMG_MONO10P",
+           "IMG_BAYER_RG10P", "IMG_BAYER_GR10P", "IMG_BAYER_BG10P", "IMG_BAYER_GB10P", "IMG_MONO12P",
+           "IMG_BAYER_RG12P", "IMG_BAYER_GR12P", "IMG_BAYER_BG12P", "IMG_BAYER_GB12P", "RAW_DEPTH_FORMATS",
            "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
            "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut", "SPECKLE_S16", "SPECKLE_F32", "SPECKLE_TYPES",
            "SpeckleParams"]

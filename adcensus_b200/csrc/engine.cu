@@ -721,7 +721,8 @@ int check_image_desc(const char* fn, const adc_image_desc* img) {
     if (!img) return ADC_OK;
     const bool known = (img->format >= ADC_IMG_BGR && img->format <= ADC_IMG_RGB_PLANAR) ||
                        (img->format >= ADC_IMG_BAYER_RGGB && img->format <= ADC_IMG_BAYER_GBRG) ||
-                       (img->format >= ADC_IMG_NV12 && img->format <= ADC_IMG_YVYU);
+                       (img->format >= ADC_IMG_NV12 && img->format <= ADC_IMG_YVYU) ||
+                       (img->format >= ADC_IMG_MONO10 && img->format <= ADC_IMG_BAYER_GB12P);
     if (!known) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
     if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
     if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
@@ -734,6 +735,17 @@ int check_image_desc(const char* fn, const adc_image_desc* img) {
     return ADC_OK;
 }
 
+// The rule the device entries add for the formats with one sample per 16-bit word (ADC_IMG_MONO10 ... _BAYER_GB16),
+// whose words the kernels load whole: both bases, the row pitch and the image stride are even.  Needs no image size.
+int check_image_align(const char* fn, const adc_image_desc* img, const void* left, const void* right) {
+    if (!img || img->format < ADC_IMG_MONO10 || img->format >= ADC_IMG_MONO10P) return ADC_OK;
+    if ((uintptr_t)left % 2) return fail(ADC_ERR_ARG, "%s: d_left must be 2-byte aligned for a 16-bit format", fn);
+    if ((uintptr_t)right % 2) return fail(ADC_ERR_ARG, "%s: d_right must be 2-byte aligned for a 16-bit format", fn);
+    if (img->row_pitch % 2) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld must be even for a 16-bit format", fn, (long long)img->row_pitch);
+    if (img->image_stride % 2) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld must be even for a 16-bit format", fn, (long long)img->image_stride);
+    return ADC_OK;
+}
+
 // The size-dependent rules of an image descriptor (NULL = tight packed BGR) for n pairs of views of w x h pixels (the
 // engine's size, or the raw frame size of the rectified entries); `g` receives the geometry with every zero default
 // replaced.
@@ -741,7 +753,9 @@ int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, int n
     const adc_image_desc d = img ? *img : adc_image_desc{};
     const long long H = h, min_row = adc_image_tight(d.format, w, h).row_pitch;
     const bool yuv420 = d.format == ADC_IMG_NV12 || d.format == ADC_IMG_NV21;
-    const char* min_row_rule = yuv420 ? "2 * ceil(W / 2)" : d.format >= ADC_IMG_YUYV ? "4 * ceil(W / 2)" : "W * bytes per pixel";
+    const char* min_row_rule = yuv420 ? "2 * ceil(W / 2)" : d.format < ADC_IMG_YUYV ? "W * bytes per pixel"
+                               : d.format <= ADC_IMG_YVYU ? "4 * ceil(W / 2)" : d.format < ADC_IMG_MONO10P ? "2 * W"
+                               : d.format < ADC_IMG_MONO12P ? "ceil(10 * W / 8)" : "ceil(12 * W / 8)";
     g->format = d.format;
     g->row_pitch = d.row_pitch ? (long long)d.row_pitch : min_row;
     if (g->row_pitch < min_row)
@@ -1280,7 +1294,7 @@ int adc_match_images_batch_device(adc_engine* e, int32_t n, const uint8_t* d_lef
                                   int32_t n_maps, void* stream) {
     const char* fn = "adc_match_images_batch_device";
     int rc = check_output_args(fn, vols, n_vols, maps, n_maps, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
-    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (rc || (rc = check_image_desc(fn, img)) || (rc = check_image_align(fn, img, d_left, d_right))) return rc;
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     AdcImageGeom g;
     if ((rc = resolve_image(fn, e->W, e->H, img, n, &g))) return rc;
@@ -1402,7 +1416,7 @@ int adc_match_rectified_batch_device(adc_engine* e, int32_t n, const uint8_t* d_
                                      const adc_map_out* maps, int32_t n_maps, void* stream) {
     const char* fn = "adc_match_rectified_batch_device";
     int rc = check_output_args(fn, vols, n_vols, maps, n_maps, d_disp != nullptr, d_cost != nullptr, cost_layout, cost_dtype, true);
-    if (rc || (rc = check_image_desc(fn, img))) return rc;
+    if (rc || (rc = check_image_desc(fn, img)) || (rc = check_image_align(fn, img, d_left, d_right))) return rc;
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     AdcImageGeom g;
     AdcRectGeom r;

@@ -10,7 +10,7 @@
 // row (of each plane): coalesced along x.  Every pixel is loaded by exactly one thread, alpha bytes are never loaded, and
 // nothing past the last pixel of the last row is touched.  All source offsets are 64-bit.
 // The kernel template (k_image_ingest) is in k_image.cuh; this file instantiates it for the six formats above, and
-// k_bayer.cu for the Bayer mosaics, k_yuv.cu for the YUV formats.
+// k_bayer.cu for the Bayer mosaics, k_yuv.cu for the YUV formats, k_rawdepth.cu for the high-bit-depth formats.
 #include <algorithm>
 
 #include "adc_common.cuh"
@@ -30,7 +30,8 @@ void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t
         case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
             adc_launch_yuv_image(P.dm, w.S, left, right, g, w.bgr, st);
             break;
-        default: launch_image<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, w.bgr, st); break;
+        case ADC_IMG_RGB_PLANAR: launch_image<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, w.bgr, st); break;
+        default: adc_launch_rawdepth_image(P.dm, w.S, left, right, g, w.bgr, st); break;
     }
     ++*launches;
 }
@@ -44,6 +45,8 @@ AdcImageGeom adc_image_tight(int format, long long w, long long h) {
         case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU: rp = 4 * ((w + 1) / 2); break;
         default: break;
     }
+    // high bit depth: one 16-bit word per sample, or the whole bytes of a row's 10- / 12-bit stream
+    if (is_rawdepth(format)) rp = rd_container(format) <= 2 ? 2 * w : (rd_bits(format) * w + 7) / 8;
     const long long plane = h * rp;
     if (format == ADC_IMG_RGB_PLANAR) return AdcImageGeom{format, rp, plane, 3 * plane};
     if (format == ADC_IMG_NV12 || format == ADC_IMG_NV21) return AdcImageGeom{format, rp, plane, plane + (h + 1) / 2 * rp};

@@ -1,6 +1,7 @@
 // k_image.cuh -- the pieces the two image ingestion kernels share (k_image.cu: images in any format / pitch,
 // k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the Bayer demosaic, the YUV
-// conversion and the store scheme that writes one view's packed BGR.
+// conversion, the 10- / 12- / 16-bit sample readers with their depth reduction, and the store scheme that writes one
+// view's packed BGR.
 //
 // The output of one view is a contiguous run of 3*N bytes.  A thread takes four consecutive pixels of it at a time:
 // 12 bytes, stored as three 32-bit words.  The view's run starts at an arbitrary byte phase (3*N*(2*pair + view) mod
@@ -62,8 +63,17 @@ __host__ __device__ constexpr int bayer_r_site(int F) {
     return F == ADC_IMG_BAYER_RGGB ? 0 : F == ADC_IMG_BAYER_GRBG ? 1 : F == ADC_IMG_BAYER_GBRG ? 2 : 3;
 }
 
-// The interior rule at (x, y) from the raw value c there and its eight neighbours.
-template <int F>
+// round_half_even(v / 2^S) saturated to 8 bits, the depth reduction of the high-bit-depth formats (S = depth - 8):
+// cv::Mat::convertTo(CV_8U, 1.0 / (1 << S)).  S = 0: 8-bit samples as they are.
+template <int S>
+static __device__ __forceinline__ int to8(int v) {
+    if constexpr (S == 0) return v;
+    else return min(255, (v + (1 << (S - 1)) - 1 + (v >> S & 1)) >> S);
+}
+
+// The interior rule at (x, y) from the raw value c there and its eight neighbours, computed at the samples' own depth
+// (8 + S bits) and then reduced to 8 bits.
+template <int F, int S = 0>
 static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n, int s, int wv, int e, int nw, int ne,
                                                       int sw, int se) {
     const int cross = (n + s + wv + e + 2) >> 2, diag = (nw + ne + sw + se + 2) >> 2;
@@ -79,7 +89,7 @@ static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n
         r = dy ? ver : hor;
         b = dy ? hor : ver;
     }
-    return (unsigned)b | (unsigned)g << 8 | (unsigned)r << 16;
+    return (unsigned)to8<S>(b) | (unsigned)to8<S>(g) << 8 | (unsigned)to8<S>(r) << 16;
 }
 
 template <int F>
@@ -126,13 +136,66 @@ static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long 
     }
 }
 
+// High-bit-depth mono and Bayer frames (ADC_IMG_MONO10 ... ADC_IMG_BAYER_GB12P; rules in include/adcensus_b200.h).
+// The code is ADC_IMG_MONO10 + 5 * container + colour: container 0 / 1 / 2 = one sample per little-endian 16-bit word
+// with 10 / 12 / 16 significant bits, 3 / 4 = the PFNC 10p / 12p bit streams; colour 0 = mono, 1..4 = the Bayer
+// patterns in the order of ADC_IMG_BAYER_RGGB ... _GBRG, whose code rd_pattern gives for bayer_rule.
+__host__ __device__ constexpr bool is_rawdepth(int F) { return F >= ADC_IMG_MONO10 && F <= ADC_IMG_BAYER_GB12P; }
+__host__ __device__ constexpr int rd_container(int F) { return (F - ADC_IMG_MONO10) / 5; }
+__host__ __device__ constexpr bool rd_mono(int F) { return (F - ADC_IMG_MONO10) % 5 == 0; }
+__host__ __device__ constexpr int rd_pattern(int F) { return ADC_IMG_BAYER_RGGB + (F - ADC_IMG_MONO10) % 5 - 1; }
+__host__ __device__ constexpr int rd_bits(int F) { return rd_container(F) == 2 ? 16 : rd_container(F) % 3 == 0 ? 10 : 12; }
+
+// Sample x of the row at `row`.  A 16-bit container is read as the whole word (bits above the nominal depth are kept
+// and saturate in to8); the words are 2-byte aligned (the device entries require it, the host entries stage
+// tightly).  A packed row is a little-endian bit stream from its first byte: the field of sample x starts at bit x * b
+// and, b being 10 or 12, always spans exactly two bytes, the second of which is for x = W - 1 the row's last byte.
+template <int F>
+static __device__ __forceinline__ int rd_sample(const uint8_t* row, int x) {
+    if constexpr (rd_container(F) <= 2) {
+        return __ldg(reinterpret_cast<const unsigned short*>(row) + x);
+    } else {
+        constexpr int b = rd_bits(F);
+        const int o = x * b;
+        const uint8_t* p = row + (o >> 3);
+        return ((__ldg(p) | (int)__ldg(p + 1) << 8) >> (o & 7)) & ((1 << b) - 1);
+    }
+}
+
+// The Bayer rule at full depth on nine samples, then the depth reduction of its three results.
+template <int F>
+static __device__ __forceinline__ unsigned rd_bayer_rule(int x, int y, int c, int n, int s, int wv, int e, int nw, int ne,
+                                                         int sw, int se) {
+    return bayer_rule<rd_pattern(F), rd_bits(F) - 8>(x, y, c, n, s, wv, e, nw, ne, sw, se);
+}
+
+// Pixel (x, y) of the w x h frame at src: a mono sample reduced and repeated, or the demosaic of bayer_px on the full
+// depth samples (same clamp, same all-zero rule below 3 x 3).
+template <int F>
+static __device__ __forceinline__ unsigned rd_px(const uint8_t* src, long long row_pitch, int w, int h, int x, int y) {
+    if constexpr (rd_mono(F)) {
+        return to8<rd_bits(F) - 8>(rd_sample<F>(src + (long long)y * row_pitch, x)) * 0x010101u;
+    } else {
+        if (w < 3 || h < 3) return 0u;
+        x = min(max(x, 1), w - 2);
+        y = min(max(y, 1), h - 2);
+        const uint8_t* m = src + (long long)y * row_pitch;
+        const uint8_t* u = m - row_pitch;
+        const uint8_t* d = m + row_pitch;
+        return rd_bayer_rule<F>(x, y, rd_sample<F>(m, x), rd_sample<F>(u, x), rd_sample<F>(d, x), rd_sample<F>(m, x - 1),
+                                rd_sample<F>(m, x + 1), rd_sample<F>(u, x - 1), rd_sample<F>(u, x + 1),
+                                rd_sample<F>(d, x - 1), rd_sample<F>(d, x + 1));
+    }
+}
+
 // Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the one-pixel readers above, the demosaic
-// of a Bayer mosaic, or the conversion of a YUV frame.
+// of a Bayer mosaic, the conversion of a YUV frame, or the reduction of a high-bit-depth frame.
 template <int F>
 static __device__ __forceinline__ unsigned view_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int w,
                                                    int h, int x, int y) {
     if constexpr (is_bayer(F)) return bayer_px<F>(src, row_pitch, w, h, x, y);
     else if constexpr (is_yuv(F)) return yuv_px<F>(src, row_pitch, plane_pitch, x, y);
+    else if constexpr (is_rawdepth(F)) return rd_px<F>(src, row_pitch, w, h, x, y);
     else return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch);
 }
 
@@ -176,7 +239,7 @@ __device__ __forceinline__ void store_view_bgr(uint8_t* __restrict__ o, int N, i
 }
 
 // ---- the kernels (instantiated per format in k_image.cu and k_rectify.cu, the Bayer formats in k_bayer.cu, the YUV
-// formats in k_yuv.cu) ----
+// formats in k_yuv.cu, the high-bit-depth formats in k_rawdepth.cu) ----
 
 // k_image.cu: pixel (x, y) of the view, read in place.
 template <int F>
@@ -238,6 +301,29 @@ static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* 
             s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? yuv_px<F>(src, row_pitch, plane_pitch, x, y)
                                                                             : 0u;
         }
+    } else if constexpr (is_rawdepth(F)) {
+        // as for the 8-bit mosaics: where no clamp applies, one 4x4 window of full-depth samples serves the four
+        // demosaics, each reduced to 8 bits before the blend; elsewhere, and for mono, neighbour by neighbour
+        if (!rd_mono(F) && x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
+            int v[4][4];
+            const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch;
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) v[i][j] = rd_sample<F>(r0 + i * row_pitch, x0 - 1 + j);
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int dx = k & 1, dy = k >> 1;
+                s[k] = rd_bayer_rule<F>(x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
+                                        v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const int x = x0 + (k & 1), y = y0 + (k >> 1);
+                s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? rd_px<F>(src, row_pitch, sw, sh, x, y) : 0u;
+            }
+        }
     } else if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
         const uint8_t* r0 = src + y0 * row_pitch;
         s[0] = ImgIn<F>::px(r0, x0, plane_pitch);
@@ -296,3 +382,9 @@ void adc_launch_yuv_image(const AdcDims& dm, int S, const uint8_t* left, const u
                           uint8_t* bgr, cudaStream_t st);
 void adc_launch_yuv_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                             const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);
+// The high-bit-depth instantiations of both kernels (k_rawdepth.cu), for g.format one of ADC_IMG_MONO10 ...
+// ADC_IMG_BAYER_GB12P.
+void adc_launch_rawdepth_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                               uint8_t* bgr, cudaStream_t st);
+void adc_launch_rawdepth_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right,
+                                 const AdcImageGeom& g, const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);

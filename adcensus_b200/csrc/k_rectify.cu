@@ -12,9 +12,10 @@
 //     both neighbours x0 and x0 + 1 lie outside the frame: the border value 0 whichever way X saturated.
 //
 // Per wave: k_rectify_ingest<F> (k_image.cuh; instantiated here for the six formats of k_image.cu, in k_bayer.cu for
-// the Bayer mosaics, in k_yuv.cu for the YUV formats) makes one launch over the wave's pairs x 2 views.  For each output pixel it gathers
-// the four neighbours of (x0, y0) from the raw view through the format readers of k_image.cuh, weights them
-// (32 - ax | ax) * (32 - ay | ay), and writes (sum + 512) >> 10 per channel with the store scheme of k_image.cuh.  When
+// the Bayer mosaics, in k_yuv.cu for the YUV formats, in k_rawdepth.cu for the high-bit-depth formats) makes one launch
+// over the wave's pairs x 2 views.  For each output pixel it gathers the four neighbours of (x0, y0) from the raw view
+// through the format readers of k_image.cuh, weights them (32 - ax | ax) * (32 - ay | ay), and writes (sum + 512) >> 10
+// per channel with the store scheme of k_image.cuh.  When
 // all four neighbours lie inside the frame (0 <= x0 < src_width - 1, 0 <= y0 < src_height - 1; never for a frame one
 // pixel wide or high) the loads are unconditional; otherwise each neighbour is loaded only if it is inside, so nothing
 // outside a view's frame is read, and alpha bytes never are.  Source offsets are 64-bit.
@@ -81,7 +82,8 @@ void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8
         case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
             adc_launch_yuv_rectify(P.dm, w.S, left, right, g, r, w.bgr, st);
             break;
-        default: launch_rectify<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
+        case ADC_IMG_RGB_PLANAR: launch_rectify<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
+        default: adc_launch_rawdepth_rectify(P.dm, w.S, left, right, g, r, w.bgr, st); break;
     }
     ++*launches;
 }

@@ -99,6 +99,20 @@ BAYER_FORMATS = {"bayer_rggb": IMG_BAYER_RGGB, "bayer_grbg": IMG_BAYER_GRBG, "ba
 # plane and an interleaved chroma plane at plane_pitch (video decoders), the others packed 4:2:2 (UVC cameras)
 IMG_NV12, IMG_NV21, IMG_YUYV, IMG_UYVY, IMG_YVYU = 32, 33, 34, 35, 36
 YUV_FORMATS = {"nv12": IMG_NV12, "nv21": IMG_NV21, "yuyv": IMG_YUYV, "uyvy": IMG_UYVY, "yvyu": IMG_YVYU}
+# high-bit-depth mono and Bayer frames under their GenICam PFNC names, reduced to 8 bits as cv2.convertScaleAbs(v,
+# alpha=2**-(bits - 8)) does (Bayer: after cv2.cvtColor on the uint16 mosaic): one sample per little-endian uint16 with
+# 10, 12 or 16 significant bits ("u16"), or the 10p / 12p bit streams ("p": 4 samples in 5 bytes, 2 in 3)
+IMG_MONO10, IMG_BAYER_RG10, IMG_BAYER_GR10, IMG_BAYER_BG10, IMG_BAYER_GB10 = 64, 65, 66, 67, 68
+IMG_MONO12, IMG_BAYER_RG12, IMG_BAYER_GR12, IMG_BAYER_BG12, IMG_BAYER_GB12 = 69, 70, 71, 72, 73
+IMG_MONO16, IMG_BAYER_RG16, IMG_BAYER_GR16, IMG_BAYER_BG16, IMG_BAYER_GB16 = 74, 75, 76, 77, 78
+IMG_MONO10P, IMG_BAYER_RG10P, IMG_BAYER_GR10P, IMG_BAYER_BG10P, IMG_BAYER_GB10P = 79, 80, 81, 82, 83
+IMG_MONO12P, IMG_BAYER_RG12P, IMG_BAYER_GR12P, IMG_BAYER_BG12P, IMG_BAYER_GB12P = 84, 85, 86, 87, 88
+# name -> (code, significant bits, container)
+RAW_DEPTH_FORMATS = {f"{colour}{suffix}": (IMG_MONO10 + 5 * k + c, bits, container)
+                     for k, (suffix, bits, container) in enumerate((("10", 10, "u16"), ("12", 12, "u16"), ("16", 16, "u16"),
+                                                                    ("10p", 10, "p"), ("12p", 12, "p")))
+                     for c, colour in enumerate(("mono", "bayer_rg", "bayer_gr", "bayer_bg", "bayer_gb"))}
+_RAW_DEPTH = {code: (bits, container) for code, bits, container in RAW_DEPTH_FORMATS.values()}
 
 
 class ImageDesc(ctypes.Structure):
@@ -117,7 +131,7 @@ def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> Imag
 
 def _img_format(v) -> int:
     if isinstance(v, str):
-        names = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS}
+        names = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS, **{k: v[0] for k, v in RAW_DEPTH_FORMATS.items()}}
         if v not in names:
             raise ValueError(f"unknown image format {v!r} (one of {sorted(names)})")
         return names[v]
@@ -127,12 +141,19 @@ def _img_format(v) -> int:
 def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
     """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray, Bayer), [3][H][W] (planar R,
     G, B), [H + ceil(H/2)][2*ceil(W/2)] (NV12 / NV21: the luma rows, then the chroma rows; OpenCV's (H*3/2, W) Mat for
-    even sizes) or [H][2*ceil(W/2)][2] (4:2:2, OpenCV's CV_8UC2) with the pixels / channels of a row contiguous; the
-    pitches come from the view's strides, so slices of a larger frame (crops, side-by-side halves) need no copy."""
-    if a.dtype != np.uint8:
-        raise ValueError(f"images must be uint8, got {a.dtype}")
+    even sizes), [H][2*ceil(W/2)][2] (4:2:2, OpenCV's CV_8UC2), uint16 [H][W] (the 16-bit containers) or
+    [H][ceil(bits*W/8)] (10p / 12p: each row's bytes) with the pixels / channels of a row contiguous; the pitches come
+    from the view's strides, so slices of a larger frame (crops, side-by-side halves) need no copy."""
+    bits, container = _RAW_DEPTH.get(fmt, (8, None))
+    dtype = np.uint16 if container == "u16" else np.uint8
+    if a.dtype != dtype:
+        raise ValueError(f"images of format {fmt} must be {np.dtype(dtype)}, got {a.dtype}")
     C = IMG_CHANNELS.get(fmt, 1)
-    if fmt == IMG_RGB_PLANAR:
+    if container == "u16":
+        shape, inner, pitches = (H, W), (2,), (0, a.strides[0], 0)
+    elif container == "p":
+        shape, inner, pitches = (H, (bits * W + 7) // 8), (1,), (0, a.strides[0], 0)
+    elif fmt == IMG_RGB_PLANAR:
         shape, inner, pitches = (3, H, W), (1,), (0, a.strides[1], a.strides[0])
     elif fmt == IMG_GRAY or fmt in BAYER_FORMATS.values():
         shape, inner, pitches = (H, W), (1,), (0, a.strides[0], 0)
@@ -525,11 +546,14 @@ class Engine:
                      cost_layout="hwd", cost_dtype=None, disparity=True):
         """match_outputs for images in any IMG_* format, read in place: `left` / `right` are uint8 numpy views of shape
         [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray, bayer_*), [3][H][W] (rgb_planar),
-        [H + ceil(H/2)][2*ceil(W/2)] (nv12, nv21) or [H][2*ceil(W/2)][2] (yuyv, uyvy, yvyu) whose rows may be pitched,
+        [H + ceil(H/2)][2*ceil(W/2)] (nv12, nv21) or [H][2*ceil(W/2)][2] (yuyv, uyvy, yvyu), uint16 views [H][W]
+        (mono10 / 12 / 16, bayer_rg10 ...) or uint8 views [H][ceil(bits*W/8)] of the rows' bytes (mono10p, bayer_rg12p
+        ...: what a camera SDK's buffer is to numpy) whose rows may be pitched,
         e.g. frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.
         The result is what match_outputs gives for the same pixels packed as BGR (for a Bayer mosaic: for
         cv2.cvtColor(view, COLOR_Bayer*2BGR), the pattern being the view's own top-left 2x2 block; for a YUV frame: for
-        cv2.cvtColor(frame, COLOR_YUV2BGR_*) cropped to W x H)."""
+        cv2.cvtColor(frame, COLOR_YUV2BGR_*) cropped to W x H; for a high-bit-depth frame: for the unpacked uint16
+        samples, demosaiced if Bayer, through cv2.convertScaleAbs(v, alpha=2**-(bits - 8)))."""
         return self._match_views(self._L.adc_match_images, self.height, self.width, left, right, format, maps, volumes,
                                  layout, dtype, cost, cost_layout, cost_dtype, disparity)
 

@@ -296,8 +296,8 @@ int adc_match_outputs(adc_engine* e, const uint8_t* left, const uint8_t* right, 
  * Rule violations fail with ADC_ERR_ARG naming the field: the rules that need no image size before the engine is
  * checked, the size-dependent ones before any device work.
  * Cost: tight packed BGR takes the packed-BGR entry points' copies; every other format or geometry runs one ingestion
- * kernel per wave that writes the wave's packed BGR in one pass.  The Bayer and YUV formats (below) are formats of this
- * list, with the geometry rules stated there. */
+ * kernel per wave that writes the wave's packed BGR in one pass.  The Bayer, YUV and high-bit-depth formats (below) are
+ * formats of this list, with the geometry rules stated there. */
 enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC_IMG_GRAY = 4, ADC_IMG_RGB_PLANAR = 5 };
 /* Bayer mosaics: raw 8-bit colour-filter frames, 1 byte per pixel in one plane (geometry and rules as for ADC_IMG_GRAY),
  * demosaiced on the way in.  The name gives the colours of the view's OWN top-left 2x2 block, row 0 then row 1, as
@@ -354,13 +354,66 @@ enum { ADC_IMG_BAYER_RGGB = 16, ADC_IMG_BAYER_GRBG = 17, ADC_IMG_BAYER_BGGR = 18
  * src_height frame is converted first and that BGR frame is resampled; a neighbour outside the frame is BGR (0, 0, 0),
  * not the conversion of YUV (0, 0, 0).  Only the view's own samples are read: nothing past the last chroma byte of an
  * NV12 / NV21 view, nothing past 4*ceil(W/2) bytes of a packed 4:2:2 row.
- * Out of scope: three-plane 4:2:0 (I420 / YV12), BT.709, full range, 10-bit (P010). */
+ * Out of scope: three-plane 4:2:0 (I420 / YV12), BT.709, full range, 10- and 16-bit YUV (P010 / P016). */
 enum { ADC_IMG_NV12 = 32, ADC_IMG_NV21 = 33, ADC_IMG_YUYV = 34, ADC_IMG_UYVY = 35, ADC_IMG_YVYU = 36 };
+/* High-bit-depth mono and Bayer frames, as GigE Vision / USB3 Vision cameras deliver them, reduced to 8 bits on the way
+ * in.  The names are the GenICam PFNC pixel formats; five containers, each as mono and as the four Bayer patterns:
+ *   ADC_IMG_MONO10   ADC_IMG_BAYER_{RG,GR,BG,GB}10    Mono10 / BayerRG10 ...: one sample per little-endian uint16,
+ *                                                     LSB-aligned, 10 significant bits; a tight row is 2*W bytes
+ *   ADC_IMG_MONO12   ADC_IMG_BAYER_{RG,GR,BG,GB}12    Mono12 / BayerRG12 ...: the same, 12 significant bits
+ *   ADC_IMG_MONO16   ADC_IMG_BAYER_{RG,GR,BG,GB}16    Mono16 / BayerRG16 ...: the same, 16 bits.  Also the format for
+ *                                                     10- / 12-bit data delivered MSB-aligned in 16-bit words
+ *   ADC_IMG_MONO10P  ADC_IMG_BAYER_{RG,GR,BG,GB}10P   Mono10p / BayerRG10p ...: 4 samples in 5 bytes; a tight row is
+ *                                                     ceil(10*W / 8) bytes
+ *   ADC_IMG_MONO12P  ADC_IMG_BAYER_{RG,GR,BG,GB}12P   Mono12p / BayerRG12p ...: 2 samples in 3 bytes; a tight row is
+ *                                                     ceil(12*W / 8) bytes
+ * The Bayer names follow the 8-bit block's convention, the colours of the view's OWN top-left 2x2 block, and map onto
+ * the same four OpenCV codes: RG = ADC_IMG_BAYER_RGGB = COLOR_BayerRGGB2BGR = legacy COLOR_BayerBG2BGR (46), GR = _GRBG
+ * = legacy COLOR_BayerGB2BGR (47), BG = _BGGR = legacy COLOR_BayerRG2BGR (48), GB = _GBRG = legacy COLOR_BayerGR2BGR
+ * (49).  The same warning applies: OpenCV's legacy names are not the sensor's, COLOR_BayerBG2BGR is the RG sensor.
+ * Sample of pixel x of a row (b = 10, 12 or 16 the depth):
+ *   16-bit containers: v = the x-th uint16 of the row, the whole word; bits above b are NOT masked off.
+ *   10p / 12p: the row is a little-endian bit stream that starts at the row's first byte (rows are not packed across
+ *     their ends); with o = x*b and k = o >> 3:  v = ((row[k] | row[k+1] << 8) >> (o & 7)) & (2^b - 1).  A field always
+ *     spans exactly two bytes, and for x = W - 1 byte k + 1 is the last byte of the tight row.  (12p: byte0 = p0[7:0],
+ *     byte1 = p0[11:8] | p1[3:0] << 4, byte2 = p1[11:4].)
+ * Depth reduction, one rule for every format, s = b - 8 (2, 4 or 8):
+ *   to8(v) = min(255, (v + 2^(s-1) - 1 + ((v >> s) & 1)) >> s)
+ * which is round_half_even(v / 2^s) saturated: cv::Mat::convertTo(dst, CV_8U, 1.0 / (1 << s)).  A 10- or 12-bit word with
+ * bits set above its depth therefore saturates to 255, as OpenCV treats the uint16 array.
+ * Semantics:
+ *   mono: the view is matched exactly as if the caller had unpacked it to CV_16UC1, run convertTo(CV_8U, 2^-s) and passed
+ *     the result as ADC_IMG_GRAY.
+ *   Bayer: as if the caller had unpacked it to CV_16UC1, run cv::cvtColor(raw16, <the code above>) at full depth (the
+ *     interior rule and border clamp stated under ADC_IMG_BAYER_* on the 16-bit values; W < 3 or H < 3 gives all-zero
+ *     views), then convertTo(CV_8U, 2^-s) on the three channels, and passed that as packed BGR.  Demosaic first, reduce
+ *     second: the other order differs in the last bit.
+ *   through the rectified entries: the whole src_width x src_height frame is converted that way first and the 8-bit BGR
+ *     frame is resampled as described there; a neighbour outside the frame is BGR 0.
+ * Geometry (both views share it): sample x of row y of pair i is read from the row at base + i*image_stride +
+ * y*row_pitch.  plane_pitch must be 0; row_pitch: 0 = the tight row above, and at least that; image_stride: 0 =
+ * H * row_pitch, and at least that.  16-bit containers on the device entries: both base pointers, row_pitch and
+ * image_stride must be even, so that the words are aligned (ADC_ERR_ARG naming the argument otherwise, before the
+ * engine is checked); the host entries take any pointer and pitch, they upload the rows tightly.  10p / 12p: any byte
+ * alignment; a crop or the right half of a side-by-side frame must start on a byte boundary of the stream (x a multiple
+ * of 4 for 10p, of 2 for 12p) and, for Bayer, at an even x and y or with the correspondingly different pattern: the
+ * caller's responsibility, as for the 8-bit mosaics.  Only the view's own samples are read: nothing past 2*W bytes of a
+ * 16-bit row, nothing past ceil(b*W / 8) bytes of a packed row.
+ * Out of scope: big-endian words, 14-bit formats, the legacy GigE Vision Mono12Packed / Bayer**12Packed nibble order,
+ * 16-bit colour images. */
+enum {
+    ADC_IMG_MONO10 = 64, ADC_IMG_BAYER_RG10 = 65, ADC_IMG_BAYER_GR10 = 66, ADC_IMG_BAYER_BG10 = 67, ADC_IMG_BAYER_GB10 = 68,
+    ADC_IMG_MONO12 = 69, ADC_IMG_BAYER_RG12 = 70, ADC_IMG_BAYER_GR12 = 71, ADC_IMG_BAYER_BG12 = 72, ADC_IMG_BAYER_GB12 = 73,
+    ADC_IMG_MONO16 = 74, ADC_IMG_BAYER_RG16 = 75, ADC_IMG_BAYER_GR16 = 76, ADC_IMG_BAYER_BG16 = 77, ADC_IMG_BAYER_GB16 = 78,
+    ADC_IMG_MONO10P = 79, ADC_IMG_BAYER_RG10P = 80, ADC_IMG_BAYER_GR10P = 81, ADC_IMG_BAYER_BG10P = 82, ADC_IMG_BAYER_GB10P = 83,
+    ADC_IMG_MONO12P = 84, ADC_IMG_BAYER_RG12P = 85, ADC_IMG_BAYER_GR12P = 86, ADC_IMG_BAYER_BG12P = 87, ADC_IMG_BAYER_GB12P = 88
+};
 typedef struct adc_image_desc {
-    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_* and the YUV formats) */
+    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_*, the YUV and the high-bit-depth formats) */
     int32_t reserved;      /* must be zero */
     int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / Bayer / planar;
-                              2*ceil(W/2) for NV12 / NV21; 4*ceil(W/2) for YUYV / UYVY / YVYU) */
+                              2*ceil(W/2) for NV12 / NV21; 4*ceil(W/2) for YUYV / UYVY / YVYU; 2*W for the 16-bit
+                              containers; ceil(10*W/8) for 10p, ceil(12*W/8) for 12p) */
     int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; NV12 / NV21: bytes
                               from the luma plane to the chroma plane, 0 = H * row_pitch; other formats: must be 0 */
     int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch;
@@ -396,7 +449,8 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
  * commutes with the resampling.  A Bayer mosaic is demosaiced over the whole src_width x src_height frame first (the
  * rule under ADC_IMG_BAYER_*, with its clamp at the frame's edges; frames narrower or lower than 3 pixels give all-zero
  * views), and that BGR frame is resampled; so is a YUV frame (each neighbour converted from its own luma and chroma,
- * a neighbour outside the frame BGR 0).  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
+ * a neighbour outside the frame BGR 0) and a high-bit-depth frame (demosaiced at full depth and reduced to 8 bits
+ * first).  For each output pixel, with (X, Y) its source coordinate in 1/32 pixel and (ax, ay)
  * the 5-bit fractions:
  *   ADC_REMAP_F32 (map1 = float x [H][W], map2 = float y [H][W], CV_32FC1 each):
  *     X = round_half_even(x * 32) saturated to int32, where NaN and values outside int32 give INT_MIN;

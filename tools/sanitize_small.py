@@ -357,4 +357,70 @@ for k, (sw, sh, fmt) in enumerate(((83, 53, "nv12"), (40, 1, "nv21"), (57, 9, "u
         cudart.cudaFree(p)
     print("yuv rectified ok", fmt, sw, sh, flush=True)
 eng.close()
+
+# High-bit-depth frames: views a few samples into wider rows, the right view of each ending with its last sample (the
+# last 16-bit word, or byte ceil(b*W/8) of the last packed row, which the last field's second byte is) at the end of
+# its own cudaMalloc allocation; plain (every container, mono and a mosaic) and rectified (one format per container,
+# maps sampling the last row and column and beyond, a 2-row frame)
+import rawdepth_testlib as XT
+
+
+def rawdepth_views(frames, fmt, n, vw, vh, lead):
+    rp = XT.tight_row(fmt, vw) + lead + 4
+    stride = vh * rp + 6
+    size = lead + (n - 1) * stride + (vh - 1) * rp + XT.tight_row(fmt, vw)
+    ptrs = []
+    for f in frames:
+        host = np.zeros(size, np.uint8)
+        for i in range(n):
+            XT.write_view(host, f, fmt, vw, vh, rp, lead + i * stride)
+        p = ctypes.c_void_p()
+        assert cudart.cudaMalloc(ctypes.byref(p), size) == 0
+        assert cudart.cudaMemcpy(p, host.ctypes.data, size, 1) == 0
+        ptrs.append(p.value)
+    return ptrs, A.image_desc(fmt, rp, 0, stride)
+
+
+w, h, D, n = 71, 47, 23, 3
+eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D), wave_pairs=2, lanes=2)
+rng = np.random.default_rng(11)
+for suffix, bits, packed in XT.CONTAINERS:
+    for colour in ("mono", "bayer_gr"):
+        fmt = colour + suffix
+        lead = bits // 2 if packed else 4   # 4 samples into the row: 5 or 6 bytes of a stream, 2 words
+        frames = [XT.random_frame(rng, fmt, w, h) for _ in range(2)]
+        ptrs, desc = rawdepth_views(frames, fmt, n, w, h, lead)
+        d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+        eng.match_images_batch_device(n, ptrs[0] + lead, ptrs[1] + lead, image=desc, d_disp=d_o.data_ptr(),
+                                      stream=torch.cuda.current_stream().cuda_stream)
+        torch.cuda.synchronize()
+        single = eng.match(XT.decode(frames[0], fmt, w, h), XT.decode(frames[1], fmt, w, h))
+        assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), fmt
+        for p in ptrs:
+            cudart.cudaFree(p)
+        print("rawdepth ok", fmt, flush=True)
+for k, (sw, sh, fmt) in enumerate(((83, 53, "bayer_rg12p"), (40, 2, "bayer_gb10p"), (57, 9, "mono12"), (31, 33, "bayer_bg10"),
+                                   (45, 3, "bayer_gr16"))):
+    edge = np.array([sw - 1, sw - 1.5, sw - 0.5, sw - 1 / 64, sw, sw + 0.5, -0.5, -1 / 64], np.float32)
+    maps = []
+    for v in range(2):
+        mx, my = R.warp_maps(w, h, sw, sh, 100 + v, specials=False)
+        mx[:, -8:] = edge
+        my[-8:, :] = (edge * sh / sw).astype(np.float32)[:, None]
+        my[-1, :] = sh - 1
+        mx[-1, ::2] = sw - 1
+        maps.append(R.convert_maps(mx, my) if k % 2 else (mx, my))
+    eng.set_rectification(maps[0], maps[1], (sw, sh))
+    frames = [XT.random_frame(rng, fmt, sw, sh) for _ in range(2)]
+    ptrs, desc = rawdepth_views(frames, fmt, n, sw, sh, 2)
+    d_o = torch.empty((n, h, w), dtype=torch.float32, device=dev)
+    eng.match_rectified_batch_device(n, ptrs[0] + 2, ptrs[1] + 2, image=desc, d_disp=d_o.data_ptr(),
+                                     stream=torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+    single = eng.match(*(R.remap(XT.decode(frames[v], fmt, sw, sh), *maps[v]) for v in range(2)))
+    assert (d_o.cpu().numpy().view(np.uint32) == single.view(np.uint32)[None]).all(), (sw, sh, fmt)
+    for p in ptrs:
+        cudart.cudaFree(p)
+    print("rawdepth rectified ok", fmt, sw, sh, flush=True)
+eng.close()
 print("all ok")
