@@ -15,7 +15,7 @@ from .engine import (ADCensusOption, ADCensusStereo, AdcError, Engine, STAGE, TA
                      IMG_YUYV, IMG_UYVY, IMG_YVYU, YUV_FORMATS, image_desc, REMAP_F32, REMAP_FIXED, Remap,
                      Rectification, REPROJ_POINTS, REPROJ_DEPTH,
                      REPROJ_DISP_S16, REPROJ_KINDS, ReprojectOut, SPECKLE_S16,
-                     SPECKLE_F32, SPECKLE_TYPES, SpeckleParams)
+                     SPECKLE_F32, SPECKLE_TYPES, SpeckleParams, CloudOut)
 from .engine import (IMG_MONO10, IMG_BAYER_RG10, IMG_BAYER_GR10, IMG_BAYER_BG10, IMG_BAYER_GB10, IMG_MONO12,
                      IMG_BAYER_RG12, IMG_BAYER_GR12, IMG_BAYER_BG12, IMG_BAYER_GB12, IMG_MONO16,
                      IMG_BAYER_RG16, IMG_BAYER_GR16, IMG_BAYER_BG16, IMG_BAYER_GB16,
@@ -37,4 +37,4 @@ __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "T
            "IMG_BAYER_RG12P", "IMG_BAYER_GR12P", "IMG_BAYER_BG12P", "IMG_BAYER_GB12P", "RAW_DEPTH_FORMATS",
            "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
            "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut", "SPECKLE_S16", "SPECKLE_F32", "SPECKLE_TYPES",
-           "SpeckleParams"]
+           "SpeckleParams", "CloudOut"]

@@ -147,14 +147,15 @@ size_t adc_cost_elem_bytes(int dtype);
 // ADC_COST_HWD / ADC_COST_DHW, element type ADC_COST_F32 / F16 / BF16 rounded to nearest even); dst aligned to its element
 void adc_launch_cost_export(const AdcParams& P, const AdcWave& w, const float* vol, void* dst, int layout, int dtype,
                             cudaStream_t st, unsigned long long* launches);
-// image ingestion (k_image.cu): the wave's views at left / right (pair i at byte i*image_stride, format ADC_IMG_*, pitches
-// resolved: no zero defaults left) -> w.bgr as packed BGR
+// image ingestion (k_image.cu): S pairs of views at left / right (pair i at byte i*image_stride, format ADC_IMG_*,
+// pitches resolved: no zero defaults left) -> bgr as packed BGR [S][2][N*3] (a wave's w.bgr, or a caller's views);
+// S <= 65535 (the grid's z)
 struct AdcImageGeom {
     int format;
     long long row_pitch, plane_pitch, image_stride;
 };
-void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
-                             const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches);
+void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                             uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
 // The tight layout of a w x h view in `format`: row pitch, plane pitch (ADC_IMG_RGB_PLANAR: from one channel plane to
 // the next; NV12 / NV21: from the luma plane to the chroma plane; else 0) and footprint (in image_stride).
 AdcImageGeom adc_image_tight(int format, long long w, long long h);
@@ -170,14 +171,30 @@ struct AdcRectGeom {
 // a view's adc_remap (map1 / map2 with byte pitches, device-readable, ADC_REMAP_F32 / ADC_REMAP_FIXED) -> out [H][W]
 void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1, long long pitch1, const void* map2,
                               long long pitch2, uint2* out, cudaStream_t st);
-// the wave's raw views at left / right (geometry g over src_w x src_h frames, pitches resolved) -> w.bgr, resampled
-void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
-                               const AdcImageGeom& g, const AdcRectGeom& r, cudaStream_t st, unsigned long long* launches);
+// S pairs of raw views at left / right (geometry g over src_w x src_h frames, pitches resolved) -> bgr [S][2][N*3],
+// resampled; S * ceil(N / 4 / II_GROUPS) < 2^31 (the grid's x)
+void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                               const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
 // reprojection to 3-D (k_reproject.cu): n maps of dm.N pixels at disp -> the outputs whose pointer is not NULL (map i
 // at pixel i*N of each), Q row-major; s16_invalid = the DISP_S16 value of a +inf pixel.  One launch.
 struct AdcReprojQ { double q[16]; };
 void adc_launch_reproject(const AdcDims& dm, long long n, const float* disp, const AdcReprojQ& Q, float* points,
                           float* depth, int16_t* s16, int16_t s16_invalid, cudaStream_t st, unsigned long long* launches);
+// point clouds (k_cloud.cu): the kept pixels of n maps of dm.N pixels at disp (finite d, finite point, z_min <= Z <=
+// z_max), compacted in raster order: map i's first `capacity` points at point i*capacity of points / colors (R, G, B of
+// the pixel of bgr + i*bgr_stride; NULL = none) / pixels (NULL = none), its full count at counts[i].  `work` holds
+// adc_point_cloud_work_bytes(dm, n) bytes, 8-byte aligned and zeroed in stream order before the launch.  One launch.
+struct AdcCloudOut {
+    float* points;
+    uint8_t* colors;
+    int32_t* pixels;
+    int32_t* counts;
+    long long capacity;
+};
+size_t adc_point_cloud_work_bytes(const AdcDims& dm, long long n);
+void adc_launch_point_cloud(const AdcDims& dm, long long n, const float* disp, const AdcReprojQ& Q, const uint8_t* bgr,
+                            long long bgr_stride, float z_min, float z_max, const AdcCloudOut& out, void* work,
+                            cudaStream_t st, unsigned long long* launches);
 // speckle removal (k_speckle.cu): the rules resolved on the host.  S16: missing = (int)v == nv_i, connected =
 // |a - b| <= md_i in int, written (int16)nv_i.  F32: missing = v == nv_f, connected = fabsf(a - b) <= md_f (the largest
 // float not above max_diff), written nv_f.  A component of at most max_size pixels is removed.

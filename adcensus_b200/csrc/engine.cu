@@ -42,6 +42,9 @@ static_assert(sizeof(adc_speckle_params) == 32 && offsetof(adc_speckle_params, m
               offsetof(adc_speckle_params, reserved) == 24, "adc_speckle_params layout (include/adcensus_b200.h)");
 static_assert(sizeof(adc_reproject_out) == 16 && offsetof(adc_reproject_out, kind) == 8 &&
               offsetof(adc_reproject_out, reserved) == 12, "adc_reproject_out layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_cloud_out) == 48 && offsetof(adc_cloud_out, colors) == 8 && offsetof(adc_cloud_out, pixels) == 16 &&
+              offsetof(adc_cloud_out, counts) == 24 && offsetof(adc_cloud_out, capacity) == 32 &&
+              offsetof(adc_cloud_out, reserved) == 40, "adc_cloud_out layout (include/adcensus_b200.h)");
 
 namespace {
 
@@ -560,9 +563,9 @@ int run_batch(adc_engine* e, int n, const BatchIO& io, const MatchReq& q, cudaSt
         if (ingest) {
             const long long off = (long long)first * q.img->image_stride;
             if (q.rect)
-                adc_launch_rectify_ingest(e->P, wave_view(e, ln, nS), io.ls + off, io.rs + off, *q.img, *q.rect, ln.st, &e->launches);
+                adc_launch_rectify_ingest(e->P.dm, nS, io.ls + off, io.rs + off, *q.img, *q.rect, w.bgr, ln.st, &e->launches);
             else
-                adc_launch_image_ingest(e->P, wave_view(e, ln, nS), io.ls + off, io.rs + off, *q.img, ln.st, &e->launches);
+                adc_launch_image_ingest(e->P.dm, nS, io.ls + off, io.rs + off, *q.img, w.bgr, ln.st, &e->launches);
         } else if (strided_copy) {
             const cudaMemcpyKind k = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
             CK(cudaMemcpy2DAsync(w.bgr, 2 * IMG, io.ls + (size_t)first * IMG, IMG, IMG, nS, k, ln.st));
@@ -828,6 +831,29 @@ size_t staged_bytes(const adc_engine* e, const MatchReq& q) {
     return 2 * (size_t)adc_image_tight(q.img->format, view_w(e, q), view_h(e, q)).image_stride;
 }
 
+// One pair's host views (geometry g, resolved, over the raw frames of `rect` or the engine's size) -> `bgr` as packed
+// BGR [2][N*3] on st: the views are uploaded tightly, view after view, to `raw` (2 * the tight footprint) and converted
+// from there by one (rectified) ingestion launch.
+int ingest_host_pair(adc_engine* e, const AdcImageGeom& g, const AdcRectGeom* rect, const uint8_t* left,
+                     const uint8_t* right, uint8_t* raw, uint8_t* bgr, cudaStream_t st) {
+    const size_t sh = rect ? rect->src_h : e->H;
+    const AdcImageGeom tight = adc_image_tight(g.format, rect ? rect->src_w : e->W, sh);
+    const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
+    // one block of tight rows per plane: the three planes of a planar image; the H luma rows and ceil(H/2) chroma
+    // rows of NV12 / NV21; the H rows of every other format
+    const bool yuv420 = g.format == ADC_IMG_NV12 || g.format == ADC_IMG_NV21;
+    const int planes = g.format == ADC_IMG_RGB_PLANAR ? 3 : yuv420 ? 2 : 1;
+    for (int v = 0; v < 2; v++)
+        for (int c = 0; c < planes; c++)
+            CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
+                                 (size_t)g.row_pitch, tp, yuv420 && c ? (sh + 1) / 2 : sh, cudaMemcpyHostToDevice, st));
+    if (rect)
+        adc_launch_rectify_ingest(e->P.dm, 1, raw, raw + foot, tight, *rect, bgr, st, &e->launches);
+    else
+        adc_launch_image_ingest(e->P.dm, 1, raw, raw + foot, tight, bgr, st, &e->launches);
+    return ADC_OK;
+}
+
 // One pair's host inputs of request q -> lane ln, for a run that stops after `last`.  Packed BGR rows (raw ==
 // nullptr) are gathered into the pinned ring and copied into ln.w.bgr at once.  Other formats and raw frames are
 // uploaded tightly, view after view, to `raw` and converted from there by the (rectified) ingestion kernel.  A host
@@ -848,23 +874,8 @@ int upload_pair(adc_engine* e, Lane& ln, const MatchReq& q, const uint8_t* left,
     if (!raw) {
         CK(cudaMemcpyAsync(ln.w.bgr, ln.pin_in, 2 * IMG, cudaMemcpyHostToDevice, ln.st));
     } else {
-        const AdcImageGeom& g = *q.img;
-        const size_t sh = view_h(e, q);
-        const AdcImageGeom tight = adc_image_tight(g.format, view_w(e, q), sh);
-        const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
-        // one block of tight rows per plane: the three planes of a planar image; the H luma rows and ceil(H/2) chroma
-        // rows of NV12 / NV21; the H rows of every other format
-        const bool yuv420 = g.format == ADC_IMG_NV12 || g.format == ADC_IMG_NV21;
-        const int planes = g.format == ADC_IMG_RGB_PLANAR ? 3 : yuv420 ? 2 : 1;
-        for (int v = 0; v < 2; v++)
-            for (int c = 0; c < planes; c++)
-                CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
-                                     (size_t)g.row_pitch, tp, yuv420 && c ? (sh + 1) / 2 : sh, cudaMemcpyHostToDevice,
-                                     ln.st));
-        if (q.rect)
-            adc_launch_rectify_ingest(e->P, wave_view(e, ln, 1), raw, raw + foot, tight, *q.rect, ln.st, &e->launches);
-        else
-            adc_launch_image_ingest(e->P, wave_view(e, ln, 1), raw, raw + foot, tight, ln.st, &e->launches);
+        int rc = ingest_host_pair(e, *q.img, q.rect, left, right, raw, ln.w.bgr, ln.st);
+        if (rc) return rc;
     }
     if (q.cost.p) {
         float* staging = lane_volumes(e, ln.w, last).other;
@@ -1027,6 +1038,56 @@ AdcSpeckle speckle_rules(const adc_speckle_params& p) {
 }
 
 size_t speckle_work_bytes(const adc_engine* e, long long n) { return 8 * (size_t)n * (size_t)e->P.dm.N; }
+
+// The rules of the view entries that need no engine: the image entries' rules on img, then rectified and views.
+int check_views_args(const char* fn, const adc_image_desc* img, int rectified, const void* views, bool device,
+                     const void* left, const void* right) {
+    int rc = check_image_desc(fn, img);
+    if (rc || (device && (rc = check_image_align(fn, img, left, right)))) return rc;
+    if (rectified != 0 && rectified != 1) return fail(ADC_ERR_ARG, "%s: rectified %d is not 0 or 1", fn, rectified);
+    if (!views) return fail(ADC_ERR_ARG, "%s: views is NULL", fn);
+    return ADC_OK;
+}
+
+// The rules of the view entries after the engine check: the size-dependent rules of img against the engine's size
+// (plain) or the raw frame size (rectified, which needs a rectification set).
+int resolve_views(adc_engine* e, const char* fn, const adc_image_desc* img, int rectified, int n, AdcImageGeom* g,
+                  AdcRectGeom* r) {
+    return rectified ? resolve_rectified(e, fn, img, n, g, r) : resolve_image(fn, e->W, e->H, img, n, g);
+}
+
+// The rules of the point-cloud entries that need no engine (device: the alignment rules too).
+int check_cloud_args(const char* fn, int n, const float* disp, const double* Q, const uint8_t* bgr, long long bgr_stride,
+                     float z_min, float z_max, const adc_cloud_out* o, const void* work, bool device) {
+    if (!o) return fail(ADC_ERR_ARG, "%s: out is NULL", fn);
+    if (!o->points) return fail(ADC_ERR_ARG, "%s: out->points is NULL", fn);
+    if (!o->counts) return fail(ADC_ERR_ARG, "%s: out->counts is NULL", fn);
+    if (!disp) return fail(ADC_ERR_ARG, "%s: disp is NULL", fn);
+    if (!Q) return fail(ADC_ERR_ARG, "%s: Q is NULL", fn);
+    if (!o->colors != !bgr)
+        return fail(ADC_ERR_ARG, "%s: out->colors is %s but bgr is %s (colours need an image, an image needs colours)", fn,
+                    o->colors ? "given" : "NULL", bgr ? "given" : "NULL");
+    if (o->capacity < 1) return fail(ADC_ERR_ARG, "%s: out->capacity %lld is below 1", fn, (long long)o->capacity);
+    if (o->reserved != 0) return fail(ADC_ERR_ARG, "%s: out->reserved must be zero", fn);
+    if (std::isnan(z_min)) return fail(ADC_ERR_ARG, "%s: z_min is NaN", fn);
+    if (std::isnan(z_max)) return fail(ADC_ERR_ARG, "%s: z_max is NaN", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (bgr_stride < 0) return fail(ADC_ERR_ARG, "%s: bgr_stride %lld is negative", fn, bgr_stride);
+    if (device) {
+        if ((uintptr_t)disp % 4) return fail(ADC_ERR_ARG, "%s: disp is not 4-byte aligned", fn);
+        if ((uintptr_t)o->points % 4) return fail(ADC_ERR_ARG, "%s: out->points is not 4-byte aligned", fn);
+        if ((uintptr_t)o->pixels % 4) return fail(ADC_ERR_ARG, "%s: out->pixels is not 4-byte aligned", fn);
+        if ((uintptr_t)o->counts % 4) return fail(ADC_ERR_ARG, "%s: out->counts is not 4-byte aligned", fn);
+        if ((uintptr_t)work % 8) return fail(ADC_ERR_ARG, "%s: work is not 8-byte aligned", fn);
+    }
+    return ADC_OK;
+}
+
+int check_cloud_capacity(const adc_engine* e, const char* fn, const adc_cloud_out* o) {
+    if (o->capacity > e->P.dm.N)
+        return fail(ADC_ERR_ARG, "%s: out->capacity %lld is above H * W (%d)", fn, (long long)o->capacity, e->P.dm.N);
+    return ADC_OK;
+}
 
 }  // namespace
 
@@ -1536,6 +1597,127 @@ int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* para
     return ADC_OK;
 }
 
+int adc_ingest_views_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                  const adc_image_desc* img, int32_t rectified, uint8_t* d_views, void* stream) {
+    const char* fn = "adc_ingest_views_batch_device";
+    int rc = check_views_args(fn, img, rectified, d_views, true, d_left, d_right);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (n > 0 && (!d_left || !d_right)) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
+    AdcImageGeom g;
+    AdcRectGeom r;
+    if ((rc = resolve_views(e, fn, img, rectified, n, &g, &r))) return rc;
+    if (n == 0) return ADC_OK;
+    CK(cudaSetDevice(e->cfg.device));
+    const size_t pair_bytes = 6 * (size_t)e->P.dm.N;
+    for (int first = 0; first < n; first += 65535) {   // k_image_ingest's blockIdx.z is the pair
+        const int count = std::min(n - first, 65535);
+        const long long off = (long long)first * g.image_stride;
+        uint8_t* out = d_views + (size_t)first * pair_bytes;
+        if (rectified)
+            adc_launch_rectify_ingest(e->P.dm, count, d_left + off, d_right + off, g, r, out, (cudaStream_t)stream, &e->launches);
+        else
+            adc_launch_image_ingest(e->P.dm, count, d_left + off, d_right + off, g, out, (cudaStream_t)stream, &e->launches);
+    }
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_ingest_views(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img,
+                     int32_t rectified, uint8_t* views) {
+    const char* fn = "adc_ingest_views";
+    int rc = check_views_args(fn, img, rectified, views, false, left, right);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if (!left || !right) return fail(ADC_ERR_ARG, "%s: NULL image", fn);
+    AdcImageGeom g;
+    AdcRectGeom r;
+    if ((rc = resolve_views(e, fn, img, rectified, 1, &g, &r))) return rc;
+    if ((rc = idle_lane0(e))) return rc;
+    Lane& ln = e->lanes[0];
+    // staging: the views, then the raw frames uploaded tightly
+    const size_t out_bytes = 6 * (size_t)e->P.dm.N, off = align_up(out_bytes, 256);
+    const AdcImageGeom tight = rectified ? adc_image_tight(g.format, r.src_w, r.src_h) : adc_image_tight(g.format, e->W, e->H);
+    if ((rc = grow_stage(e, fn, off + 2 * (size_t)tight.image_stride, "the raw views and the packed BGR views"))) return rc;
+    uint8_t* stage = static_cast<uint8_t*>(e->vol_stage);
+    if ((rc = ingest_host_pair(e, g, rectified ? &r : nullptr, left, right, stage + off, stage, ln.st))) return rc;
+    CK(cudaMemcpyAsync(views, stage, out_bytes, cudaMemcpyDeviceToHost, ln.st));
+    CK(cudaStreamSynchronize(ln.st));
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_point_cloud_workspace_bytes(const adc_engine* e, int32_t n, size_t* out) {
+    const char* fn = "adc_point_cloud_workspace_bytes";
+    if (!out) return fail(ADC_ERR_ARG, "%s: out is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    *out = adc_point_cloud_work_bytes(e->P.dm, n);
+    return ADC_OK;
+}
+
+int adc_point_cloud_batch_device(adc_engine* e, int32_t n, const float* d_disp, const double Q[16], const uint8_t* d_bgr,
+                                 int64_t bgr_stride, float z_min, float z_max, const adc_cloud_out* out, void* d_work,
+                                 size_t work_bytes, void* stream) {
+    const char* fn = "adc_point_cloud_batch_device";
+    int rc = check_cloud_args(fn, n, d_disp, Q, d_bgr, bgr_stride, z_min, z_max, out, d_work, true);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if ((rc = check_cloud_capacity(e, fn, out))) return rc;
+    const size_t need = adc_point_cloud_work_bytes(e->P.dm, n);
+    if (work_bytes < need) return fail(ADC_ERR_ARG, "%s: work_bytes %zu below the %zu bytes of %d maps", fn, work_bytes, need, n);
+    if (n == 0) return ADC_OK;
+    if (!d_work) return fail(ADC_ERR_ARG, "%s: work is NULL", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    const cudaStream_t st = (cudaStream_t)stream;
+    CK(cudaMemsetAsync(d_work, 0, need, st));
+    const AdcCloudOut o{out->points, out->colors, out->pixels, out->counts, (long long)out->capacity};
+    adc_launch_point_cloud(e->P.dm, n, d_disp, reproj_q(Q), d_bgr, bgr_stride ? (long long)bgr_stride : 3ll * e->P.dm.N,
+                           z_min, z_max, o, d_work, st, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
+int adc_point_cloud(adc_engine* e, const float* disp, const double Q[16], const uint8_t* bgr, float z_min, float z_max,
+                    const adc_cloud_out* out) {
+    const char* fn = "adc_point_cloud";
+    int rc = check_cloud_args(fn, 1, disp, Q, bgr, 0, z_min, z_max, out, nullptr, false);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    if ((rc = check_cloud_capacity(e, fn, out))) return rc;
+    if ((rc = idle_lane0(e))) return rc;
+    Lane& ln = e->lanes[0];
+    // staging, each part 256-byte aligned: workspace, map, image, points, colours, pixel indices, count
+    const size_t N = (size_t)e->P.dm.N, cap = (size_t)out->capacity;
+    const size_t sizes[7] = {adc_point_cloud_work_bytes(e->P.dm, 1), N * sizeof(float), bgr ? 3 * N : 0,
+                             12 * cap, out->colors ? 3 * cap : 0, out->pixels ? 4 * cap : 0, sizeof(int32_t)};
+    size_t off[7], need = 0;
+    for (int i = 0; i < 7; i++) {
+        off[i] = need;
+        need += align_up(sizes[i], 256);
+    }
+    if ((rc = grow_stage(e, fn, need, "the map, its image and its point cloud"))) return rc;
+    char* stage = static_cast<char*>(e->vol_stage);
+    CK(cudaMemcpyAsync(stage + off[1], disp, sizes[1], cudaMemcpyHostToDevice, ln.st));
+    if (bgr) CK(cudaMemcpyAsync(stage + off[2], bgr, sizes[2], cudaMemcpyHostToDevice, ln.st));
+    CK(cudaMemsetAsync(stage, 0, sizes[0], ln.st));
+    const AdcCloudOut o{reinterpret_cast<float*>(stage + off[3]), out->colors ? reinterpret_cast<uint8_t*>(stage + off[4]) : nullptr,
+                        out->pixels ? reinterpret_cast<int32_t*>(stage + off[5]) : nullptr,
+                        reinterpret_cast<int32_t*>(stage + off[6]), (long long)cap};
+    adc_launch_point_cloud(e->P.dm, 1, reinterpret_cast<const float*>(stage + off[1]), reproj_q(Q),
+                           bgr ? reinterpret_cast<const uint8_t*>(stage + off[2]) : nullptr, 3ll * e->P.dm.N, z_min, z_max,
+                           o, stage, ln.st, &e->launches);
+    CK(cudaMemcpyAsync(out->counts, o.counts, sizeof(int32_t), cudaMemcpyDeviceToHost, ln.st));
+    CK(cudaStreamSynchronize(ln.st));
+    CK(cudaGetLastError());
+    const size_t kept = std::min((size_t)std::max(out->counts[0], 0), cap);
+    CK(cudaMemcpy(out->points, o.points, 12 * kept, cudaMemcpyDeviceToHost));
+    if (out->colors) CK(cudaMemcpy(out->colors, o.colors, 3 * kept, cudaMemcpyDeviceToHost));
+    if (out->pixels) CK(cudaMemcpy(out->pixels, o.pixels, 4 * kept, cudaMemcpyDeviceToHost));
+    return ADC_OK;
+}
+
 void* adc_host_alloc(size_t bytes) {
     void* p = nullptr;
     if (cudaHostAlloc(&p, bytes, cudaHostAllocDefault) != cudaSuccess) { cudaGetLastError(); return nullptr; }
@@ -1673,7 +1855,7 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 const long long foot = g.image_stride;
                 g.image_stride = 2 * foot;
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
-                adc_launch_image_ingest(P, w, src, src + foot, g, ln.st, &e->launches);
+                adc_launch_image_ingest(P.dm, w.S, src, src + foot, g, w.bgr, ln.st, &e->launches);
                 bytes = 2.0 * adc_image_read_bytes(e->img_format, P.dm.W, P.dm.H) + 2 * 3.0 * N;
                 break;
             }
@@ -1686,7 +1868,7 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 g.image_stride = 2 * foot;
                 const AdcRectGeom rg{{e->rect_map, e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h};
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
-                adc_launch_rectify_ingest(P, w, src, src + foot, g, rg, ln.st, &e->launches);
+                adc_launch_rectify_ingest(P.dm, w.S, src, src + foot, g, rg, w.bgr, ln.st, &e->launches);
                 bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
                 break;
             }

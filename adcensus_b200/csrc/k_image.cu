@@ -16,22 +16,22 @@
 #include "adc_common.cuh"
 #include "k_image.cuh"
 
-void adc_launch_image_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
-                             const AdcImageGeom& g, cudaStream_t st, unsigned long long* launches) {
+void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                             uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
-        case ADC_IMG_BGR: launch_image<ADC_IMG_BGR>(P.dm, w.S, left, right, g, w.bgr, st); break;
-        case ADC_IMG_RGB: launch_image<ADC_IMG_RGB>(P.dm, w.S, left, right, g, w.bgr, st); break;
-        case ADC_IMG_BGRA: launch_image<ADC_IMG_BGRA>(P.dm, w.S, left, right, g, w.bgr, st); break;
-        case ADC_IMG_RGBA: launch_image<ADC_IMG_RGBA>(P.dm, w.S, left, right, g, w.bgr, st); break;
-        case ADC_IMG_GRAY: launch_image<ADC_IMG_GRAY>(P.dm, w.S, left, right, g, w.bgr, st); break;
+        case ADC_IMG_BGR: launch_image<ADC_IMG_BGR>(dm, S, left, right, g, bgr, st); break;
+        case ADC_IMG_RGB: launch_image<ADC_IMG_RGB>(dm, S, left, right, g, bgr, st); break;
+        case ADC_IMG_BGRA: launch_image<ADC_IMG_BGRA>(dm, S, left, right, g, bgr, st); break;
+        case ADC_IMG_RGBA: launch_image<ADC_IMG_RGBA>(dm, S, left, right, g, bgr, st); break;
+        case ADC_IMG_GRAY: launch_image<ADC_IMG_GRAY>(dm, S, left, right, g, bgr, st); break;
         case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
-            adc_launch_bayer_image(P.dm, w.S, left, right, g, w.bgr, st);
+            adc_launch_bayer_image(dm, S, left, right, g, bgr, st);
             break;
         case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
-            adc_launch_yuv_image(P.dm, w.S, left, right, g, w.bgr, st);
+            adc_launch_yuv_image(dm, S, left, right, g, bgr, st);
             break;
-        case ADC_IMG_RGB_PLANAR: launch_image<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, w.bgr, st); break;
-        default: adc_launch_rawdepth_image(P.dm, w.S, left, right, g, w.bgr, st); break;
+        case ADC_IMG_RGB_PLANAR: launch_image<ADC_IMG_RGB_PLANAR>(dm, S, left, right, g, bgr, st); break;
+        default: adc_launch_rawdepth_image(dm, S, left, right, g, bgr, st); break;
     }
     ++*launches;
 }

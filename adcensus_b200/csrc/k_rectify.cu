@@ -68,22 +68,22 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
     else k_remap_convert_fixed<<<grid, RC_THREADS, 0, st>>>(dm.W, dm.N, m1, pitch1, m2, pitch2, out);
 }
 
-void adc_launch_rectify_ingest(const AdcParams& P, const AdcWave& w, const uint8_t* left, const uint8_t* right,
-                               const AdcImageGeom& g, const AdcRectGeom& r, cudaStream_t st, unsigned long long* launches) {
+void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                               const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
-        case ADC_IMG_BGR: launch_rectify<ADC_IMG_BGR>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
-        case ADC_IMG_RGB: launch_rectify<ADC_IMG_RGB>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
-        case ADC_IMG_BGRA: launch_rectify<ADC_IMG_BGRA>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
-        case ADC_IMG_RGBA: launch_rectify<ADC_IMG_RGBA>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
-        case ADC_IMG_GRAY: launch_rectify<ADC_IMG_GRAY>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
+        case ADC_IMG_BGR: launch_rectify<ADC_IMG_BGR>(dm, S, left, right, g, r, bgr, st); break;
+        case ADC_IMG_RGB: launch_rectify<ADC_IMG_RGB>(dm, S, left, right, g, r, bgr, st); break;
+        case ADC_IMG_BGRA: launch_rectify<ADC_IMG_BGRA>(dm, S, left, right, g, r, bgr, st); break;
+        case ADC_IMG_RGBA: launch_rectify<ADC_IMG_RGBA>(dm, S, left, right, g, r, bgr, st); break;
+        case ADC_IMG_GRAY: launch_rectify<ADC_IMG_GRAY>(dm, S, left, right, g, r, bgr, st); break;
         case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
-            adc_launch_bayer_rectify(P.dm, w.S, left, right, g, r, w.bgr, st);
+            adc_launch_bayer_rectify(dm, S, left, right, g, r, bgr, st);
             break;
         case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
-            adc_launch_yuv_rectify(P.dm, w.S, left, right, g, r, w.bgr, st);
+            adc_launch_yuv_rectify(dm, S, left, right, g, r, bgr, st);
             break;
-        case ADC_IMG_RGB_PLANAR: launch_rectify<ADC_IMG_RGB_PLANAR>(P.dm, w.S, left, right, g, r, w.bgr, st); break;
-        default: adc_launch_rawdepth_rectify(P.dm, w.S, left, right, g, r, w.bgr, st); break;
+        case ADC_IMG_RGB_PLANAR: launch_rectify<ADC_IMG_RGB_PLANAR>(dm, S, left, right, g, r, bgr, st); break;
+        default: adc_launch_rawdepth_rectify(dm, S, left, right, g, r, bgr, st); break;
     }
     ++*launches;
 }

@@ -6,9 +6,7 @@
 //             double, P_c = (float)((double)(float)h_c * (1.0 / h_3))
 //   DEPTH     P_2 alone
 //   DISP_S16  saturate_cast<short>(d * 16) as x86 computes it, (min_disparity - 1) * 16 for +inf
-// The double arithmetic is written with the _rn intrinsics, so nvcc can neither contract a multiply and an add into a
-// DFMA nor fold the +0.0 that turns a -0 first product into +0 (OpenCV's sum starts at +0.0).  Q[i][3] is added as it
-// is: OpenCV multiplies it by 1.0, which changes no value.
+// The double arithmetic (q_row, coord) is in k_reproject.cuh, shared with the point clouds of k_cloud.cu.
 // Each template instance computes only what its outputs need: the S16-only kernel does no double arithmetic, the
 // depth-only kernel evaluates rows 2 and 3.
 // Grid: blockIdx.x = a run of RP_PIX consecutive pixels of a map, blockIdx.y (striding by gridDim.y) = the map.  Offsets
@@ -18,25 +16,13 @@
 #include <algorithm>
 
 #include "adc_common.cuh"
+#include "k_reproject.cuh"
 
 #define RP_THREADS 256
 #define RP_PER_THREAD 4
 #define RP_PIX (RP_THREADS * RP_PER_THREAD)   // pixels per CTA and map
 
 enum { RP_POINTS = 1, RP_DEPTH = 2, RP_S16 = 4 };
-
-// h_i of pixel (x, y) with value d, one rounding per operation
-static __device__ __forceinline__ double q_row(const AdcReprojQ& Q, int i, double x, double y, double d) {
-    double h = __dadd_rn(0.0, __dmul_rn(Q.q[4 * i], x));
-    h = __dadd_rn(h, __dmul_rn(Q.q[4 * i + 1], y));
-    h = __dadd_rn(h, __dmul_rn(Q.q[4 * i + 2], d));
-    return __dadd_rn(h, Q.q[4 * i + 3]);
-}
-
-// OpenCV's double-rounded coordinate: (float)((double)(float)h * ia)
-static __device__ __forceinline__ float coord(double h, double ia) {
-    return __double2float_rn(__dmul_rn((double)__double2float_rn(h), ia));
-}
 
 // cv::saturate_cast<short>(d * 16) on x86, the engine's invalid value for +inf
 static __device__ __forceinline__ int16_t disp_s16(float d, int16_t invalid) {

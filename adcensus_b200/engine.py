@@ -262,6 +262,16 @@ class SpeckleParams(ctypes.Structure):
 assert ctypes.sizeof(SpeckleParams) == 32
 
 
+class CloudOut(ctypes.Structure):
+    """adc_cloud_out: the destinations of a point cloud (points, colors or None, pixels or None, counts), the points
+    per map they hold (capacity) and a reserved zero."""
+    _fields_ = [("points", ctypes.c_void_p), ("colors", ctypes.c_void_p), ("pixels", ctypes.c_void_p),
+                ("counts", ctypes.c_void_p), ("capacity", ctypes.c_int64), ("reserved", ctypes.c_int64)]
+
+
+assert ctypes.sizeof(CloudOut) == 48
+
+
 class AdcError(RuntimeError):
     pass
 
@@ -336,6 +346,14 @@ def load_library() -> ctypes.CDLL:
     L.adc_speckle_workspace_bytes.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_size_t)]
     L.adc_filter_speckles.argtypes = [vp, vp, ctypes.POINTER(SpeckleParams)]
     L.adc_filter_speckles_batch_device.argtypes = [vp, i32, vp, ctypes.POINTER(SpeckleParams), vp, ctypes.c_size_t, vp]
+    L.adc_ingest_views.argtypes = [vp, u8p, u8p, ctypes.POINTER(ImageDesc), i32, u8p]
+    L.adc_ingest_views_batch_device.argtypes = [vp, i32, u8p, u8p, ctypes.POINTER(ImageDesc), i32, u8p, vp]
+    L.adc_point_cloud_workspace_bytes.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_size_t)]
+    L.adc_point_cloud.argtypes = [vp, f32p, ctypes.POINTER(ctypes.c_double), u8p, ctypes.c_float, ctypes.c_float,
+                                  ctypes.POINTER(CloudOut)]
+    L.adc_point_cloud_batch_device.argtypes = [vp, i32, f32p, ctypes.POINTER(ctypes.c_double), u8p, ctypes.c_int64,
+                                               ctypes.c_float, ctypes.c_float, ctypes.POINTER(CloudOut), vp,
+                                               ctypes.c_size_t, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -690,6 +708,75 @@ class Engine:
         nv = self.speckle_invalid(t) if new_val is None else new_val
         p = SpeckleParams(t, int(max_size), float(nv), float(max_diff), 0)
         _check(self._L.adc_filter_speckles_batch_device(self._h, n, d_maps, ctypes.byref(p), d_work, work_bytes, stream))
+
+    # ---- the views as the engine matches them (adc_ingest_views*) ---------------------------------------
+    def ingest_views(self, left, right, format="bgr", rectified=False) -> np.ndarray:
+        """uint8 [2][H][W][3]: the packed BGR left and right views that match_images (rectified=False) or
+        match_rectified (rectified=True) feed to stage 1 for the same views, in the shapes those entries take."""
+        fmt = _img_format(format)
+        if rectified and self.rect_src_size is None:
+            raise AdcError("no rectification is set (set_rectification)")
+        vw, vh = self.rect_src_size if rectified else (self.width, self.height)
+        desc = _image_view_desc(left, fmt, vh, vw)
+        if _image_view_desc(right, fmt, vh, vw).row_pitch != desc.row_pitch or \
+                (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
+            raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
+        views = np.empty((2, self.height, self.width, 3), np.uint8)
+        _check(self._L.adc_ingest_views(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc),
+                                        1 if rectified else 0, views.ctypes.data))
+        return views
+
+    def ingest_views_batch_device(self, n: int, d_left: int, d_right: int, d_views: int, image=None, rectified=False,
+                                  stream: int = 0):
+        """Device pointers (ints): n pairs described by `image` (an ImageDesc, None = tight packed BGR), plain or through
+        the rectification, written to d_views as packed BGR [n][2][H][W][3].  One launch per 65535 pairs enqueued on
+        `stream` without synchronising."""
+        _check(self._L.adc_ingest_views_batch_device(self._h, n, d_left, d_right,
+                                                     None if image is None else ctypes.byref(image),
+                                                     1 if rectified else 0, d_views, stream))
+
+    # ---- point clouds (adc_point_cloud*) ------------------------------------------------------------------
+    def point_cloud(self, disp, Q, bgr=None, z_range=(-np.inf, np.inf), pixels=False):
+        """The valid points of one disparity map (float32 [H][W]) in raster order: points float32 [k][3], plus colors
+        uint8 [k][3] (R, G, B of `bgr`, a packed BGR [H][W][3] image) and pixels int32 [k] (y*W + x) when requested --
+        cv2.reprojectImageTo3D(disp, Q)[keep] with keep = finite d, finite point, z_range[0] <= Z <= z_range[1].
+        Returns points alone, or a tuple (points[, colors][, pixels])."""
+        H, W = self.height, self.width
+        disp = np.ascontiguousarray(disp, np.float32)
+        if disp.shape != (H, W):
+            raise ValueError(f"expected a disparity map of shape {(H, W)}, got {disp.shape}")
+        img = None if bgr is None else _img(bgr, (H, W, 3))
+        N = H * W
+        pts = np.empty((N, 3), np.float32)
+        cols = np.empty((N, 3), np.uint8) if img is not None else None
+        pix = np.empty(N, np.int32) if pixels else None
+        count = np.zeros(1, np.int32)
+        out = CloudOut(pts.ctypes.data, None if cols is None else cols.ctypes.data, None if pix is None else pix.ctypes.data,
+                       count.ctypes.data, N, 0)
+        _check(self._L.adc_point_cloud(self._h, disp.ctypes.data, _q_matrix(Q), None if img is None else img.ctypes.data,
+                                       float(z_range[0]), float(z_range[1]), ctypes.byref(out)))
+        k = int(count[0])
+        res = [pts[:k].copy()] + ([cols[:k].copy()] if cols is not None else []) + ([pix[:k].copy()] if pixels else [])
+        return res[0] if len(res) == 1 else tuple(res)
+
+    def point_cloud_workspace_bytes(self, n: int) -> int:
+        """Bytes of device workspace that point_cloud_batch_device needs for n maps."""
+        out = ctypes.c_size_t()
+        _check(self._L.adc_point_cloud_workspace_bytes(self._h, n, ctypes.byref(out)))
+        return int(out.value)
+
+    def point_cloud_batch_device(self, n: int, d_disp: int, Q, d_points: int, d_counts: int, capacity: int,
+                                 d_work: int, work_bytes: int, d_bgr: int = 0, bgr_stride: int = 0, d_colors: int = 0,
+                                 d_pixels: int = 0, z_range=(-np.inf, np.inf), stream: int = 0):
+        """Device pointers (ints): n maps of H*W float32 at d_disp; map i's first `capacity` kept points at point
+        i*capacity of d_points (float32 x3), d_colors (uint8 R, G, B of d_bgr + i*bgr_stride, 0 = 3*H*W) and d_pixels
+        (int32), its full count at d_counts[i]; work_bytes >= point_cloud_workspace_bytes(n) of workspace at d_work.  A
+        memset and one launch enqueued on `stream` without synchronising; in pipelined mode the maps must be joined on
+        `stream` first."""
+        out = CloudOut(d_points, d_colors or None, d_pixels or None, d_counts, int(capacity), 0)
+        _check(self._L.adc_point_cloud_batch_device(self._h, n, d_disp, _q_matrix(Q), d_bgr or None, int(bgr_stride),
+                                                    float(z_range[0]), float(z_range[1]), ctypes.byref(out), d_work,
+                                                    work_bytes, stream))
 
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""

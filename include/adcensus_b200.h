@@ -592,6 +592,82 @@ int adc_filter_speckles_batch_device(adc_engine* e, int32_t n, void* d_maps, con
  * concurrently with another call on the same engine. */
 int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* params);
 
+/* ---- the views as the engine matches them ----------------------------------------------------------------
+ * The packed BGR views that stage 1 of a match reads, handed to the caller: n pairs described by `img` (NULL = tight
+ * packed BGR), plain (rectified = 0, what adc_match_images* ingests) or resampled through the maps set with
+ * adc_set_rectification (rectified = 1, what adc_match_rectified* ingests), written as packed BGR u8 [n][2][H][W][3]:
+ * pair i's left view at byte i*6*H*W, its right view 3*H*W bytes after it.  The bytes are exactly those the image or
+ * rectified entries feed to stage 1 for the same arguments, so every rule of those entries carries over: formats,
+ * geometry, alignment, the demosaic, YUV and depth-reduction rules, cv::remap, and BGR 0 outside the frame.  Passing
+ * d_views back to adc_match_images_batch_device as tight packed BGR therefore matches exactly what the raw-format call
+ * matches, and d_views with a stride of 6*H*W colours adc_point_cloud_batch_device's points by the left view.
+ * Fails with ADC_ERR_ARG naming the field: the image entries' rules on img (before the engine is checked, and on the
+ * device entry the 16-bit alignment rule), rectified not 0 or 1, views NULL, then (after the engine check) a negative
+ * n, a NULL view with n > 0, the size-dependent rules of img against W x H (plain) or the raw frame size (rectified),
+ * and, rectified, no rectification set.  d_views needs no alignment.
+ * The device entry enqueues ceil(n / 65535) ingestion launches (one per 65535 pairs) on `stream` (a cudaStream_t,
+ * NULL = legacy default stream), not synchronised; the caller's views must stay untouched until they complete.  It touches no engine buffer but the rectification maps, which adc_set_rectification replaces only
+ * after synchronising the device, so it may run next to the engine's batch calls. */
+int adc_ingest_views_batch_device(adc_engine* e, int32_t n, const uint8_t* d_left, const uint8_t* d_right,
+                                  const adc_image_desc* img, int32_t rectified, uint8_t* d_views, void* stream);
+/* One pair, host pointers (image_stride is not used), synchronous: views = [2][H][W][3].  The raw views and the output
+ * pass through the device staging of adc_match_volumes (allocated on first use, grown when needed; ADC_ERR_NOMEM
+ * before any work if that fails); one ingestion launch.  Not concurrently with another call on the same engine. */
+int adc_ingest_views(adc_engine* e, const uint8_t* left, const uint8_t* right, const adc_image_desc* img,
+                     int32_t rectified, uint8_t* views);
+
+/* ---- point clouds -------------------------------------------------------------------------------------------
+ * The valid points of f32 [H][W] disparity maps of the engine's size, compacted in raster order, with their colours:
+ * what cv::reprojectImageTo3D followed by boolean indexing gives (OpenCV's samples/python/stereo_match.py), in one pass
+ * and without a host round trip.  Let P be ADC_REPROJ_POINTS of pixel (x, y) with value d (the reprojection formula
+ * above, bit for bit).  The pixel is kept iff d is finite, P_x, P_y and P_z are finite, and z_min <= P_z <= z_max as
+ * IEEE float comparisons (z_min > z_max keeps nothing; +-inf bounds keep every finite Z).  A non-finite d never has a
+ * finite point (with Q[i][2] = 0 the product 0 * inf is NaN), so the d-finite term states the rule without changing the
+ * result for any Q; an invalid (+inf) pixel is never kept.  Kept pixels
+ * are written in raster order, each with P (f32 x, y, z), then (R, G, B) = (bgr[2], bgr[1], bgr[0]) of pixel (x, y) of
+ * that map's colour image, then y*W + x.  When a map keeps more than `capacity` pixels only the first `capacity` are
+ * written, nothing past them is touched, and counts[i] still holds the full number.  Kept points are finite, so every
+ * output compares bit for bit (no NaN payloads).  In numpy:
+ *   P = cv2.reprojectImageTo3D(disp, Q)
+ *   keep = np.isfinite(disp) & np.isfinite(P).all(-1) & (P[..., 2] >= z_min) & (P[..., 2] <= z_max)
+ *   points, colors, pixels = P[keep], cv2.cvtColor(bgr, cv2.COLOR_BGR2RGB)[keep], np.flatnonzero(keep)
+ * Colour: packed BGR u8 [H][W][3] per map, bgr_stride bytes from one map's image to the next (0 = 3*H*W): the images
+ * the maps were matched from, e.g. adc_ingest_views_batch_device's views with stride 6*H*W (the left views). */
+typedef struct adc_cloud_out {
+    float*   points;    /* f32 [capacity][3] per map, map i's points at point i*capacity (required) */
+    uint8_t* colors;    /* u8 [capacity][3] R, G, B per map, or NULL; non-NULL iff a colour image is given */
+    int32_t* pixels;    /* int32 [capacity] per map, y*W + x of each point, or NULL */
+    int32_t* counts;    /* int32 [n]: the points each map keeps, the true number even beyond capacity (required) */
+    int64_t  capacity;  /* points per map in the destinations, 1..H*W */
+    int64_t  reserved;  /* must be zero */
+} adc_cloud_out;        /* 48 bytes */
+
+/* *out = the device workspace adc_point_cloud_batch_device needs for n maps: 8 * (1 + n * ceil(H*W / 2048)) bytes, 0 for
+ * n = 0. */
+int adc_point_cloud_workspace_bytes(const adc_engine* e, int32_t n, size_t* out);
+/* n maps in device memory (map i at element i*H*W), colour images d_bgr (or NULL) and the destinations of `out` in
+ * device memory, using only the caller's workspace d_work of work_bytes bytes, which the call initialises itself: one
+ * cudaMemsetAsync of the workspace and one kernel launch enqueued on `stream` (a cudaStream_t, NULL = legacy default
+ * stream) for any n and any content, not synchronised, no host round trip.  The kernel is a single pass: each tile of
+ * 2048 pixels computes its points once, and finds its place in the map's output by a decoupled look-back over the
+ * map's earlier tiles.  Q is passed by value: the caller may free it on return.  No engine buffer is touched, so the
+ * call may run next to the engine's batch calls; the maps must be complete in `stream`'s order (in pipelined mode,
+ * after adc_join on that stream).
+ * Fails with ADC_ERR_ARG naming the field, before the engine is checked: out NULL; out->points, out->counts, the map or
+ * Q NULL; out->colors and the colour image not both given or both NULL; capacity below 1; a non-zero reserved; z_min or
+ * z_max NaN; a negative n or bgr_stride; on the device entry the map, out->points, out->pixels or out->counts not
+ * 4-byte aligned, or d_work not 8-byte aligned; then capacity above H*W, work_bytes below
+ * adc_point_cloud_workspace_bytes for n maps, d_work NULL while n > 0.  n == 0 is a no-op. */
+int adc_point_cloud_batch_device(adc_engine* e, int32_t n, const float* d_disp, const double Q[16], const uint8_t* d_bgr,
+                                 int64_t bgr_stride, float z_min, float z_max, const adc_cloud_out* out, void* d_work,
+                                 size_t work_bytes, void* stream);
+/* One map, host pointers (bgr [H][W][3] or NULL; out's arrays and counts[0]), synchronous.  The map, the image, the
+ * workspace and the outputs pass through the device staging of adc_match_volumes (allocated on first use, grown when
+ * needed; ADC_ERR_NOMEM before any work if that fails); only the min(count, capacity) kept points are copied back.
+ * Not concurrently with another call on the same engine. */
+int adc_point_cloud(adc_engine* e, const float* disp, const double Q[16], const uint8_t* bgr, float z_min, float z_max,
+                    const adc_cloud_out* out);
+
 void* adc_host_alloc(size_t bytes);  /* pinned host memory (cudaHostAlloc) */
 void  adc_host_free(void* p);
 int   adc_synchronize(adc_engine* e);
