@@ -122,6 +122,9 @@ struct adc_engine {
     // device staging of adc_match_volumes' exported volumes: allocated on first use, grown when needed
     void* vol_stage = nullptr;
     size_t vol_stage_bytes = 0;
+    // [N] pinned: the right-view map of the latest one-pair host match with a final map (adc_get_right_disparity), kept
+    // apart from lane 0's arena, which every batch call's first wave overwrites
+    float* pin_disp_r = nullptr;
 };
 
 namespace {
@@ -929,6 +932,7 @@ int match_host(adc_engine* e, const char* fn, const MatchReq& q, const uint8_t* 
     if (disp) {
         CK(cudaMemcpyAsync(ln.pin_out, ln.w.disp_l, N * sizeof(float), cudaMemcpyDeviceToHost, ln.st));
         CK(cudaEventRecord(ev[6], ln.st));
+        CK(cudaMemcpyAsync(e->pin_disp_r, ln.w.disp_r, N * sizeof(float), cudaMemcpyDeviceToHost, ln.st));
     }
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
@@ -1129,6 +1133,7 @@ void adc_destroy(adc_engine* e) {
     if (e->d_ray_off) cudaFree(e->d_ray_off);
     if (e->vol_stage) cudaFree(e->vol_stage);
     if (e->rect_map) cudaFree(e->rect_map);
+    if (e->pin_disp_r) cudaFreeHost(e->pin_disp_r);
     if (e->ev_fork) cudaEventDestroy(e->ev_fork);
     for (auto& ev : e->ev_stage) if (ev) cudaEventDestroy(ev);
     if (e->main_st) cudaStreamDestroy(e->main_st);
@@ -1224,6 +1229,11 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
             return bail(fail(ADC_ERR_NOMEM, "pinned staging allocation failed"));
         }
     }
+    if (cudaHostAlloc((void**)&e->pin_disp_r, N * sizeof(float), cudaHostAllocDefault) != cudaSuccess) {
+        cudaGetLastError();
+        return bail(fail(ADC_ERR_NOMEM, "pinned staging allocation failed"));
+    }
+    memset(e->pin_disp_r, 0, N * sizeof(float));
     if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail(ADC_ERR_CUDA, "device sync failed: %s", cudaGetErrorString(cudaGetLastError())));
     *out = e;
     return ADC_OK;
@@ -1249,10 +1259,7 @@ int adc_match_cost(adc_engine* e, const uint8_t* img_left, const uint8_t* img_ri
 
 int adc_get_right_disparity(adc_engine* e, float* disp_right) {
     if (!e || !disp_right) return fail(ADC_ERR_ARG, "adc_get_right_disparity: bad arguments");
-    CK(cudaSetDevice(e->cfg.device));
-    Lane& ln = e->lanes[0];
-    CK(cudaStreamSynchronize(ln.st));
-    CK(cudaMemcpy(disp_right, ln.w.disp_r, (size_t)e->P.dm.N * sizeof(float), cudaMemcpyDeviceToHost));
+    memcpy(disp_right, e->pin_disp_r, (size_t)e->P.dm.N * sizeof(float));   // complete: match_host synchronised
     return ADC_OK;
 }
 

@@ -110,7 +110,9 @@ int adc_match(adc_engine* e, const uint8_t* img_left, const uint8_t* img_right, 
 /* The right-view disparity map of the most recent adc_match call: what the reference computes into its private
  * disp_right_ (ADCensusStereo::ComputeDisparityRight, ADCensusStereo.cpp:245-310) for the left-right check and never
  * hands out -- float32 [H][W], sub-pixel, not refined (a minimum at either end of the range is the integer disparity).
- * Host pointer.  SURVEY.md 8(f) rank 4. */
+ * Host pointer.  The one-pair host entries with a final map (adc_match, adc_match_cost and, with disp, the volumes,
+ * outputs, images and rectified ones) count as adc_match calls here; batch calls, synchronous or not, pipelined or not,
+ * made since do not change the map this returns.  SURVEY.md 8(f) rank 4. */
 int adc_get_right_disparity(adc_engine* e, float* disp_right);
 
 /* Batched Match over n independent pairs (the data-parallel form of the call above; the
