@@ -119,7 +119,6 @@ struct AdcWave {            // device pointers of one wave (S pairs)
     unsigned* so_bitrows;   // [S][4][H][row words] mirrored per-row bit vectors of the right image (scanline optimiser)
     unsigned* so_rec;       // [S][4][N][rec words] per-pixel penalty records of the four pass directions
     const AdcSoTmaps* so_tm;     // host memory, owned by the lane: tensor maps of the scanline passes
-    unsigned long long* wta_key;  // [S][N] right-view WTA keys (ordered cost << 32 | disparity index)
     int* vote_work;         // [S][N]     region voting: slots whose histogram changed, to derive this round
     int2* vote_chg;         // [S][N]     region voting: change records of the current round / fills of a commit
     uchar2* vote_alr;       // [S][N]     region voting: horizontal arms only (left, right)

@@ -175,7 +175,6 @@ size_t carve_lane(void* base, const AdcDims& dm, int L1, int S, AdcWave* w) {
     t.vote_dirtyb = c.take<uint8_t>((size_t)S * N);
     t.vote_state = c.take<int>((size_t)S * N);
     t.vote_off = c.take<int>((size_t)S * (N + 1));
-    t.wta_key = c.take<unsigned long long>((size_t)S * N);
     t.rowcnt = c.take<int>((size_t)S * 2 * dm.H);
     t.so_bitrows = c.take<unsigned>((size_t)S * adc_so_bitrow_bytes(dm) / 4);
     t.so_rec = c.take<unsigned>((size_t)S * adc_so_rec_bytes(dm) / 4);
@@ -253,6 +252,22 @@ int upload_tables(adc_engine* e) {
             CK(cudaMemcpy(e->d_ray_off, off.data(), sizeof(short2) * off.size(), cudaMemcpyHostToDevice));
         }
     }
+    return ADC_OK;
+}
+
+bool poisoned(const adc_engine* e) { return (e->cfg.debug_flags & ADC_DBG_POISON) != 0; }
+int poison_byte(const adc_engine* e) { return (e->cfg.debug_flags >> 8) & 0xff; }
+
+// Fills lane ln's whole arena on its stream: every buffer carve_lane cuts, the unused slots of a partial wave and the
+// arm-sum over-read tail behind the volumes.  With ADC_DBG_POISON the fill is the test pattern, so that a kernel that
+// reads what its wave or call did not write shows in the outputs; otherwise zeros, which nothing relies on (the poison
+// tests run every entry point without them) but which keep a fresh engine's buffers deterministic for adc_debug_get and
+// adc_profile_kernel before its first run.  Then comes the state a kernel relies on from adc_create, restored after
+// every poison fill; each entry names the kernel.  There is none: every buffer a kernel reads is written earlier in the
+// same wave or call.
+int fill_arena(adc_engine* e, Lane& ln) {
+    const size_t bytes = carve_lane(nullptr, e->P.dm, e->P.L1, e->S, nullptr);
+    CK(cudaMemsetAsync(ln.arena, poisoned(e) ? poison_byte(e) : 0, bytes, ln.st));
     return ADC_OK;
 }
 
@@ -562,6 +577,10 @@ int run_batch(adc_engine* e, int n, const BatchIO& io, const MatchReq& q, cudaSt
         Lane& ln = e->lanes[wv % nl];
         const int first = wv * S, nS = std::min(S, n - first);
         const AdcWave& w = ln.w;   // where the images go in and the map comes out
+        if (poisoned(e)) {
+            int rcp = fill_arena(e, ln);
+            if (rcp) return rcp;
+        }
         // ---- inputs -> w.bgr  ([S][2][IMG])
         if (ingest) {
             const long long off = (long long)first * q.img->image_stride;
@@ -800,18 +819,21 @@ int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, 
 }
 
 // Makes the device staging of the host entries (e->vol_stage) at least `need` bytes: freed and re-allocated when it is
-// smaller, ADC_ERR_NOMEM if that fails.
+// smaller, ADC_ERR_NOMEM if that fails.  With ADC_DBG_POISON the whole staging is filled with the pattern on lane 0's
+// stream, which every caller (a one-pair host call) works on.
 int grow_stage(adc_engine* e, const char* fn, size_t need, const char* what) {
-    if (need <= e->vol_stage_bytes) return ADC_OK;
-    if (e->vol_stage) CK(cudaFree(e->vol_stage));
-    e->vol_stage = nullptr;
-    e->vol_stage_bytes = 0;
-    if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
-        cudaGetLastError();
+    if (need > e->vol_stage_bytes) {
+        if (e->vol_stage) CK(cudaFree(e->vol_stage));
         e->vol_stage = nullptr;
-        return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for %s", fn, need, what);
+        e->vol_stage_bytes = 0;
+        if (cudaMalloc(&e->vol_stage, need) != cudaSuccess) {
+            cudaGetLastError();
+            e->vol_stage = nullptr;
+            return fail(ADC_ERR_NOMEM, "%s: device staging of %zu bytes for %s", fn, need, what);
+        }
+        e->vol_stage_bytes = need;
     }
-    e->vol_stage_bytes = need;
+    if (poisoned(e) && e->vol_stage) CK(cudaMemsetAsync(e->vol_stage, poison_byte(e), e->vol_stage_bytes, e->lanes[0].st));
     return ADC_OK;
 }
 
@@ -925,6 +947,7 @@ int match_host(adc_engine* e, const char* fn, const MatchReq& q, const uint8_t* 
     }
     uint8_t* raw = !ingest ? nullptr : raw_in_volume ? reinterpret_cast<uint8_t*>(lane_volumes(e, ln.w, last).c0)
                                                      : reinterpret_cast<uint8_t*>(stage);
+    if (poisoned(e) && (rc = fill_arena(e, ln))) return rc;
     cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
     CostSrc src;
     if ((rc = upload_pair(e, ln, q, left, right, raw, last, ev ? ev[0] : nullptr, &src))) return rc;
@@ -1222,7 +1245,7 @@ int adc_create(int32_t width, int32_t height, const adc_option* opt, const adc_c
         if (!adc_so_tmaps_encode(e->P, S, ln.w.volA, ln.w.volB, ln.w.so_rec, &ln.so_tm))
             return bail(fail(ADC_ERR_CUDA, "adc_create: the scanline passes' tensor maps could not be encoded (cuTensorMapEncodeTiled)"));
         ln.w.so_tm = &ln.so_tm;
-        if (cudaMemsetAsync(ln.arena, 0, bytes, ln.st) != cudaSuccess) return bail(fail(ADC_ERR_CUDA, "memset failed"));
+        if ((rc = fill_arena(e, ln))) return bail(rc);
         if (cudaHostAlloc((void**)&ln.pin_in, (size_t)S * 2 * N * 3, cudaHostAllocDefault) != cudaSuccess ||
             cudaHostAlloc((void**)&ln.pin_out, (size_t)S * N * sizeof(float), cudaHostAllocDefault) != cudaSuccess) {
             cudaGetLastError();
@@ -1783,6 +1806,7 @@ int adc_render_disparity(adc_engine* e, const float* disp, uint8_t* gray8, uint8
     float* d_disp = ln.w.disp_t;
     unsigned* d_mm = reinterpret_cast<unsigned*>(ln.w.rowcnt);
     float* d_mm_out = reinterpret_cast<float*>(ln.w.rowcnt) + 2;
+    if (poisoned(e) && (rc = fill_arena(e, ln))) return rc;
     CK(cudaMemcpyAsync(d_disp, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
     if (adc_launch_render(e->P.dm, d_disp, d_mm, ln.w.flag, ln.w.bgr, d_mm_out, ln.st, &e->launches))
         return fail(ADC_ERR_CUDA, "adc_render_disparity: colour table upload failed");
@@ -1804,6 +1828,7 @@ int adc_disparity_cloud(adc_engine* e, const uint8_t* img_left, const float* dis
     const AdcWave w1 = wave_view(e, ln, 1);
     float* d_cloud = ln.w.volA;                       // 6 floats per pixel at most; a volume has Dp >= 4 ... use both volumes' span
     if ((size_t)e->P.dm.vol_stride * 2 < N * 6) return fail(ADC_ERR_UNSUPPORTED, "adc_disparity_cloud: disparity range too small for the scratch volume");
+    if (poisoned(e) && (rc = fill_arena(e, ln))) return rc;
     CK(cudaMemcpyAsync(ln.w.disp_t, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
     CK(cudaMemcpyAsync(ln.w.bgr, img_left, 3 * N, cudaMemcpyHostToDevice, ln.st));
     CK(cudaMemsetAsync(ln.w.counters, 0, ADC_CNT * sizeof(int), ln.st));

@@ -51,7 +51,13 @@ class _Config(ctypes.Structure):
 
 
 # adc_config.debug_flags (test hooks)
-DBG_NO_RAY_TABLE, DBG_VOTE_ENUM, DBG_VOTE_GLOBAL_STATE, DBG_UNFUSED_AGG = 1, 2, 4, 8
+DBG_NO_RAY_TABLE, DBG_VOTE_ENUM, DBG_VOTE_GLOBAL_STATE, DBG_UNFUSED_AGG, DBG_POISON = 1, 2, 4, 8, 16
+
+
+def poison_flags(byte: int) -> int:
+    """debug_flags that fill every lane arena with `byte` before each wave and call (ADC_DBG_POISON with
+    ADC_DBG_POISON_BYTE(byte))."""
+    return DBG_POISON | ((int(byte) & 0xff) << 8)
 
 # cost-input mode (adc_match_cost*): volume layouts, element types and the value domain's ceiling
 COST_HWD, COST_DHW = 0, 1

@@ -81,8 +81,22 @@ enum {
     ADC_DBG_NO_RAY_TABLE = 1,     /* interpolation evaluates lround(y + m*sin) in double per step instead of the verified integer table */
     ADC_DBG_VOTE_ENUM = 2,        /* region voting finds the affected histograms by enumeration instead of adjacency lists */
     ADC_DBG_VOTE_GLOBAL_STATE = 4,/* region voting keeps its per-slot state in global instead of shared memory */
-    ADC_DBG_UNFUSED_AGG = 8       /* aggregation as eight single passes instead of five (three of them fused double passes) */
+    ADC_DBG_UNFUSED_AGG = 8,      /* aggregation as eight single passes instead of five (three of them fused double passes) */
+    ADC_DBG_POISON = 16           /* every byte of a lane's device arena is set to the pattern ADC_DBG_POISON_BYTE gives, on
+                                     the lane's stream: at adc_create instead of zeros; at the start of every wave of a batch
+                                     call, after the lane has joined the caller's stream and before the wave's inputs
+                                     arrive; in the one-pair host calls (and adc_debug_run*) before the pair is uploaded;
+                                     in adc_render_disparity and adc_disparity_cloud before their uploads.  The device
+                                     staging of the one-pair host calls is filled too, whenever a call takes it.  So a
+                                     kernel that reads memory its wave or call did not write meets the pattern, not zeros or
+                                     a plausible earlier pair.  Not filled: what explicit calls set and later calls rely
+                                     on -- the cost and ray tables, the integer ray offsets, the tensor maps, the
+                                     rectification maps (adc_set_rectification), the right-view map adc_get_right_disparity
+                                     returns and the pinned host staging.  A test hook: the fills cost bandwidth */
 };
+/* The pattern byte of ADC_DBG_POISON (bits 8-15 of debug_flags): 0xFF makes floats NaN and integers -1, 0x7F floats
+ * 3.4e38 and integers large and positive, 0x01 every byte label a mismatch. */
+#define ADC_DBG_POISON_BYTE(b) (((b) & 0xff) << 8)
 
 /* stands in for: ADCensusOption::ADCensusOption() defaults (adcensus_types.h:67-74) */
 void adc_default_option(adc_option* opt);

@@ -1,5 +1,6 @@
-"""Test infrastructure of the per-pixel side maps (adc_match_outputs*): what the confidence maps must hold, and the
-outlier map in the form of the reference's mismatch / occlusion lists."""
+"""Test infrastructure of the per-pixel side maps (adc_match_outputs*): what the confidence maps must hold, the outlier
+map in the form of the reference's mismatch / occlusion lists, and the demo's 8-bit rendering of a map
+(adc_render_disparity)."""
 from __future__ import annotations
 
 import numpy as np
@@ -55,3 +56,17 @@ def outlier_lists(label: np.ndarray):
         ys, xs = np.nonzero(np.asarray(label) == want)
         out.append(np.ascontiguousarray(np.stack([xs, ys], 1).astype(np.int32).reshape(-1, 2)))
     return out
+
+
+def gray8(disp: np.ndarray, width: int):
+    """ShowDisparityMap / SaveDisparityMap (main.cpp:147-170, 180-201) in float32."""
+    d = np.abs(disp.astype(np.float32))
+    valid = ~np.isinf(d)                                   # disp != Invalid_Float
+    mn = np.float32(min(np.float32(width), d[valid].min())) if valid.any() else np.float32(width)
+    mx = np.float32(max(np.float32(-width), d[valid].max())) if valid.any() else np.float32(-width)
+    out = np.zeros(d.shape, np.uint8)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        v = (d - mn) / np.float32(mx - mn) * np.float32(255)
+    ok = valid & np.isfinite(v)
+    out[ok] = v[ok].astype(np.uint8)                       # static_cast<uchar>: truncation
+    return out, float(mn), float(mx)

@@ -3,12 +3,16 @@ for it (printed by tests/c/ca_plan_main.cpp and so_plan_main.cpp from the header
 template instantiations one run of it launches, and the run itself against the oracle."""
 from __future__ import annotations
 
+import os
+import re
 import subprocess
 from concurrent.futures import ThreadPoolExecutor
+from pathlib import Path
 
 import numpy as np
 import pytest
 
+import adc_testlib as T
 import engine_testlib as E  # puts tools/ on sys.path
 import maps_testlib as MT
 import make_golden_sweep as GS
@@ -25,6 +29,81 @@ class Case:
         self.Dp = (self.D + 3) // 4 * 4
         self.L1 = opt.cross_L1
         self.wave_pairs, self.lanes, self.n = wave_pairs, lanes, n
+
+
+# ---- cases ----------------------------------------------------------------------------------------------------------
+def sweep_case(D):
+    W, H, opt, seed = GS.sweep_case(D)
+    return Case(f"D{D}", W, H, opt, seed)
+
+
+def _opt(D, **kw):
+    return T.default_option(max_disparity=D, **kw)
+
+
+LONG_ARMS = dict(cross_L1=255, cross_L2=120, cross_t1=50, cross_t2=25)
+# name -> (case, what its plans must be).  Shapes found with the plan executables; test_plan_branch_cases checks them.
+PLAN_CASES = {
+    # fused cost + first horizontal pass (ca_plan): rows in 2 and 3 segments at L1 = 34, qc = 8, exact and not
+    "cost_rows_2seg": (Case("cost_rows_2seg", 501, 23, _opt(45), 61), dict(ca_nseg=2, ca_qc=8)),
+    "cost_rows_3seg": (Case("cost_rows_3seg", 861, 19, _opt(64), 62), dict(ca_nseg=3, ca_qc=8)),
+    # L1 = 130: 3 segments of 164 outputs, shorter than 2 L1, so a segment's halos span a whole neighbouring segment
+    "cost_rows_l1_130": (Case("cost_rows_l1_130", 486, 17, _opt(61, cross_L1=130, cross_L2=40, cross_t1=60, cross_t2=30), 63),
+                         dict(ca_nseg=3, ca_qc=8, ca_short=True)),
+    # D < 32: four quads per CTA, D not a multiple of 4, rows in 2 segments
+    "cost_rows_qc4": (Case("cost_rows_qc4", 825, 13, _opt(23), 64), dict(ca_nseg=2, ca_qc=4)),
+    # arms too long for the fused cost plan: the separate cost kernel, exact and padded D; at W = 701 the row does not
+    # fit k_arm_sum2t's plan either, so both axes take the LDG double pass with eight quads
+    "cost_volume_exact": (Case("cost_volume_exact", 509, 13, _opt(32, **LONG_ARMS), 65), dict(ca_ok=False)),
+    "cost_volume_padded_ldg": (Case("cost_volume_padded_ldg", 701, 13, _opt(37, **LONG_ARMS), 66),
+                               dict(ca_ok=False, tmaps=False)),
+    # k_arm_sum2t down columns cut into segments, one line per CTA, eight and four quads
+    "cols_seg_qc8": (Case("cols_seg_qc8", 21, 709, _opt(64), 67), dict(t1_nseg=3, t1_qc=8, t1_lpc=1)),
+    "cols_seg_qc4": (Case("cols_seg_qc4", 13, 809, _opt(23), 68), dict(t1_nseg=2, t1_qc=4, t1_lpc=1)),
+    # the LDG double pass on rows in segments: Q = 4 (generic QC) and Q = 3 (no TMA plan at all, Q < 4)
+    "ldg_rows_q4": (Case("ldg_rows_q4", 1001, 13, _opt(14), 69), dict(ldg0_nseg=2, ldg0_qc=0, t0_nseg=2)),
+    "ldg_rows_q3": (Case("ldg_rows_q3", 1001, 13, _opt(11), 70), dict(ldg0_nseg=2, ldg0_qc=0, tmaps=False)),
+    # scanline slots of T = 2 steps on the row passes, for 8, 16 and 32 lanes per line, K not FULL, an odd step count
+    "so_t2_lps8": (Case("so_t2_lps8", 33, 1057, _opt(61), 71, wave_pairs=8, lanes=1), dict(so_T0=2, lps=8)),
+    "so_t2_lps16": (Case("so_t2_lps16", 33, 659, _opt(93), 72, wave_pairs=8, lanes=1), dict(so_T0=2, lps=16)),
+    "so_t2_lps32": (Case("so_t2_lps32", 33, 329, _opt(200), 73, wave_pairs=8, lanes=1), dict(so_T0=2, lps=32)),
+}
+
+SWEEP_DS = list(range(1, 257))
+
+
+def all_cases():
+    return [sweep_case(D) for D in SWEEP_DS] + [c for c, _ in PLAN_CASES.values()]
+
+
+SYMBOLS = {
+    "k_scanline": re.compile(r"_Z10k_scanlineILi(\d+)ELi(\d+)ELb([01])EE"),
+    "k_cost_volume": re.compile(r"_Z13k_cost_volumeILb([01])EE"),
+    "k_cost_arm_sum_h": re.compile(r"_Z16k_cost_arm_sum_hILb([01])ELi(\d+)EE"),
+    "k_arm_sum2t": re.compile(r"_Z11k_arm_sum2tILb([01])ELi(\d+)EE"),
+    "k_arm_sum2": re.compile(r"_Z10k_arm_sum2ILb([01])ELi(\d+)EE"),
+    "k_vote_scan": re.compile(r"_Z11k_vote_scanILb([01])EE"),
+    "k_vote_push": re.compile(r"_Z11k_vote_pushILb([01])EE"),
+}
+
+
+def library_instantiations():
+    """{(template, args...)} of the seven templates, read from the built library's device symbols."""
+    from adcensus_b200.build import build_library
+    cuobjdump = Path(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")).parent / "cuobjdump"
+    if not cuobjdump.exists():
+        pytest.skip(f"cuobjdump not found at {cuobjdump}")
+    r = subprocess.run([str(cuobjdump), "-symbols", str(build_library())], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-2000:]
+    found = set()
+    for name, rx in SYMBOLS.items():
+        for m in rx.finditer(r.stdout):
+            args = tuple(int(g) for g in m.groups())
+            if name == "k_scanline":
+                found.add((name, args[0], args[1], bool(args[2])))
+            else:
+                found.add((name, bool(args[0]), *args[1:]))
+    return found
 
 
 # ---- plans ----------------------------------------------------------------------------------------------------------
@@ -110,10 +189,10 @@ def reached(c, plans):
 
 
 # ---- the GPU run ----------------------------------------------------------------------------------------------------
-def check_case(c):
+def check_case(c, debug_flags=0):
     """One match_outputs_batch_device call over the case's pairs, exporting the three volumes (f32, [H][W][D]), the
-    WTA maps, the outlier map and the final map, each pair compared bit for bit with its own oracle run; returns every
-    output of the call on the host."""
+    WTA maps, the outlier map and the final map, each pair compared bit for bit with its own oracle run, on an engine
+    created with `debug_flags`; returns every output of the call on the host."""
     torch, dev = E.cuda()
     # the oracle runs overlap in threads (ctypes releases the GIL during the call) while the GPU runs the batch
     pairs = GS.sweep_pairs(c.W, c.H, c.D, c.seed)[:c.n]
@@ -121,7 +200,7 @@ def check_case(c):
         futs = [ex.submit(E.oracle_outputs, c.W, c.H, c.opt, l, r) for l, r in pairs]
         d_l = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev)
         d_r = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev)
-        eng = E.engine(c.W, c.H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes)
+        eng = E.engine(c.W, c.H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes, debug_flags=debug_flags)
         assert (eng.wave_pairs, eng.lanes) == (c.wave_pairs, c.lanes), (eng.wave_pairs, eng.lanes)
         got = E.batch_outputs(eng, eng.match_outputs_batch_device, len(pairs), d_l.data_ptr(), d_r.data_ptr(),
                               3 * c.W * c.H, volumes=[(s, "hwd", "f32") for s in ("cost", "aggr", "opt")],
@@ -135,6 +214,7 @@ def check_case(c):
         E.same(f"{tag} SO4/VOL_AGGR", got["opt"][i], w["opt"])
         E.same(f"{tag} WTA/DISP_L", got["wta_left"][i], w["wta_left"])
         E.same(f"{tag} WTA/DISP_R", got["wta_right"][i], w["wta_right"])
+        assert set(np.unique(got["outliers"][i])) <= {0, 1, 2}, f"{tag} OUTLIER: labels other than 0, 1, 2"
         mis, occ = MT.outlier_lists(got["outliers"][i])
         E.same(f"{tag} OUTLIER/MISMATCHES", mis, w["mismatches"].reshape(-1, 2))
         E.same(f"{tag} OUTLIER/OCCLUSIONS", occ, w["occlusions"].reshape(-1, 2))
