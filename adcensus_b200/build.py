@@ -14,7 +14,7 @@ def _stale() -> bool:
     if not LIB.exists():
         return True
     t = LIB.stat().st_mtime
-    srcs = list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.cpp")) + \
+    srcs = list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + list(CSRC.glob("*.h")) + list(CSRC.glob("*.cpp")) + \
         list((PKG.parent / "include").glob("*.h")) + [CSRC / "Makefile"]
     return any(s.stat().st_mtime > t for s in srcs)
 

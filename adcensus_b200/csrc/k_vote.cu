@@ -39,6 +39,7 @@
 // L1 <= 255.  For L1 > 127 the uint16 support counts the forward lists are reserved from may wrap, so those pairs
 // always enumerate.
 #include "adc_common.cuh"
+#include "vote_plan.h"
 #include <type_traits>
 
 #define VP_THREADS 1024
@@ -95,18 +96,25 @@ k_vote_slots(AdcDims dm, const int* __restrict__ vlist, int* __restrict__ counte
              int* __restrict__ pslotT, const uint16_t* __restrict__ sup) {
     const int pair = blockIdx.y;
     const int n0 = counters[pair * ADC_CNT + 10], n1 = counters[pair * ADC_CNT + 11];
-    unsigned room = 0;   // sum of the region sizes = upper bound of the forward lists (saturating)
+    unsigned room = 0;   // sum of the region sizes = size of the forward lists (saturating, vote_plan.h)
     for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < n0 + n1; s += gridDim.x * blockDim.x) {
         const int p = s < n0 ? vlist[((size_t)pair * 2 + 0) * dm.N + s] : vlist[((size_t)pair * 2 + 1) * dm.N + (s - n0)];
         const int y = p / dm.W, x = p - y * dm.W;
         vstate[(size_t)pair * dm.N + p] = -(s + 2);
         pslotT[(size_t)pair * dm.N + (size_t)x * dm.H + y] = s;
-        room += sup[(size_t)pair * dm.N + p];
+        room = vote_room_add(room, sup[(size_t)pair * dm.N + p]);
     }
-    room = __reduce_add_sync(0xffffffffu, min(room, 0x00ffffffu));
-    if ((threadIdx.x & 31) == 0 && room) {
-        const unsigned old = atomicAdd(reinterpret_cast<unsigned*>(counters + pair * ADC_CNT + 15), min(room, 0x1fffffffu));
-        if (old > 0x3fffffffu) atomicExch(reinterpret_cast<unsigned*>(counters + pair * ADC_CNT + 15), 0x7fffffffu);   // stays "too big"
+    __shared__ unsigned s_part[256 / 32];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) room = vote_room_add(room, __shfl_xor_sync(0xffffffffu, room, o));
+    if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = room;
+    __syncthreads();
+    if (threadIdx.x == 0) {   // the CTA's part, merged as vote_room_merge does
+        unsigned part = 0;
+        for (int i = 0; i < 256 / 32; i++) part = vote_room_add(part, s_part[i]);
+        unsigned* c = reinterpret_cast<unsigned*>(counters + pair * ADC_CNT + 15);
+        if (part > VOTE_ROOM_PART_MAX) atomicOr(c, VOTE_ROOM_OVER);
+        else if (part) atomicAdd(c, part);
     }
 }
 
@@ -176,7 +184,6 @@ __device__ __forceinline__ void vote_scan_region(int p, int W, const uchar4* __r
 // of slot s, written compacted at a base taken from the pair's cursor (counters[9]).  A slot reserves as many entries as
 // its region has pixels and marks the ones it does not use (-1): the lists of a pair are ONE dense array of `room`
 // entries that k_vote_push streams through.
-__host__ __device__ inline long long vote_fwd_offset(long long ns, int HW) { return (ns * HW + 1) & ~1ll; }   // in 32-bit words, 8-byte aligned
 template <bool WIDE>
 __global__ void __launch_bounds__(VI_WARPS * 32)
 k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restrict__ alr_all, const int* __restrict__ vstate_all,
@@ -186,11 +193,11 @@ k_vote_scan(AdcParams P, const uchar4* __restrict__ arms, const uchar2* __restri
     const AdcDims& dm = P.dm;
     const int pair = blockIdx.y;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int W = dm.W, D = dm.D, HW = WIDE ? D : (D + 1) >> 1;
+    const int W = dm.W, D = dm.D, HW = vote_hist_words(D, WIDE);
     int* cnt = counters + pair * ADC_CNT;
     const int n0 = cnt[10], n1 = cnt[11], ns = n0 + n1;
     const long long room = (unsigned)cnt[15];
-    const bool use_fwd = !force_enum && vote_fwd_offset(ns, HW) + 2 * room <= hist_stride;
+    const bool use_fwd = !force_enum && vote_use_fwd(ns, HW, room, hist_stride);
     const uchar4* A = arms + (size_t)pair * dm.N;
     const uchar2* ALR = alr_all + (size_t)pair * dm.N;
     const int* VS = vstate_all + (size_t)pair * dm.N;
@@ -253,11 +260,11 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     constexpr int VB = WIDE ? 16 : 8;
     constexpr int NHW = WIDE ? 8 : 4;           // histogram words per lane, at most
     extern __shared__ __align__(16) unsigned char vp_smem[];
-    __shared__ int s_nwork, s_nchg, s_warp[32], s_base, s_fits;
+    __shared__ int s_nwork, s_nchg, s_warp[32], s_base;
     const AdcDims& dm = P.dm;
     const int pair = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-    const int W = dm.W, H = dm.H, D = dm.D, HW = WIDE ? D : (D + 1) >> 1;
+    const int W = dm.W, H = dm.H, D = dm.D, HW = vote_hist_words(D, WIDE);
     const int L1 = max(P.L1, 0), R = 2 * L1 + 1;
     const uchar2* ALR = alr_all + (size_t)pair * dm.N;
     const uchar2* ATB = atbT_all + (size_t)pair * dm.N;
@@ -297,7 +304,7 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     // ---- adjacency lists (CSR by target) from the forward lists of k_vote_scan: count, prefix, fill
     const long long room = (unsigned)__ldcg(cnt + 15);
     const long long fwd_off = vote_fwd_offset(ns, HW);
-    const bool use_fwd = !force_enum && fwd_off + 2 * room <= hist_stride;
+    const bool use_fwd = !force_enum && vote_use_fwd(ns, HW, room, hist_stride);
     const int2* fwd = reinterpret_cast<const int2*>(hist + fwd_off);
     // adjacency entry = the slot whose histogram counts the target.  (Whether that slot's pixel comes after the target in
     // raster order -- all a push needs to know about it -- is a comparison of slot numbers: the lists are in raster order.)
@@ -307,7 +314,7 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     // Both passes stream through the pair's forward entries, eight independent 8-byte loads per thread in flight (the
     // first version walked list by list, two entries per lane in flight, and spent 1.9 of the kernel's 3.6 ms here).
     auto for_each_edge = [&](auto&& f) {
-        const int n = (int)room;                       // (< 2^30: use_fwd)
+        const int n = (int)room;                       // (<= VOTE_ROOM_MAX: use_fwd)
         for (int i0 = tid; i0 < n; i0 += 8 * VP_THREADS) {
             int2 e[8];
 #pragma unroll
@@ -320,7 +327,7 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
     if (use_fwd) for_each_edge([&](int t, int) { atomicAdd(&cur[t + 1], 1); });   // length of t's list, kept at index t + 1
     __syncthreads();
     // ---- inclusive prefix sum over cur[0..ns]: cur[t] = start of t's list, cur[ns] = number of entries
-    if (tid == 0) { s_base = 0; s_fits = 1; }
+    if (tid == 0) s_base = 0;
     __syncthreads();
     for (int i0 = 0; i0 <= ns; i0 += VP_THREADS) {
         const int i = i0 + tid;
@@ -343,13 +350,12 @@ k_vote_push(AdcParams P, const uchar2* __restrict__ alr_all,
         __syncthreads();
         if (tid == VP_THREADS - 1) {
             const long long nb = (long long)base + s_warp[VP_WARPS - 1] + inc;
-            if (nb > 0x3fffffff) s_fits = 0;
-            s_base = (int)min(nb, (long long)0x3fffffff);
+            s_base = (int)min(nb, (long long)VOTE_ROOM_SAT);   // (nb <= room when use_fwd)
         }
         __syncthreads();
     }
     const int n_adj = s_base;
-    const bool use_adj = use_fwd && s_fits && fwd_off + 2 * room + n_adj <= hist_stride;
+    const bool use_adj = vote_use_adj(use_fwd, ns, HW, room, n_adj, hist_stride);
     // ---- fill (afterwards cur[t] = end of t's list = start of t + 1's)
     if (use_adj) for_each_edge([&](int t, int s) { adj[atomicAdd(&cur[t], 1)] = s; });
     __syncthreads();
@@ -650,11 +656,11 @@ void adc_launch_voting(const AdcParams& P, const AdcWave& w, cudaStream_t st, un
     cudaMemsetAsync(w.vote_pslotT, 0xff, (size_t)w.S * dm.N * sizeof(int), st);
     dim3 tgrid((dm.W + 31) / 32, (dm.H + 31) / 32, w.S);
     k_vote_transpose<<<tgrid, 256, 0, st>>>(dm, w.arms, w.vote_atbT);
-    dim3 sgrid(64, w.S);
+    dim3 sgrid(VOTE_ROOM_CTAS, w.S);
     k_vote_slots<<<sgrid, 256, 0, st>>>(dm, w.vlist, w.counters, w.vote_state, w.vote_pslotT, w.sup_h);
     // ADC_DBG_VOTE_ENUM forces the enumeration fallback (tests); L1 > 127 takes it always (the support counts may wrap)
     const int force_enum = (P.dbg & 2) || L1 > 127 ? 1 : 0;
-    if (dm.D > 254 || L1 > 127) launch_scan_push<true>(P, w, L1, force_enum, st);
+    if (vote_wide(dm.D, L1)) launch_scan_push<true>(P, w, L1, force_enum, st);
     else                        launch_scan_push<false>(P, w, L1, force_enum, st);
     *launches += 5;
     adc_launch_build_lists(P, w, st, launches);

@@ -534,6 +534,22 @@ int orc_begin(orc_ctx* c, const uint8_t* left, const uint8_t* right) {
     return 1;
 }
 
+/* Refinement only: the staged runner from OUTLIER on, with the given WTA maps and the arms of the left image.  It never
+ * touches the cost volumes (calloc leaves them unmapped), so it runs at sizes whose volumes would not fit in host
+ * memory.  The discontinuity adjustment reads the aggregated volume, so a context with it enabled is refused. */
+int orc_begin_refine(orc_ctx* c, const uint8_t* left, const uint8_t* right, const float* disp_left, const float* disp_right) {
+    if (!c || !left || !right || !disp_left || !disp_right || c->opt.do_discontinuity_adjustment) return 0;
+    const size_t n = (size_t)c->w * c->h;
+    c->left = left; c->right = right;
+    memcpy(c->disp_l, disp_left, n * sizeof(float));
+    memcpy(c->disp_r, disp_right, n * sizeof(float));
+    build_arms(c);
+    support_counts(c);
+    c->n_mism = c->n_occl = 0;
+    c->next_stage = ADC_STAGE_OUTLIER;
+    return 1;
+}
+
 int orc_step(orc_ctx* c) {
     const int st = c->next_stage;
     const size_t nd = (size_t)c->w * c->h * c->D;

@@ -43,6 +43,9 @@ int orc_match(orc_ctx* c, const uint8_t* left, const uint8_t* right, float* disp
 /* staged runner, mirrors oracle/ref_harness.cpp */
 int orc_begin(orc_ctx* c, const uint8_t* left, const uint8_t* right);
 int orc_step(orc_ctx* c);
+/* the staged runner from OUTLIER on, from given WTA maps (float [H][W] each); the arms come from the left image and the
+ * cost volumes are never touched.  Returns 0 with do_discontinuity_adjustment set (that stage reads the volume). */
+int orc_begin_refine(orc_ctx* c, const uint8_t* left, const uint8_t* right, const float* disp_left, const float* disp_right);
 size_t orc_tap(orc_ctx* c, int tap, void* dst, size_t cap);
 double orc_time_match(orc_ctx* c, const uint8_t* left, const uint8_t* right, float* disp, int iters);
 

@@ -179,6 +179,19 @@ class Oracle(_Checker):
         build_oracle()
         super().__init__(ORACLE_DIR / "_build" / "libadc_oracle.so", "orc", width, height, opt or default_option())
 
+    def begin_refine(self, left: np.ndarray, right: np.ndarray, disp_left: np.ndarray, disp_right: np.ndarray):
+        """Start the staged runner at OUTLIER from the given WTA maps (orc_begin_refine): the arms come from the left
+        image, the cost volumes are never touched."""
+        left = np.ascontiguousarray(left, np.uint8)
+        right = np.ascontiguousarray(right, np.uint8)
+        dl = np.ascontiguousarray(disp_left, np.float32)
+        dr = np.ascontiguousarray(disp_right, np.float32)
+        assert dl.size == dr.size == self.w * self.h
+        self._keep = (left, right)
+        f = self._f("begin_refine")
+        f.argtypes = [ctypes.c_void_p] * 5
+        assert f(self.ctx, left.ctypes.data, right.ctypes.data, dl.ctypes.data, dr.ctypes.data) == 1
+
 
 class Reference(_Checker):
     """The unmodified reference (oracle/_ref), available where it was built."""
