@@ -18,6 +18,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "img_format.h"
+
 #define ADC_INVALID_F (__int_as_float(0x7f800000))  // +inf  (adcensus_types.h:33)
 #define ADC_LARGE_F 99999.0f                         // adcensus_types.h:35
 #define ADC_CNT 16                                   // ints of per-pair counters
@@ -147,20 +149,10 @@ size_t adc_cost_elem_bytes(int dtype);
 void adc_launch_cost_export(const AdcParams& P, const AdcWave& w, const float* vol, void* dst, int layout, int dtype,
                             cudaStream_t st, unsigned long long* launches);
 // image ingestion (k_image.cu): S pairs of views at left / right (pair i at byte i*image_stride, format ADC_IMG_*,
-// pitches resolved: no zero defaults left) -> bgr as packed BGR [S][2][N*3] (a wave's w.bgr, or a caller's views);
-// S <= 65535 (the grid's z)
-struct AdcImageGeom {
-    int format;
-    long long row_pitch, plane_pitch, image_stride;
-};
+// pitches resolved: no zero defaults left; the formats, their geometry and adc_image_tight are in img_format.h) ->
+// bgr as packed BGR [S][2][N*3] (a wave's w.bgr, or a caller's views); S <= 65535 (the grid's z)
 void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                              uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
-// The tight layout of a w x h view in `format`: row pitch, plane pitch (ADC_IMG_RGB_PLANAR: from one channel plane to
-// the next; NV12 / NV21: from the luma plane to the chroma plane; else 0) and footprint (in image_stride).
-AdcImageGeom adc_image_tight(int format, long long w, long long h);
-// The bytes of a w x h view the ingestion kernels read (the tight footprint without the padding byte of odd-width
-// 4:2:0 luma rows).
-long long adc_image_read_bytes(int format, long long w, long long h);
 // rectified ingestion (k_rectify.cu).  The engine's internal form of a view's remap table: one uint2 per output pixel,
 // .x = (u16)x0 | (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
 struct AdcRectGeom {

@@ -744,26 +744,21 @@ MatchReq output_req(const void* cost, int cost_layout, int cost_dtype, const flo
 // The rules of an image descriptor that need no image size (adc_match_images*, checked before the engine).
 int check_image_desc(const char* fn, const adc_image_desc* img) {
     if (!img) return ADC_OK;
-    const bool known = (img->format >= ADC_IMG_BGR && img->format <= ADC_IMG_RGB_PLANAR) ||
-                       (img->format >= ADC_IMG_BAYER_RGGB && img->format <= ADC_IMG_BAYER_GBRG) ||
-                       (img->format >= ADC_IMG_NV12 && img->format <= ADC_IMG_YVYU) ||
-                       (img->format >= ADC_IMG_MONO10 && img->format <= ADC_IMG_BAYER_GB12P);
-    if (!known) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
+    if (img_family(img->format) == IMG_UNKNOWN) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
     if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
     if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
     if (img->plane_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is negative", fn, (long long)img->plane_pitch);
     if (img->image_stride < 0) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld is negative", fn, (long long)img->image_stride);
-    const bool planes = img->format == ADC_IMG_RGB_PLANAR || img->format == ADC_IMG_NV12 || img->format == ADC_IMG_NV21;
-    if (!planes && img->plane_pitch != 0)
+    if (img_planes(img->format) == 1 && img->plane_pitch != 0)
         return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format other than ADC_IMG_RGB_PLANAR, ADC_IMG_NV12 "
                     "and ADC_IMG_NV21", fn);
     return ADC_OK;
 }
 
-// The rule the device entries add for the formats with one sample per 16-bit word (ADC_IMG_MONO10 ... _BAYER_GB16),
-// whose words the kernels load whole: both bases, the row pitch and the image stride are even.  Needs no image size.
+// The rule the device entries add for the formats with one sample per 16-bit word (img_words), whose words the kernels
+// load whole: both bases, the row pitch and the image stride are even.  Needs no image size.
 int check_image_align(const char* fn, const adc_image_desc* img, const void* left, const void* right) {
-    if (!img || img->format < ADC_IMG_MONO10 || img->format >= ADC_IMG_MONO10P) return ADC_OK;
+    if (!img || !img_words(img->format)) return ADC_OK;
     if ((uintptr_t)left % 2) return fail(ADC_ERR_ARG, "%s: d_left must be 2-byte aligned for a 16-bit format", fn);
     if ((uintptr_t)right % 2) return fail(ADC_ERR_ARG, "%s: d_right must be 2-byte aligned for a 16-bit format", fn);
     if (img->row_pitch % 2) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld must be even for a 16-bit format", fn, (long long)img->row_pitch);
@@ -776,27 +771,21 @@ int check_image_align(const char* fn, const adc_image_desc* img, const void* lef
 // replaced.
 int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, int n, AdcImageGeom* g) {
     const adc_image_desc d = img ? *img : adc_image_desc{};
-    const long long H = h, min_row = adc_image_tight(d.format, w, h).row_pitch;
-    const bool yuv420 = d.format == ADC_IMG_NV12 || d.format == ADC_IMG_NV21;
-    const char* min_row_rule = yuv420 ? "2 * ceil(W / 2)" : d.format < ADC_IMG_YUYV ? "W * bytes per pixel"
-                               : d.format <= ADC_IMG_YVYU ? "4 * ceil(W / 2)" : d.format < ADC_IMG_MONO10P ? "2 * W"
-                               : d.format < ADC_IMG_MONO12P ? "ceil(10 * W / 8)" : "ceil(12 * W / 8)";
+    const long long H = h, min_row = img_row_pitch(d.format, w);
     g->format = d.format;
     g->row_pitch = d.row_pitch ? (long long)d.row_pitch : min_row;
     if (g->row_pitch < min_row)
-        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is less than %s (%lld)", fn, g->row_pitch, min_row_rule, min_row);
+        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is less than %s (%lld)", fn, g->row_pitch, img_row_rule(d.format),
+                    min_row);
     long long foot = 0;
     if (__builtin_mul_overflow(H, g->row_pitch, &foot)) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is too large", fn, g->row_pitch);
     g->plane_pitch = 0;
-    if (d.format == ADC_IMG_RGB_PLANAR || yuv420) {
+    if (img_planes(d.format) > 1) {
         g->plane_pitch = d.plane_pitch ? (long long)d.plane_pitch : foot;
         if (g->plane_pitch < foot)
             return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is less than H * row_pitch (%lld)", fn, g->plane_pitch, foot);
-        long long chroma = 0;   // NV12 / NV21: ceil(H/2) chroma rows after the plane pitch
-        const bool over = yuv420 ? __builtin_mul_overflow((H + 1) / 2, g->row_pitch, &chroma) ||
-                                       __builtin_add_overflow(g->plane_pitch, chroma, &foot)
-                                 : __builtin_mul_overflow(3ll, g->plane_pitch, &foot);
-        if (over) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is too large", fn, g->plane_pitch);
+        if (!img_footprint(d.format, H, g->row_pitch, g->plane_pitch, &foot))
+            return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is too large", fn, g->plane_pitch);
     }
     g->image_stride = d.image_stride ? (long long)d.image_stride : foot;
     if (g->image_stride < foot)
@@ -864,14 +853,12 @@ int ingest_host_pair(adc_engine* e, const AdcImageGeom& g, const AdcRectGeom* re
     const size_t sh = rect ? rect->src_h : e->H;
     const AdcImageGeom tight = adc_image_tight(g.format, rect ? rect->src_w : e->W, sh);
     const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
-    // one block of tight rows per plane: the three planes of a planar image; the H luma rows and ceil(H/2) chroma
-    // rows of NV12 / NV21; the H rows of every other format
-    const bool yuv420 = g.format == ADC_IMG_NV12 || g.format == ADC_IMG_NV21;
-    const int planes = g.format == ADC_IMG_RGB_PLANAR ? 3 : yuv420 ? 2 : 1;
+    // one block of tight rows per plane
     for (int v = 0; v < 2; v++)
-        for (int c = 0; c < planes; c++)
+        for (int c = 0; c < img_planes(g.format); c++)
             CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
-                                 (size_t)g.row_pitch, tp, yuv420 && c ? (sh + 1) / 2 : sh, cudaMemcpyHostToDevice, st));
+                                 (size_t)g.row_pitch, tp, (size_t)img_plane_rows(g.format, c, sh), cudaMemcpyHostToDevice,
+                                 st));
     if (rect)
         adc_launch_rectify_ingest(e->P.dm, 1, raw, raw + foot, tight, *rect, bgr, st, &e->launches);
     else

@@ -1,7 +1,8 @@
 // k_image.cuh -- the pieces the two image ingestion kernels share (k_image.cu: images in any format / pitch,
-// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the Bayer demosaic, the YUV
-// conversion, the 10- / 12- / 16-bit sample readers with their depth reduction, and the store scheme that writes one
-// view's packed BGR.
+// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the one demosaic reader of
+// the 8-bit and high-bit-depth mosaics, the YUV conversion, the 10- / 12- / 16-bit sample readers with their depth
+// reduction, the store scheme that writes one view's packed BGR, and the kernels' launchers.  The formats and their
+// constants come from img_format.h.
 //
 // The output of one view is a contiguous run of 3*N bytes.  A thread takes four consecutive pixels of it at a time:
 // 12 bytes, stored as three 32-bit words.  The view's run starts at an arbitrary byte phase (3*N*(2*pair + view) mod
@@ -53,16 +54,6 @@ template <> struct ImgIn<ADC_IMG_RGB_PLANAR> {
     }
 };
 
-// Bayer mosaics (ADC_IMG_BAYER_*): the demosaiced pixel (x, y) of a w x h mosaic at src as B | G << 8 | R << 16,
-// equal to cv::cvtColor(mosaic, COLOR_Bayer*2BGR) (the rule is in include/adcensus_b200.h).  Frames narrower or lower
-// than 3 pixels are all zero.  The position is clamped to [1, w - 2] x [1, h - 2] first, which is the border rule and
-// also keeps all nine loads of the 3x3 neighbourhood inside the frame, so none of them needs a predicate.  The colour of
-// a site comes from the parities of x and y against the R site of the pattern (bit 0: its column, bit 1: its row).
-__host__ __device__ constexpr bool is_bayer(int F) { return F >= ADC_IMG_BAYER_RGGB && F <= ADC_IMG_BAYER_GBRG; }
-__host__ __device__ constexpr int bayer_r_site(int F) {
-    return F == ADC_IMG_BAYER_RGGB ? 0 : F == ADC_IMG_BAYER_GRBG ? 1 : F == ADC_IMG_BAYER_GBRG ? 2 : 3;
-}
-
 // round_half_even(v / 2^S) saturated to 8 bits, the depth reduction of the high-bit-depth formats (S = depth - 8):
 // cv::Mat::convertTo(CV_8U, 1.0 / (1 << S)).  S = 0: 8-bit samples as they are.
 template <int S>
@@ -71,14 +62,15 @@ static __device__ __forceinline__ int to8(int v) {
     else return min(255, (v + (1 << (S - 1)) - 1 + (v >> S & 1)) >> S);
 }
 
-// The interior rule at (x, y) from the raw value c there and its eight neighbours, computed at the samples' own depth
-// (8 + S bits) and then reduced to 8 bits.
-template <int F, int S = 0>
+// The demosaic rule of Bayer pattern P (an ADC_IMG_BAYER_* code) at interior site (x, y) from the raw value c there and
+// its eight neighbours, computed at the samples' own depth (8 + S bits) and then reduced to 8 bits.  The colour of a
+// site comes from the parities of x and y against the pattern's R site.
+template <int P, int S>
 static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n, int s, int wv, int e, int nw, int ne,
                                                       int sw, int se) {
     const int cross = (n + s + wv + e + 2) >> 2, diag = (nw + ne + sw + se + 2) >> 2;
     const int hor = (wv + e + 1) >> 1, ver = (n + s + 1) >> 1;
-    const int dx = (x ^ bayer_r_site(F)) & 1, dy = (y ^ bayer_r_site(F) >> 1) & 1;
+    const int dx = (x ^ img_r_site(P)) & 1, dy = (y ^ img_r_site(P) >> 1) & 1;
     int r, g, b;
     if (dx == dy) {   // an R (dy = 0) or B (dy = 1) site
         g = cross;
@@ -92,24 +84,9 @@ static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n
     return (unsigned)to8<S>(b) | (unsigned)to8<S>(g) << 8 | (unsigned)to8<S>(r) << 16;
 }
 
-template <int F>
-static __device__ __forceinline__ unsigned bayer_px(const uint8_t* src, long long row_pitch, int w, int h, int x, int y) {
-    if (w < 3 || h < 3) return 0u;
-    x = min(max(x, 1), w - 2);
-    y = min(max(y, 1), h - 2);
-    const uint8_t* m = src + (long long)y * row_pitch + x;
-    const uint8_t* u = m - row_pitch;
-    const uint8_t* d = m + row_pitch;
-    return bayer_rule<F>(x, y, __ldg(m), __ldg(u), __ldg(d), __ldg(m - 1), __ldg(m + 1), __ldg(u - 1), __ldg(u + 1),
-                         __ldg(d - 1), __ldg(d + 1));
-}
-
 // YUV frames (ADC_IMG_NV12 ... ADC_IMG_YVYU): pixel (x, y) of the frame at src as B | G << 8 | R << 16, equal to
 // cv::cvtColor(frame, COLOR_YUV2BGR_*) (BT.601 limited range, the rule and geometry are in include/adcensus_b200.h).
 // One luma and two chroma byte loads; neighbouring pixels share their chroma, so L1 serves that reuse.
-__host__ __device__ constexpr bool is_yuv(int F) { return F >= ADC_IMG_NV12 && F <= ADC_IMG_YVYU; }
-__host__ __device__ constexpr bool is_yuv420(int F) { return F == ADC_IMG_NV12 || F == ADC_IMG_NV21; }
-
 static __device__ __forceinline__ unsigned yuv_rule(int Y, int U, int V) {
     const int y = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
     const int r = min(max((y + 1673527 * v) >> 20, 0), 255);
@@ -121,7 +98,7 @@ static __device__ __forceinline__ unsigned yuv_rule(int Y, int U, int V) {
 template <int F>
 static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int x,
                                                   int y) {
-    if constexpr (is_yuv420(F)) {
+    if constexpr (img_yuv420(F)) {
         const uint8_t* c = src + plane_pitch + (long long)(y >> 1) * row_pitch + (x & ~1);
         const int c0 = __ldg(c), c1 = __ldg(c + 1);
         return yuv_rule(__ldg(src + (long long)y * row_pitch + x), F == ADC_IMG_NV12 ? c0 : c1,
@@ -136,66 +113,59 @@ static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long 
     }
 }
 
-// High-bit-depth mono and Bayer frames (ADC_IMG_MONO10 ... ADC_IMG_BAYER_GB12P; rules in include/adcensus_b200.h).
-// The code is ADC_IMG_MONO10 + 5 * container + colour: container 0 / 1 / 2 = one sample per little-endian 16-bit word
-// with 10 / 12 / 16 significant bits, 3 / 4 = the PFNC 10p / 12p bit streams; colour 0 = mono, 1..4 = the Bayer
-// patterns in the order of ADC_IMG_BAYER_RGGB ... _GBRG, whose code rd_pattern gives for bayer_rule.
-__host__ __device__ constexpr bool is_rawdepth(int F) { return F >= ADC_IMG_MONO10 && F <= ADC_IMG_BAYER_GB12P; }
-__host__ __device__ constexpr int rd_container(int F) { return (F - ADC_IMG_MONO10) / 5; }
-__host__ __device__ constexpr bool rd_mono(int F) { return (F - ADC_IMG_MONO10) % 5 == 0; }
-__host__ __device__ constexpr int rd_pattern(int F) { return ADC_IMG_BAYER_RGGB + (F - ADC_IMG_MONO10) % 5 - 1; }
-__host__ __device__ constexpr int rd_bits(int F) { return rd_container(F) == 2 ? 16 : rd_container(F) % 3 == 0 ? 10 : 12; }
-
-// Sample x of the row at `row`.  A 16-bit container is read as the whole word (bits above the nominal depth are kept
-// and saturate in to8); the words are 2-byte aligned (the device entries require it, the host entries stage
-// tightly).  A packed row is a little-endian bit stream from its first byte: the field of sample x starts at bit x * b
-// and, b being 10 or 12, always spans exactly two bytes, the second of which is for x = W - 1 the row's last byte.
+// High-bit-depth frames (ADC_IMG_MONO10 ... ADC_IMG_BAYER_GB12P; rules in include/adcensus_b200.h, container and bits
+// in img_format.h): sample x of the row at `row`.  A 16-bit container is read as the whole word (bits above the nominal
+// depth are kept and saturate in to8); the words are 2-byte aligned (the device entries require it, the host entries
+// stage tightly).  A packed row is a little-endian bit stream from its first byte: the field of sample x starts at bit
+// x * b and, b being 10 or 12, always spans exactly two bytes, the second of which is for x = W - 1 the row's last byte.
 template <int F>
 static __device__ __forceinline__ int rd_sample(const uint8_t* row, int x) {
-    if constexpr (rd_container(F) <= 2) {
+    if constexpr (img_words(F)) {
         return __ldg(reinterpret_cast<const unsigned short*>(row) + x);
     } else {
-        constexpr int b = rd_bits(F);
+        constexpr int b = img_bits(F);
         const int o = x * b;
         const uint8_t* p = row + (o >> 3);
         return ((__ldg(p) | (int)__ldg(p + 1) << 8) >> (o & 7)) & ((1 << b) - 1);
     }
 }
 
-// The Bayer rule at full depth on nine samples, then the depth reduction of its three results.
+// Sample x + dx of a mosaic row: a byte for an 8-bit Bayer mosaic, a full-depth sample for a high-bit-depth one.  The
+// neighbour offset dx is a constant, which an 8-bit load takes as its immediate offset.
 template <int F>
-static __device__ __forceinline__ unsigned rd_bayer_rule(int x, int y, int c, int n, int s, int wv, int e, int nw, int ne,
-                                                         int sw, int se) {
-    return bayer_rule<rd_pattern(F), rd_bits(F) - 8>(x, y, c, n, s, wv, e, nw, ne, sw, se);
+static __device__ __forceinline__ int mosaic_sample(const uint8_t* row, int x, int dx) {
+    if constexpr (img_family(F) == IMG_BAYER) return __ldg(row + x + dx);
+    else return rd_sample<F>(row, x + dx);
 }
 
-// Pixel (x, y) of the w x h frame at src: a mono sample reduced and repeated, or the demosaic of bayer_px on the full
-// depth samples (same clamp, same all-zero rule below 3 x 3).
+// Mosaics (ADC_IMG_BAYER_* and the high-bit-depth Bayer formats): the demosaiced pixel (x, y) of a w x h mosaic at src
+// as B | G << 8 | R << 16, equal to cv::cvtColor(mosaic, COLOR_Bayer*2BGR) (the rule is in include/adcensus_b200.h) on
+// the full-depth samples, then reduced to 8 bits.  Frames narrower or lower than 3 pixels are all zero.  The position is
+// clamped to [1, w - 2] x [1, h - 2] first, which is the border rule and also keeps all nine loads of the 3x3
+// neighbourhood inside the frame, so none of them needs a predicate.
 template <int F>
-static __device__ __forceinline__ unsigned rd_px(const uint8_t* src, long long row_pitch, int w, int h, int x, int y) {
-    if constexpr (rd_mono(F)) {
-        return to8<rd_bits(F) - 8>(rd_sample<F>(src + (long long)y * row_pitch, x)) * 0x010101u;
-    } else {
-        if (w < 3 || h < 3) return 0u;
-        x = min(max(x, 1), w - 2);
-        y = min(max(y, 1), h - 2);
-        const uint8_t* m = src + (long long)y * row_pitch;
-        const uint8_t* u = m - row_pitch;
-        const uint8_t* d = m + row_pitch;
-        return rd_bayer_rule<F>(x, y, rd_sample<F>(m, x), rd_sample<F>(u, x), rd_sample<F>(d, x), rd_sample<F>(m, x - 1),
-                                rd_sample<F>(m, x + 1), rd_sample<F>(u, x - 1), rd_sample<F>(u, x + 1),
-                                rd_sample<F>(d, x - 1), rd_sample<F>(d, x + 1));
-    }
+static __device__ __forceinline__ unsigned mosaic_px(const uint8_t* src, long long row_pitch, int w, int h, int x, int y) {
+    if (w < 3 || h < 3) return 0u;
+    x = min(max(x, 1), w - 2);
+    y = min(max(y, 1), h - 2);
+    const uint8_t* m = src + (long long)y * row_pitch;
+    const uint8_t* u = m - row_pitch;
+    const uint8_t* d = m + row_pitch;
+    return bayer_rule<img_pattern(F), img_shift(F)>(
+        x, y, mosaic_sample<F>(m, x, 0), mosaic_sample<F>(u, x, 0), mosaic_sample<F>(d, x, 0), mosaic_sample<F>(m, x, -1),
+        mosaic_sample<F>(m, x, 1), mosaic_sample<F>(u, x, -1), mosaic_sample<F>(u, x, 1), mosaic_sample<F>(d, x, -1),
+        mosaic_sample<F>(d, x, 1));
 }
 
-// Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the one-pixel readers above, the demosaic
-// of a Bayer mosaic, the conversion of a YUV frame, or the reduction of a high-bit-depth frame.
+// Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the demosaic of a mosaic, the conversion of
+// a YUV frame, a high-bit-depth mono sample reduced and repeated, or one of the one-pixel readers above.
 template <int F>
 static __device__ __forceinline__ unsigned view_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int w,
                                                    int h, int x, int y) {
-    if constexpr (is_bayer(F)) return bayer_px<F>(src, row_pitch, w, h, x, y);
-    else if constexpr (is_yuv(F)) return yuv_px<F>(src, row_pitch, plane_pitch, x, y);
-    else if constexpr (is_rawdepth(F)) return rd_px<F>(src, row_pitch, w, h, x, y);
+    if constexpr (img_mosaic(F)) return mosaic_px<F>(src, row_pitch, w, h, x, y);
+    else if constexpr (img_family(F) == IMG_YUV) return yuv_px<F>(src, row_pitch, plane_pitch, x, y);
+    else if constexpr (img_family(F) == IMG_RAWDEPTH)
+        return to8<img_shift(F)>(rd_sample<F>(src + (long long)y * row_pitch, x)) * 0x010101u;
     else return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch);
 }
 
@@ -238,8 +208,7 @@ __device__ __forceinline__ void store_view_bgr(uint8_t* __restrict__ o, int N, i
     }
 }
 
-// ---- the kernels (instantiated per format in k_image.cu and k_rectify.cu, the Bayer formats in k_bayer.cu, the YUV
-// formats in k_yuv.cu, the high-bit-depth formats in k_rawdepth.cu) ----
+// ---- the kernels (instantiated per format in the file of its family, see the end of this file) ----
 
 // k_image.cu: pixel (x, y) of the view, read in place.
 template <int F>
@@ -254,8 +223,8 @@ k_image_ingest(int W, int H, int N, const uint8_t* __restrict__ left, const uint
 }
 
 template <int F>
-static void launch_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                         uint8_t* bgr, cudaStream_t st) {
+void launch_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                  uint8_t* bgr, cudaStream_t st) {
     const int groups = dm.N / 4;
     dim3 grid(std::max(1, (groups + II_GROUPS - 1) / II_GROUPS), 2, S);
     k_image_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.H, dm.N, left, right, g.row_pitch, g.plane_pitch, g.image_stride, bgr);
@@ -268,74 +237,49 @@ static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* 
     const int x0 = (short)(m.x & 0xffffu), y0 = (short)(m.x >> 16);
     const int ax = m.y & 31, ay = m.y >> 5;
     unsigned s[4];   // (x0, y0), (x0 + 1, y0), (x0, y0 + 1), (x0 + 1, y0 + 1)
-    if constexpr (is_bayer(F)) {
-        // each neighbour inside the frame is demosaiced from its clamped 3x3 neighbourhood.  When no clamp applies
-        // (1 <= x0, x0 + 1 <= sw - 2, likewise y0), the four neighbourhoods are one 4x4 window, loaded once.
-        if (x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
-            int v[4][4];
-            const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch + (x0 - 1);
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) v[i][j] = __ldg(r0 + i * row_pitch + j);
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const int dx = k & 1, dy = k >> 1;
-                s[k] = bayer_rule<F>(x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
-                                     v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const int x = x0 + (k & 1), y = y0 + (k >> 1);
-                s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? bayer_px<F>(src, row_pitch, sw, sh, x, y)
-                                                                                : 0u;
-            }
-        }
-    } else if constexpr (is_yuv(F)) {
-        // each neighbour inside the frame is converted from its own luma and chroma (nearest chroma, no chroma
-        // interpolation); one outside the frame is BGR 0, not the conversion of zero samples
+    // neighbour by neighbour: each one inside the frame through view_px (a mosaic site demosaiced from its clamped 3x3
+    // neighbourhood, a YUV pixel from its own luma and nearest chroma), one outside the frame BGR 0, not the
+    // conversion of zero samples
+    const auto each = [&] {
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const int x = x0 + (k & 1), y = y0 + (k >> 1);
-            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? yuv_px<F>(src, row_pitch, plane_pitch, x, y)
-                                                                            : 0u;
+            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh
+                       ? view_px<F>(src, row_pitch, plane_pitch, sw, sh, x, y) : 0u;
         }
-    } else if constexpr (is_rawdepth(F)) {
-        // as for the 8-bit mosaics: where no clamp applies, one 4x4 window of full-depth samples serves the four
-        // demosaics, each reduced to 8 bits before the blend; elsewhere, and for mono, neighbour by neighbour
-        if (!rd_mono(F) && x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
+    };
+    if constexpr (img_mosaic(F)) {
+        // when no clamp applies (1 <= x0, x0 + 1 <= sw - 2, likewise y0), the four 3x3 neighbourhoods are one 4x4
+        // window of full-depth samples, loaded once; each demosaic is reduced to 8 bits before the blend
+        if (x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
             int v[4][4];
             const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch;
 #pragma unroll
             for (int i = 0; i < 4; i++)
 #pragma unroll
-                for (int j = 0; j < 4; j++) v[i][j] = rd_sample<F>(r0 + i * row_pitch, x0 - 1 + j);
+                for (int j = 0; j < 4; j++) v[i][j] = mosaic_sample<F>(r0 + i * row_pitch, x0 - 1, j);
 #pragma unroll
             for (int k = 0; k < 4; k++) {
                 const int dx = k & 1, dy = k >> 1;
-                s[k] = rd_bayer_rule<F>(x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
-                                        v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
+                s[k] = bayer_rule<img_pattern(F), img_shift(F)>(
+                    x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
+                    v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
             }
         } else {
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const int x = x0 + (k & 1), y = y0 + (k >> 1);
-                s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? rd_px<F>(src, row_pitch, sw, sh, x, y) : 0u;
-            }
+            each();
         }
-    } else if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
-        const uint8_t* r0 = src + y0 * row_pitch;
-        s[0] = ImgIn<F>::px(r0, x0, plane_pitch);
-        s[1] = ImgIn<F>::px(r0, x0 + 1, plane_pitch);
-        s[2] = ImgIn<F>::px(r0 + row_pitch, x0, plane_pitch);
-        s[3] = ImgIn<F>::px(r0 + row_pitch, x0 + 1, plane_pitch);
+    } else if constexpr (img_family(F) == IMG_PACKED) {
+        if ((unsigned)x0 < (unsigned)(sw - 1) && (unsigned)y0 < (unsigned)(sh - 1)) {
+            const uint8_t* r0 = src + y0 * row_pitch;
+            s[0] = ImgIn<F>::px(r0, x0, plane_pitch);
+            s[1] = ImgIn<F>::px(r0, x0 + 1, plane_pitch);
+            s[2] = ImgIn<F>::px(r0 + row_pitch, x0, plane_pitch);
+            s[3] = ImgIn<F>::px(r0 + row_pitch, x0 + 1, plane_pitch);
+        } else {
+            each();
+        }
     } else {
-#pragma unroll
-        for (int k = 0; k < 4; k++) {
-            const int x = x0 + (k & 1), y = y0 + (k >> 1);
-            s[k] = (unsigned)x < (unsigned)sw && (unsigned)y < (unsigned)sh ? ImgIn<F>::px(src + y * row_pitch, x, plane_pitch) : 0u;
-        }
+        each();
     }
     const int w[4] = {(32 - ax) * (32 - ay), ax * (32 - ay), (32 - ax) * ay, ax * ay};
     unsigned out = 0;
@@ -364,27 +308,22 @@ k_rectify_ingest(int W, int N, int S, int sw, int sh, const uint2* __restrict__ 
 }
 
 template <int F>
-static void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                           const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
+void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                    const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
     const int tiles = std::max(1, (dm.N / 4 + II_GROUPS - 1) / II_GROUPS);
     dim3 grid((unsigned)(tiles * S), 2);
     k_rectify_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.N, S, r.src_w, r.src_h, r.map[0], r.map[1], left, right,
                                                      g.row_pitch, g.plane_pitch, g.image_stride, bgr);
 }
 
-// The Bayer instantiations of both kernels (k_bayer.cu), for g.format one of ADC_IMG_BAYER_*.
-void adc_launch_bayer_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                            uint8_t* bgr, cudaStream_t st);
-void adc_launch_bayer_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                              const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);
-// The YUV instantiations of both kernels (k_yuv.cu), for g.format one of ADC_IMG_NV12 ... ADC_IMG_YVYU.
-void adc_launch_yuv_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                          uint8_t* bgr, cudaStream_t st);
-void adc_launch_yuv_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                            const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);
-// The high-bit-depth instantiations of both kernels (k_rawdepth.cu), for g.format one of ADC_IMG_MONO10 ...
-// ADC_IMG_BAYER_GB12P.
-void adc_launch_rawdepth_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                               uint8_t* bgr, cudaStream_t st);
-void adc_launch_rawdepth_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right,
-                                 const AdcImageGeom& g, const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st);
+// The launchers of format F are instantiated in the file of F's family (img_format.h): II_IMAGE(F) / II_RECTIFY(F)
+// there, and nowhere else, so each file compiles only its own formats' kernels.
+#define II_IMAGE(F)                                                                                                    \
+    template void launch_image<F>(const AdcDims&, int, const uint8_t*, const uint8_t*, const AdcImageGeom&, uint8_t*,   \
+                                  cudaStream_t);
+#define II_RECTIFY(F)                                                                                                  \
+    template void launch_rectify<F>(const AdcDims&, int, const uint8_t*, const uint8_t*, const AdcImageGeom&,          \
+                                    const AdcRectGeom&, uint8_t*, cudaStream_t);
+#define II_EXTERN(F) extern II_IMAGE(F) extern II_RECTIFY(F)
+ADC_IMG_FORMATS(II_EXTERN)
+#undef II_EXTERN

@@ -1,8 +1,9 @@
 // k_rawdepth.cu -- the high-bit-depth instantiations of the two image ingestion kernels (k_image.cuh): k_image_ingest
 // for adc_match_images* and k_rectify_ingest for adc_match_rectified*, one per format: five containers (16-bit words
 // holding 10, 12 or 16 significant bits; the PFNC 10p and 12p bit streams) x mono and the four Bayer patterns, all
-// reading through rd_px.  Container, depth and pattern are template constants, so the shift of the depth reduction and
-// the field width of the packed readers are immediates and the kernels take the arguments every other format takes.
+// reading through rd_sample, the mosaics through mosaic_px.  Container, depth and pattern are template constants, so
+// the shift of the depth reduction and the field width of the packed readers are immediates and the kernels take the
+// arguments every other format takes.
 //
 // Plain ingestion: each thread converts four consecutive output pixels; a mono pixel is one sample (one 16-bit load, or
 // two byte loads for a packed field), a Bayer pixel nine samples from the clamped 3x3 neighbourhood, demosaiced at full
@@ -12,29 +13,5 @@
 // see DESIGN.md section 19.
 #include "k_image.cuh"
 
-#define RD_COLOURS(LAUNCH, M)                                   \
-    case M: LAUNCH(M); break;                                   \
-    case M + 1: LAUNCH(M + 1); break;                           \
-    case M + 2: LAUNCH(M + 2); break;                           \
-    case M + 3: LAUNCH(M + 3); break;                           \
-    case M + 4: LAUNCH(M + 4); break;
-#define RD_FORMATS(LAUNCH)                                      \
-    switch (g.format) {                                         \
-        RD_COLOURS(LAUNCH, ADC_IMG_MONO10)                      \
-        RD_COLOURS(LAUNCH, ADC_IMG_MONO12)                      \
-        RD_COLOURS(LAUNCH, ADC_IMG_MONO16)                      \
-        RD_COLOURS(LAUNCH, ADC_IMG_MONO10P)                     \
-        RD_COLOURS(LAUNCH, ADC_IMG_MONO12P)                     \
-    }
-
-void adc_launch_rawdepth_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                               uint8_t* bgr, cudaStream_t st) {
-#define RD_IMAGE(F) launch_image<F>(dm, S, left, right, g, bgr, st)
-    RD_FORMATS(RD_IMAGE)
-}
-
-void adc_launch_rawdepth_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right,
-                                 const AdcImageGeom& g, const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
-#define RD_RECTIFY(F) launch_rectify<F>(dm, S, left, right, g, r, bgr, st)
-    RD_FORMATS(RD_RECTIFY)
-}
+ADC_IMG_RAWDEPTH_FORMATS(II_IMAGE)
+ADC_IMG_RAWDEPTH_FORMATS(II_RECTIFY)

@@ -11,9 +11,9 @@
 //     [-2^20, 2^20] has x0 = +-32767 / -32768 after the int16 saturation, and since src_width, src_height <= 32767
 //     both neighbours x0 and x0 + 1 lie outside the frame: the border value 0 whichever way X saturated.
 //
-// Per wave: k_rectify_ingest<F> (k_image.cuh; instantiated here for the six formats of k_image.cu, in k_bayer.cu for
-// the Bayer mosaics, in k_yuv.cu for the YUV formats, in k_rawdepth.cu for the high-bit-depth formats) makes one launch
-// over the wave's pairs x 2 views.  For each output pixel it gathers the four neighbours of (x0, y0) from the raw view
+// Per wave: k_rectify_ingest<F> (k_image.cuh; dispatched here over every format of img_format.h, instantiated here for
+// the six formats of k_image.cu and in the family files for the others) makes one launch over the wave's pairs x 2
+// views.  For each output pixel it gathers the four neighbours of (x0, y0) from the raw view
 // through the format readers of k_image.cuh, weights them (32 - ax | ax) * (32 - ay | ay), and writes (sum + 512) >> 10
 // per channel with the store scheme of k_image.cuh.  When
 // all four neighbours lie inside the frame (0 <= x0 < src_width - 1, 0 <= y0 < src_height - 1; never for a frame one
@@ -71,19 +71,11 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
 void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                                const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
-        case ADC_IMG_BGR: launch_rectify<ADC_IMG_BGR>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_RGB: launch_rectify<ADC_IMG_RGB>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_BGRA: launch_rectify<ADC_IMG_BGRA>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_RGBA: launch_rectify<ADC_IMG_RGBA>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_GRAY: launch_rectify<ADC_IMG_GRAY>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_BAYER_RGGB: case ADC_IMG_BAYER_GRBG: case ADC_IMG_BAYER_BGGR: case ADC_IMG_BAYER_GBRG:
-            adc_launch_bayer_rectify(dm, S, left, right, g, r, bgr, st);
-            break;
-        case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_YUYV: case ADC_IMG_UYVY: case ADC_IMG_YVYU:
-            adc_launch_yuv_rectify(dm, S, left, right, g, r, bgr, st);
-            break;
-        case ADC_IMG_RGB_PLANAR: launch_rectify<ADC_IMG_RGB_PLANAR>(dm, S, left, right, g, r, bgr, st); break;
-        default: adc_launch_rawdepth_rectify(dm, S, left, right, g, r, bgr, st); break;
+#define RC_CASE(F) case F: launch_rectify<F>(dm, S, left, right, g, r, bgr, st); break;
+        ADC_IMG_FORMATS(RC_CASE)
+#undef RC_CASE
     }
     ++*launches;
 }
+
+ADC_IMG_PACKED_FORMATS(II_RECTIFY)

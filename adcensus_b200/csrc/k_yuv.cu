@@ -9,24 +9,5 @@
 // neighbour outside the frame is 0.  No shared memory: see DESIGN.md section 18.
 #include "k_image.cuh"
 
-void adc_launch_yuv_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                          uint8_t* bgr, cudaStream_t st) {
-    switch (g.format) {
-        case ADC_IMG_NV12: launch_image<ADC_IMG_NV12>(dm, S, left, right, g, bgr, st); break;
-        case ADC_IMG_NV21: launch_image<ADC_IMG_NV21>(dm, S, left, right, g, bgr, st); break;
-        case ADC_IMG_YUYV: launch_image<ADC_IMG_YUYV>(dm, S, left, right, g, bgr, st); break;
-        case ADC_IMG_UYVY: launch_image<ADC_IMG_UYVY>(dm, S, left, right, g, bgr, st); break;
-        default: launch_image<ADC_IMG_YVYU>(dm, S, left, right, g, bgr, st); break;
-    }
-}
-
-void adc_launch_yuv_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                            const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
-    switch (g.format) {
-        case ADC_IMG_NV12: launch_rectify<ADC_IMG_NV12>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_NV21: launch_rectify<ADC_IMG_NV21>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_YUYV: launch_rectify<ADC_IMG_YUYV>(dm, S, left, right, g, r, bgr, st); break;
-        case ADC_IMG_UYVY: launch_rectify<ADC_IMG_UYVY>(dm, S, left, right, g, r, bgr, st); break;
-        default: launch_rectify<ADC_IMG_YVYU>(dm, S, left, right, g, r, bgr, st); break;
-    }
-}
+ADC_IMG_YUV_FORMATS(II_IMAGE)
+ADC_IMG_YUV_FORMATS(II_RECTIFY)

@@ -135,12 +135,14 @@ def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> Imag
     return ImageDesc(_img_format(format), 0, int(row_pitch), int(plane_pitch), int(image_stride))
 
 
+_IMG_NAMES = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS, **{k: v[0] for k, v in RAW_DEPTH_FORMATS.items()}}
+
+
 def _img_format(v) -> int:
     if isinstance(v, str):
-        names = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS, **{k: v[0] for k, v in RAW_DEPTH_FORMATS.items()}}
-        if v not in names:
-            raise ValueError(f"unknown image format {v!r} (one of {sorted(names)})")
-        return names[v]
+        if v not in _IMG_NAMES:
+            raise ValueError(f"unknown image format {v!r} (one of {sorted(_IMG_NAMES)})")
+        return _IMG_NAMES[v]
     return int(v)
 
 
@@ -174,6 +176,15 @@ def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
     if tuple(a.strides[-len(inner):]) != inner or min(a.strides) < 0:
         raise ValueError(f"the pixels of an image row must be contiguous (strides {a.strides})")
     return ImageDesc(fmt, 0, pitches[1], pitches[2], 0)
+
+
+def _image_pair_desc(left: np.ndarray, right: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
+    """The one descriptor of a left and a right numpy view (_image_view_desc), which need the same strides."""
+    desc = _image_view_desc(left, fmt, H, W)
+    if _image_view_desc(right, fmt, H, W).row_pitch != desc.row_pitch or \
+            (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
+        raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
+    return desc
 
 
 # rectification on the way in (adc_set_rectification, adc_match_rectified*): remap tables as cv2.initUndistortRectifyMap
@@ -585,11 +596,7 @@ class Engine:
                      cost_dtype, disparity):
         """The host entries that take views in an IMG_* format: adc_match_images (views of H x W) and
         adc_match_rectified (raw frames of vh x vw)."""
-        fmt = _img_format(format)
-        desc = _image_view_desc(left, fmt, vh, vw)
-        if _image_view_desc(right, fmt, vh, vw).row_pitch != desc.row_pitch or \
-                (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
-            raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
+        desc = _image_pair_desc(left, right, _img_format(format), vh, vw)
         disp, out, args = self._outputs(maps, volumes, layout, dtype, cost, cost_layout, cost_dtype, disparity)
         _check(call(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc), *args))
         return disp, out
@@ -723,10 +730,7 @@ class Engine:
         if rectified and self.rect_src_size is None:
             raise AdcError("no rectification is set (set_rectification)")
         vw, vh = self.rect_src_size if rectified else (self.width, self.height)
-        desc = _image_view_desc(left, fmt, vh, vw)
-        if _image_view_desc(right, fmt, vh, vw).row_pitch != desc.row_pitch or \
-                (fmt == IMG_RGB_PLANAR and right.strides != left.strides):
-            raise ValueError(f"left and right must have the same strides, got {left.strides} and {right.strides}")
+        desc = _image_pair_desc(left, right, fmt, vh, vw)
         views = np.empty((2, self.height, self.width, 3), np.uint8)
         _check(self._L.adc_ingest_views(self._h, left.ctypes.data, right.ctypes.data, ctypes.byref(desc),
                                         1 if rectified else 0, views.ctypes.data))
