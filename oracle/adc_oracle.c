@@ -39,6 +39,7 @@ struct orc_ctx {
     uint8_t* edge;
     int next_stage;
     int horizontal_first;
+    uint64_t tie[ORC_TIE_N]; /* orc_tie_counts: since orc_begin / orc_begin_refine */
 };
 
 /* ------------------------------------------------------------------------------------------ */
@@ -160,7 +161,7 @@ static int colour_dist(const uint8_t* a, const uint8_t* b) { /* cross_aggregator
 }
 
 /* One arm: walk from (x,y) in direction (sx,sy).  cross_aggregator.cpp:135-201 / 203-269. */
-static uint8_t grow_arm(const orc_ctx* c, int x, int y, int sx, int sy) {
+static uint8_t grow_arm(orc_ctx* c, int x, int y, int sx, int sy) {
     const int w = c->w, h = c->h;
     const int limit = c->opt.cross_L1 < 255 ? c->opt.cross_L1 : 255; /* min(L1, MAX_ARM_LENGTH) :151 */
     const uint8_t* p0 = c->left + ((size_t)y * w + x) * 3;
@@ -171,8 +172,13 @@ static uint8_t grow_arm(const orc_ctx* c, int x, int y, int sx, int sy) {
         if (px < 0 || px >= w || py < 0 || py >= h) break;          /* :154-163 */
         const uint8_t* p = c->left + ((size_t)py * w + px) * 3;
         const int dist_anchor = colour_dist(p, p0);
+        c->tie[ORC_TIE_ARM_T1] += dist_anchor == c->opt.cross_t1;
         if (dist_anchor >= c->opt.cross_t1) break;                    /* :169-172 */
-        if (n > 0 && colour_dist(p, prev) >= c->opt.cross_t1) break;  /* :175-180 (t1 again) */
+        const int dist_prev = n > 0 ? colour_dist(p, prev) : 0;
+        c->tie[ORC_TIE_ARM_T1] += n > 0 && dist_prev == c->opt.cross_t1;
+        if (n > 0 && dist_prev >= c->opt.cross_t1) break;             /* :175-180 (t1 again) */
+        c->tie[ORC_TIE_ARM_L2] += n + 1 == c->opt.cross_L2 && dist_anchor >= c->opt.cross_t2;
+        c->tie[ORC_TIE_ARM_T2] += n + 1 > c->opt.cross_L2 && dist_anchor == c->opt.cross_t2;
         if (n + 1 > c->opt.cross_L2 && dist_anchor >= c->opt.cross_t2) break; /* :183-187 */
         len++;
         prev = p;
@@ -309,8 +315,9 @@ static void so_pass(const orc_ctx* c, const float* src, float* dst, int sx, int 
 }
 
 /* ---- stage 4: winner-takes-all with parabola ---------------------------------------------- */
-static float subpixel(float c1, float c2, float cmin, int best) { /* ADCensusStereo.cpp:234-240 */
+static float subpixel(orc_ctx* c, float c1, float c2, float cmin, int best) { /* ADCensusStereo.cpp:234-240 */
     const float denom = c1 + c2 - 2 * cmin;
+    c->tie[ORC_TIE_SUBPIX_FLAT] += c1 == c2 || denom == 0.0f;
     if (denom != 0.0f) return (float)best + (c1 - c2) / (denom * 2.0f);
     return (float)best;
 }
@@ -321,10 +328,12 @@ static void wta_left(orc_ctx* c) { /* ADCensusStereo.cpp:188-243 */
         const float* v = c->vol_aggr + p * D;
         float best_cost = ORC_LARGE;
         int best = 0;
-        for (int d = dmin; d < dmax; d++)
+        for (int d = dmin; d < dmax; d++) {
+            c->tie[ORC_TIE_WTA_L] += v[d - dmin] == best_cost;
             if (best_cost > v[d - dmin]) { best_cost = v[d - dmin]; best = d; } /* strict: first minimum */
+        }
         if (best == dmin || best == dmax - 1) { c->disp_l[p] = ORC_INVALID; continue; }
-        c->disp_l[p] = subpixel(v[best - 1 - dmin], v[best + 1 - dmin], best_cost, best);
+        c->disp_l[p] = subpixel(c, v[best - 1 - dmin], v[best + 1 - dmin], best_cost, best);
     }
 }
 
@@ -340,6 +349,7 @@ static void wta_right(orc_ctx* c) { /* ADCensusStereo.cpp:245-310: cost_R(x,d) =
                 if (xl >= 0 && xl < w) {
                     const float v = c->vol_aggr[((size_t)y * w + xl) * D + (d - dmin)];
                     local[d - dmin] = v;
+                    c->tie[ORC_TIE_WTA_R] += v == best_cost;
                     if (best_cost > v) { best_cost = v; best = d; }
                 } else {
                     local[d - dmin] = ORC_LARGE; /* :286 */
@@ -351,7 +361,7 @@ static void wta_right(orc_ctx* c) { /* ADCensusStereo.cpp:245-310: cost_R(x,d) =
              * guarded, the reference's behaviour is undefined in that corner (SURVEY 8a/A10) */
             const int i1 = best - 1 - dmin, i2 = best + 1 - dmin;
             if (i1 < 0 || i2 >= D) { *out = (float)best; continue; }
-            *out = subpixel(local[i1], local[i2], best_cost, best);
+            *out = subpixel(c, local[i1], local[i2], best_cost, best);
         }
     free(local);
 }
@@ -369,10 +379,15 @@ static void outlier_detection(orc_ctx* c) { /* multistep_refiner.cpp:90-151, ras
             const long col_r = lroundf((float)x - disp);
             if (col_r >= 0 && col_r < w) {
                 const float disp_r = c->disp_r[(size_t)y * w + col_r];
+                c->tie[ORC_TIE_LR_EQ] += fabsf(disp - disp_r) == thres;
                 if (fabsf(disp - disp_r) > thres) {
                     const int col_rl = (int)lroundf((float)col_r + disp_r);
                     int is_occl = 0;
-                    if (col_rl > 0 && col_rl < w) is_occl = c->disp_l[(size_t)y * w + col_rl] > disp; /* may already be +inf */
+                    if (col_rl > 0 && col_rl < w) {
+                        const float dl = c->disp_l[(size_t)y * w + col_rl]; /* may already be +inf */
+                        c->tie[ORC_TIE_OCCL_EQ] += dl == disp;
+                        is_occl = dl > disp;
+                    }
                     if (is_occl) { c->occl[2 * c->n_occl] = x; c->occl[2 * c->n_occl + 1] = y; c->n_occl++; }
                     else         { c->mism[2 * c->n_mism] = x; c->mism[2 * c->n_mism + 1] = y; c->n_mism++; }
                     *dp = ORC_INVALID;
@@ -413,8 +428,15 @@ static void region_voting(orc_ctx* c) { /* multistep_refiner.cpp:153-227 */
                     if (peak < hist[d]) { peak = hist[d]; best = d; }
                     total += hist[d];
                 }
-                if (peak > 0 && total > c->opt.irv_ts && (float)peak * 1.0f / (float)total > c->opt.irv_th)
+                c->tie[ORC_TIE_VOTE_TS] += peak > 0 && total == c->opt.irv_ts;
+                c->tie[ORC_TIE_VOTE_TH] += peak > 0 && total > c->opt.irv_ts && (float)peak * 1.0f / (float)total == c->opt.irv_th;
+                if (peak > 0 && total > c->opt.irv_ts && (float)peak * 1.0f / (float)total > c->opt.irv_th) {
+                    int later = 0;
+                    for (int d = best + 1; d < D; d++) later |= hist[d] == peak;
+                    c->tie[ORC_TIE_VOTE_PEAK] += later;
+                    c->tie[ORC_TIE_VOTE_PAIR] += best % 2 == 0 && best + 1 < D && hist[best + 1] == peak;
                     *dp = (float)(best + dmin); /* visible to later pixels of this sweep */
+                }
             }
             size_t keep = 0; /* erase filled, order preserved (:217-224) */
             for (size_t i = 0; i < *cnt; i++) {
@@ -454,6 +476,7 @@ static void proper_interpolation(orc_ctx* c) { /* multistep_refiner.cpp:229-305 
                     if (d != ORC_INVALID) {
                         const uint8_t* q = c->left + ((size_t)yy * w + xx) * 3;
                         const int dist = abs(pc[0] - q[0]) + abs(pc[1] - q[1]) + abs(pc[2] - q[2]);
+                        c->tie[ORC_TIE_INTERP_DIST] += k == 0 && dist == best_dist && d != best_d;
                         if (best_dist > dist) { best_dist = dist; best_d = d; } /* first closest wins */
                         min_d = fminf2(min_d, d);
                         n_cand++;
@@ -462,6 +485,7 @@ static void proper_interpolation(orc_ctx* c) { /* multistep_refiner.cpp:229-305 
                 }
                 ang += pi / 16; /* float quotient accumulated in double (:234,268) */
             }
+            c->tie[ORC_TIE_INTERP_NONE] += n_cand == 0;
             if (n_cand == 0) continue;
             fill[i] = k == 0 ? best_d : min_d;
         }
@@ -482,6 +506,7 @@ static void discontinuity_adjustment(orc_ctx* c) { /* multistep_refiner.cpp:307-
             const float* r2 = p + (size_t)(y + 1) * w + x;
             const float gx = (-r0[-1] + r0[1]) + (-2 * r1[-1] + 2 * r1[1]) + (-r2[-1] + r2[1]);
             const float gy = (-r0[-1] - 2 * r0[0] - r0[1]) + (r2[-1] + 2 * r2[0] + r2[1]);
+            c->tie[ORC_TIE_EDGE_EQ] += fabsf(gx) + fabsf(gy) == 5.0f;
             if (fabsf(gx) + fabsf(gy) > 5.0f) c->edge[(size_t)y * w + x] = 1;
         }
     for (int y = 0; y < h; y++)
@@ -500,6 +525,7 @@ static void discontinuity_adjustment(orc_ctx* c) { /* multistep_refiner.cpp:307-
                 const long d2i = lroundf(d2);
                 if (d2i < 0 || d2i >= D) continue;
                 const float cc = k == 0 ? cost[-D + d2i] : cost[D + d2i];
+                c->tie[ORC_TIE_DISC_EQ] += cc == c0;
                 if (cc < c0) { row[x] = d2; c0 = cc; }
             }
         }
@@ -529,6 +555,7 @@ static void median3_inplace(float* img, int w, int h) { /* adcensus_util.cpp:55-
 int orc_begin(orc_ctx* c, const uint8_t* left, const uint8_t* right) {
     if (!c || !left || !right) return 0;
     c->left = left; c->right = right;
+    memset(c->tie, 0, sizeof(c->tie));
     c->next_stage = ADC_STAGE_COST;
     c->horizontal_first = 1;
     return 1;
@@ -543,6 +570,7 @@ int orc_begin_refine(orc_ctx* c, const uint8_t* left, const uint8_t* right, cons
     c->left = left; c->right = right;
     memcpy(c->disp_l, disp_left, n * sizeof(float));
     memcpy(c->disp_r, disp_right, n * sizeof(float));
+    memset(c->tie, 0, sizeof(c->tie));
     build_arms(c);
     support_counts(c);
     c->n_mism = c->n_occl = 0;
@@ -614,6 +642,8 @@ size_t orc_tap(orc_ctx* c, int tap, void* dst, size_t cap) {
     default: return 0;
     }
 }
+
+void orc_tie_counts(const orc_ctx* c, uint64_t* out) { memcpy(out, c->tie, sizeof(c->tie)); }
 
 double orc_time_match(orc_ctx* c, const uint8_t* left, const uint8_t* right, float* disp, int iters) {
     struct timespec t0, t1;

@@ -35,6 +35,26 @@ typedef struct orc_option {
 
 typedef struct orc_ctx orc_ctx;
 
+/* Tie counters: each is one increment at a comparison that an exact equality decided, where the neighbouring
+ * comparison (>= for >, another reduction order) would have decided otherwise.  They never change a result.
+ *   WTA_L / WTA_R   a later d with cost == the best so far (the strict > keeps the first minimum)
+ *   SUBPIX_FLAT     the parabola's neighbours are equal or its denominator is 0
+ *   LR_EQ           |disp - disp_r| == lrcheck_thres (kept)
+ *   OCCL_EQ         disp_l[col_rl] == disp (a mismatch, not an occlusion)
+ *   VOTE_PEAK       a filled pixel whose histogram has a later bin equal to the peak (the lowest disparity keeps it)
+ *   VOTE_TS         total == irv_ts (not filled);  VOTE_TH  peak / total == irv_th (not filled)
+ *   INTERP_DIST     a mismatch whose later ray meets the best colour distance with another disparity (the earliest
+ *                   ray keeps it; occlusions take the smallest disparity, which no tie decides)
+ *   INTERP_NONE     no ray found a candidate (the pixel becomes 0.0)
+ *   EDGE_EQ         |gx| + |gy| == 5 (not an edge);  DISC_EQ  cc == c0 (not adjusted)
+ *   ARM_T1 / ARM_T2 a colour distance equal to cross_t1 / cross_t2 where it is compared (the arm stops)
+ *   ARM_L2          a step at exactly n + 1 == cross_L2 whose anchor distance is >= cross_t2 (the arm goes on)
+ *   VOTE_PAIR       a filled pixel whose peak is an even bin 2k with bin 2k + 1 equal to it (the two bins of one word of
+ *                   the GPU's narrow histogram, where the lane's own scan, not the cross-lane minimum, breaks the tie) */
+enum { ORC_TIE_WTA_L, ORC_TIE_WTA_R, ORC_TIE_SUBPIX_FLAT, ORC_TIE_LR_EQ, ORC_TIE_OCCL_EQ, ORC_TIE_VOTE_PEAK,
+       ORC_TIE_VOTE_TS, ORC_TIE_VOTE_TH, ORC_TIE_INTERP_DIST, ORC_TIE_INTERP_NONE, ORC_TIE_EDGE_EQ, ORC_TIE_DISC_EQ,
+       ORC_TIE_ARM_T1, ORC_TIE_ARM_T2, ORC_TIE_ARM_L2, ORC_TIE_VOTE_PAIR, ORC_TIE_N };
+
 void orc_default_option(orc_option* o);
 orc_ctx* orc_create(int width, int height, const orc_option* opt);
 void orc_destroy(orc_ctx* c);
@@ -47,6 +67,8 @@ int orc_step(orc_ctx* c);
  * cost volumes are never touched.  Returns 0 with do_discontinuity_adjustment set (that stage reads the volume). */
 int orc_begin_refine(orc_ctx* c, const uint8_t* left, const uint8_t* right, const float* disp_left, const float* disp_right);
 size_t orc_tap(orc_ctx* c, int tap, void* dst, size_t cap);
+/* the tie counters accumulated since orc_begin / orc_begin_refine (ORC_TIE_N values) */
+void orc_tie_counts(const orc_ctx* c, uint64_t* out);
 double orc_time_match(orc_ctx* c, const uint8_t* left, const uint8_t* right, float* disp, int iters);
 
 /* leaf functions exposed for exhaustive micro-tests */

@@ -43,6 +43,9 @@ STAGE_TAPS = {
     "VOTE": ["DISP_L", "MISMATCHES", "OCCLUSIONS"],
     "INTERP": ["DISP_L"], "DISC": ["DISP_L"], "MEDIAN": ["DISP_L"],
 }
+# the oracle's tie counters (oracle/adc_oracle.h ORC_TIE_*), in order
+TIES = ["WTA_L", "WTA_R", "SUBPIX_FLAT", "LR_EQ", "OCCL_EQ", "VOTE_PEAK", "VOTE_TS", "VOTE_TH", "INTERP_DIST",
+        "INTERP_NONE", "EDGE_EQ", "DISC_EQ", "ARM_T1", "ARM_T2", "ARM_L2", "VOTE_PAIR"]
 
 
 class Option(ctypes.Structure):
@@ -164,6 +167,14 @@ class _Checker:
         while self.step() >= 0:
             pass
         return self.tap("DISP_L").copy()
+
+    def tie_counts(self) -> dict:
+        """{name: count} of the restatement's tie counters since the last begin (TIES; oracle/adc_oracle.h)."""
+        out = (ctypes.c_uint64 * len(TIES))()
+        f = self._f("tie_counts")
+        f.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        f(self.ctx, out)
+        return dict(zip(TIES, map(int, out)))
 
     def time_match(self, left, right, iters=1) -> float:
         left = np.ascontiguousarray(left, np.uint8)

@@ -69,3 +69,5 @@ double occ_time_match(occ_ctx* x, const uint8_t* left, const uint8_t* right, flo
     x->injected = 0;
     return orc_time_match(x->c, left, right, disp, iters);
 }
+
+void occ_tie_counts(const occ_ctx* x, uint64_t* out) { orc_tie_counts(x->c, out); }

@@ -189,22 +189,57 @@ def reached(c, plans):
 
 
 # ---- the GPU run ----------------------------------------------------------------------------------------------------
-def check_case(c, debug_flags=0):
+def _oracle_outputs(c, left, right, cost):
+    if cost is None:
+        return E.oracle_outputs(c.W, c.H, c.opt, left, right)
+    import cost_testlib as CT
+    orc = CT.CostOracle(c.W, c.H, c.opt)
+    orc.begin_cost(left, right, cost)
+    out = {}
+    for st in T.STAGES:
+        orc.step()
+        for tap in T.STAGE_TAPS[st]:
+            if (st, tap) in E.ORACLE_OUTPUTS:
+                out[E.ORACLE_OUTPUTS[(st, tap)]] = orc.tap(tap).copy()
+    orc.close()
+    return out
+
+
+def check_case(c, debug_flags=0, pairs=None, confidence=False, pipelined=False, cost_layout="hwd", cost_dtype="f32"):
     """One match_outputs_batch_device call over the case's pairs, exporting the three volumes (f32, [H][W][D]), the
     WTA maps, the outlier map and the final map, each pair compared bit for bit with its own oracle run, on an engine
-    created with `debug_flags`; returns every output of the call on the host."""
+    created with `debug_flags`; returns every output of the call on the host.
+    pairs: [(left, right)] or [(left, right, cost volume f32 [H][W][D])] instead of the sweep's pairs; with cost volumes
+    the call matches from them (given as `cost_layout` / `cost_dtype`; their values must be exact in that type).
+    confidence: also export MIN_COST / PEAK_RATIO and compare them with maps_testlib.confidence of the oracle's SO4
+    volume.  pipelined: the batch as two calls that flow into each other."""
     torch, dev = E.cuda()
+    if pairs is None:
+        pairs = GS.sweep_pairs(c.W, c.H, c.D, c.seed)[:c.n]
+    pairs = [(p[0], p[1], p[2] if len(p) > 2 else None) for p in pairs]
+    has_cost = pairs[0][2] is not None
+    assert all((p[2] is not None) == has_cost for p in pairs)
+    maps = ["wta_left", "wta_right", "outliers"] + (["min_cost", "peak_ratio"] if confidence else [])
     # the oracle runs overlap in threads (ctypes releases the GIL during the call) while the GPU runs the batch
-    pairs = GS.sweep_pairs(c.W, c.H, c.D, c.seed)[:c.n]
     with ThreadPoolExecutor(len(pairs)) as ex:
-        futs = [ex.submit(E.oracle_outputs, c.W, c.H, c.opt, l, r) for l, r in pairs]
+        futs = [ex.submit(_oracle_outputs, c, l, r, v) for l, r, v in pairs]
         d_l = torch.from_numpy(np.stack([p[0] for p in pairs])).to(dev)
         d_r = torch.from_numpy(np.stack([p[1] for p in pairs])).to(dev)
+        cost = {}
+        if has_cost:
+            import cost_testlib as CT
+            vols = [v if cost_layout == "hwd" else np.ascontiguousarray(v.transpose(2, 0, 1)) for _, _, v in pairs]
+            vols = [CT.to_bf16_bits(v) if cost_dtype == "bf16" else v.astype({"f32": np.float32, "f16": np.float16}[cost_dtype])
+                    for v in vols]
+            for v, (_, _, v32) in zip(vols, pairs):
+                back = (v.astype(np.uint32) << 16).view(np.float32) if cost_dtype == "bf16" else v.astype(np.float32)
+                assert np.array_equal(back, v32 if cost_layout == "hwd" else v32.transpose(2, 0, 1)), "volume not exact"
+            cost = dict(d_cost=torch.from_numpy(np.stack(vols).view(np.int16) if cost_dtype == "bf16" else np.stack(vols)).to(dev), cost_layout=cost_layout, cost_dtype=cost_dtype)
         eng = E.engine(c.W, c.H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes, debug_flags=debug_flags)
         assert (eng.wave_pairs, eng.lanes) == (c.wave_pairs, c.lanes), (eng.wave_pairs, eng.lanes)
         got = E.batch_outputs(eng, eng.match_outputs_batch_device, len(pairs), d_l.data_ptr(), d_r.data_ptr(),
                               3 * c.W * c.H, volumes=[(s, "hwd", "f32") for s in ("cost", "aggr", "opt")],
-                              maps=["wta_left", "wta_right", "outliers"])
+                              maps=maps, pipelined=pipelined, **cost)
         eng.close()
         want = [f.result() for f in futs]
     for i, w in enumerate(want):
@@ -218,5 +253,9 @@ def check_case(c, debug_flags=0):
         mis, occ = MT.outlier_lists(got["outliers"][i])
         E.same(f"{tag} OUTLIER/MISMATCHES", mis, w["mismatches"].reshape(-1, 2))
         E.same(f"{tag} OUTLIER/OCCLUSIONS", occ, w["occlusions"].reshape(-1, 2))
+        if confidence:
+            c1, ratio = MT.confidence(w["opt"])
+            E.same(f"{tag} MIN_COST", got["min_cost"][i], c1)
+            E.same(f"{tag} PEAK_RATIO", got["peak_ratio"][i], ratio)
         E.same(f"{tag} MEDIAN/DISP_L", got["disp"][i], w["final"])
     return got
