@@ -62,6 +62,14 @@ __device__ __forceinline__ float adc_key2f(unsigned k) {
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
+// Parabola through (best-1, best, best+1), ADCensusStereo.cpp:234-240 (k_wta.cu, k_scanline.cu).  Explicit _rn
+// intrinsics keep nvcc from contracting c1 + c2 - 2*min into an FMA.
+__device__ __forceinline__ float adc_subpixel(float c1, float c2, float cmin, int best) {
+    const float denom = __fsub_rn(__fadd_rn(c1, c2), __fmul_rn(2.0f, cmin));
+    if (denom != 0.0f) return __fadd_rn((float)best, __fdiv_rn(__fsub_rn(c1, c2), __fmul_rn(denom, 2.0f)));
+    return (float)best;
+}
+
 // Function attributes and __device__ / __constant__ symbols exist once per device: one-time set-up is keyed by the
 // current device (one process may own engines on several GPUs, driven from several threads: the flags are atomics, and
 // a thread that loses the race may run the kernel before the winner's attribute call has returned -- so every caller
@@ -228,6 +236,11 @@ bool adc_so_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, un
 int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
                         cudaStream_t st, unsigned long long* launches);
 int adc_launch_wta(const AdcParams& P, const AdcWave& w, const float* vol, cudaStream_t st, unsigned long long* launches);
+// the last scanline pass (-y) fused with the WTA (so_wta_fused, so_plan.h): src = w.volB's optimised-so-far volume; writes
+// disp_l and the right view's partial records to rec; k_wta_merge folds them into disp_r
+int adc_launch_scanline_wta(const AdcParams& P, const AdcWave& w, const float* src, float* rec, cudaStream_t st,
+                            unsigned long long* launches);
+int adc_launch_wta_merge(const AdcParams& P, const AdcWave& w, const float* rec, cudaStream_t st, unsigned long long* launches);
 // cost-curve confidence (k_confidence.cu): per pixel of the wave's volume `vol`, c1 = C(d1) -> min_cost and c1 / c2 ->
 // peak_ratio (either may be NULL; pair i at element i*N, 4-byte aligned)
 void adc_launch_confidence(const AdcParams& P, const AdcWave& w, const float* vol, float* min_cost, float* peak_ratio,

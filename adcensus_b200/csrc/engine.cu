@@ -24,6 +24,7 @@
 #include "../../include/adcensus_b200.h"
 #include "adc_common.cuh"
 #include "ca_plan.h"
+#include "so_plan.h"
 
 static_assert(sizeof(adc_option) == 60, "adc_option must match the reference's ADCensusOption (60 bytes)");
 static_assert(offsetof(adc_option, so_p1) == 32 && offsetof(adc_option, irv_th) == 48 &&
@@ -379,7 +380,7 @@ LaneVols lane_volumes(const adc_engine* e, const AdcWave& w, int last_stage) {
 // OPT in volA after scanline pass 4, which nothing later writes.  `maps` (possibly none) likewise (DESIGN.md section 12): the
 // WTA maps and the confidence right after the WTA (disp_l is overwritten by the LR check), the outlier map right after
 // the LR check (region voting changes label).
-int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_t* ev, const CostSrc& cost,
+int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, bool debug_run, cudaEvent_t* ev, const CostSrc& cost,
                      const VolOuts& outs, const MapOuts& maps) {
     const AdcParams& P = e->P;
     const AdcWave w = wave_view(e, ln, nS);
@@ -462,11 +463,22 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
     // ---- stage 3: scanline optimisation, 4 chained passes (scanline_optimizer.cpp:54-60)
     adc_launch_diffmaps(P, w, st, L);
     adc_launch_so_bitrows(P, w, st, L);
+    // Pass 4 takes both WTA views as its epilogue where nothing else reads the optimised volume: it then writes disp_l and
+    // the right view's partial records into A instead of the volume, and k_wta_merge finishes disp_r (so_plan.h).
+    SoVolumeUse vol_use{};
+    for (int i = 0; i < outs.n; i++) vol_use.opt_export |= outs.o[i].stage == ADC_VOL_OPT;
+    vol_use.confidence = maps.dst[ADC_MAP_MIN_COST] || maps.dst[ADC_MAP_PEAK_RATIO];
+    vol_use.discontinuity = e->opt.do_discontinuity_adjustment != 0;
+    vol_use.debug_run = debug_run || last_stage < ADC_STAGE_WTA;
+    const int wta_force = (e->cfg.debug_flags & ADC_DBG_UNFUSED_SO_WTA) ? SO_WTA_NEVER
+                          : (e->cfg.debug_flags & ADC_DBG_FUSED_SO_WTA) ? SO_WTA_ALWAYS : SO_WTA_AUTO;
+    const bool so_wta = so_wta_fused(vol_use, wta_force, P.dm.W, P.dm.H, P.dm.D, P.dm.Dp, P.dm.dmin, P.dm.vol_stride);
     static const int dirs[4][2] = {{1, 0}, {-1, 0}, {0, 1}, {0, -1}};
     for (int ps = 0; ps < 4; ps++) {
         const float* src = (ps % 2 == 0) ? A : B;
         float* dst = (ps % 2 == 0) ? B : A;
-        if (adc_launch_scanline(P, w, src, dst, dirs[ps][0], dirs[ps][1], st, L))
+        if (ps == 3 && so_wta ? adc_launch_scanline_wta(P, w, src, dst, st, L)
+                              : adc_launch_scanline(P, w, src, dst, dirs[ps][0], dirs[ps][1], st, L))
             return fail(ADC_ERR_UNSUPPORTED, "scanline pass not launched (disparity range %d, limit 256)", P.dm.D);
         if (ps % 2 == 0) e->dbg_init = B; else e->dbg_aggr = A;
         if (ps == 3) export_vol(ADC_VOL_OPT, A);
@@ -476,7 +488,8 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, cudaEvent_
     if (ev) CK(cudaEventRecord(ev[3], st));
 
     // ---- stage 4: left + right disparity (ADCensusStereo.cpp:108-109)
-    if (adc_launch_wta(P, w, A, st, L)) return fail(ADC_ERR_UNSUPPORTED, "WTA launch failed");
+    if (so_wta) adc_launch_wta_merge(P, w, A, st, L);
+    else if (adc_launch_wta(P, w, A, st, L)) return fail(ADC_ERR_UNSUPPORTED, "WTA launch failed");
     if (maps.dst[ADC_MAP_WTA_LEFT])
         CK(cudaMemcpyAsync(maps.dst[ADC_MAP_WTA_LEFT], w.disp_l, mapN * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (maps.dst[ADC_MAP_WTA_RIGHT])
@@ -625,7 +638,7 @@ int run_batch(adc_engine* e, int n, const BatchIO& io, const MatchReq& q, cudaSt
         MapOuts wave_maps;
         for (int i = 0; i < q.n_maps; i++)
             wave_maps.dst[q.maps[i].kind] = static_cast<char*>(q.maps[i].dst) + (size_t)first * N * map_elem_bytes(q.maps[i].kind);
-        int rc = enqueue_pipeline(e, ln, nS, last, nullptr, wave_cost, wave_outs, wave_maps);
+        int rc = enqueue_pipeline(e, ln, nS, last, q.debug_stage >= 0, nullptr, wave_cost, wave_outs, wave_maps);
         if (rc) return rc;
         // ---- outputs (a device call without a map output gives exported volumes / side maps only)
         if (strided_copy) {
@@ -938,7 +951,7 @@ int match_host(adc_engine* e, const char* fn, const MatchReq& q, const uint8_t* 
     cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
     CostSrc src;
     if ((rc = upload_pair(e, ln, q, left, right, raw, last, ev ? ev[0] : nullptr, &src))) return rc;
-    if ((rc = enqueue_pipeline(e, ln, 1, last, ev, src, dev, dev_maps))) return rc;
+    if ((rc = enqueue_pipeline(e, ln, 1, last, q.debug_stage >= 0, ev, src, dev, dev_maps))) return rc;
     if (disp) {
         CK(cudaMemcpyAsync(ln.pin_out, ln.w.disp_l, N * sizeof(float), cudaMemcpyDeviceToHost, ln.st));
         CK(cudaEventRecord(ev[6], ln.st));
@@ -1896,6 +1909,21 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                     return fail(ADC_ERR_UNSUPPORTED, "fused cost and horizontal arm sums not applicable");
                 bytes = V + 24 * N + (double)arm_line_rec(P.dm.W, P.dm.H, 1, 0) * arm_rec_words(P.L1) * 4.0;   // + horizontal records (all before the vertical axis's first)
                 break;
+            case 16:    // the -y pass fused with the WTA: volA's volumes in, disp_l and the right view's records into volB
+            case 17: {  // the records in volB folded into disp_r
+                const long long plane = so_wta_plane(P.dm.W, P.dm.H, P.dm.D, P.dm.Dp);
+                if (SO_WTA_FIELDS * plane > P.dm.vol_stride)
+                    return fail(ADC_ERR_UNSUPPORTED, "adc_profile_kernel: the WTA records do not fit in a pair's volume");
+                const double recs = 4.0 * SO_WTA_FIELDS * P.dm.H * (double)so_wta_row_records(P.dm.W, P.dm.D, P.dm.Dp, P.dm.dmin);
+                if (kernel_id == 16) {
+                    if (adc_launch_scanline_wta(P, w, w.volA, w.volB, ln.st, &e->launches)) return fail(ADC_ERR_UNSUPPORTED, "scanline");
+                    bytes = V + 6 * N + recs + 4 * N;
+                } else {
+                    adc_launch_wta_merge(P, w, w.volB, ln.st, &e->launches);
+                    bytes = recs + 4 * N;
+                }
+                break;
+            }
             default: return fail(ADC_ERR_ARG, "adc_profile_kernel: unknown kernel id %d", kernel_id);
         }
     }

@@ -188,11 +188,16 @@ __device__ __forceinline__ void tma_load_4d(unsigned dst, const CUtensorMap* map
                  : "memory");
 }
 
-template <int K, int LPS, bool FULL>   // FULL: D == LPS*K, every lane's K values are real disparities (no padding logic)
-__global__ void __launch_bounds__(SO_WARPS * 32, SO_MIN_CTAS)
-k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ CUtensorMap tm_rec, AdcParams P,
-           float* __restrict__ dst, int sx, int sy, int T, int NS) {
+// WTA: the last pass (-y) with the winner-takes-all as its epilogue (DESIGN.md 5.5).  It stores no volume: each warp
+// overwrites the costs of a step in its ring slot with the step's L, takes the left view's first minimum of each of its
+// columns from the registers, and once all warps of the CTA have finished a slot, the CTA reads the slot's rows along the
+// right view's diagonals and writes one partial record per (row, right pixel) to dst (so_plan.h).  The slot is refilled
+// only after that.
+template <int K, int LPS, bool FULL, bool WTA>   // FULL: D == LPS*K, every lane's K values are real disparities (no padding logic)
+__device__ __forceinline__ void so_pass(const CUtensorMap& tm_cost, const CUtensorMap& tm_rec, const AdcParams& P,
+                                        float* __restrict__ dst, float* __restrict__ disp_l, int sx, int sy, int T, int NS) {
     constexpr int LPW = 32 / LPS;               // lines per warp
+    if constexpr (WTA) { sx = 0; sy = -1; }
     extern __shared__ __align__(128) unsigned char so_smem[];
     const AdcDims& dm = P.dm;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -239,12 +244,12 @@ k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ 
     int c = 0, t = 0, slot = 0;
     unsigned phase = 0;
     const int bit0 = gl * K;   // first disparity of this lane inside the record's bit string
-    auto fetch = [&](float (&C)[K], bool& a1, unsigned& bits) {
+    auto fetch = [&](float (&C)[K], bool& a1, unsigned& bits) -> float* {   // returns the step's row of costs in the slot
         if (t == 0) mbar_wait(bar0 + 8u * (unsigned)slot, phase);
         const int pos = fwd ? t : T - 1 - t;
         const int row = sx ? sub * T + pos : pos * LPW + sub;   // box {Dp, T, LPW} or {Dp, LPW, T}
-        const unsigned char* sl = wring + (size_t)slot * slot_bytes;
-        const float* cs = reinterpret_cast<const float*>(sl) + row * Dp;
+        unsigned char* sl = wring + (size_t)slot * slot_bytes;
+        float* cs = reinterpret_cast<float*>(sl) + row * Dp;
         if constexpr (FULL && K == 8) {
             // a lane's eight costs are two 16-byte chunks 32 bytes apart: the lanes of a 128-bit load phase would hit four bank
             // groups twice, so lanes with (gl >> 2) & 1 read their second chunk first -- eight different bank groups per phase
@@ -258,7 +263,7 @@ k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ 
         const unsigned* rw = reinterpret_cast<const unsigned*>(sl + cost_region) + row * nrec;
         a1 = rw[0] != 0u;
         bits = __funnelshift_r(rw[1 + (bit0 >> 5)], rw[2 + (bit0 >> 5)], bit0 & 31);
-        if (++t == T) {
+        if (!WTA && ++t == T) {   // WTA: the slot is advanced by wta_advance, after the CTA has read it
             // Every lane has read the slot before it is refilled.  The refill is a write of the ASYNC proxy (the TMA engine),
             // the reads above went through the generic proxy: each lane orders its reads against that proxy before the
             // barrier (DESIGN.md 5.3: without the proxy fence pairs of a loaded GPU came out wrong).
@@ -269,22 +274,102 @@ k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ 
             c++;
             if (++slot == NS) { slot = 0; phase ^= 1u; }
         }
+        return cs;
     };
 
     bool valid[K];
 #pragma unroll
     for (int k = 0; k < K; k++) valid[k] = FULL || (gl * K + k) < D;
 
+    // ---- WTA epilogue (WTA only; step s of the pass is image row H - 1 - s)
+    // the CTA's warps that own columns: they alone take part in its barriers
+    const int wta_threads = 32 * min(SO_WARPS, (n_lines - (int)blockIdx.x * SO_WARPS * LPW + LPW - 1) / LPW);
+    // Left view of this group's column: the first minimum over d is the lowest d holding the group's minimum m (the
+    // reference's strict '>' scan from Large_Float, ADCensusStereo.cpp:209-222); its neighbours are read from the row.
+    auto wta_left = [&](const float* row, const float (&V)[K], float m, int step) {
+        int kk = K;
+#pragma unroll
+        for (int k = K - 1; k >= 0; k--)
+            if (valid[k] && V[k] == m) kk = k;
+        const unsigned bal = __ballot_sync(0xffffffffu, kk < K);
+        const unsigned grp = LPS == 32 ? bal : (bal >> (sub * LPS)) & ((1u << LPS) - 1u);
+        __syncwarp();   // the row's values stored by the other lanes
+        if (live && gl == __ffs(grp) - 1) {
+            const int bd = gl * K + kk;
+            float out = ADC_INVALID_F;   // a minimum at either end of the range (or none) is Invalid (:224-227)
+            if (m < ADC_LARGE_F && bd > 0 && bd < D - 1) out = adc_subpixel(row[bd - 1], row[bd + 1], m, dm.dmin + bd);
+            disp_l[(size_t)pair * dm.N + (size_t)(dm.H - 1 - step) * W + line] = out;
+        }
+    };
+    // Right view: cost_R(xr, d) = cost(xr + dmin + d, d).  For each step of the slot and each right pixel whose diagonal
+    // crosses the band, the first minimum over the diagonal's d-range inside the band, its in-range neighbours and the
+    // range's first and last cost (the fields of so_plan.h; k_wta_merge folds them).
+    auto wta_records = [&](int nt, int s0) {
+        constexpr int CB = SO_WARPS * LPW;   // band width
+        const int x0 = blockIdx.x * CB, NJ = CB + D - 1, nb = (W + CB - 1) / CB, dmin = dm.dmin;
+        const long long plane = (long long)dm.H * nb * NJ;
+        float* R = dst + (size_t)pair * dm.vol_stride;
+        const size_t wstride = (size_t)NS * slot_bytes / 4;   // floats between two warps' rings
+        const int xcap = W - 1 - x0;                           // the band's last column inside the image
+        for (int tt = 0; tt < nt; tt++) {
+            const int y = dm.H - 1 - (s0 + tt);
+            const float* rb = reinterpret_cast<const float*>(so_smem + (size_t)slot * slot_bytes) + (T - 1 - tt) * LPW * Dp;
+            for (int j = threadIdx.x; j < NJ; j += wta_threads) {
+                const int xr = x0 - dmin - (D - 1) + j;
+                const int ilo = max(0, j - (D - 1)), ihi = min(min(CB - 1, j), xcap);   // band columns on the diagonal
+                if (xr < 0 || xr >= W || ilo > ihi) continue;
+                const int dd0 = D - 1 - j;                                              // d of band column i: i + dd0
+                auto at = [&](int i) { return rb[(size_t)(i / LPW) * wstride + (i % LPW) * Dp + i + dd0]; };
+                float m = ADC_LARGE_F;
+                int a = -1;
+                const float* pw = rb + dd0;   // band column i = w * LPW + s sits at pw + w * (wstride + LPW) + s * (Dp + 1)
+#pragma unroll 1
+                for (int w = 0; w < SO_WARPS; w++, pw += wstride + LPW) {
+                    const float* p = pw;
+#pragma unroll
+                    for (int s = 0; s < LPW; s++, p += Dp + 1) {
+                        const int i = w * LPW + s;
+                        if (i >= ilo && i <= ihi) {
+                            const float v = *p;
+                            if (m > v) { m = v; a = i; }
+                        }
+                    }
+                }
+                const long long r = ((long long)y * nb + blockIdx.x) * NJ + j;
+                R[r] = m;
+                R[plane + r] = __int_as_float(a < 0 ? -1 : a + dd0);
+                R[2 * plane + r] = a > ilo ? at(a - 1) : ADC_LARGE_F;
+                R[3 * plane + r] = a >= 0 && a < ihi ? at(a + 1) : ADC_LARGE_F;
+                R[4 * plane + r] = at(ilo);
+                R[5 * plane + r] = at(ihi);
+            }
+        }
+    };
+    // after step `step`: at the end of a slot (or of the pass) the CTA takes the slot's records, then the slot is refilled
+    auto wta_advance = [&](int step) {
+        if (++t < T && step + 1 < n_steps) return;
+        asm volatile("bar.sync 1, %0;" ::"r"(wta_threads) : "memory");   // every warp's rows of the slot are stored
+        wta_records(t, step + 1 - t);
+        // the refill is a write of the async proxy after generic reads and writes of the slot (see fetch)
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        asm volatile("bar.sync 1, %0;" ::"r"(wta_threads) : "memory");   // nobody reads the slot any more
+        if (lane == 0 && c + NS < nch) issue(c + NS);
+        t = 0;
+        c++;
+        if (++slot == NS) { slot = 0; phase ^= 1u; }
+    };
+
     // the path head: L = C  (scanline_optimizer.cpp:99-100)
     long long pi = (long long)(sy ? (sy > 0 ? 0 : dm.H - 1) : line) * W + (sx ? (sx > 0 ? 0 : W - 1) : line);
     float* O = dst + (size_t)pair * dm.vol_stride;
     float L[K];
+    float* row;
     {
         bool a1;
         unsigned bits;
-        fetch(L, a1, bits);
+        row = fetch(L, a1, bits);
     }
-    if (live) st_vec<K>(O + (size_t)pi * Dp, gl, Dp, L);
+    if (!WTA && live) st_vec<K>(O + (size_t)pi * Dp, gl, Dp, L);
     float minL = ADC_LARGE_F;
 #pragma unroll
     for (int k = 0; k < K; k++) {
@@ -293,12 +378,16 @@ k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ 
     }
 #pragma unroll
     for (int o = LPS / 2; o >= 1; o >>= 1) minL = fminf(minL, __shfl_xor_sync(0xffffffffu, minL, o));
+    if constexpr (WTA) {   // the head's row in the slot holds L already
+        wta_left(row, L, minL, 0);
+        wta_advance(0);
+    }
 
     for (int step = 1; step < n_steps; step++) {
         float C[K];
         bool a1;
         unsigned bits;
-        fetch(C, a1, bits);
+        row = fetch(C, a1, bits);
         pi += pstep;
 
         const float up = __shfl_up_sync(0xffffffffu, L[K - 1], 1, LPS);
@@ -325,29 +414,56 @@ k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ 
             Ln[k] = v;
             if (valid[k]) mn = fminf(mn, v);
         }
-        if (live) st_vec<K>(O + (size_t)pi * Dp, gl, Dp, Ln);
+        if constexpr (WTA) {
+            if constexpr (FULL && K == 8) {   // the bank-group order of fetch's loads
+                const int b = (gl >> 2) & 1;
+                const float4 lo = make_float4(Ln[0], Ln[1], Ln[2], Ln[3]), hi = make_float4(Ln[4], Ln[5], Ln[6], Ln[7]);
+                *reinterpret_cast<float4*>(row + 8 * gl + 4 * b) = b ? hi : lo;
+                *reinterpret_cast<float4*>(row + 8 * gl + 4 - 4 * b) = b ? lo : hi;
+            } else st_vec<K>(row, gl, Dp, Ln);
+        } else if (live) st_vec<K>(O + (size_t)pi * Dp, gl, Dp, Ln);
 #pragma unroll
         for (int k = 0; k < K; k++) L[k] = valid[k] ? Ln[k] : ADC_LARGE_F;
 #pragma unroll
         for (int o = LPS / 2; o >= 1; o >>= 1) mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
         minL = mn;
+        if constexpr (WTA) {
+            wta_left(row, Ln, mn, step);
+            wta_advance(step);
+        }
     }
 }
 
 template <int K, int LPS, bool FULL>
+__global__ void __launch_bounds__(SO_WARPS * 32, SO_MIN_CTAS)
+k_scanline(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ CUtensorMap tm_rec, AdcParams P,
+           float* __restrict__ dst, int sx, int sy, int T, int NS) {
+    so_pass<K, LPS, FULL, false>(tm_cost, tm_rec, P, dst, nullptr, sx, sy, T, NS);
+}
+
+template <int K, int LPS, bool FULL>   // the -y pass; rec = the right view's records
+__global__ void __launch_bounds__(SO_WARPS * 32, SO_MIN_CTAS)
+k_scanline_wta(const __grid_constant__ CUtensorMap tm_cost, const __grid_constant__ CUtensorMap tm_rec, AdcParams P,
+               float* __restrict__ rec, float* __restrict__ disp_l, int T, int NS) {
+    so_pass<K, LPS, FULL, true>(tm_cost, tm_rec, P, rec, disp_l, 0, -1, T, NS);
+}
+
+template <int K, int LPS, bool FULL, bool WTA>
 static void launch_scanline_kf(const AdcParams& P, const AdcWave& w, const CUtensorMap& tc, const CUtensorMap& tr,
                                int T, int NS, size_t smem, float* dst, int sx, int sy, cudaStream_t st) {
     constexpr int LPW = 32 / LPS;
     const int n_lines = sx ? P.dm.H : P.dm.W;
+    const void* fn = WTA ? (const void*)k_scanline_wta<K, LPS, FULL> : (const void*)k_scanline<K, LPS, FULL>;
     static AdcOnce attr_once;
     if (adc_once_needed(attr_once)) {
-        cudaFuncSetAttribute(k_scanline<K, LPS, FULL>, cudaFuncAttributeMaxDynamicSharedMemorySize, SO_SMEM_MAX);
-        cudaFuncSetAttribute(k_scanline<K, LPS, FULL>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SO_SMEM_MAX);
+        cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         adc_once_done(attr_once);
     }
     const int lines_per_block = SO_WARPS * LPW;
     dim3 grid((n_lines + lines_per_block - 1) / lines_per_block, w.S);
-    k_scanline<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, sx, sy, T, NS);
+    if constexpr (WTA) k_scanline_wta<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, w.disp_l, T, NS);
+    else k_scanline<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, sx, sy, T, NS);
 }
 
 void adc_launch_so_bitrows(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
@@ -400,8 +516,9 @@ bool adc_so_tmaps_encode(const AdcParams& P, int S, float* volA, float* volB, un
     return true;
 }
 
-int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
-                        cudaStream_t st, unsigned long long* launches) {
+template <bool WTA>
+static int launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
+                           cudaStream_t st, unsigned long long* launches) {
     const int Dp = P.dm.Dp;
     if (Dp > 256 || !w.so_tm || (src != w.volA && src != w.volB)) return 1;   // D > 256 not supported; a source without a map
     const int axis = sx ? 0 : 1;
@@ -410,8 +527,8 @@ int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, 
     memcpy(&tr, w.so_tm->rec[axis], 128);
     const int T = w.so_tm->T[axis], NS = w.so_tm->NS[axis];
     const size_t smem = w.so_tm->smem[axis];
-#define SO_GO(KK, LL) (P.dm.D == KK * LL ? launch_scanline_kf<KK, LL, true>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st) \
-                                             : launch_scanline_kf<KK, LL, false>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st))
+#define SO_GO(KK, LL) (P.dm.D == KK * LL ? launch_scanline_kf<KK, LL, true, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st) \
+                                             : launch_scanline_kf<KK, LL, false, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st))
     switch (so_lanes_per_line(Dp)) {
         case 8:   // K = ceil(Dp / 8)
             switch ((Dp + 7) / 8) { case 1: SO_GO(1, 8); break; case 2: SO_GO(2, 8); break; case 3: SO_GO(3, 8); break; case 4: SO_GO(4, 8); break;
@@ -426,6 +543,16 @@ int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, 
 #undef SO_GO
     ++*launches;
     return 0;
+}
+
+int adc_launch_scanline(const AdcParams& P, const AdcWave& w, const float* src, float* dst, int sx, int sy,
+                        cudaStream_t st, unsigned long long* launches) {
+    return launch_scanline<false>(P, w, src, dst, sx, sy, st, launches);
+}
+
+int adc_launch_scanline_wta(const AdcParams& P, const AdcWave& w, const float* src, float* rec, cudaStream_t st,
+                            unsigned long long* launches) {
+    return launch_scanline<true>(P, w, src, rec, 0, -1, st, launches);
 }
 
 size_t adc_so_rec_bytes(const AdcDims& dm) { return (size_t)4 * dm.N * so_rec_words(dm.Dp) * 4; }   // four pass directions

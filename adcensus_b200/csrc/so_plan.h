@@ -55,3 +55,52 @@ inline SoPlan so_plan(int W, int H, int Dp, int S, int axis_y, int sm_count, siz
     }
     return best;
 }
+
+// ---- the last pass (-y) with the winner-takes-all as its epilogue (k_scanline_wta, k_wta_merge) ----------
+// A CTA of the y pass owns a band of so_wta_band columns.  Per row it writes disp_l and, for every right pixel xr whose
+// diagonal x = xr + dmin + d crosses the band, one partial record of the right view over that diagonal's d-range inside
+// the band (SO_WTA_FIELDS floats, field-major); k_wta_merge folds a right pixel's records in band order.
+#define SO_WTA_FIELDS 6     // minimum, first argmin (d, as int bits), cost at argmin-1 and argmin+1, at the range's first and last d
+SO_HD inline int so_wta_band(int Dp) { return SO_WARPS * (32 / so_lanes_per_line(Dp)); }
+// record slots of one band in one row: j = 0 .. band + D - 2 holds right pixel xr = x0 - dmin - (D - 1) + j
+SO_HD inline int so_wta_slots(int Dp, int D) { return so_wta_band(Dp) + D - 1; }
+// floats of one field plane of one pair: H rows x bands x slots
+inline long long so_wta_plane(int W, int H, int D, int Dp) {
+    const int c = so_wta_band(Dp);
+    return (long long)H * ((W + c - 1) / c) * so_wta_slots(Dp, D);
+}
+// records one row actually carries: slots whose right pixel lies in the image and whose diagonal meets a band column < W
+inline long long so_wta_row_records(int W, int D, int Dp, int dmin) {
+    const int c = so_wta_band(Dp);
+    long long n = 0;
+    for (int x0 = 0; x0 < W; x0 += c) {
+        const int lo = x0 - dmin - (D - 1) > 0 ? x0 - dmin - (D - 1) : 0;
+        const int xe = x0 + c < W ? x0 + c : W;
+        const int hi = xe - 1 - dmin < W - 1 ? xe - 1 - dmin : W - 1;
+        if (hi >= lo) n += hi - lo + 1;
+    }
+    return n;
+}
+
+// What else a run does with the optimised volume of pass 4, besides the winner-takes-all.
+struct SoVolumeUse {
+    bool opt_export;      // an ADC_VOL_OPT export
+    bool confidence;      // a MIN_COST or PEAK_RATIO map
+    bool discontinuity;   // the discontinuity adjustment (reads the volume at the end of the refinement)
+    bool debug_run;       // adc_debug_run*: it may stop at SO4, and adc_debug_get may tap the volume afterwards
+};
+enum SoWtaForce { SO_WTA_AUTO = 0, SO_WTA_NEVER = 1, SO_WTA_ALWAYS = 2 };   // ALWAYS: still only where the records fit
+
+// Whether pass 4 runs fused with the winner-takes-all.  The fused form never stores the optimised volume, so it needs
+// nobody to read it afterwards; its records take the volume's place in the pair's slice (vol_floats floats), so they must
+// fit there.  It replaces a volume store and the WTA's volume read (2V per pair) by the records written and read again; it
+// is taken where that traffic is at most half of 2V, i.e. where the band is wide against the disparity range (Cone,
+// D = 64 on 16 columns: 44 %; 1242 x 375 x 128 on 8 columns: 80 %; 1920 x 1080 x 192 on 4 columns: 152 %).
+inline bool so_wta_fused(const SoVolumeUse& use, int force, int W, int H, int D, int Dp, int dmin, long long vol_floats) {
+    if (use.opt_export || use.confidence || use.discontinuity || use.debug_run || force == SO_WTA_NEVER) return false;
+    if ((long long)SO_WTA_FIELDS * so_wta_plane(W, H, D, Dp) > vol_floats) return false;
+    if (force == SO_WTA_ALWAYS) return true;
+    const double traffic = 2.0 * SO_WTA_FIELDS * 4.0 * (double)so_wta_row_records(W, D, Dp, dmin);   // per row: written + read
+    const double staged = 2.0 * 4.0 * W * Dp;                                                         // per row: volume store + WTA read
+    return traffic <= 0.5 * staged;
+}

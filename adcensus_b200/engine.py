@@ -52,6 +52,7 @@ class _Config(ctypes.Structure):
 
 # adc_config.debug_flags (test hooks)
 DBG_NO_RAY_TABLE, DBG_VOTE_ENUM, DBG_VOTE_GLOBAL_STATE, DBG_UNFUSED_AGG, DBG_POISON = 1, 2, 4, 8, 16
+DBG_UNFUSED_SO_WTA, DBG_FUSED_SO_WTA = 32, 64
 
 
 def poison_flags(byte: int) -> int:
@@ -832,7 +833,7 @@ class Engine:
     PROFILE_KERNELS = {"cost_volume": 0, "arm_sum_h": 1, "arm_sum_v_div": 2, "scanline_x": 3, "scanline_y": 4, "wta": 5,
                        "arm_sum2_v": 6, "arm_sum2_h": 7, "arm_sum_h_div": 8, "arm_sum_v": 9, "cost_ingest": 10,
                        "cost_export": 11, "confidence": 12, "image_ingest": 13,
-                       "rectify": 14, "cost_arm_sum_h": 15}
+                       "rectify": 14, "cost_arm_sum_h": 15, "scanline_y_wta": 16, "wta_merge": 17}
 
     def profile_kernel(self, name: str, reps: int = 5):
         """(mean ms per launch over one wave, algorithmic bytes per launch) of one pipeline kernel."""

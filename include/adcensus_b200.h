@@ -82,6 +82,11 @@ enum {
     ADC_DBG_VOTE_ENUM = 2,        /* region voting finds the affected histograms by enumeration instead of adjacency lists */
     ADC_DBG_VOTE_GLOBAL_STATE = 4,/* region voting keeps its per-slot state in global instead of shared memory */
     ADC_DBG_UNFUSED_AGG = 8,      /* aggregation as eight single passes instead of five (three of them fused double passes) */
+    ADC_DBG_UNFUSED_SO_WTA = 32,  /* the last scanline pass stores the optimised volume and the WTA reads it back, also where
+                                     the pass would take the WTA as its epilogue */
+    ADC_DBG_FUSED_SO_WTA = 64,    /* the last scanline pass takes the WTA as its epilogue wherever nothing else reads the
+                                     optimised volume and its partial records fit in a pair's volume, also where the
+                                     records' traffic would not pay for it */
     ADC_DBG_POISON = 16           /* every byte of a lane's device arena is set to the pattern ADC_DBG_POISON_BYTE gives, on
                                      the lane's stream: at adc_create instead of zeros; at the start of every wave of a batch
                                      call, after the lane has joined the caller's stream and before the wave's inputs
@@ -713,7 +718,10 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * ADC_IMG_BGR if there was none, tight raw frames; needs a rectification set; per pair the bytes of both raw frames +
  * 2*3*N written, plus both views' internal maps, 2*8*N, once per wave), 15 = the AD-census cost computed inside the first
  * horizontal arm sum, which the fused pipeline runs in place of ids 0 and 1 (per pair one volume written, 24*N bytes of
- * packed pixels and census words read, plus the horizontal window records).
+ * packed pixels and census words read, plus the horizontal window records), 16 = the scanline pass along -y with the WTA
+ * as its epilogue, which the pipeline runs in place of ids 4 and 5 where nothing else reads the optimised volume (per pair
+ * one volume read, disp_l and the right view's partial records written), 17 = the fold of those records into the
+ * right-view map (records read, disp_r written).
  * algorithmic_bytes (optional) receives the bytes one launch must move (SURVEY.md section 8d). */
 int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* avg_ms, double* algorithmic_bytes);
 
