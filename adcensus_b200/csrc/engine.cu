@@ -555,6 +555,20 @@ int drain_lane(adc_engine* e, Lane& ln) {
     return ADC_OK;
 }
 
+// n pairs of views at left / right (pair i at byte i * g.image_stride; geometry g, resolved, over the raw frames of
+// `rect` or the engine's size) -> `bgr` as packed BGR [n][2][N*3] on st: a plain or rectified ingestion launch per
+// 65535 pairs (k_image_ingest's blockIdx.z is the pair).
+void ingest_views(adc_engine* e, int n, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                  const AdcRectGeom* rect, uint8_t* bgr, cudaStream_t st) {
+    for (int first = 0; first < n; first += 65535) {
+        const int count = std::min(n - first, 65535);
+        const long long off = (long long)first * g.image_stride;
+        uint8_t* out = bgr + (size_t)first * 6 * e->P.dm.N;
+        if (rect) adc_launch_rectify_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
+        else adc_launch_image_ingest(e->P.dm, count, left + off, right + off, g, out, st, &e->launches);
+    }
+}
+
 enum SrcKind { SRC_HOST_PTRS, SRC_HOST_STRIDED, SRC_DEVICE_STRIDED };
 
 // Where the pairs of a batch live: strided views and maps (ls / rs / ds, pair i at i times a tight pair's size, or at
@@ -597,10 +611,7 @@ int run_batch(adc_engine* e, int n, const BatchIO& io, const MatchReq& q, cudaSt
         // ---- inputs -> w.bgr  ([S][2][IMG])
         if (ingest) {
             const long long off = (long long)first * q.img->image_stride;
-            if (q.rect)
-                adc_launch_rectify_ingest(e->P.dm, nS, io.ls + off, io.rs + off, *q.img, *q.rect, w.bgr, ln.st, &e->launches);
-            else
-                adc_launch_image_ingest(e->P.dm, nS, io.ls + off, io.rs + off, *q.img, w.bgr, ln.st, &e->launches);
+            ingest_views(e, nS, io.ls + off, io.rs + off, *q.img, q.rect, w.bgr, ln.st);
         } else if (strided_copy) {
             const cudaMemcpyKind k = on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
             CK(cudaMemcpy2DAsync(w.bgr, 2 * IMG, io.ls + (size_t)first * IMG, IMG, IMG, nS, k, ln.st));
@@ -820,10 +831,15 @@ int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, 
     return ADC_OK;
 }
 
-// Makes the device staging of the host entries (e->vol_stage) at least `need` bytes: freed and re-allocated when it is
-// smaller, ADC_ERR_NOMEM if that fails.  With ADC_DBG_POISON the whole staging is filled with the pattern on lane 0's
-// stream, which every caller (a one-pair host call) works on.
-int grow_stage(adc_engine* e, const char* fn, size_t need, const char* what) {
+// Lays out the device staging of a one-pair host call (e->vol_stage): `carve` takes the call's parts from a Carver, first
+// to size them, then to point them into the staging, which is freed and re-allocated when it is smaller (ADC_ERR_NOMEM
+// if that fails).  With ADC_DBG_POISON the whole staging is filled with the pattern on lane 0's stream, which every
+// caller (a one-pair host call) works on.
+template <typename Carve>
+int grow_stage(adc_engine* e, const char* fn, const char* what, Carve carve) {
+    Carver sizing(nullptr);
+    carve(sizing);
+    const size_t need = sizing.off;
     if (need > e->vol_stage_bytes) {
         if (e->vol_stage) CK(cudaFree(e->vol_stage));
         e->vol_stage = nullptr;
@@ -836,6 +852,8 @@ int grow_stage(adc_engine* e, const char* fn, size_t need, const char* what) {
         e->vol_stage_bytes = need;
     }
     if (poisoned(e) && e->vol_stage) CK(cudaMemsetAsync(e->vol_stage, poison_byte(e), e->vol_stage_bytes, e->lanes[0].st));
+    Carver parts(e->vol_stage);
+    carve(parts);
     return ADC_OK;
 }
 
@@ -849,22 +867,17 @@ int idle_lane0(adc_engine* e) {
     return ADC_OK;
 }
 
-// The frame size of a request's views: the raw frames' with a rectification, else the engine's.
-int view_w(const adc_engine* e, const MatchReq& q) { return q.rect ? q.rect->src_w : e->W; }
-int view_h(const adc_engine* e, const MatchReq& q) { return q.rect ? q.rect->src_h : e->H; }
-
-// Bytes of one pair's views of an ingesting request, uploaded tightly (upload_pair).
-size_t staged_bytes(const adc_engine* e, const MatchReq& q) {
-    return 2 * (size_t)adc_image_tight(q.img->format, view_w(e, q), view_h(e, q)).image_stride;
+// The tight geometry of a view of `format`: over the raw frames of `rect`, or the engine's size without one.
+AdcImageGeom tight_view(const adc_engine* e, int format, const AdcRectGeom* rect) {
+    return rect ? adc_image_tight(format, rect->src_w, rect->src_h) : adc_image_tight(format, e->W, e->H);
 }
 
-// One pair's host views (geometry g, resolved, over the raw frames of `rect` or the engine's size) -> `bgr` as packed
-// BGR [2][N*3] on st: the views are uploaded tightly, view after view, to `raw` (2 * the tight footprint) and converted
-// from there by one (rectified) ingestion launch.
+// One pair's host views (geometry g, resolved) -> `bgr` as packed BGR [2][N*3] on st: the views are uploaded tightly,
+// view after view, to `raw` (2 * the tight footprint) and converted from there by ingest_views.
 int ingest_host_pair(adc_engine* e, const AdcImageGeom& g, const AdcRectGeom* rect, const uint8_t* left,
                      const uint8_t* right, uint8_t* raw, uint8_t* bgr, cudaStream_t st) {
     const size_t sh = rect ? rect->src_h : e->H;
-    const AdcImageGeom tight = adc_image_tight(g.format, rect ? rect->src_w : e->W, sh);
+    const AdcImageGeom tight = tight_view(e, g.format, rect);
     const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
     // one block of tight rows per plane
     for (int v = 0; v < 2; v++)
@@ -872,10 +885,7 @@ int ingest_host_pair(adc_engine* e, const AdcImageGeom& g, const AdcRectGeom* re
             CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
                                  (size_t)g.row_pitch, tp, (size_t)img_plane_rows(g.format, c, sh), cudaMemcpyHostToDevice,
                                  st));
-    if (rect)
-        adc_launch_rectify_ingest(e->P.dm, 1, raw, raw + foot, tight, *rect, bgr, st, &e->launches);
-    else
-        adc_launch_image_ingest(e->P.dm, 1, raw, raw + foot, tight, bgr, st, &e->launches);
+    ingest_views(e, 1, raw, raw + foot, tight, rect, bgr, st);
     return ADC_OK;
 }
 
@@ -924,29 +934,22 @@ int match_host(adc_engine* e, const char* fn, const MatchReq& q, const uint8_t* 
     note_formats(e, q);
     const int last = last_stage(q);
     const size_t N = (size_t)e->P.dm.N, ND = N * e->P.dm.D;
-    size_t need = 0;
-    for (int i = 0; i < q.n_vols; i++) need += align_up(ND * adc_cost_elem_bytes(q.vols[i].dtype), 256);
-    for (int i = 0; i < q.n_maps; i++) need += align_up(N * map_elem_bytes(q.maps[i].kind), 256);
     const bool ingest = needs_ingest(e, q, true);
-    const size_t raw_bytes = ingest ? staged_bytes(e, q) : 0;
+    const size_t raw_bytes = ingest ? 2 * (size_t)tight_view(e, q.img->format, q.rect).image_stride : 0;
     const bool raw_in_volume = raw_bytes <= (size_t)e->S * e->P.dm.vol_stride * sizeof(float);
-    if (!raw_in_volume) need += raw_bytes;
-    if ((rc = grow_stage(e, fn, need, "the exported volumes and maps"))) return rc;
-    char* stage = static_cast<char*>(e->vol_stage);
     VolOuts dev;
     dev.n = q.n_vols;
-    for (int i = 0; i < q.n_vols; i++) {
-        dev.o[i] = q.vols[i];
-        dev.o[i].dst = stage;
-        stage += align_up(ND * adc_cost_elem_bytes(q.vols[i].dtype), 256);
-    }
     MapOuts dev_maps;
-    for (int i = 0; i < q.n_maps; i++) {
-        dev_maps.dst[q.maps[i].kind] = stage;
-        stage += align_up(N * map_elem_bytes(q.maps[i].kind), 256);
-    }
-    uint8_t* raw = !ingest ? nullptr : raw_in_volume ? reinterpret_cast<uint8_t*>(lane_volumes(e, ln.w, last).c0)
-                                                     : reinterpret_cast<uint8_t*>(stage);
+    uint8_t* raw = ingest && raw_in_volume ? reinterpret_cast<uint8_t*>(lane_volumes(e, ln.w, last).c0) : nullptr;
+    rc = grow_stage(e, fn, "the exported volumes and maps", [&](Carver& c) {
+        for (int i = 0; i < q.n_vols; i++) {
+            dev.o[i] = q.vols[i];
+            dev.o[i].dst = c.take<char>(ND * adc_cost_elem_bytes(q.vols[i].dtype));
+        }
+        for (int i = 0; i < q.n_maps; i++) dev_maps.dst[q.maps[i].kind] = c.take<char>(N * map_elem_bytes(q.maps[i].kind));
+        if (!raw_in_volume) raw = c.take<uint8_t>(raw_bytes);
+    });
+    if (rc) return rc;
     if (poisoned(e) && (rc = fill_arena(e, ln))) return rc;
     cudaEvent_t* ev = disp ? e->ev_stage : nullptr;
     CostSrc src;
@@ -1007,16 +1010,21 @@ int check_reproject_args(const char* fn, int n, const float* disp, const double*
     return ADC_OK;
 }
 
-// The DISP_S16 value of a +inf pixel: (min_disparity - 1) * 16 saturated to int16.
-int16_t reproj_s16_invalid(const adc_engine* e) {
-    const long long v = ((long long)e->opt.min_disparity - 1) * 16;
-    return (int16_t)std::min(32767ll, std::max(-32768ll, v));
-}
-
 AdcReprojQ reproj_q(const double* Q) {
     AdcReprojQ q;
     memcpy(q.q, Q, sizeof(q.q));
     return q;
+}
+
+// Reprojects n maps at device address disp into the device outputs `o` on st.  A +inf pixel's DISP_S16 value is
+// (min_disparity - 1) * 16 saturated to int16.
+int reproject_enqueue(adc_engine* e, long long n, const float* disp, const double* Q, const ReprojOuts& o, cudaStream_t st) {
+    const long long s16_invalid = std::min(32767ll, std::max(-32768ll, ((long long)e->opt.min_disparity - 1) * 16));
+    adc_launch_reproject(e->P.dm, n, disp, reproj_q(Q), static_cast<float*>(o.dst[ADC_REPROJ_POINTS]),
+                         static_cast<float*>(o.dst[ADC_REPROJ_DEPTH]), static_cast<int16_t*>(o.dst[ADC_REPROJ_DISP_S16]),
+                         (int16_t)s16_invalid, st, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
 }
 
 // cvRound on x86 (cvtsd2si): round half to even, INT_MIN for NaN and for anything outside int32.
@@ -1054,14 +1062,17 @@ int check_speckle_args(const char* fn, int n, const void* maps, const adc_speckl
     return ADC_OK;
 }
 
-AdcSpeckle speckle_rules(const adc_speckle_params& p) {
+// Filters n maps at device address maps in place on st, with the workspace at device address work.
+int speckles_enqueue(adc_engine* e, long long n, void* maps, void* work, const adc_speckle_params& p, cudaStream_t st) {
     AdcSpeckle s;
     s.nv_i = cv_round(p.new_val);
     s.md_i = cv_round(p.max_diff);
     s.nv_f = (float)p.new_val;
     s.md_f = p.type == ADC_SPECKLE_F32 ? float_at_most(p.max_diff) : 0.0f;
     s.max_size = p.max_size;
-    return s;
+    adc_launch_speckles(e->P.dm, n, p.type == ADC_SPECKLE_F32, maps, work, s, st, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
 }
 
 size_t speckle_work_bytes(const adc_engine* e, long long n) { return 8 * (size_t)n * (size_t)e->P.dm.N; }
@@ -1113,6 +1124,18 @@ int check_cloud_args(const char* fn, int n, const float* disp, const double* Q, 
 int check_cloud_capacity(const adc_engine* e, const char* fn, const adc_cloud_out* o) {
     if (o->capacity > e->P.dm.N)
         return fail(ADC_ERR_ARG, "%s: out->capacity %lld is above H * W (%d)", fn, (long long)o->capacity, e->P.dm.N);
+    return ADC_OK;
+}
+
+// The point clouds of n maps at device address disp into the device outputs `o` on st: zeroes the workspace `work`,
+// then one launch.  bgr_stride 0 = tight images (3 * N bytes apart).
+int cloud_enqueue(adc_engine* e, long long n, const float* disp, const double* Q, const uint8_t* bgr, long long bgr_stride,
+                  float z_min, float z_max, const adc_cloud_out& o, void* work, cudaStream_t st) {
+    CK(cudaMemsetAsync(work, 0, adc_point_cloud_work_bytes(e->P.dm, n), st));
+    adc_launch_point_cloud(e->P.dm, n, disp, reproj_q(Q), bgr, bgr_stride ? bgr_stride : 3ll * e->P.dm.N, z_min, z_max,
+                           AdcCloudOut{o.points, o.colors, o.pixels, o.counts, (long long)o.capacity}, work, st,
+                           &e->launches);
+    CK(cudaGetLastError());
     return ADC_OK;
 }
 
@@ -1543,11 +1566,7 @@ int adc_reproject_batch_device(adc_engine* e, int32_t n, const float* d_disp, co
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if (n == 0) return ADC_OK;
     CK(cudaSetDevice(e->cfg.device));
-    adc_launch_reproject(e->P.dm, n, d_disp, reproj_q(Q), static_cast<float*>(o.dst[ADC_REPROJ_POINTS]),
-                         static_cast<float*>(o.dst[ADC_REPROJ_DEPTH]), static_cast<int16_t*>(o.dst[ADC_REPROJ_DISP_S16]),
-                         reproj_s16_invalid(e), (cudaStream_t)stream, &e->launches);
-    CK(cudaGetLastError());
-    return ADC_OK;
+    return reproject_enqueue(e, n, d_disp, Q, o, (cudaStream_t)stream);
 }
 
 int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const adc_reproject_out* outs, int32_t n_outs) {
@@ -1558,24 +1577,18 @@ int adc_reproject(adc_engine* e, const float* disp, const double Q[16], const ad
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if ((rc = idle_lane0(e))) return rc;
     Lane& ln = e->lanes[0];
-    // staging: the map, then each requested output, 256-byte aligned
     const size_t N = (size_t)e->P.dm.N;
-    size_t off[3] = {0, 0, 0}, need = align_up(N * sizeof(float), 256);
+    float* d_disp = nullptr;
+    ReprojOuts d;
+    rc = grow_stage(e, fn, "the disparity map and its reprojection", [&](Carver& c) {
+        d_disp = c.take<float>(N);
+        for (int k = 0; k < 3; k++) d.dst[k] = o.dst[k] ? c.take<char>(N * reproj_elem_bytes(k)) : nullptr;
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_disp, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
+    if ((rc = reproject_enqueue(e, 1, d_disp, Q, d, ln.st))) return rc;
     for (int k = 0; k < 3; k++)
-        if (o.dst[k]) {
-            off[k] = need;
-            need += align_up(N * reproj_elem_bytes(k), 256);
-        }
-    if ((rc = grow_stage(e, fn, need, "the disparity map and its reprojection"))) return rc;
-    char* stage = static_cast<char*>(e->vol_stage);
-    CK(cudaMemcpyAsync(stage, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
-    adc_launch_reproject(e->P.dm, 1, reinterpret_cast<const float*>(stage), reproj_q(Q),
-                         o.dst[ADC_REPROJ_POINTS] ? reinterpret_cast<float*>(stage + off[ADC_REPROJ_POINTS]) : nullptr,
-                         o.dst[ADC_REPROJ_DEPTH] ? reinterpret_cast<float*>(stage + off[ADC_REPROJ_DEPTH]) : nullptr,
-                         o.dst[ADC_REPROJ_DISP_S16] ? reinterpret_cast<int16_t*>(stage + off[ADC_REPROJ_DISP_S16]) : nullptr,
-                         reproj_s16_invalid(e), ln.st, &e->launches);
-    for (int k = 0; k < 3; k++)
-        if (o.dst[k]) CK(cudaMemcpyAsync(o.dst[k], stage + off[k], N * reproj_elem_bytes(k), cudaMemcpyDeviceToHost, ln.st));
+        if (o.dst[k]) CK(cudaMemcpyAsync(o.dst[k], d.dst[k], N * reproj_elem_bytes(k), cudaMemcpyDeviceToHost, ln.st));
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
     return ADC_OK;
@@ -1601,10 +1614,7 @@ int adc_filter_speckles_batch_device(adc_engine* e, int32_t n, void* d_maps, con
     if (n == 0) return ADC_OK;
     if (!d_work) return fail(ADC_ERR_ARG, "%s: work is NULL", fn);
     CK(cudaSetDevice(e->cfg.device));
-    adc_launch_speckles(e->P.dm, n, params->type == ADC_SPECKLE_F32, d_maps, d_work, speckle_rules(*params),
-                        (cudaStream_t)stream, &e->launches);
-    CK(cudaGetLastError());
-    return ADC_OK;
+    return speckles_enqueue(e, n, d_maps, d_work, *params, (cudaStream_t)stream);
 }
 
 int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* params) {
@@ -1614,14 +1624,16 @@ int adc_filter_speckles(adc_engine* e, void* map, const adc_speckle_params* para
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     if ((rc = idle_lane0(e))) return rc;
     Lane& ln = e->lanes[0];
-    // staging: the workspace, then the map
-    const size_t bytes = (size_t)e->P.dm.N * speckle_elem_bytes(params->type), off = align_up(speckle_work_bytes(e, 1), 256);
-    if ((rc = grow_stage(e, fn, off + bytes, "the map and its speckle workspace"))) return rc;
-    char* stage = static_cast<char*>(e->vol_stage);
-    CK(cudaMemcpyAsync(stage + off, map, bytes, cudaMemcpyHostToDevice, ln.st));
-    adc_launch_speckles(e->P.dm, 1, params->type == ADC_SPECKLE_F32, stage + off, stage, speckle_rules(*params), ln.st,
-                        &e->launches);
-    CK(cudaMemcpyAsync(map, stage + off, bytes, cudaMemcpyDeviceToHost, ln.st));
+    const size_t bytes = (size_t)e->P.dm.N * speckle_elem_bytes(params->type);
+    char *work = nullptr, *d_map = nullptr;
+    rc = grow_stage(e, fn, "the map and its speckle workspace", [&](Carver& c) {
+        work = c.take<char>(speckle_work_bytes(e, 1));
+        d_map = c.take<char>(bytes);
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_map, map, bytes, cudaMemcpyHostToDevice, ln.st));
+    if ((rc = speckles_enqueue(e, 1, d_map, work, *params, ln.st))) return rc;
+    CK(cudaMemcpyAsync(map, d_map, bytes, cudaMemcpyDeviceToHost, ln.st));
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
     return ADC_OK;
@@ -1640,16 +1652,7 @@ int adc_ingest_views_batch_device(adc_engine* e, int32_t n, const uint8_t* d_lef
     if ((rc = resolve_views(e, fn, img, rectified, n, &g, &r))) return rc;
     if (n == 0) return ADC_OK;
     CK(cudaSetDevice(e->cfg.device));
-    const size_t pair_bytes = 6 * (size_t)e->P.dm.N;
-    for (int first = 0; first < n; first += 65535) {   // k_image_ingest's blockIdx.z is the pair
-        const int count = std::min(n - first, 65535);
-        const long long off = (long long)first * g.image_stride;
-        uint8_t* out = d_views + (size_t)first * pair_bytes;
-        if (rectified)
-            adc_launch_rectify_ingest(e->P.dm, count, d_left + off, d_right + off, g, r, out, (cudaStream_t)stream, &e->launches);
-        else
-            adc_launch_image_ingest(e->P.dm, count, d_left + off, d_right + off, g, out, (cudaStream_t)stream, &e->launches);
-    }
+    ingest_views(e, n, d_left, d_right, g, rectified ? &r : nullptr, d_views, (cudaStream_t)stream);
     CK(cudaGetLastError());
     return ADC_OK;
 }
@@ -1666,13 +1669,15 @@ int adc_ingest_views(adc_engine* e, const uint8_t* left, const uint8_t* right, c
     if ((rc = resolve_views(e, fn, img, rectified, 1, &g, &r))) return rc;
     if ((rc = idle_lane0(e))) return rc;
     Lane& ln = e->lanes[0];
-    // staging: the views, then the raw frames uploaded tightly
-    const size_t out_bytes = 6 * (size_t)e->P.dm.N, off = align_up(out_bytes, 256);
-    const AdcImageGeom tight = rectified ? adc_image_tight(g.format, r.src_w, r.src_h) : adc_image_tight(g.format, e->W, e->H);
-    if ((rc = grow_stage(e, fn, off + 2 * (size_t)tight.image_stride, "the raw views and the packed BGR views"))) return rc;
-    uint8_t* stage = static_cast<uint8_t*>(e->vol_stage);
-    if ((rc = ingest_host_pair(e, g, rectified ? &r : nullptr, left, right, stage + off, stage, ln.st))) return rc;
-    CK(cudaMemcpyAsync(views, stage, out_bytes, cudaMemcpyDeviceToHost, ln.st));
+    const AdcRectGeom* rect = rectified ? &r : nullptr;
+    const size_t out_bytes = 6 * (size_t)e->P.dm.N;
+    uint8_t *d_views = nullptr, *raw = nullptr;
+    rc = grow_stage(e, fn, "the raw views and the packed BGR views", [&](Carver& c) {
+        d_views = c.take<uint8_t>(out_bytes);
+        raw = c.take<uint8_t>(2 * (size_t)tight_view(e, g.format, rect).image_stride);
+    });
+    if (rc || (rc = ingest_host_pair(e, g, rect, left, right, raw, d_views, ln.st))) return rc;
+    CK(cudaMemcpyAsync(views, d_views, out_bytes, cudaMemcpyDeviceToHost, ln.st));
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
     return ADC_OK;
@@ -1700,13 +1705,7 @@ int adc_point_cloud_batch_device(adc_engine* e, int32_t n, const float* d_disp, 
     if (n == 0) return ADC_OK;
     if (!d_work) return fail(ADC_ERR_ARG, "%s: work is NULL", fn);
     CK(cudaSetDevice(e->cfg.device));
-    const cudaStream_t st = (cudaStream_t)stream;
-    CK(cudaMemsetAsync(d_work, 0, need, st));
-    const AdcCloudOut o{out->points, out->colors, out->pixels, out->counts, (long long)out->capacity};
-    adc_launch_point_cloud(e->P.dm, n, d_disp, reproj_q(Q), d_bgr, bgr_stride ? (long long)bgr_stride : 3ll * e->P.dm.N,
-                           z_min, z_max, o, d_work, st, &e->launches);
-    CK(cudaGetLastError());
-    return ADC_OK;
+    return cloud_enqueue(e, n, d_disp, Q, d_bgr, bgr_stride, z_min, z_max, *out, d_work, (cudaStream_t)stream);
 }
 
 int adc_point_cloud(adc_engine* e, const float* disp, const double Q[16], const uint8_t* bgr, float z_min, float z_max,
@@ -1718,26 +1717,24 @@ int adc_point_cloud(adc_engine* e, const float* disp, const double Q[16], const 
     if ((rc = check_cloud_capacity(e, fn, out))) return rc;
     if ((rc = idle_lane0(e))) return rc;
     Lane& ln = e->lanes[0];
-    // staging, each part 256-byte aligned: workspace, map, image, points, colours, pixel indices, count
     const size_t N = (size_t)e->P.dm.N, cap = (size_t)out->capacity;
-    const size_t sizes[7] = {adc_point_cloud_work_bytes(e->P.dm, 1), N * sizeof(float), bgr ? 3 * N : 0,
-                             12 * cap, out->colors ? 3 * cap : 0, out->pixels ? 4 * cap : 0, sizeof(int32_t)};
-    size_t off[7], need = 0;
-    for (int i = 0; i < 7; i++) {
-        off[i] = need;
-        need += align_up(sizes[i], 256);
-    }
-    if ((rc = grow_stage(e, fn, need, "the map, its image and its point cloud"))) return rc;
-    char* stage = static_cast<char*>(e->vol_stage);
-    CK(cudaMemcpyAsync(stage + off[1], disp, sizes[1], cudaMemcpyHostToDevice, ln.st));
-    if (bgr) CK(cudaMemcpyAsync(stage + off[2], bgr, sizes[2], cudaMemcpyHostToDevice, ln.st));
-    CK(cudaMemsetAsync(stage, 0, sizes[0], ln.st));
-    const AdcCloudOut o{reinterpret_cast<float*>(stage + off[3]), out->colors ? reinterpret_cast<uint8_t*>(stage + off[4]) : nullptr,
-                        out->pixels ? reinterpret_cast<int32_t*>(stage + off[5]) : nullptr,
-                        reinterpret_cast<int32_t*>(stage + off[6]), (long long)cap};
-    adc_launch_point_cloud(e->P.dm, 1, reinterpret_cast<const float*>(stage + off[1]), reproj_q(Q),
-                           bgr ? reinterpret_cast<const uint8_t*>(stage + off[2]) : nullptr, 3ll * e->P.dm.N, z_min, z_max,
-                           o, stage, ln.st, &e->launches);
+    void* work = nullptr;
+    float* d_disp = nullptr;
+    uint8_t* d_bgr = nullptr;
+    adc_cloud_out o = *out;
+    rc = grow_stage(e, fn, "the map, its image and its point cloud", [&](Carver& c) {
+        work = c.take<char>(adc_point_cloud_work_bytes(e->P.dm, 1));
+        d_disp = c.take<float>(N);
+        d_bgr = bgr ? c.take<uint8_t>(3 * N) : nullptr;
+        o.points = c.take<float>(3 * cap);
+        o.colors = out->colors ? c.take<uint8_t>(3 * cap) : nullptr;
+        o.pixels = out->pixels ? c.take<int32_t>(cap) : nullptr;
+        o.counts = c.take<int32_t>(1);
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_disp, disp, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
+    if (bgr) CK(cudaMemcpyAsync(d_bgr, bgr, 3 * N, cudaMemcpyHostToDevice, ln.st));
+    if ((rc = cloud_enqueue(e, 1, d_disp, Q, d_bgr, 0, z_min, z_max, o, work, ln.st))) return rc;
     CK(cudaMemcpyAsync(out->counts, o.counts, sizeof(int32_t), cudaMemcpyDeviceToHost, ln.st));
     CK(cudaStreamSynchronize(ln.st));
     CK(cudaGetLastError());
@@ -1887,7 +1884,7 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 const long long foot = g.image_stride;
                 g.image_stride = 2 * foot;
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
-                adc_launch_image_ingest(P.dm, w.S, src, src + foot, g, w.bgr, ln.st, &e->launches);
+                ingest_views(e, w.S, src, src + foot, g, nullptr, w.bgr, ln.st);
                 bytes = 2.0 * adc_image_read_bytes(e->img_format, P.dm.W, P.dm.H) + 2 * 3.0 * N;
                 break;
             }
@@ -1900,7 +1897,7 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 g.image_stride = 2 * foot;
                 const AdcRectGeom rg{{e->rect_map, e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h};
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
-                adc_launch_rectify_ingest(P.dm, w.S, src, src + foot, g, rg, w.bgr, ln.st, &e->launches);
+                ingest_views(e, w.S, src, src + foot, g, &rg, w.bgr, ln.st);
                 bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
                 break;
             }
