@@ -107,7 +107,8 @@ struct adc_engine {
     cudaEvent_t ev_stage[8] = {};
     // debug state (adc_debug_run): which buffer plays the reference's cost_init_ / cost_aggr_
     const float* dbg_init = nullptr;
-    const float* dbg_aggr = nullptr;
+    const float* dbg_aggr = nullptr;   // nullptr also after a run whose last scanline pass took the WTA (dbg_so_wta)
+    bool dbg_so_wta = false;           // the last run's pass 4 stored partial WTA records, not the optimised volume
     int dbg_stage = -1;
     // layout / element type of the last cost-input call (adc_profile_kernel's ingestion timing)
     int cost_layout = ADC_COST_DHW, cost_dtype = ADC_COST_F32;
@@ -404,6 +405,7 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, bool debug
     for (int i = 0; i < outs.n; i++) cost_exported |= outs.o[i].stage == ADC_VOL_COST;
     e->dbg_init = cost_in_agg && !cost_exported ? nullptr : C0;   // no tap of a cost volume that was never written
     e->dbg_aggr = C0;
+    e->dbg_so_wta = false;
     auto stop = [&](int stage) { e->dbg_stage = stage; return stage >= last_stage; };
     // launch errors surface where they happen: a stage boundary reports the first failed launch since the previous one
     auto launched = [&](const char* what) -> int {
@@ -480,7 +482,8 @@ int enqueue_pipeline(adc_engine* e, Lane& ln, int nS, int last_stage, bool debug
         if (ps == 3 && so_wta ? adc_launch_scanline_wta(P, w, src, dst, st, L)
                               : adc_launch_scanline(P, w, src, dst, dirs[ps][0], dirs[ps][1], st, L))
             return fail(ADC_ERR_UNSUPPORTED, "scanline pass not launched (disparity range %d, limit 256)", P.dm.D);
-        if (ps % 2 == 0) e->dbg_init = B; else e->dbg_aggr = A;
+        if (ps % 2 == 0) e->dbg_init = B; else e->dbg_aggr = ps == 3 && so_wta ? nullptr : A;   // the fused pass leaves records in A
+        if (ps == 3) e->dbg_so_wta = so_wta;
         if (ps == 3) export_vol(ADC_VOL_OPT, A);
         if (stop(ADC_STAGE_SO1 + ps)) return launched("scanline optimisation");
     }
@@ -1990,7 +1993,11 @@ size_t adc_debug_get(adc_engine* e, int32_t tap, void* dst, size_t cap) {
             const float* v = tap == ADC_TAP_VOL_INIT ? e->dbg_init : e->dbg_aggr;
             bytes = N * dm.D * sizeof(float);
             if (dst && cap >= bytes && !v) {
-                fail(ADC_ERR_ARG, "adc_debug_get: no such volume: no run yet, or the last run computed the cost inside the aggregation");
+                if (tap == ADC_TAP_VOL_AGGR && e->dbg_so_wta)
+                    fail(ADC_ERR_ARG, "adc_debug_get: no such volume: the last run's final scanline pass took the WTA as its "
+                                      "epilogue (fused scanline + WTA) and stored no optimised volume");
+                else
+                    fail(ADC_ERR_ARG, "adc_debug_get: no such volume: no run yet, or the last run computed the cost inside the aggregation");
                 return 0;
             }
             if (!dst || cap < bytes || !v) return bytes;

@@ -448,22 +448,35 @@ k_scanline_wta(const __grid_constant__ CUtensorMap tm_cost, const __grid_constan
     so_pass<K, LPS, FULL, true>(tm_cost, tm_rec, P, rec, disp_l, 0, -1, T, NS);
 }
 
+// The fused pass exists only where its records can fit a pair's volume for some shape adc_create accepts
+// (so_wta_fused): never with 32 lanes per line (a band of 4 columns), nor at D = 8 (K = 1, FULL).
+// tests/test_fused_wta_parity.py derives that set over the whole domain and compares it with the library's kernels.
+template <int K, int LPS, bool FULL>
+constexpr bool so_wta_built() { return LPS != 32 && !(K == 1 && FULL); }
+
 template <int K, int LPS, bool FULL, bool WTA>
-static void launch_scanline_kf(const AdcParams& P, const AdcWave& w, const CUtensorMap& tc, const CUtensorMap& tr,
-                               int T, int NS, size_t smem, float* dst, int sx, int sy, cudaStream_t st) {
-    constexpr int LPW = 32 / LPS;
-    const int n_lines = sx ? P.dm.H : P.dm.W;
-    const void* fn = WTA ? (const void*)k_scanline_wta<K, LPS, FULL> : (const void*)k_scanline<K, LPS, FULL>;
-    static AdcOnce attr_once;
-    if (adc_once_needed(attr_once)) {
-        cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SO_SMEM_MAX);
-        cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-        adc_once_done(attr_once);
+static int launch_scanline_kf(const AdcParams& P, const AdcWave& w, const CUtensorMap& tc, const CUtensorMap& tr,
+                              int T, int NS, size_t smem, float* dst, int sx, int sy, cudaStream_t st) {
+    if constexpr (WTA && !so_wta_built<K, LPS, FULL>()) {
+        return 1;
+    } else {
+        constexpr int LPW = 32 / LPS;
+        const int n_lines = sx ? P.dm.H : P.dm.W;
+        const void* fn;
+        if constexpr (WTA) fn = (const void*)k_scanline_wta<K, LPS, FULL>;
+        else fn = (const void*)k_scanline<K, LPS, FULL>;
+        static AdcOnce attr_once;
+        if (adc_once_needed(attr_once)) {
+            cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, SO_SMEM_MAX);
+            cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+            adc_once_done(attr_once);
+        }
+        const int lines_per_block = SO_WARPS * LPW;
+        dim3 grid((n_lines + lines_per_block - 1) / lines_per_block, w.S);
+        if constexpr (WTA) k_scanline_wta<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, w.disp_l, T, NS);
+        else k_scanline<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, sx, sy, T, NS);
+        return 0;
     }
-    const int lines_per_block = SO_WARPS * LPW;
-    dim3 grid((n_lines + lines_per_block - 1) / lines_per_block, w.S);
-    if constexpr (WTA) k_scanline_wta<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, w.disp_l, T, NS);
-    else k_scanline<K, LPS, FULL><<<grid, SO_WARPS * 32, smem, st>>>(tc, tr, P, dst, sx, sy, T, NS);
 }
 
 void adc_launch_so_bitrows(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches) {
@@ -527,8 +540,9 @@ static int launch_scanline(const AdcParams& P, const AdcWave& w, const float* sr
     memcpy(&tr, w.so_tm->rec[axis], 128);
     const int T = w.so_tm->T[axis], NS = w.so_tm->NS[axis];
     const size_t smem = w.so_tm->smem[axis];
-#define SO_GO(KK, LL) (P.dm.D == KK * LL ? launch_scanline_kf<KK, LL, true, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st) \
-                                             : launch_scanline_kf<KK, LL, false, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st))
+    int rc = 1;
+#define SO_GO(KK, LL) rc = (P.dm.D == KK * LL ? launch_scanline_kf<KK, LL, true, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st) \
+                                                  : launch_scanline_kf<KK, LL, false, WTA>(P, w, tc, tr, T, NS, smem, dst, sx, sy, st))
     switch (so_lanes_per_line(Dp)) {
         case 8:   // K = ceil(Dp / 8)
             switch ((Dp + 7) / 8) { case 1: SO_GO(1, 8); break; case 2: SO_GO(2, 8); break; case 3: SO_GO(3, 8); break; case 4: SO_GO(4, 8); break;
@@ -541,6 +555,7 @@ static int launch_scanline(const AdcParams& P, const AdcWave& w, const float* sr
             switch ((Dp + 31) / 32) { case 5: SO_GO(5, 32); break; case 6: SO_GO(6, 32); break; case 7: SO_GO(7, 32); break; default: SO_GO(8, 32); }
     }
 #undef SO_GO
+    if (rc) return rc;
     ++*launches;
     return 0;
 }

@@ -87,8 +87,9 @@ SYMBOLS = {
 }
 
 
-def library_instantiations():
-    """{(template, args...)} of the seven templates, read from the built library's device symbols."""
+def library_instantiations(symbols=SYMBOLS):
+    """{(template, args...)} of the templates in `symbols` (by default the seven above), read from the built library's
+    device symbols."""
     from adcensus_b200.build import build_library
     cuobjdump = Path(os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")).parent / "cuobjdump"
     if not cuobjdump.exists():
@@ -96,10 +97,10 @@ def library_instantiations():
     r = subprocess.run([str(cuobjdump), "-symbols", str(build_library())], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr[-2000:]
     found = set()
-    for name, rx in SYMBOLS.items():
+    for name, rx in symbols.items():
         for m in rx.finditer(r.stdout):
             args = tuple(int(g) for g in m.groups())
-            if name == "k_scanline":
+            if name in ("k_scanline", "k_scanline_wta"):
                 found.add((name, args[0], args[1], bool(args[2])))
             else:
                 found.add((name, bool(args[0]), *args[1:]))
@@ -146,6 +147,14 @@ class Plans:
         v = list(map(int, self._run("so_plan_main", c.W, c.H, c.Dp, c.wave_pairs, axis, *self.dev).split()))
         return dict(zip(("T", "NS", "smem", "ctas", "ctas_per_sm", "waves"), v))
 
+    def so_wta(self, c, debug_flags=0, volumes=True, confidence=False):
+        """so_wta_fused for a batched run of case c (check_case's requests): dict(fused, band, row_records, plane, vol)."""
+        import adcensus_b200 as A
+        force = 1 if debug_flags & A.engine.DBG_UNFUSED_SO_WTA else 2 if debug_flags & A.engine.DBG_FUSED_SO_WTA else 0
+        v = list(map(int, self._run("so_wta_main", c.W, c.H, c.D, c.opt.min_disparity, int(volumes), int(confidence),
+                                    int(c.opt.do_discontinuity_adjustment != 0), 0, force).split()))
+        return dict(zip(("fused", "band", "row_records", "plane", "vol"), v))
+
 
 def so_lanes_per_line(Dp):
     return 8 if Dp <= 64 else (16 if Dp <= 128 else 32)
@@ -154,7 +163,7 @@ def so_lanes_per_line(Dp):
 A2_TMA, A2_LDG = 1, 0     # the forms arm_sum2_form (ca_plan.h) picks
 
 
-def reached(c, plans):
+def reached(c, plans, fused=False):
     """The instantiations of the seven templates one batched run of case c launches, by the launch rules of
     k_aggregate.cu, k_cost.cu, k_scanline.cu and k_vote.cu (a run that matches, so every stage runs, with the fused
     aggregation):
@@ -162,7 +171,8 @@ def reached(c, plans):
       axis dir:  k_arm_sum2t<dir, qc> where the TMA plans of both axes are ok and, on rows, the row is one segment; else
                  k_arm_sum2<dir, 8 if Qc == 8 else 0> (generic QC).  This restates arm_sum2_form, and the form the plan
                  executable prints for the axis must agree with it;
-      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp);
+      scanline:  k_scanline<ceil(Dp / LPS), LPS, D == K * LPS>, LPS = so_lanes_per_line(Dp), and with the same
+                 arguments k_scanline_wta where the last pass runs `fused` with the WTA (Plans.so_wta);
       voting:    k_vote_scan<WIDE> and k_vote_push<WIDE>, WIDE iff D > 254 or L1 > 127."""
     out = set()
     exact = c.D == c.Dp
@@ -182,6 +192,8 @@ def reached(c, plans):
     lps = so_lanes_per_line(c.Dp)
     K = -(-c.Dp // lps)
     out.add(("k_scanline", K, lps, c.D == K * lps))
+    if fused:
+        out.add(("k_scanline_wta", K, lps, c.D == K * lps))
     wide = c.D > 254 or min(c.L1, 255) > 127
     out.add(("k_vote_scan", wide))
     out.add(("k_vote_push", wide))
@@ -205,10 +217,14 @@ def _oracle_outputs(c, left, right, cost):
     return out
 
 
-def check_case(c, debug_flags=0, pairs=None, confidence=False, pipelined=False, cost_layout="hwd", cost_dtype="f32"):
+def check_case(c, debug_flags=0, pairs=None, confidence=False, pipelined=False, cost_layout="hwd", cost_dtype="f32",
+               volumes=True, after=None):
     """One match_outputs_batch_device call over the case's pairs, exporting the three volumes (f32, [H][W][D]), the
     WTA maps, the outlier map and the final map, each pair compared bit for bit with its own oracle run, on an engine
     created with `debug_flags`; returns every output of the call on the host.
+    volumes=False: no volume export (the call then reads the optimised volume only where the options do, so the last
+    scanline pass may take the WTA as its epilogue); not with confidence.  after(eng): called with the engine after the
+    call, before it is closed.
     pairs: [(left, right)] or [(left, right, cost volume f32 [H][W][D])] instead of the sweep's pairs; with cost volumes
     the call matches from them (given as `cost_layout` / `cost_dtype`; their values must be exact in that type).
     confidence: also export MIN_COST / PEAK_RATIO and compare them with maps_testlib.confidence of the oracle's SO4
@@ -219,6 +235,7 @@ def check_case(c, debug_flags=0, pairs=None, confidence=False, pipelined=False, 
     pairs = [(p[0], p[1], p[2] if len(p) > 2 else None) for p in pairs]
     has_cost = pairs[0][2] is not None
     assert all((p[2] is not None) == has_cost for p in pairs)
+    assert volumes or not confidence, "the confidence maps read the optimised volume"
     maps = ["wta_left", "wta_right", "outliers"] + (["min_cost", "peak_ratio"] if confidence else [])
     # the oracle runs overlap in threads (ctypes releases the GIL during the call) while the GPU runs the batch
     with ThreadPoolExecutor(len(pairs)) as ex:
@@ -238,15 +255,18 @@ def check_case(c, debug_flags=0, pairs=None, confidence=False, pipelined=False, 
         eng = E.engine(c.W, c.H, c.opt, wave_pairs=c.wave_pairs, lanes=c.lanes, debug_flags=debug_flags)
         assert (eng.wave_pairs, eng.lanes) == (c.wave_pairs, c.lanes), (eng.wave_pairs, eng.lanes)
         got = E.batch_outputs(eng, eng.match_outputs_batch_device, len(pairs), d_l.data_ptr(), d_r.data_ptr(),
-                              3 * c.W * c.H, volumes=[(s, "hwd", "f32") for s in ("cost", "aggr", "opt")],
+                              3 * c.W * c.H, volumes=[(s, "hwd", "f32") for s in ("cost", "aggr", "opt") if volumes],
                               maps=maps, pipelined=pipelined, **cost)
+        if after is not None:
+            after(eng)
         eng.close()
         want = [f.result() for f in futs]
     for i, w in enumerate(want):
         tag = f"{c.name} ({c.W}x{c.H}x{c.D}, dmin {c.opt.min_disparity}) pair {i}"
-        E.same(f"{tag} COST/VOL_INIT", got["cost"][i], w["cost"])
-        E.same(f"{tag} AGG4/VOL_AGGR", got["aggr"][i], w["aggr"])
-        E.same(f"{tag} SO4/VOL_AGGR", got["opt"][i], w["opt"])
+        if volumes:
+            E.same(f"{tag} COST/VOL_INIT", got["cost"][i], w["cost"])
+            E.same(f"{tag} AGG4/VOL_AGGR", got["aggr"][i], w["aggr"])
+            E.same(f"{tag} SO4/VOL_AGGR", got["opt"][i], w["opt"])
         E.same(f"{tag} WTA/DISP_L", got["wta_left"][i], w["wta_left"])
         E.same(f"{tag} WTA/DISP_R", got["wta_right"][i], w["wta_right"])
         assert set(np.unique(got["outliers"][i])) <= {0, 1, 2}, f"{tag} OUTLIER: labels other than 0, 1, 2"

@@ -8,6 +8,9 @@ per-pair volumes of tests/test_size_limits.py, which no test can afford to recom
        with int32 (cost_computor.cpp: y * width_ * disp_range + ...; cross_aggregator.cpp: width_ * height_ *
        disp_range * sizeof(...)), so it is undefined here; the hashes are the oracle's (oracle/adc_oracle.c), which
        indexes with size_t and agrees with the reference wherever the reference is defined.  About 18 GB of host memory.
+  F1   4000 x 2100 x 64, seeds 1 and 2: 537.6 M elements, 2.15 GB per volume -- past 2^31 bytes, at a shape where the
+       last scanline pass takes both WTA views as its epilogue (so_wta_fused, so_plan.h), so that a wave of the two
+       pairs writes the second pair's partial records past 2^32 bytes.  The UNMODIFIED reference's hashes.
 
 Usage: make_golden_limits.py [case ...]   (all cases by default; each case runs in its own process, in parallel)
 Rerunning it reproduces the file byte for byte.
@@ -27,6 +30,8 @@ CASES = {
     "L1_s1": (2100, 1024, 256, 1, "reference"),
     "L1_s2": (2100, 1024, 256, 2, "reference"),
     "L2_s1": (8400, 1024, 256, 1, "oracle"),
+    "F1_s1": (4000, 2100, 64, 1, "reference"),
+    "F1_s2": (4000, 2100, 64, 2, "reference"),
 }
 
 
