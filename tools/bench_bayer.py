@@ -8,9 +8,9 @@ process so that every figure comes from the same run:
 * bayer_bgr    : adc_match_batch_device on the same mosaics demosaiced beforehand (cv2.cvtColor), packed BGR on the
                  device: the yardstick for `bayer`, whose image content differs from Cone's
 * rect_bayer   : adc_match_rectified_batch_device on raw BayerRG8 frames [N, 480, 640]: Cone resized to 640x480 and
-                 mosaiced, rectified through initUndistortRectifyMap maps (CV_16SC2) of bench_rectify's made-up rig
+                 mosaiced, rectified through initUndistortRectifyMap maps (CV_16SC2) of rectify_testlib's made-up rig
 * rect_bgr_raw : adc_match_rectified_batch_device on the same raw frames demosaiced beforehand, [N, 480, 640, 3]
-  The four are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The four are timed in alternating windows (`--rounds`); the medians are reported.
 * host         : the same raw frames through cv2.cvtColor and cv2.remap on the host (both views of every pair, OpenCV's
                  own threading) followed by adc_match_batch on the rectified images: wall clock over one batch, after a
                  warm-up batch.
@@ -21,51 +21,33 @@ process so that every figure comes from the same run:
 Every Bayer map is checked bit for bit against the packed-BGR maps of the demosaiced images (and the host path's).  The
 card's name and power limit are recorded beside the numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
 import statistics
 import sys
-import time
-from pathlib import Path
 
 import cv2
-import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import bayer_testlib as B  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_rectify import rig_maps  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import bayer_testlib as BT
+import rectify_testlib as R
 
 PAT = "bayer_rggb"
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_bayer.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
     sw, sh = 640, 480
-    D, n = 64, args.pairs
-    mos = [B.mosaic(img, PAT) for img in (left, right)]
-    demo = [B.cv_demosaic(cv2, m, PAT) for m in mos]
-    raw = [B.mosaic(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR), PAT) for img in (left, right)]
-    raw_bgr = [B.cv_demosaic(cv2, r, PAT) for r in raw]
-    maps = [rig_maps(sw, sh, w, h, s) for s in (1, -1)]
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)
+    D = 64
+    mos = [BT.mosaic(img, PAT) for img in (left, right)]
+    demo = [BT.cv_demosaic(cv2, m, PAT) for m in mos]
+    raw = [BT.mosaic(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR), PAT) for img in (left, right)]
+    raw_bgr = [BT.cv_demosaic(cv2, r, PAT) for r in raw]
+    maps = [R.cone_rig(cv2, sw, sh, w, h, cv2.CV_16SC2, s) for s in (1, -1)]
     m_left, m_right = rep(mos[0]), rep(mos[1])
     b_left, b_right = rep(demo[0]), rep(demo[1])
     r_left, r_right = rep(raw[0]), rep(raw[1])
@@ -78,39 +60,33 @@ def main():
     st = torch.cuda.current_stream()
     desc = A.image_desc(PAT)
 
-    def bayer():
+    def bayer(_):
         eng.match_images_batch_device(n, m_left.data_ptr(), m_right.data_ptr(), image=desc,
                                       d_disp=out["bayer"].data_ptr(), stream=st.cuda_stream)
 
-    def bayer_bgr():
+    def bayer_bgr(_):
         eng.match_batch_device(n, b_left.data_ptr(), b_right.data_ptr(), out["bayer_bgr"].data_ptr(), st.cuda_stream)
 
-    def rect_bayer():
+    def rect_bayer(_):
         eng.match_rectified_batch_device(n, r_left.data_ptr(), r_right.data_ptr(), image=desc,
                                          d_disp=out["rect_bayer"].data_ptr(), stream=st.cuda_stream)
 
-    def rect_bgr_raw():
+    def rect_bgr_raw(_):
         eng.match_rectified_batch_device(n, rb_left.data_ptr(), rb_right.data_ptr(),
                                          d_disp=out["rect_bgr_raw"].data_ptr(), stream=st.cuda_stream)
 
-    ms = alternating_windows(eng, st, (bayer, bayer_bgr, rect_bayer, rect_bgr_raw), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (bayer, bayer_bgr, rect_bayer, rect_bgr_raw), args.steps, args.warmup, args.rounds)
     eng.set_pipelined(False)
 
     # host path: cv2.cvtColor + cv2.remap of every view, then adc_match_batch (pointer-array form)
-    remap = lambda img, m: cv2.remap(img, *m, cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT, borderValue=0)
-    code = getattr(cv2, B.CV_NAME[PAT])
+    code = getattr(cv2, BT.CV_NAME[PAT])
     lefts, rights = [raw[0]] * n, [raw[1]] * n
 
     def host():
-        return eng.match_batch_ptrs([remap(cv2.cvtColor(x, code), maps[0]) for x in lefts],
-                                    [remap(cv2.cvtColor(x, code), maps[1]) for x in rights])
+        return eng.match_batch_ptrs([B.remap(cv2.cvtColor(x, code), maps[0]) for x in lefts],
+                                    [B.remap(cv2.cvtColor(x, code), maps[1]) for x in rights])
 
-    host()
-    host_s = []
-    for _ in range(args.rounds):
-        t0 = time.perf_counter()
-        host_maps = host()
-        host_s.append(time.perf_counter() - t0)
+    host_s, host_maps = B.host_seconds(host, args.rounds)
     got = {k: v.cpu().numpy() for k, v in out.items()}
     checks = {"bayer_vs_bayer_bgr": got["bayer"].tobytes() == got["bayer_bgr"].tobytes(),
               "rect_bayer_vs_rect_bgr_raw": got["rect_bayer"].tobytes() == got["rect_bgr_raw"].tobytes(),
@@ -118,46 +94,33 @@ def main():
               "bayer_vs_single_pair": all(got["bayer"][i].tobytes() == eng.match(demo[0], demo[1]).tobytes()
                                           for i in (0, n - 1))}
 
-    reps = 50
-    kernels = {}
-    # the profile ids replay the format of the engine's last images / rectified call: make one of each first
-    for name, pid, call in (("image_ingest_bayer", "image_ingest",
-                             lambda: eng.match_images(mos[0], mos[1], format=PAT)),
-                            ("rectify_bayer", "rectify", lambda: eng.match_rectified(raw[0], raw[1], format=PAT)),
-                            ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))):
-        call()
-        k_ms, k_bytes = eng.profile_kernel(pid, reps=reps)
-        cp_bytes = int(k_bytes // 2)
-        cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
-        kernels[name] = {"ms_per_wave": round(k_ms, 4), "algorithmic_bytes": k_bytes,
-                         "achieved_gbs": round(k_bytes / (k_ms * 1e-3) / 1e9, 1),
-                         "d2d_copy_same_bytes_ms": round(cp_ms, 4), "d2d_copy_gbs": round(cp_gbs, 1),
-                         "kernel_vs_copy": round(cp_ms / k_ms, 4)}
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    kernels = B.kernels_vs_copy(eng, (
+        ("image_ingest_bayer", "image_ingest", lambda: eng.match_images(mos[0], mos[1], format=PAT)),
+        ("rectify_bayer", "rectify", lambda: eng.match_rectified(raw[0], raw[1], format=PAT)),
+        ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))), reps=50, dev=dev)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     host_rate = round(n / statistics.median(host_s), 2)
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "bayer": {"value": rate(ms["bayer"]), "call": "adc_match_images_batch_device ([N, H, W] BayerRG8)"},
-            "bayer_bgr": {"value": rate(ms["bayer_bgr"]),
+            "bayer": {"value": rate["bayer"], "call": "adc_match_images_batch_device ([N, H, W] BayerRG8)"},
+            "bayer_bgr": {"value": rate["bayer_bgr"],
                           "call": "adc_match_batch_device (the same mosaics demosaiced beforehand, packed BGR)"},
-            "rect_bayer": {"value": rate(ms["rect_bayer"]),
+            "rect_bayer": {"value": rate["rect_bayer"],
                            "call": "adc_match_rectified_batch_device (640x480 raw BayerRG8, CV_16SC2 maps)"},
-            "rect_bgr_raw": {"value": rate(ms["rect_bgr_raw"]),
+            "rect_bgr_raw": {"value": rate["rect_bgr_raw"],
                              "call": "adc_match_rectified_batch_device (the same raw frames demosaiced beforehand, BGR)"},
             "host_cvtcolor_remap": {"value": host_rate,
                                     "call": "cv2.cvtColor + cv2.remap on the host (both views) + adc_match_batch",
                                     "cv2_threads": cv2.getNumThreads(), "opencv": cv2.__version__},
-            "bayer_vs_bayer_bgr": round(rate(ms["bayer"]) / rate(ms["bayer_bgr"]), 4),
-            "rect_bayer_vs_rect_bgr_raw": round(rate(ms["rect_bayer"]) / rate(ms["rect_bgr_raw"]), 4),
-            "rect_bayer_vs_host": round(rate(ms["rect_bayer"]) / host_rate, 2),
+            "bayer_vs_bayer_bgr": round(rate["bayer"] / rate["bayer_bgr"], 4),
+            "rect_bayer_vs_rect_bgr_raw": round(rate["rect_bayer"] / rate["rect_bgr_raw"], 4),
+            "rect_bayer_vs_host": round(rate["rect_bayer"] / host_rate, 2),
             "windows_ms": {k: [round(x, 2) for x in v] for k, v in ms.items()},
             "checks": checks,
             "rounds": args.rounds, "steps_per_round": args.steps, "wave_pairs": eng.wave_pairs, "lanes": eng.lanes,
-            "kernels": {**kernels, "note": f"one wave; CUDA events over {reps} launches; the copy is one cudaMemcpyAsync "
-                                           f"of algorithmic_bytes / 2, read + write counted"},
-            "card": card()}
+            "kernels": kernels,
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

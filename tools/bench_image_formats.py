@@ -10,7 +10,7 @@ device-resident, pipelined), in one process so that every figure comes from the 
 * gray_bgr   : adc_match_batch_device on the same gray images replicated to packed BGR: the yardstick for `gray`, whose
                image content (and so the data-dependent refinement work) differs from Cone's colour images
 * sbs_bgra   : adc_match_images_batch_device on side-by-side BGRA frames [N, H, 2W, 4], right view at +4W bytes
-  The four are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The four are timed in alternating windows (`--rounds`); the medians are reported.
 * kernel     : the ingestion kernel alone over one wave (adc_profile_kernel id 13, CUDA events) in each format, next to
                a device-to-device cudaMemcpyAsync (torch copy_) of the bytes the two cudaMemcpy2DAsync calls of the
                packed-BGR path move for one wave (both views: 2*3*N per pair), timed in the same process.
@@ -18,42 +18,25 @@ Every timed colour map is checked against the unmodified reference's sha256 (tes
 single-pair adc_match_images result of the same gray images.  The card's name and power limit are recorded beside the
 numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
-import statistics
 import sys
-from pathlib import Path
 
 import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import images_testlib as IT  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import adc_testlib as T
+import images_testlib as IT
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_image_formats.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
-    D, n = 64, args.pairs
-    hashes = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
-    golden = hashes["MEDIAN/DISP_L"]
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)
+    D = 64
+    golden = B.golden()
     d_left, d_right = rep(left), rep(right)
     p_left, p_right = rep(IT.from_bgr(left, "rgb_planar")), rep(IT.from_bgr(right, "rgb_planar"))
     g_left, g_right = rep(left[:, :, 1].copy()), rep(right[:, :, 1].copy())
@@ -68,25 +51,25 @@ def main():
     desc_g = A.image_desc("gray")
     desc_s = A.image_desc("bgra", 8 * w, 0, 8 * w * h)
 
-    def bgr():
+    def bgr(_):
         eng.match_batch_device(n, d_left.data_ptr(), d_right.data_ptr(), out["bgr"].data_ptr(), st.cuda_stream)
 
-    def rgb_planar():
+    def rgb_planar(_):
         eng.match_images_batch_device(n, p_left.data_ptr(), p_right.data_ptr(), image=desc_p,
                                       d_disp=out["rgb_planar"].data_ptr(), stream=st.cuda_stream)
 
-    def gray():
+    def gray(_):
         eng.match_images_batch_device(n, g_left.data_ptr(), g_right.data_ptr(), image=desc_g,
                                       d_disp=out["gray"].data_ptr(), stream=st.cuda_stream)
 
-    def gray_bgr():
+    def gray_bgr(_):
         eng.match_batch_device(n, gb_left.data_ptr(), gb_right.data_ptr(), out["gray_bgr"].data_ptr(), st.cuda_stream)
 
-    def sbs_bgra():
+    def sbs_bgra(_):
         eng.match_images_batch_device(n, sbs.data_ptr(), sbs.data_ptr() + 4 * w, image=desc_s,
                                       d_disp=out["sbs_bgra"].data_ptr(), stream=st.cuda_stream)
 
-    ms = alternating_windows(eng, st, (bgr, rgb_planar, gray, gray_bgr, sbs_bgra), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (bgr, rgb_planar, gray, gray_bgr, sbs_bgra), args.steps, args.warmup, args.rounds)
     eng.set_pipelined(False)
     gray_single, _ = eng.match_images(left[:, :, 1].copy(), right[:, :, 1].copy(), format="gray")
 
@@ -110,17 +93,17 @@ def main():
         kernels[fmt] = {"ms_per_wave": round(k_ms, 4), "algorithmic_bytes": k_bytes,
                         "achieved_gbs": round(k_bytes / (k_ms * 1e-3) / 1e9, 1)}
     cp_bytes = S * 2 * 3 * N
-    cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    cp_ms, cp_gbs = B.d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "bgr": {"value": rate(ms["bgr"]), "call": "adc_match_batch_device (packed BGR)"},
-            "rgb_planar": {"value": rate(ms["rgb_planar"]), "call": "adc_match_images_batch_device ([N, 3, H, W] RGB)"},
-            "gray": {"value": rate(ms["gray"]), "call": "adc_match_images_batch_device ([N, H, W] gray)"},
-            "gray_bgr": {"value": rate(ms["gray_bgr"]), "call": "adc_match_batch_device (the gray images as packed BGR)"},
-            "sbs_bgra": {"value": rate(ms["sbs_bgra"]),
+            "bgr": {"value": rate["bgr"], "call": "adc_match_batch_device (packed BGR)"},
+            "rgb_planar": {"value": rate["rgb_planar"], "call": "adc_match_images_batch_device ([N, 3, H, W] RGB)"},
+            "gray": {"value": rate["gray"], "call": "adc_match_images_batch_device ([N, H, W] gray)"},
+            "gray_bgr": {"value": rate["gray_bgr"], "call": "adc_match_batch_device (the gray images as packed BGR)"},
+            "sbs_bgra": {"value": rate["sbs_bgra"],
                          "call": "adc_match_images_batch_device ([N, H, 2W, 4] side-by-side BGRA)"},
-            "vs_bgr": {k: round(rate(ms[k]) / rate(ms["bgr"]), 4) for k in ("rgb_planar", "sbs_bgra")},
-            "gray_vs_gray_bgr": round(rate(ms["gray"]) / rate(ms["gray_bgr"]), 4),
+            "vs_bgr": {k: round(rate[k] / rate["bgr"], 4) for k in ("rgb_planar", "sbs_bgra")},
+            "gray_vs_gray_bgr": round(rate["gray"] / rate["gray_bgr"], 4),
             "checks": checks,
             "checked_against": "colour: sha256 of the unmodified reference's MEDIAN/DISP_L; gray: the single-pair "
                                "adc_match_images map of the same gray images (also for gray_bgr)",
@@ -130,10 +113,9 @@ def main():
             "bgr_copies": {"bytes": cp_bytes, "ms": round(cp_ms, 4), "achieved_gbs": round(cp_gbs, 1),
                            "note": "one device-to-device cudaMemcpyAsync of the bytes the packed-BGR path's two "
                                    "cudaMemcpy2DAsync calls move per wave; read + write counted"},
-            "card": card()}
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

@@ -7,7 +7,7 @@ pipelined), in one process so that every figure comes from the same run:
 * plain     : adc_match_batch_device (what bench.py's "value" times)
 * side_maps : adc_match_outputs_batch_device with the final map + MIN_COST + PEAK_RATIO + OUTLIERS
 * map_only  : adc_match_outputs_batch_device with WTA_LEFT + PEAK_RATIO and no final map: the pipeline stops after the WTA
-  The three are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The three are timed in alternating windows (`--rounds`); the medians are reported.
 * kernels   : k_confidence alone over one wave (adc_profile_kernel id 12, both confidence maps) next to k_wta (id 5) and a
               device-to-device cudaMemcpyAsync (torch copy_) that reads and writes k_confidence's bytes, in the same call.
 Every timed map is checked against the unmodified reference's sha256 (tests/golden): the final maps against
@@ -16,43 +16,26 @@ confidence maps against the numpy helper (tests/maps_testlib.py) on the engine's
 sha256 must be the reference's SO4/VOL_AGGR.  The card's name and power limit are recorded beside the numbers.  Prints
 one JSON line; writes nothing.
 """
-import argparse
-import json
-import statistics
 import sys
-from pathlib import Path
 
-import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import maps_testlib as MT  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import adc_testlib as T
+import maps_testlib as MT
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_output_maps.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
-    D, n = 64, args.pairs
-    hashes = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
+    D = 64
+    hashes = B.cone_hashes()
     f32 = lambda: torch.empty((n, h, w), dtype=torch.float32, device=dev)
-    d_left = torch.from_numpy(np.repeat(left[None], n, 0)).to(dev)
-    d_right = torch.from_numpy(np.repeat(right[None], n, 0)).to(dev)
+    d_left, d_right = rep(left), rep(right)
     d_disp, d_disp_s = f32(), f32()
     side = {"min_cost": f32(), "peak_ratio": f32(), "outliers": torch.empty((n, h, w), dtype=torch.uint8, device=dev)}
     only = {"wta_left": f32(), "peak_ratio": f32()}
@@ -64,19 +47,19 @@ def main():
     c1, ratio = MT.confidence(single["opt"])
     del single
 
-    def plain():
+    def plain(_):
         eng.match_batch_device(n, d_left.data_ptr(), d_right.data_ptr(), d_disp.data_ptr(), st.cuda_stream)
 
-    def side_maps():
+    def side_maps(_):
         eng.match_outputs_batch_device(n, d_left.data_ptr(), d_right.data_ptr(),
                                        maps=[(b.data_ptr(), m) for m, b in side.items()], d_disp=d_disp_s.data_ptr(),
                                        stream=st.cuda_stream)
 
-    def map_only():
+    def map_only(_):
         eng.match_outputs_batch_device(n, d_left.data_ptr(), d_right.data_ptr(),
                                        maps=[(b.data_ptr(), m) for m, b in only.items()], stream=st.cuda_stream)
 
-    ms = alternating_windows(eng, st, (plain, side_maps, map_only), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (plain, side_maps, map_only), args.steps, args.warmup, args.rounds)
 
     def all_equal(t, want_sha):
         a = t.cpu().numpy()
@@ -101,20 +84,18 @@ def main():
     }
 
     reps = 50
-    k_ms, k_bytes = eng.profile_kernel("confidence", reps=reps)
+    k_ms, k_bytes, cp_ms, cp_gbs = B.kernel_vs_copy(eng, "confidence", reps, dev)
     w_ms, w_bytes = eng.profile_kernel("wta", reps=reps)
-    cp_bytes = int(k_bytes // 2)                         # a copy of B bytes reads B and writes B
-    cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
     k_gbs = k_bytes / (k_ms * 1e-3) / 1e9
     w_gbs = w_bytes / (w_ms * 1e-3) / 1e9
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "plain": {"value": rate(ms["plain"]), "call": "adc_match_batch_device"},
-            "side_maps": {"value": rate(ms["side_maps"]),
+            "plain": {"value": rate["plain"], "call": "adc_match_batch_device"},
+            "side_maps": {"value": rate["side_maps"],
                           "call": "adc_match_outputs_batch_device (final map + MIN_COST + PEAK_RATIO + OUTLIERS)"},
-            "map_only": {"value": rate(ms["map_only"]),
+            "map_only": {"value": rate["map_only"],
                          "call": "adc_match_outputs_batch_device (WTA_LEFT + PEAK_RATIO, no final map)"},
-            "side_maps_vs_plain": round(rate(ms["side_maps"]) / rate(ms["plain"]), 4),
+            "side_maps_vs_plain": round(rate["side_maps"] / rate["plain"], 4),
             "checks": checks,
             "checked_against": "sha256 of the unmodified reference's MEDIAN/DISP_L, WTA/DISP_L, OUTLIER/MISMATCHES, "
                                "OUTLIER/OCCLUSIONS; confidence: numpy helper on the pair's optimised volume "
@@ -124,13 +105,12 @@ def main():
                                   "note": f"N*Dp*4 read + 2*4*N written per pair; CUDA events over {reps} launches"},
             "wta_kernel": {"ms_per_wave": round(w_ms, 4), "algorithmic_bytes": w_bytes, "achieved_gbs": round(w_gbs, 1),
                            "note": "N*D*4 read + 8*N written per pair (both views)"},
-            "d2d_copy": {"bytes": cp_bytes, "ms": round(cp_ms, 4), "achieved_gbs": round(cp_gbs, 1),
+            "d2d_copy": {"bytes": int(k_bytes // 2), "ms": round(cp_ms, 4), "achieved_gbs": round(cp_gbs, 1),
                          "note": "cudaMemcpyAsync device to device of half of k_confidence's bytes; read + write counted"},
             "confidence_vs_copy": round(k_gbs / cp_gbs, 3), "confidence_vs_wta_time": round(k_ms / w_ms, 3),
-            "card": card()}
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

@@ -11,7 +11,8 @@ every figure comes from the same run:
                  rig maps): the camera path
 * rect_cloud   : the camera path, then on the second stream adc_ingest_views_batch_device of the raw frames and the
                  coloured cloud of the maps by the left views
-  Each path is timed in `rounds` alternating windows of `steps` steps (bench_reproject.windows); medians reported.
+  Each path is timed in `rounds` alternating windows of `steps` steps (CUDA events on the first stream, which waits for
+  the second at the end of a window); medians reported.
 * kernel       : adc_point_cloud_batch_device alone over 256 Cone maps (coloured, with pixels), next to
                  adc_reproject_batch_device (points) on the same maps and a device-to-device copy of as many bytes
                  (read + write) as the cloud moves; and reprojection followed by torch boolean indexing (a host sync
@@ -19,67 +20,38 @@ every figure comes from the same run:
 Every timed output is checked against the numpy restatement (tests/cloud_testlib.py).  The card's name and power limit
 are recorded beside the numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
-import statistics
 import sys
-from pathlib import Path
 
 import cv2
 import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import cloud_testlib as C  # noqa: E402
-import rawdepth_testlib as RD  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_rectify import rig_maps  # noqa: E402
-from bench_reproject import windows  # noqa: E402
-from bench_volume_export import d2d_copy  # noqa: E402
-from make_golden_reproject import rig_Q  # noqa: E402
-
-
-def events_ms(fn, reps, st):
-    fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record(st)
-    for _ in range(reps):
-        fn()
-    e1.record(st)
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
+import benchlib as B
+import adcensus_b200 as A
+import cloud_testlib as C
+import rawdepth_testlib as RD
+import rectify_testlib as R
+from make_golden_reproject import rig_Q
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_point_cloud.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
-    N, D, n = w * h, 64, args.pairs
+    N, D = w * h, 64
     sw, sh = 640, 480
     fmt = "bayer_rg12p"
     rng = np.random.default_rng(0)
     raw = [RD.encode(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR), fmt, rng) for img in (left, right)]
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)
     d_left, d_right = rep(left), rep(right)
     r_left, r_right = rep(raw[0]), rep(raw[1])
     raw_desc = A.image_desc(fmt)
     Q = rig_Q(w, h, True)
     eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D))
-    eng.set_rectification(rig_maps(sw, sh, w, h, 1), rig_maps(sw, sh, w, h, -1), (sw, sh))
+    maps = [R.cone_rig(cv2, sw, sh, w, h, cv2.CV_16SC2, s) for s in (1, -1)]
+    eng.set_rectification(maps[0], maps[1], (sw, sh))
     eng.set_pipelined(True)
     st = torch.cuda.current_stream()
     s2 = torch.cuda.Stream()
@@ -120,7 +92,7 @@ def main():
                                       s2.cuda_stream)
         cloud_of(d, views.data_ptr(), 6 * N, s2)
 
-    ms = windows(eng, st, s2, (plain, cloud, rect, rect_cloud), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (plain, cloud, rect, rect_cloud), args.steps, args.warmup, args.rounds, side=s2)
     eng.set_pipelined(False)
 
     # checks: the last cloud (camera path, coloured by the left views) and a plain one against the restatement
@@ -137,12 +109,12 @@ def main():
               "camera_cloud_vs_restatement": cloud_ok(cam, views[0, 0].cpu().numpy())}
     m0 = disp["cloud"][0][0].cpu().numpy()
     reps = 20
-    k_cloud = events_ms(lambda: cloud_of(disp["cloud"][0], d_left.data_ptr(), 0, st), reps, st)
+    k_cloud = B.events_ms(lambda: cloud_of(disp["cloud"][0], d_left.data_ptr(), 0, st), reps, st)
     checks["cloud_vs_restatement"] = cloud_ok(m0, left)
     kept = int(counts.sum())
     rp = torch.empty((n, h, w, 3), dtype=torch.float32, device=dev)
-    k_reproj = events_ms(lambda: eng.reproject_batch_device(n, disp["cloud"][0].data_ptr(), Q, [(rp.data_ptr(), "points")],
-                                                            st.cuda_stream), reps, st)
+    k_reproj = B.events_ms(lambda: eng.reproject_batch_device(n, disp["cloud"][0].data_ptr(), Q,
+                                                              [(rp.data_ptr(), "points")], st.cuda_stream), reps, st)
 
     def torch_index():
         eng.reproject_batch_device(n, disp["cloud"][0].data_ptr(), Q, [(rp.data_ptr(), "points")], st.cuda_stream)
@@ -150,26 +122,26 @@ def main():
         keep = torch.isfinite(d) & torch.isfinite(rp).all(-1)
         return rp[keep], d_left[keep.view(n, h, w)].flip(-1)
 
-    k_index = events_ms(torch_index, reps, st)
+    k_index = B.events_ms(torch_index, reps, st)
     p_idx, c_idx = torch_index()
     checks["torch_indexing_same_points"] = bool(p_idx.shape[0] == kept and torch.equal(
         p_idx.view(torch.int32), torch.cat([pts[i, :int(counts[i])] for i in range(n)]).view(torch.int32)))
     # bytes the cloud moves: maps read, colours read and written, points and pixel indices written
     cloud_bytes = n * N * 4 + kept * (3 + 12 + 3 + 4)
     cp = torch.empty(cloud_bytes // 2 + 1, dtype=torch.uint8, device=dev)
-    cp_ms, cp_gbs = d2d_copy(cp, cloud_bytes // 2, reps)
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    cp_ms, cp_gbs = B.d2d_copy(cp, cloud_bytes // 2, reps)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "plain": {"value": rate(ms["plain"]), "call": "adc_match_batch_device"},
-            "cloud": {"value": rate(ms["cloud"]),
+            "plain": {"value": rate["plain"], "call": "adc_match_batch_device"},
+            "cloud": {"value": rate["cloud"],
                       "call": "adc_match_batch_device + adc_point_cloud_batch_device (colours, pixels) on a second stream "
                               "after adc_join"},
-            "cloud_vs_plain": round(rate(ms["cloud"]) / rate(ms["plain"]), 4),
-            "rect": {"value": rate(ms["rect"]), "call": "adc_match_rectified_batch_device (640x480 BayerRG12p)"},
-            "rect_cloud": {"value": rate(ms["rect_cloud"]),
+            "cloud_vs_plain": round(rate["cloud"] / rate["plain"], 4),
+            "rect": {"value": rate["rect"], "call": "adc_match_rectified_batch_device (640x480 BayerRG12p)"},
+            "rect_cloud": {"value": rate["rect_cloud"],
                            "call": "adc_match_rectified_batch_device + adc_ingest_views_batch_device + "
                                    "adc_point_cloud_batch_device coloured by the left views"},
-            "rect_cloud_vs_rect": round(rate(ms["rect_cloud"]) / rate(ms["rect"]), 4),
+            "rect_cloud_vs_rect": round(rate["rect_cloud"] / rate["rect"], 4),
             "kernel": {"cloud_ms_per_256_maps": round(k_cloud, 4), "kept_points": kept, "bytes": cloud_bytes,
                        "achieved_gbs": round(cloud_bytes / (k_cloud * 1e-3) / 1e9, 1),
                        "d2d_copy_same_bytes_ms": round(cp_ms, 4), "d2d_copy_gbs": round(cp_gbs, 1),
@@ -178,10 +150,9 @@ def main():
                        "reproject_then_torch_indexing_ms": round(k_index, 4)},
             "checks": checks,
             "rounds": args.rounds, "steps_per_round": args.steps, "wave_pairs": eng.wave_pairs, "lanes": eng.lanes,
-            "card": card()}
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

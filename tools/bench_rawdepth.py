@@ -10,9 +10,9 @@ pipelined), in one process so that every figure comes from the same run:
                  uint16, cv2.convertScaleAbs), packed BGR on the device: the yardsticks (BayerRG12 holds the samples of
                  BayerRG12p, so rg12p_bgr is its yardstick too)
 * rect_rg12p   : adc_match_rectified_batch_device on raw 640 x 480 BayerRG12p frames (Cone resized and synthesised),
-                 rectified through initUndistortRectifyMap maps (CV_16SC2) of bench_rectify's made-up rig
+                 rectified through initUndistortRectifyMap maps (CV_16SC2) of rectify_testlib's made-up rig
 * rect_bgr_raw : adc_match_rectified_batch_device on the same raw frames converted beforehand, [N, 480, 640, 3]
-  The seven are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The seven are timed in alternating windows (`--rounds`); the medians are reported.
 * host         : the same raw BayerRG12p frames through a numpy unpack, cv2.cvtColor, cv2.convertScaleAbs and cv2.remap
                  on the host (both views of every pair, 16 OpenCV threads) followed by adc_match_batch on the rectified
                  images: wall clock over one batch, after a warm-up batch.
@@ -24,27 +24,17 @@ pipelined), in one process so that every figure comes from the same run:
 Every map is checked bit for bit against the packed-BGR maps of the converted images (and the host path's).  The card's
 name and power limit are recorded beside the numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
 import statistics
 import sys
-import time
-from pathlib import Path
 
 import cv2
 import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import rawdepth_testlib as X  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_rectify import rig_maps  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import rawdepth_testlib as X
+import rectify_testlib as R
 
 
 def unpack12p(rows, W):
@@ -57,20 +47,13 @@ def unpack12p(rows, W):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_rawdepth.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n, raw=True)
     h, w, _ = left.shape
     sw, sh = 640, 480
-    D, n = 64, args.pairs
-    rep = lambda a: torch.from_numpy(np.repeat(np.ascontiguousarray(a).view(np.uint8)[None], n, 0)).to(dev)   # noqa: E731
+    D = 64
     rng = np.random.default_rng(12)
 
     rg12p = [X.encode(img, "bayer_rg12p", rng) for img in (left, right)]
@@ -80,7 +63,7 @@ def main():
     mono_dec = [X.cv_decode(cv2, f, "mono12p", w, h) for f in mono12p]
     raw = [X.encode(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR), "bayer_rg12p", rng) for img in (left, right)]
     raw_bgr = [X.cv_decode(cv2, r, "bayer_rg12p", sw, sh) for r in raw]
-    maps = [rig_maps(sw, sh, w, h, s) for s in (1, -1)]
+    maps = [R.cone_rig(cv2, sw, sh, w, h, cv2.CV_16SC2, s) for s in (1, -1)]
     d = {"rg12p": [rep(x) for x in rg12p], "rg12": [rep(x) for x in rg12], "mono12p": [rep(x) for x in mono12p],
          "rg12p_bgr": [rep(x) for x in rg_dec], "mono12p_bgr": [rep(x) for x in mono_dec],
          "rect_rg12p": [rep(x) for x in raw], "rect_bgr_raw": [rep(x) for x in raw_bgr]}
@@ -91,20 +74,20 @@ def main():
     st = torch.cuda.current_stream()
 
     def images(name, fmt):
-        def call():
+        def call(_):
             eng.match_images_batch_device(n, d[name][0].data_ptr(), d[name][1].data_ptr(), image=A.image_desc(fmt),
                                           d_disp=out[name].data_ptr(), stream=st.cuda_stream)
         call.__name__ = name
         return call
 
     def packed_bgr(name):
-        def call():
+        def call(_):
             eng.match_batch_device(n, d[name][0].data_ptr(), d[name][1].data_ptr(), out[name].data_ptr(), st.cuda_stream)
         call.__name__ = name
         return call
 
     def rectified(name, fmt):
-        def call():
+        def call(_):
             eng.match_rectified_batch_device(n, d[name][0].data_ptr(), d[name][1].data_ptr(), image=A.image_desc(fmt),
                                              d_disp=out[name].data_ptr(), stream=st.cuda_stream)
         call.__name__ = name
@@ -113,26 +96,18 @@ def main():
     paths = (images("rg12p", "bayer_rg12p"), packed_bgr("rg12p_bgr"), images("rg12", "bayer_rg12"),
              images("mono12p", "mono12p"), packed_bgr("mono12p_bgr"), rectified("rect_rg12p", "bayer_rg12p"),
              rectified("rect_bgr_raw", "bgr"))
-    ms = alternating_windows(eng, st, paths, args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, paths, args.steps, args.warmup, args.rounds)
     eng.set_pipelined(False)
 
     # host path: unpack + cvtColor + convertScaleAbs + remap of every view on 16 threads, then adc_match_batch
-    threads = cv2.getNumThreads()
-    cv2.setNumThreads(16)
-    remap = lambda img, m: cv2.remap(img, *m, cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT, borderValue=0)  # noqa: E731
     convert = lambda x: cv2.convertScaleAbs(cv2.cvtColor(unpack12p(x, sw), cv2.COLOR_BayerBG2BGR), alpha=1 / 16)  # noqa: E731
     lefts, rights = [raw[0]] * n, [raw[1]] * n
 
     def host():
-        return eng.match_batch_ptrs([remap(convert(x), maps[0]) for x in lefts], [remap(convert(x), maps[1]) for x in rights])
+        return eng.match_batch_ptrs([B.remap(convert(x), maps[0]) for x in lefts],
+                                    [B.remap(convert(x), maps[1]) for x in rights])
 
-    host()
-    host_s = []
-    for _ in range(args.rounds):
-        t0 = time.perf_counter()
-        host_maps = host()
-        host_s.append(time.perf_counter() - t0)
-    cv2.setNumThreads(threads)
+    host_s, host_maps = B.host_seconds(host, args.rounds, threads=16)
     got = {k: v.cpu().numpy() for k, v in out.items()}
     checks = {"rg12p_vs_rg12p_bgr": got["rg12p"].tobytes() == got["rg12p_bgr"].tobytes(),
               "rg12_vs_rg12p_bgr": got["rg12"].tobytes() == got["rg12p_bgr"].tobytes(),
@@ -142,28 +117,17 @@ def main():
               "rg12p_vs_single_pair": all(got["rg12p"][i].tobytes() == eng.match(rg_dec[0], rg_dec[1]).tobytes()
                                           for i in (0, n - 1))}
 
-    reps = 50
-    kernels = {}
     rg10p = [X.from_samples(v >> 2, "bayer_rg10p") for v in rg12]
     rg8 = [(v >> 4).astype(np.uint8) for v in rg12]
-    # the profile ids replay the format of the engine's last images / rectified call: make one of each first
-    for name, pid, call in (
+    kernels = B.kernels_vs_copy(eng, (
             ("image_ingest_rg12p", "image_ingest", lambda: eng.match_images(rg12p[0], rg12p[1], format="bayer_rg12p")),
             ("image_ingest_rg10p", "image_ingest", lambda: eng.match_images(rg10p[0], rg10p[1], format="bayer_rg10p")),
             ("image_ingest_rg12", "image_ingest", lambda: eng.match_images(rg12[0], rg12[1], format="bayer_rg12")),
             ("image_ingest_mono12p", "image_ingest", lambda: eng.match_images(mono12p[0], mono12p[1], format="mono12p")),
             ("image_ingest_rg8", "image_ingest", lambda: eng.match_images(rg8[0], rg8[1], format="bayer_rggb")),
             ("rectify_rg12p", "rectify", lambda: eng.match_rectified(raw[0], raw[1], format="bayer_rg12p")),
-            ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))):
-        call()
-        k_ms, k_bytes = eng.profile_kernel(pid, reps=reps)
-        cp_bytes = int(k_bytes // 2)
-        cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
-        kernels[name] = {"ms_per_wave": round(k_ms, 4), "algorithmic_bytes": k_bytes,
-                         "achieved_gbs": round(k_bytes / (k_ms * 1e-3) / 1e9, 1),
-                         "d2d_copy_same_bytes_ms": round(cp_ms, 4), "d2d_copy_gbs": round(cp_gbs, 1),
-                         "kernel_vs_copy": round(cp_ms / k_ms, 4)}
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)   # noqa: E731
+            ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))), reps=50, dev=dev)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     host_rate = round(n / statistics.median(host_s), 2)
     calls = {"rg12p": "adc_match_images_batch_device (BayerRG12p, tight rows of 675 bytes)",
              "rg12p_bgr": "adc_match_batch_device (the same frames converted beforehand, packed BGR)",
@@ -173,25 +137,23 @@ def main():
              "rect_rg12p": "adc_match_rectified_batch_device (640x480 raw BayerRG12p, CV_16SC2 maps)",
              "rect_bgr_raw": "adc_match_rectified_batch_device (the same raw frames converted beforehand, BGR)"}
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            **{k: {"value": rate(ms[k]), "call": c} for k, c in calls.items()},
+            **{k: {"value": rate[k], "call": c} for k, c in calls.items()},
             "host_unpack_cvtcolor_scale_remap": {
                 "value": host_rate, "opencv": cv2.__version__,
                 "call": "numpy unpack + cv2.cvtColor + cv2.convertScaleAbs + cv2.remap on the host (both views, 16 threads) "
                         "+ adc_match_batch"},
-            "rg12p_vs_rg12p_bgr": round(rate(ms["rg12p"]) / rate(ms["rg12p_bgr"]), 4),
-            "rg12_vs_rg12p_bgr": round(rate(ms["rg12"]) / rate(ms["rg12p_bgr"]), 4),
-            "mono12p_vs_mono12p_bgr": round(rate(ms["mono12p"]) / rate(ms["mono12p_bgr"]), 4),
-            "rect_rg12p_vs_rect_bgr_raw": round(rate(ms["rect_rg12p"]) / rate(ms["rect_bgr_raw"]), 4),
-            "rect_rg12p_vs_host": round(rate(ms["rect_rg12p"]) / host_rate, 2),
+            "rg12p_vs_rg12p_bgr": round(rate["rg12p"] / rate["rg12p_bgr"], 4),
+            "rg12_vs_rg12p_bgr": round(rate["rg12"] / rate["rg12p_bgr"], 4),
+            "mono12p_vs_mono12p_bgr": round(rate["mono12p"] / rate["mono12p_bgr"], 4),
+            "rect_rg12p_vs_rect_bgr_raw": round(rate["rect_rg12p"] / rate["rect_bgr_raw"], 4),
+            "rect_rg12p_vs_host": round(rate["rect_rg12p"] / host_rate, 2),
             "windows_ms": {k: [round(x, 2) for x in v] for k, v in ms.items()},
             "checks": checks,
             "rounds": args.rounds, "steps_per_round": args.steps, "wave_pairs": eng.wave_pairs, "lanes": eng.lanes,
-            "kernels": {**kernels, "note": f"one wave; CUDA events over {reps} launches; the copy is one cudaMemcpyAsync "
-                                           f"of algorithmic_bytes / 2, read + write counted"},
-            "card": card()}
+            "kernels": kernels,
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

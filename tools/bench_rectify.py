@@ -10,7 +10,7 @@ from 640x480 raw BGR frames, in one process so that every figure comes from the 
 * rect_bgr  : adc_match_batch_device on the same frames rectified by cv2.remap beforehand, packed BGR on the device: the
               yardstick for `rectified`, whose image content (black borders, resampled texture, and so the work of the
               data-dependent refinement) differs from Cone's
-  The three are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The three are timed in alternating windows (`--rounds`); the medians are reported.
 * host      : the same raw frames through cv2.remap on the host (both views of every pair, OpenCV's own threading)
               followed by adc_match_batch on the rectified images: wall clock over one batch, after a warm-up batch.
 * kernel    : the rectified ingestion kernel alone over one wave (adc_profile_kernel id 14, CUDA events), next to a
@@ -19,112 +19,80 @@ from 640x480 raw BGR frames, in one process so that every figure comes from the 
 Every map of the rectified batch is checked bit for bit against the host path's and rect_bgr's.  The card's name and power limit are
 recorded beside the numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
 import statistics
 import sys
-import time
-from pathlib import Path
 
 import cv2
-import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
-
-
-def rig_maps(sw, sh, W, H, baseline):
-    K = np.array([[0.9 * sw, 0, sw / 2 - 3.3], [0, 0.9 * sw, sh / 2 + 2.1], [0, 0, 1]], np.float64)
-    dist = np.array([-0.12, 0.05, 0.0008, -0.0006, -0.004])
-    R, _ = cv2.Rodrigues(np.array([0.004, -0.011 * baseline, 0.002]))
-    P = np.array([[0.95 * W, 0, W / 2, 0], [0, 0.95 * W, H / 2, 0], [0, 0, 1, 0]], np.float64)
-    return cv2.initUndistortRectifyMap(K, dist, R, P, (W, H), cv2.CV_16SC2)
+import benchlib as B
+import adcensus_b200 as A
+import adc_testlib as T
+import rectify_testlib as R
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_rectify.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
     sw, sh = 640, 480
-    D, n = 64, args.pairs
+    D = 64
     raw = [cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR) for img in (left, right)]
-    maps = [rig_maps(sw, sh, w, h, s) for s in (1, -1)]
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)
+    maps = [R.cone_rig(cv2, sw, sh, w, h, cv2.CV_16SC2, s) for s in (1, -1)]
     d_left, d_right = rep(left), rep(right)
     r_left, r_right = rep(raw[0]), rep(raw[1])
-    remap = lambda img, m: cv2.remap(img, *m, cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT, borderValue=0)
-    b_left, b_right = rep(remap(raw[0], maps[0])), rep(remap(raw[1], maps[1]))
+    b_left, b_right = rep(B.remap(raw[0], maps[0])), rep(B.remap(raw[1], maps[1]))
     out = {k: torch.empty((n, h, w), dtype=torch.float32, device=dev) for k in ("bgr", "rectified", "rect_bgr")}
     eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D))
     eng.set_rectification(maps[0], maps[1], (sw, sh))
     eng.set_pipelined(True)
     st = torch.cuda.current_stream()
 
-    def bgr():
+    def bgr(_):
         eng.match_batch_device(n, d_left.data_ptr(), d_right.data_ptr(), out["bgr"].data_ptr(), st.cuda_stream)
 
-    def rectified():
+    def rectified(_):
         eng.match_rectified_batch_device(n, r_left.data_ptr(), r_right.data_ptr(), d_disp=out["rectified"].data_ptr(),
                                          stream=st.cuda_stream)
 
-    def rect_bgr():
+    def rect_bgr(_):
         eng.match_batch_device(n, b_left.data_ptr(), b_right.data_ptr(), out["rect_bgr"].data_ptr(), st.cuda_stream)
 
-    ms = alternating_windows(eng, st, (bgr, rectified, rect_bgr), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (bgr, rectified, rect_bgr), args.steps, args.warmup, args.rounds)
     eng.set_pipelined(False)
 
     # host path: cv2.remap of every view, then adc_match_batch (pointer-array form) on the rectified images
     lefts, rights = [raw[0]] * n, [raw[1]] * n
 
     def host():
-        return eng.match_batch_ptrs([remap(x, maps[0]) for x in lefts], [remap(x, maps[1]) for x in rights])
+        return eng.match_batch_ptrs([B.remap(x, maps[0]) for x in lefts], [B.remap(x, maps[1]) for x in rights])
 
-    host()
-    host_s = []
-    for _ in range(args.rounds):
-        t0 = time.perf_counter()
-        host_maps = host()
-        host_s.append(time.perf_counter() - t0)
+    host_s, host_maps = B.host_seconds(host, args.rounds)
     got = out["rectified"].cpu().numpy()
     got_b = out["rect_bgr"].cpu().numpy()
+    golden = B.golden()
     checks = {"rectified_vs_host": all(got[i].tobytes() == host_maps[i].tobytes() for i in range(n)),
               "rectified_vs_rect_bgr": got.tobytes() == got_b.tobytes(),
-              "bgr_vs_reference": all(T.sha(m) == json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))
-                                      ["MEDIAN/DISP_L"] for m in out["bgr"].cpu().numpy())}
+              "bgr_vs_reference": all(T.sha(m) == golden for m in out["bgr"].cpu().numpy())}
 
     reps = 50
-    k_ms, k_bytes = eng.profile_kernel("rectify", reps=reps)
-    cp_bytes = int(k_bytes // 2)
-    cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    k_ms, k_bytes, cp_ms, cp_gbs = B.kernel_vs_copy(eng, "rectify", reps, dev)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     host_rate = round(n / statistics.median(host_s), 2)
     line = {"workload": "cone_450x375_d64_batch256_from_640x480", "unit": "maps/s",
-            "bgr": {"value": rate(ms["bgr"]), "call": "adc_match_batch_device (packed BGR, already rectified)"},
-            "rectified": {"value": rate(ms["rectified"]),
+            "bgr": {"value": rate["bgr"], "call": "adc_match_batch_device (packed BGR, already rectified)"},
+            "rectified": {"value": rate["rectified"],
                           "call": "adc_match_rectified_batch_device (640x480 raw BGR, CV_16SC2 maps)"},
             "host_remap": {"value": host_rate,
                            "call": "cv2.remap on the host (both views) + adc_match_batch on the rectified images",
                            "cv2_threads": cv2.getNumThreads(), "opencv": cv2.__version__},
-            "rect_bgr": {"value": rate(ms["rect_bgr"]),
+            "rect_bgr": {"value": rate["rect_bgr"],
                          "call": "adc_match_batch_device (the same frames rectified beforehand, packed BGR)"},
-            "rectified_vs_bgr": round(rate(ms["rectified"]) / rate(ms["bgr"]), 4),
-            "rectified_vs_rect_bgr": round(rate(ms["rectified"]) / rate(ms["rect_bgr"]), 4),
-            "rectified_vs_host_remap": round(rate(ms["rectified"]) / host_rate, 2),
+            "rectified_vs_bgr": round(rate["rectified"] / rate["bgr"], 4),
+            "rectified_vs_rect_bgr": round(rate["rectified"] / rate["rect_bgr"], 4),
+            "rectified_vs_host_remap": round(rate["rectified"] / host_rate, 2),
             "checks": checks,
             "rounds": args.rounds, "steps_per_round": args.steps, "wave_pairs": eng.wave_pairs, "lanes": eng.lanes,
             "rectify_kernel": {"ms_per_wave": round(k_ms, 4), "algorithmic_bytes": k_bytes,
@@ -134,10 +102,9 @@ def main():
             "d2d_copy_same_bytes": {"ms": round(cp_ms, 4), "achieved_gbs": round(cp_gbs, 1),
                                     "note": "one cudaMemcpyAsync of algorithmic_bytes / 2, read + write counted"},
             "kernel_vs_copy": round(cp_ms / k_ms, 4),
-            "card": card()}
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

@@ -9,8 +9,8 @@ that every figure comes from the same run:
             256 f32 maps (+inf = missing, max_size 200, max_diff 2)
 * s16     : the same batch, then on the second stream the DISP_S16 reprojection and the S16 filter
             ((min_disparity - 1) * 16 missing, max_size 200, max_diff 2 * 16: INTEGRATION.md's call)
-  Each path is timed in `rounds` alternating windows of `steps` steps (tools/bench_reproject.windows); the medians are
-  reported.  Consecutive steps alternate between two map buffers.
+  Each path is timed in `rounds` alternating windows of `steps` steps (CUDA events on the first stream, which waits for
+  the second at the end of a window); the medians are reported.  Consecutive steps alternate between two map buffers.
 * kernel  : the filter alone over the 256 Cone maps, F32 and S16, CUDA events around each call (a fresh copy of the
             maps is made before each, outside the events), next to a device-to-device copy of the map bytes.
 * adversarial : one 1920x1080 S16 map each: a one-pixel serpentine that makes one component, a constant map, a
@@ -21,43 +21,22 @@ Every filtered map is checked against the numpy restatement (tests/speckle_testl
 the reference's Cone MEDIAN/DISP_L hash.  The card's name, power limit and clocks are recorded beside the numbers.
 Prints one JSON line; writes nothing.
 """
-import argparse
-import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 from concurrent.futures import ThreadPoolExecutor
-from pathlib import Path
 
 import cv2
 import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import speckle_testlib as S  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_reproject import windows  # noqa: E402
-from bench_volume_export import d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import adc_testlib as T
+import speckle_testlib as S
 
 MAX_SIZE, MAX_DIFF = 200, 2
-
-
-def clocks():
-    """SM clock now and its maximum (read-only nvidia-smi query)."""
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i",
-                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=10).stdout
-        sm, mx = [c.strip() for c in out.strip().splitlines()[0].split(",")]
-        return {"sm_clock": sm, "max_sm_clock": mx}
-    except Exception as ex:
-        return {"error": str(ex)}
 
 
 def filter_ms(eng, n, src, dst, t, nv, md, work, wb, reps, st):
@@ -77,19 +56,12 @@ def filter_ms(eng, n, src, dst, t, nv, md, work, wb, reps, st):
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_speckles.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
-    N, D, n = w * h, 64, args.pairs
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)
+    N, D = w * h, 64
     d_left, d_right = rep(left), rep(right)
     eng = A.Engine(w, h, A.ADCensusOption(max_disparity=D))
     eng.set_pipelined(True)
@@ -120,11 +92,11 @@ def main():
                                          work.data_ptr(), wb, s2.cuda_stream)
     s16_path.__name__ = "s16"
 
-    ms = windows(eng, st, s2, (plain, f32, s16_path), args.steps, args.warmup, args.rounds)
+    ms = B.windows(eng, st, (plain, f32, s16_path), args.steps, args.warmup, args.rounds, side=s2)
     eng.set_pipelined(False)
 
     # checks: the matched maps are the reference's, the filtered ones the restatement's
-    golden = json.loads(str(np.load(T.GOLDEN_DIR / "golden_cone_full.npz")["hashes"]))["MEDIAN/DISP_L"]
+    golden = B.golden()
     m0 = disp["plain"][0][0].cpu().numpy()
     raw16 = eng.reproject(m0, np.eye(4), ["disp_s16"])["disp_s16"]
     want_f = S.filter_f32(m0, np.inf, MAX_SIZE, MAX_DIFF)
@@ -146,8 +118,8 @@ def main():
     checks["kernel_f32_vs_restatement"] = S.same_bits(dst_f[-1].cpu().numpy(), want_f)
     checks["kernel_s16_vs_restatement"] = bool(np.array_equal(dst_s[-1].cpu().numpy(), want_s))
     cp = torch.empty(n * N * 4, dtype=torch.uint8, device=dev)
-    cp_f_ms, cp_f_gbs = d2d_copy(cp, n * N * 4, 20)
-    cp_s_ms, cp_s_gbs = d2d_copy(cp, n * N * 2, 20)
+    cp_f_ms, cp_f_gbs = B.d2d_copy(cp, n * N * 4, 20)
+    cp_s_ms, cp_s_gbs = B.d2d_copy(cp, n * N * 2, 20)
     eng.close()
 
     # adversarial 1920x1080 maps (S16; new_val 0 marks the serpentine's background as missing)
@@ -184,17 +156,17 @@ def main():
         cv_ms = (time.perf_counter() - t0) * 1e3
     checks["opencv_vs_restatement"] = all(np.array_equal(a, want_s) for a in host)
 
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "plain": {"value": rate(ms["plain"]), "call": "adc_match_batch_device"},
-            "f32": {"value": rate(ms["f32"]),
+            "plain": {"value": rate["plain"], "call": "adc_match_batch_device"},
+            "f32": {"value": rate["f32"],
                     "call": "adc_match_batch_device + adc_filter_speckles_batch_device (F32) on a second stream after "
                             "adc_join"},
-            "f32_vs_plain": round(rate(ms["f32"]) / rate(ms["plain"]), 4),
-            "s16": {"value": rate(ms["s16"]),
+            "f32_vs_plain": round(rate["f32"] / rate["plain"], 4),
+            "s16": {"value": rate["s16"],
                     "call": "adc_match_batch_device + adc_reproject_batch_device (disp_s16) + "
                             "adc_filter_speckles_batch_device (S16) on a second stream after adc_join"},
-            "s16_vs_plain": round(rate(ms["s16"]) / rate(ms["plain"]), 4),
+            "s16_vs_plain": round(rate["s16"] / rate["plain"], 4),
             "kernel_f32": {"ms_per_256_maps": round(k_f32, 4), "d2d_copy_of_map_bytes_ms": round(cp_f_ms, 4),
                            "d2d_copy_gbs": round(cp_f_gbs, 1)},
             "kernel_s16": {"ms_per_256_maps": round(k_s16, 4), "d2d_copy_of_map_bytes_ms": round(cp_s_ms, 4),
@@ -203,9 +175,8 @@ def main():
             "opencv_host_256_s16_maps": {"ms": round(cv_ms, 2), "threads": cores, "opencv": cv2.__version__,
                                          "ipp": bool(cv2.ipp.useIPP())},
             "checks": checks,
-            "rounds": args.rounds, "steps_per_round": args.steps, "card": {**card(), **clocks()}}
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+            "rounds": args.rounds, "steps_per_round": args.steps, "card": {**B.card(), **B.clocks()}}
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":

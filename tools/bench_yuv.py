@@ -12,9 +12,9 @@ process so that every figure comes from the same run:
                  into each row) (ADC_IMG_YUYV)
 * yuyv_bgr     : adc_match_batch_device on the same views decoded beforehand, packed BGR
 * rect_nv12    : adc_match_rectified_batch_device on raw 640 x 480 NV12 frames (Cone resized and encoded), rectified
-                 through initUndistortRectifyMap maps (CV_16SC2) of bench_rectify's made-up rig
+                 through initUndistortRectifyMap maps (CV_16SC2) of rectify_testlib's made-up rig
 * rect_bgr_raw : adc_match_rectified_batch_device on the same raw frames decoded beforehand, [N, 480, 640, 3]
-  The six are timed in alternating windows (`--rounds`, bench_volume_export's timing); the medians are reported.
+  The six are timed in alternating windows (`--rounds`); the medians are reported.
 * host         : the same raw NV12 frames through cv2.cvtColor and cv2.remap on the host (both views of every pair, 16
                  OpenCV threads) followed by adc_match_batch on the rectified images: wall clock over one batch, after a
                  warm-up batch.
@@ -26,44 +26,27 @@ process so that every figure comes from the same run:
 Every YUV map is checked bit for bit against the packed-BGR maps of the decoded images (and the host path's).  The
 card's name and power limit are recorded beside the numbers.  Prints one JSON line; writes nothing.
 """
-import argparse
-import json
 import statistics
 import sys
-import time
-from pathlib import Path
 
 import cv2
 import numpy as np
 import torch
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
-sys.path.insert(0, str(ROOT / "tools"))
-import adcensus_b200 as A  # noqa: E402
-import adc_testlib as T  # noqa: E402
-import yuv_testlib as Y  # noqa: E402
-from bench_cost_input import card  # noqa: E402
-from bench_rectify import rig_maps  # noqa: E402
-from bench_volume_export import alternating_windows, d2d_copy  # noqa: E402
+import benchlib as B
+import adcensus_b200 as A
+import rectify_testlib as R
+import yuv_testlib as Y
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--rounds", type=int, default=3, help="alternating timed windows of each path")
-    ap.add_argument("--pairs", type=int, default=256)
-    args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_yuv.py: no CUDA device (there is no CPU fallback)")
+    args = B.args(__file__)
     dev = torch.device("cuda", 0)
-    left, right = T.load_cone()
+    n = args.pairs
+    left, right, rep = B.cone(n)
     h, w, _ = left.shape
     sw, sh = 640, 480
-    D, n = 64, args.pairs
-    rep = lambda a: torch.from_numpy(np.repeat(a[None], n, 0)).to(dev)   # noqa: E731
+    D = 64
 
     # NV12 in 450 x 376 surfaces
     nv = [Y.encode(img, "nv12") for img in (left, right)]
@@ -81,7 +64,7 @@ def main():
     # raw 640 x 480 NV12 frames
     raw = [Y.encode(cv2.resize(img, (sw, sh), interpolation=cv2.INTER_LINEAR), "nv12") for img in (left, right)]
     raw_bgr = [Y.cv_decode(cv2, r, "nv12", sw, sh) for r in raw]
-    maps = [rig_maps(sw, sh, w, h, s) for s in (1, -1)]
+    maps = [R.cone_rig(cv2, sw, sh, w, h, cv2.CV_16SC2, s) for s in (1, -1)]
     b_nv = [rep(x) for x in nv_dec]
     b_yu = [rep(x) for x in yu_dec]
     r_nv = [rep(x) for x in raw]
@@ -94,50 +77,41 @@ def main():
     st = torch.cuda.current_stream()
     nv_raw_desc = A.image_desc("nv12")
 
-    def nv12():
+    def nv12(_):
         eng.match_images_batch_device(n, nv_d[0].data_ptr(), nv_d[1].data_ptr(), image=nv_desc,
                                       d_disp=out["nv12"].data_ptr(), stream=st.cuda_stream)
 
-    def nv12_bgr():
+    def nv12_bgr(_):
         eng.match_batch_device(n, b_nv[0].data_ptr(), b_nv[1].data_ptr(), out["nv12_bgr"].data_ptr(), st.cuda_stream)
 
-    def yuyv_sbs():
+    def yuyv_sbs(_):
         eng.match_images_batch_device(n, sbs_d.data_ptr(), sbs_d.data_ptr() + 2 * w, image=yu_desc,
                                       d_disp=out["yuyv_sbs"].data_ptr(), stream=st.cuda_stream)
 
-    def yuyv_bgr():
+    def yuyv_bgr(_):
         eng.match_batch_device(n, b_yu[0].data_ptr(), b_yu[1].data_ptr(), out["yuyv_bgr"].data_ptr(), st.cuda_stream)
 
-    def rect_nv12():
+    def rect_nv12(_):
         eng.match_rectified_batch_device(n, r_nv[0].data_ptr(), r_nv[1].data_ptr(), image=nv_raw_desc,
                                          d_disp=out["rect_nv12"].data_ptr(), stream=st.cuda_stream)
 
-    def rect_bgr_raw():
+    def rect_bgr_raw(_):
         eng.match_rectified_batch_device(n, r_bgr[0].data_ptr(), r_bgr[1].data_ptr(),
                                          d_disp=out["rect_bgr_raw"].data_ptr(), stream=st.cuda_stream)
 
-    ms = alternating_windows(eng, st, (nv12, nv12_bgr, yuyv_sbs, yuyv_bgr, rect_nv12, rect_bgr_raw), args.steps,
-                             args.warmup, args.rounds)
+    ms = B.windows(eng, st, (nv12, nv12_bgr, yuyv_sbs, yuyv_bgr, rect_nv12, rect_bgr_raw), args.steps, args.warmup,
+                   args.rounds)
     eng.set_pipelined(False)
 
     # host path: cv2.cvtColor + cv2.remap of every view on 16 threads, then adc_match_batch (pointer-array form)
-    threads = cv2.getNumThreads()
-    cv2.setNumThreads(16)
-    remap = lambda img, m: cv2.remap(img, *m, cv2.INTER_LINEAR, borderMode=cv2.BORDER_CONSTANT, borderValue=0)  # noqa: E731
     code = cv2.COLOR_YUV2BGR_NV12
     lefts, rights = [raw[0]] * n, [raw[1]] * n
 
     def host():
-        return eng.match_batch_ptrs([remap(cv2.cvtColor(x, code), maps[0]) for x in lefts],
-                                    [remap(cv2.cvtColor(x, code), maps[1]) for x in rights])
+        return eng.match_batch_ptrs([B.remap(cv2.cvtColor(x, code), maps[0]) for x in lefts],
+                                    [B.remap(cv2.cvtColor(x, code), maps[1]) for x in rights])
 
-    host()
-    host_s = []
-    for _ in range(args.rounds):
-        t0 = time.perf_counter()
-        host_maps = host()
-        host_s.append(time.perf_counter() - t0)
-    cv2.setNumThreads(threads)
+    host_s, host_maps = B.host_seconds(host, args.rounds, threads=16)
     got = {k: v.cpu().numpy() for k, v in out.items()}
     checks = {"nv12_vs_nv12_bgr": got["nv12"].tobytes() == got["nv12_bgr"].tobytes(),
               "yuyv_sbs_vs_yuyv_bgr": got["yuyv_sbs"].tobytes() == got["yuyv_bgr"].tobytes(),
@@ -146,52 +120,39 @@ def main():
               "nv12_vs_single_pair": all(got["nv12"][i].tobytes() == eng.match(nv_dec[0], nv_dec[1]).tobytes()
                                          for i in (0, n - 1))}
 
-    reps = 50
-    kernels = {}
-    # the profile ids replay the format of the engine's last images / rectified call: make one of each first
     sbs_views = [np.ascontiguousarray(sbs[:, x:x + w]) for x in (0, w)]
-    for name, pid, call in (("image_ingest_nv12", "image_ingest", lambda: eng.match_images(nv[0], nv[1], format="nv12")),
-                            ("image_ingest_yuyv", "image_ingest",
-                             lambda: eng.match_images(sbs_views[0], sbs_views[1], format="yuyv")),
-                            ("rectify_nv12", "rectify", lambda: eng.match_rectified(raw[0], raw[1], format="nv12")),
-                            ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))):
-        call()
-        k_ms, k_bytes = eng.profile_kernel(pid, reps=reps)
-        cp_bytes = int(k_bytes // 2)
-        cp_ms, cp_gbs = d2d_copy(torch.zeros(cp_bytes, dtype=torch.uint8, device=dev), cp_bytes, reps)
-        kernels[name] = {"ms_per_wave": round(k_ms, 4), "algorithmic_bytes": k_bytes,
-                         "achieved_gbs": round(k_bytes / (k_ms * 1e-3) / 1e9, 1),
-                         "d2d_copy_same_bytes_ms": round(cp_ms, 4), "d2d_copy_gbs": round(cp_gbs, 1),
-                         "kernel_vs_copy": round(cp_ms / k_ms, 4)}
-    rate = lambda v: round(n * args.steps / (statistics.median(v) * 1e-3), 2)   # noqa: E731
+    kernels = B.kernels_vs_copy(eng, (
+        ("image_ingest_nv12", "image_ingest", lambda: eng.match_images(nv[0], nv[1], format="nv12")),
+        ("image_ingest_yuyv", "image_ingest", lambda: eng.match_images(sbs_views[0], sbs_views[1], format="yuyv")),
+        ("rectify_nv12", "rectify", lambda: eng.match_rectified(raw[0], raw[1], format="nv12")),
+        ("rectify_bgr", "rectify", lambda: eng.match_rectified(raw_bgr[0], raw_bgr[1]))), reps=50, dev=dev)
+    rate = {k: B.maps_per_s(v, n, args.steps) for k, v in ms.items()}
     host_rate = round(n / statistics.median(host_s), 2)
     line = {"workload": "cone_450x375_d64_batch256", "unit": "maps/s",
-            "nv12": {"value": rate(ms["nv12"]), "call": "adc_match_images_batch_device (NV12, 450x376 surfaces, pitch 512)"},
-            "nv12_bgr": {"value": rate(ms["nv12_bgr"]),
+            "nv12": {"value": rate["nv12"], "call": "adc_match_images_batch_device (NV12, 450x376 surfaces, pitch 512)"},
+            "nv12_bgr": {"value": rate["nv12_bgr"],
                          "call": "adc_match_batch_device (the same frames decoded beforehand, packed BGR)"},
-            "yuyv_sbs": {"value": rate(ms["yuyv_sbs"]), "call": "adc_match_images_batch_device (side-by-side YUYV 900x375)"},
-            "yuyv_bgr": {"value": rate(ms["yuyv_bgr"]),
+            "yuyv_sbs": {"value": rate["yuyv_sbs"], "call": "adc_match_images_batch_device (side-by-side YUYV 900x375)"},
+            "yuyv_bgr": {"value": rate["yuyv_bgr"],
                          "call": "adc_match_batch_device (the same views decoded beforehand, packed BGR)"},
-            "rect_nv12": {"value": rate(ms["rect_nv12"]),
+            "rect_nv12": {"value": rate["rect_nv12"],
                           "call": "adc_match_rectified_batch_device (640x480 raw NV12, CV_16SC2 maps)"},
-            "rect_bgr_raw": {"value": rate(ms["rect_bgr_raw"]),
+            "rect_bgr_raw": {"value": rate["rect_bgr_raw"],
                              "call": "adc_match_rectified_batch_device (the same raw frames decoded beforehand, BGR)"},
             "host_cvtcolor_remap": {"value": host_rate,
                                     "call": "cv2.cvtColor + cv2.remap on the host (both views, 16 threads) + adc_match_batch",
                                     "opencv": cv2.__version__},
-            "nv12_vs_nv12_bgr": round(rate(ms["nv12"]) / rate(ms["nv12_bgr"]), 4),
-            "yuyv_sbs_vs_yuyv_bgr": round(rate(ms["yuyv_sbs"]) / rate(ms["yuyv_bgr"]), 4),
-            "rect_nv12_vs_rect_bgr_raw": round(rate(ms["rect_nv12"]) / rate(ms["rect_bgr_raw"]), 4),
-            "rect_nv12_vs_host": round(rate(ms["rect_nv12"]) / host_rate, 2),
+            "nv12_vs_nv12_bgr": round(rate["nv12"] / rate["nv12_bgr"], 4),
+            "yuyv_sbs_vs_yuyv_bgr": round(rate["yuyv_sbs"] / rate["yuyv_bgr"], 4),
+            "rect_nv12_vs_rect_bgr_raw": round(rate["rect_nv12"] / rate["rect_bgr_raw"], 4),
+            "rect_nv12_vs_host": round(rate["rect_nv12"] / host_rate, 2),
             "windows_ms": {k: [round(x, 2) for x in v] for k, v in ms.items()},
             "checks": checks,
             "rounds": args.rounds, "steps_per_round": args.steps, "wave_pairs": eng.wave_pairs, "lanes": eng.lanes,
-            "kernels": {**kernels, "note": f"one wave; CUDA events over {reps} launches; the copy is one cudaMemcpyAsync "
-                                           f"of algorithmic_bytes / 2, read + write counted"},
-            "card": card()}
+            "kernels": kernels,
+            "card": B.card()}
     eng.close()
-    print(json.dumps(line), flush=True)
-    return 0 if all(checks.values()) else 1
+    return B.emit(line, all(checks.values()))
 
 
 if __name__ == "__main__":
