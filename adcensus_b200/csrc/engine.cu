@@ -771,24 +771,33 @@ MatchReq output_req(const void* cost, int cost_layout, int cost_dtype, const flo
 // The rules of an image descriptor that need no image size (adc_match_images*, checked before the engine).
 int check_image_desc(const char* fn, const adc_image_desc* img) {
     if (!img) return ADC_OK;
-    if (img_family(img->format) == IMG_UNKNOWN) return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
+    switch (img_code_error(img->format)) {
+        case 1: return fail(ADC_ERR_ARG, "%s: img->format %d unknown", fn, img->format);
+        case 2: return fail(ADC_ERR_ARG, "%s: img->format %d: ADC_IMG_YUV_BT709 and ADC_IMG_YUV_FULL_RANGE apply to the "
+                            "YUV formats only", fn, img->format);
+    }
     if (img->reserved != 0) return fail(ADC_ERR_ARG, "%s: img->reserved must be zero", fn);
     if (img->row_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld is negative", fn, (long long)img->row_pitch);
     if (img->plane_pitch < 0) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld is negative", fn, (long long)img->plane_pitch);
     if (img->image_stride < 0) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld is negative", fn, (long long)img->image_stride);
     if (img_planes(img->format) == 1 && img->plane_pitch != 0)
-        return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format other than ADC_IMG_RGB_PLANAR, ADC_IMG_NV12 "
-                    "and ADC_IMG_NV21", fn);
+        return fail(ADC_ERR_ARG, "%s: img->plane_pitch must be 0 for a format other than ADC_IMG_RGB_PLANAR and the 4:2:0 "
+                    "YUV formats", fn);
+    if (img_yuv_planar(img->format) && img->row_pitch % 2)
+        return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld must be even for I420 / YV12 (the chroma pitch is row_pitch / 2)",
+                    fn, (long long)img->row_pitch);
     return ADC_OK;
 }
 
 // The rule the device entries add for the formats with one sample per 16-bit word (img_words), whose words the kernels
-// load whole: both bases, the row pitch and the image stride are even.  Needs no image size.
+// load whole: both bases, the row pitch, the plane pitch (P016's chroma plane) and the image stride are even.  Needs no
+// image size.
 int check_image_align(const char* fn, const adc_image_desc* img, const void* left, const void* right) {
     if (!img || !img_words(img->format)) return ADC_OK;
     if ((uintptr_t)left % 2) return fail(ADC_ERR_ARG, "%s: d_left must be 2-byte aligned for a 16-bit format", fn);
     if ((uintptr_t)right % 2) return fail(ADC_ERR_ARG, "%s: d_right must be 2-byte aligned for a 16-bit format", fn);
     if (img->row_pitch % 2) return fail(ADC_ERR_ARG, "%s: img->row_pitch %lld must be even for a 16-bit format", fn, (long long)img->row_pitch);
+    if (img->plane_pitch % 2) return fail(ADC_ERR_ARG, "%s: img->plane_pitch %lld must be even for a 16-bit format", fn, (long long)img->plane_pitch);
     if (img->image_stride % 2) return fail(ADC_ERR_ARG, "%s: img->image_stride %lld must be even for a 16-bit format", fn, (long long)img->image_stride);
     return ADC_OK;
 }
@@ -884,10 +893,13 @@ int ingest_host_pair(adc_engine* e, const AdcImageGeom& g, const AdcRectGeom* re
     const size_t foot = (size_t)tight.image_stride, tp = (size_t)tight.row_pitch;
     // one block of tight rows per plane
     for (int v = 0; v < 2; v++)
-        for (int c = 0; c < img_planes(g.format); c++)
-            CK(cudaMemcpy2DAsync(raw + v * foot + c * tight.plane_pitch, tp, (v ? right : left) + c * g.plane_pitch,
-                                 (size_t)g.row_pitch, tp, (size_t)img_plane_rows(g.format, c, sh), cudaMemcpyHostToDevice,
-                                 st));
+        for (int c = 0; c < img_planes(g.format); c++) {
+            const size_t ctp = (size_t)img_plane_row_pitch(g.format, c, (long long)tp);
+            CK(cudaMemcpy2DAsync(raw + v * foot + img_plane_offset(g.format, c, sh, tight.row_pitch, tight.plane_pitch), ctp,
+                                 (v ? right : left) + img_plane_offset(g.format, c, sh, g.row_pitch, g.plane_pitch),
+                                 (size_t)img_plane_row_pitch(g.format, c, g.row_pitch), ctp,
+                                 (size_t)img_plane_rows(g.format, c, sh), cudaMemcpyHostToDevice, st));
+        }
     ingest_views(e, 1, raw, raw + foot, tight, rect, bgr, st);
     return ADC_OK;
 }

@@ -10,7 +10,8 @@
 // row (of each plane): coalesced along x.  Every pixel is loaded by exactly one thread, alpha bytes are never loaded, and
 // nothing past the last pixel of the last row is touched.  All source offsets are 64-bit.
 // The kernel template (k_image_ingest) is in k_image.cuh.  This file holds the one dispatch over every format of
-// img_format.h and instantiates the six formats above; k_bayer.cu, k_yuv.cu and k_rawdepth.cu instantiate the others.
+// img_format.h and instantiates the six formats above; k_bayer.cu, k_yuv.cu, k_yuv_video.cu, k_yuv_encodings.cu and
+// k_rawdepth.cu instantiate the others.
 #include <algorithm>
 
 #include "adc_common.cuh"
@@ -20,7 +21,7 @@ void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, cons
                              uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
 #define II_CASE(F) case F: launch_image<F>(dm, S, left, right, g, bgr, st); break;
-        ADC_IMG_FORMATS(II_CASE)
+        ADC_IMG_CODES(II_CASE)
 #undef II_CASE
     }
     ++*launches;

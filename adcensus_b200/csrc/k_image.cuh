@@ -84,32 +84,70 @@ static __device__ __forceinline__ unsigned bayer_rule(int x, int y, int c, int n
     return (unsigned)to8<S>(b) | (unsigned)to8<S>(g) << 8 | (unsigned)to8<S>(r) << 16;
 }
 
-// YUV frames (ADC_IMG_NV12 ... ADC_IMG_YVYU): pixel (x, y) of the frame at src as B | G << 8 | R << 16, equal to
-// cv::cvtColor(frame, COLOR_YUV2BGR_*) (BT.601 limited range, the rule and geometry are in include/adcensus_b200.h).
-// One luma and two chroma byte loads; neighbouring pixels share their chroma, so L1 serves that reuse.
+// YUV frames (ADC_IMG_NV12 ... ADC_IMG_P016, with or without the colour encoding flags): the conversion of one pixel's
+// Y, U, V to B | G << 8 | R << 16 under encoding E (img_encoding: bit 0 BT.709, bit 1 full range; the rules and their
+// constants are in include/adcensus_b200.h).  One constant row per encoding and two shift structures: limited range is
+// OpenCV's 20-bit rule (E = 0 is cv::cvtColor's COLOR_YUV2BGR_*), full range its 14-bit YCrCb rule.
+struct YuvCoef {
+    int rv, gu, gv, bu;
+};
+__host__ __device__ constexpr YuvCoef yuv_coef(int e) {
+    return e == 0 ? YuvCoef{1673527, -409993, -852492, 2116026} : e == 1 ? YuvCoef{1879825, -223607, -558796, 2215014}
+         : e == 2 ? YuvCoef{22987, -5636, -11698, 29049} : YuvCoef{25802, -3069, -7670, 30402};
+}
+
+template <int E>
 static __device__ __forceinline__ unsigned yuv_rule(int Y, int U, int V) {
-    const int y = max(Y - 16, 0) * 1220542 + (1 << 19), u = U - 128, v = V - 128;
-    const int r = min(max((y + 1673527 * v) >> 20, 0), 255);
-    const int g = min(max((y - 852492 * v - 409993 * u) >> 20, 0), 255);
-    const int b = min(max((y + 2116026 * u) >> 20, 0), 255);
+    constexpr YuvCoef k = yuv_coef(E);
+    const int u = U - 128, v = V - 128;
+    int r, g, b;
+    if constexpr (E & 2) {
+        r = Y + ((k.rv * v + 8192) >> 14);
+        g = Y + ((k.gu * u + k.gv * v + 8192) >> 14);
+        b = Y + ((k.bu * u + 8192) >> 14);
+    } else {
+        const int y = max(Y - 16, 0) * 1220542 + (1 << 19);
+        r = (y + k.rv * v) >> 20;
+        g = (y + k.gv * v + k.gu * u) >> 20;
+        b = (y + k.bu * u) >> 20;
+    }
+    r = min(max(r, 0), 255);
+    g = min(max(g, 0), 255);
+    b = min(max(b, 0), 255);
     return (unsigned)b | (unsigned)g << 8 | (unsigned)r << 16;
 }
 
+// Pixel (x, y) of the YUV view at src (h rows) in format F.  One luma and two chroma loads; neighbouring pixels share
+// their chroma, so L1 serves that reuse.  8-bit samples are single bytes (any alignment); P016's are whole 16-bit words
+// (2-byte aligned: the device entries require it, the host entries stage tightly), reduced to 8 bits before the rule.
 template <int F>
-static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int x,
-                                                  int y) {
-    if constexpr (img_yuv420(F)) {
+static __device__ __forceinline__ unsigned yuv_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int h,
+                                                  int x, int y) {
+    constexpr int C = img_base(F), E = img_encoding(F);
+    if constexpr (C == ADC_IMG_P016) {
+        const unsigned short* l = reinterpret_cast<const unsigned short*>(src + (long long)y * row_pitch);
+        const unsigned short* c =
+            reinterpret_cast<const unsigned short*>(src + plane_pitch + (long long)(y >> 1) * row_pitch) + (x & ~1);
+        return yuv_rule<E>(to8<8>(__ldg(l + x)), to8<8>(__ldg(c)), to8<8>(__ldg(c + 1)));
+    } else if constexpr (img_yuv_planar(F)) {
+        const long long cp = row_pitch >> 1;
+        const uint8_t* c0 = src + plane_pitch + (long long)(y >> 1) * cp + (x >> 1);
+        const uint8_t* c1 = c0 + (long long)((h + 1) >> 1) * cp;
+        const int s0 = __ldg(c0), s1 = __ldg(c1);
+        return yuv_rule<E>(__ldg(src + (long long)y * row_pitch + x), C == ADC_IMG_I420 ? s0 : s1,
+                           C == ADC_IMG_I420 ? s1 : s0);
+    } else if constexpr (img_yuv420(F)) {
         const uint8_t* c = src + plane_pitch + (long long)(y >> 1) * row_pitch + (x & ~1);
         const int c0 = __ldg(c), c1 = __ldg(c + 1);
-        return yuv_rule(__ldg(src + (long long)y * row_pitch + x), F == ADC_IMG_NV12 ? c0 : c1,
-                        F == ADC_IMG_NV12 ? c1 : c0);
+        return yuv_rule<E>(__ldg(src + (long long)y * row_pitch + x), C == ADC_IMG_NV12 ? c0 : c1,
+                           C == ADC_IMG_NV12 ? c1 : c0);
     } else {
         // byte offsets of Y0, U and V in the 4-byte macropixel; Y1 is Y0 + 2
-        constexpr int oy = F == ADC_IMG_UYVY ? 1 : 0;
-        constexpr int ou = F == ADC_IMG_YUYV ? 1 : F == ADC_IMG_UYVY ? 0 : 3;
-        constexpr int ov = F == ADC_IMG_YUYV ? 3 : F == ADC_IMG_UYVY ? 2 : 1;
+        constexpr int oy = C == ADC_IMG_UYVY ? 1 : 0;
+        constexpr int ou = C == ADC_IMG_YUYV ? 1 : C == ADC_IMG_UYVY ? 0 : 3;
+        constexpr int ov = C == ADC_IMG_YUYV ? 3 : C == ADC_IMG_UYVY ? 2 : 1;
         const uint8_t* m = src + (long long)y * row_pitch + 2ll * (x & ~1);
-        return yuv_rule(__ldg(m + oy + 2 * (x & 1)), __ldg(m + ou), __ldg(m + ov));
+        return yuv_rule<E>(__ldg(m + oy + 2 * (x & 1)), __ldg(m + ou), __ldg(m + ov));
     }
 }
 
@@ -163,7 +201,7 @@ template <int F>
 static __device__ __forceinline__ unsigned view_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int w,
                                                    int h, int x, int y) {
     if constexpr (img_mosaic(F)) return mosaic_px<F>(src, row_pitch, w, h, x, y);
-    else if constexpr (img_family(F) == IMG_YUV) return yuv_px<F>(src, row_pitch, plane_pitch, x, y);
+    else if constexpr (img_family(F) == IMG_YUV) return yuv_px<F>(src, row_pitch, plane_pitch, h, x, y);
     else if constexpr (img_family(F) == IMG_RAWDEPTH)
         return to8<img_shift(F)>(rd_sample<F>(src + (long long)y * row_pitch, x)) * 0x010101u;
     else return ImgIn<F>::px(src + y * row_pitch, x, plane_pitch);
@@ -325,5 +363,5 @@ void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t
     template void launch_rectify<F>(const AdcDims&, int, const uint8_t*, const uint8_t*, const AdcImageGeom&,          \
                                     const AdcRectGeom&, uint8_t*, cudaStream_t);
 #define II_EXTERN(F) extern II_IMAGE(F) extern II_RECTIFY(F)
-ADC_IMG_FORMATS(II_EXTERN)
+ADC_IMG_CODES(II_EXTERN)
 #undef II_EXTERN

@@ -72,7 +72,7 @@ void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, co
                                const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
     switch (g.format) {
 #define RC_CASE(F) case F: launch_rectify<F>(dm, S, left, right, g, r, bgr, st); break;
-        ADC_IMG_FORMATS(RC_CASE)
+        ADC_IMG_CODES(RC_CASE)
 #undef RC_CASE
     }
     ++*launches;

@@ -106,6 +106,16 @@ BAYER_FORMATS = {"bayer_rggb": IMG_BAYER_RGGB, "bayer_grbg": IMG_BAYER_GRBG, "ba
 # plane and an interleaved chroma plane at plane_pitch (video decoders), the others packed 4:2:2 (UVC cameras)
 IMG_NV12, IMG_NV21, IMG_YUYV, IMG_UYVY, IMG_YVYU = 32, 33, 34, 35, 36
 YUV_FORMATS = {"nv12": IMG_NV12, "nv21": IMG_NV21, "yuyv": IMG_YUYV, "uyvy": IMG_UYVY, "yvyu": IMG_YVYU}
+# the YUV containers of video decoders: I420 / YV12 (a Y plane, then U and V planes, resp. V and U, of half the row
+# pitch: FFmpeg yuv420p, PyAV, OpenCV's (H*3/2, W) I420 Mat) and P016 (NV12's layout in little-endian 16-bit words, the
+# samples MSB-aligned: NVDEC's 10- / 12- / 16-bit surface, FFmpeg p016le / p010le)
+IMG_I420, IMG_YV12, IMG_P016 = 38, 39, 40
+YUV_VIDEO_FORMATS = {"i420": IMG_I420, "yv12": IMG_YV12, "p016": IMG_P016}
+# colour encoding flags, OR-ed into the code of any YUV format (YUV_FORMATS, YUV_VIDEO_FORMATS); no flag is BT.601
+# limited range.  In a format name the encoding follows the container after a slash: "p016/bt709", "nv12/bt601_full".
+IMG_YUV_BT709, IMG_YUV_FULL_RANGE = 0x100, 0x200
+YUV_ENCODINGS = {"bt601": 0, "bt709": IMG_YUV_BT709, "bt601_full": IMG_YUV_FULL_RANGE,
+                 "bt709_full": IMG_YUV_BT709 | IMG_YUV_FULL_RANGE}
 # high-bit-depth mono and Bayer frames under their GenICam PFNC names, reduced to 8 bits as cv2.convertScaleAbs(v,
 # alpha=2**-(bits - 8)) does (Bayer: after cv2.cvtColor on the uint16 mosaic): one sample per little-endian uint16 with
 # 10, 12 or 16 significant bits ("u16"), or the 10p / 12p bit streams ("p": 4 samples in 5 bytes, 2 in 3)
@@ -136,29 +146,44 @@ def image_desc(format="bgr", row_pitch=0, plane_pitch=0, image_stride=0) -> Imag
     return ImageDesc(_img_format(format), 0, int(row_pitch), int(plane_pitch), int(image_stride))
 
 
-_IMG_NAMES = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS, **{k: v[0] for k, v in RAW_DEPTH_FORMATS.items()}}
+_IMG_NAMES = {**IMG_FORMATS, **BAYER_FORMATS, **YUV_FORMATS, **YUV_VIDEO_FORMATS,
+              **{k: v[0] for k, v in RAW_DEPTH_FORMATS.items()}}
+_YUV_CODES = set(YUV_FORMATS.values()) | set(YUV_VIDEO_FORMATS.values())
 
 
 def _img_format(v) -> int:
+    """The code of a format name ("i420", or a YUV container and an encoding: "i420/bt709") or IMG_* code."""
     if isinstance(v, str):
-        if v not in _IMG_NAMES:
-            raise ValueError(f"unknown image format {v!r} (one of {sorted(_IMG_NAMES)})")
-        return _IMG_NAMES[v]
+        name, _, enc = v.partition("/")
+        if name not in _IMG_NAMES or (enc and (enc not in YUV_ENCODINGS or _IMG_NAMES[name] not in _YUV_CODES)):
+            raise ValueError(f"unknown image format {v!r} (one of {sorted(_IMG_NAMES)}; a YUV format may be followed by "
+                             f"/ and one of {sorted(YUV_ENCODINGS)})")
+        return _IMG_NAMES[name] | YUV_ENCODINGS.get(enc, 0)
     return int(v)
 
 
 def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
     """The descriptor of one numpy view of an image: [H][W][C] (packed), [H][W] (gray, Bayer), [3][H][W] (planar R,
     G, B), [H + ceil(H/2)][2*ceil(W/2)] (NV12 / NV21: the luma rows, then the chroma rows; OpenCV's (H*3/2, W) Mat for
-    even sizes), [H][2*ceil(W/2)][2] (4:2:2, OpenCV's CV_8UC2), uint16 [H][W] (the 16-bit containers) or
-    [H][ceil(bits*W/8)] (10p / 12p: each row's bytes) with the pixels / channels of a row contiguous; the pitches come
-    from the view's strides, so slices of a larger frame (crops, side-by-side halves) need no copy."""
+    even sizes; the same shape in uint16 words for P016), [H][2*ceil(W/2)][2] (4:2:2, OpenCV's CV_8UC2), uint16 [H][W]
+    (the 16-bit containers) or [H][ceil(bits*W/8)] (10p / 12p: each row's bytes) with the pixels / channels of a row
+    contiguous; the pitches come from the view's strides, so slices of a larger frame (crops, side-by-side halves) need
+    no copy.  I420 / YV12: [H + ceil(H/2)][2*ceil(W/2)] as well (the luma rows, then the U and V planes, each
+    ceil(H/2) rows of ceil(W/2) bytes), with contiguous rows: a chroma plane's rows are half a luma row apart, which a
+    slice of a wider array does not hold.  A YUV format may carry the encoding flags (IMG_YUV_BT709, ...)."""
+    base = fmt & 0xff if (fmt & 0xff) in _YUV_CODES else fmt
     bits, container = _RAW_DEPTH.get(fmt, (8, None))
+    if base == IMG_P016:
+        container = "u16"
     dtype = np.uint16 if container == "u16" else np.uint8
     if a.dtype != dtype:
         raise ValueError(f"images of format {fmt} must be {np.dtype(dtype)}, got {a.dtype}")
     C = IMG_CHANNELS.get(fmt, 1)
-    if container == "u16":
+    if base in (IMG_NV12, IMG_NV21, IMG_P016, IMG_I420, IMG_YV12):
+        shape, inner, pitches = (H + (H + 1) // 2, 2 * ((W + 1) // 2)), (a.itemsize,), (0, a.strides[0], H * a.strides[0])
+        if base in (IMG_I420, IMG_YV12) and a.strides[0] != shape[1]:
+            raise ValueError(f"an I420 / YV12 image needs contiguous rows (row stride {shape[1]}), got {a.strides}")
+    elif container == "u16":
         shape, inner, pitches = (H, W), (2,), (0, a.strides[0], 0)
     elif container == "p":
         shape, inner, pitches = (H, (bits * W + 7) // 8), (1,), (0, a.strides[0], 0)
@@ -166,9 +191,7 @@ def _image_view_desc(a: np.ndarray, fmt: int, H: int, W: int) -> ImageDesc:
         shape, inner, pitches = (3, H, W), (1,), (0, a.strides[1], a.strides[0])
     elif fmt == IMG_GRAY or fmt in BAYER_FORMATS.values():
         shape, inner, pitches = (H, W), (1,), (0, a.strides[0], 0)
-    elif fmt in (IMG_NV12, IMG_NV21):
-        shape, inner, pitches = (H + (H + 1) // 2, 2 * ((W + 1) // 2)), (1,), (0, a.strides[0], H * a.strides[0])
-    elif fmt in YUV_FORMATS.values():
+    elif base in YUV_FORMATS.values():
         shape, inner, pitches = (H, 2 * ((W + 1) // 2), 2), (2, 1), (0, a.strides[0], 0)
     else:
         shape, inner, pitches = (H, W, C), (C, 1), (0, a.strides[0], 0)
@@ -584,11 +607,13 @@ class Engine:
         [H][W][3 or 4] (bgr, rgb, bgra, rgba), [H][W] (gray, bayer_*), [3][H][W] (rgb_planar),
         [H + ceil(H/2)][2*ceil(W/2)] (nv12, nv21) or [H][2*ceil(W/2)][2] (yuyv, uyvy, yvyu), uint16 views [H][W]
         (mono10 / 12 / 16, bayer_rg10 ...) or uint8 views [H][ceil(bits*W/8)] of the rows' bytes (mono10p, bayer_rg12p
-        ...: what a camera SDK's buffer is to numpy) whose rows may be pitched,
+        ...: what a camera SDK's buffer is to numpy), [H + ceil(H/2)][2*ceil(W/2)] uint8 (i420, yv12, contiguous rows)
+        or uint16 (p016), whose rows may be pitched,
         e.g. frame[:, :W] and frame[:, W:] of a side-by-side frame or a crop; both views need the same strides.
         The result is what match_outputs gives for the same pixels packed as BGR (for a Bayer mosaic: for
         cv2.cvtColor(view, COLOR_Bayer*2BGR), the pattern being the view's own top-left 2x2 block; for a YUV frame: for
-        cv2.cvtColor(frame, COLOR_YUV2BGR_*) cropped to W x H; for a high-bit-depth frame: for the unpacked uint16
+        cv2.cvtColor(frame, COLOR_YUV2BGR_*) cropped to W x H, or its BT.709 / full-range rule for a format name with
+        an encoding such as "p016/bt709" (include/adcensus_b200.h); for a high-bit-depth frame: for the unpacked uint16
         samples, demosaiced if Bayer, through cv2.convertScaleAbs(v, alpha=2**-(bits - 8)))."""
         return self._match_views(self._L.adc_match_images, self.height, self.width, left, right, format, maps, volumes,
                                  layout, dtype, cost, cost_layout, cost_dtype, disparity)

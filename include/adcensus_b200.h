@@ -342,20 +342,41 @@ enum { ADC_IMG_BGR = 0, ADC_IMG_RGB = 1, ADC_IMG_BGRA = 2, ADC_IMG_RGBA = 3, ADC
  *     = (N + S + 1) >> 1.
  * Only the view's own pixels are read. */
 enum { ADC_IMG_BAYER_RGGB = 16, ADC_IMG_BAYER_GRBG = 17, ADC_IMG_BAYER_BGGR = 18, ADC_IMG_BAYER_GBRG = 19 };
-/* YUV video and camera frames, 8-bit, converted on the way in:
+/* YUV video and camera frames, converted on the way in:
  *   ADC_IMG_NV12  Y plane, then one plane of interleaved U V   OpenCV COLOR_YUV2BGR_NV12 (91)   (NVDEC, V4L2, Jetson)
  *   ADC_IMG_NV21  Y plane, then one plane of interleaved V U   OpenCV COLOR_YUV2BGR_NV21 (93)   (Android)
  *   ADC_IMG_YUYV  packed 4:2:2, macropixel Y0 U Y1 V           OpenCV COLOR_YUV2BGR_YUYV (116) = _YUY2   (UVC, ZED)
  *   ADC_IMG_UYVY  packed 4:2:2, macropixel U Y0 V Y1           OpenCV COLOR_YUV2BGR_UYVY (108) = _Y422
  *   ADC_IMG_YVYU  packed 4:2:2, macropixel Y0 V Y1 U           OpenCV COLOR_YUV2BGR_YVYU (118)
- * Conversion: OpenCV's ITU-R BT.601 limited-range fixed-point rule (20-bit shift, arithmetic shifts), per pixel from
- * its own Y and the U, V of its chroma sample:
- *   y' = max(0, Y - 16) * 1220542,  u = U - 128,  v = V - 128,  h = 1 << 19
- *   R = sat_u8((y' + h + 1673527*v) >> 20)
- *   G = sat_u8((y' + h - 852492*v - 409993*u) >> 20)
- *   B = sat_u8((y' + h + 2116026*u) >> 20)
- * Every intermediate fits in int32.  Limited range means Y = 16..235 is expanded to 0..255: Y = U = V = 128 gives
- * (130, 130, 130), and Y = U = V = 0 gives (0, 154, 0).
+ *   ADC_IMG_I420  Y plane, then a U plane, then a V plane      OpenCV COLOR_YUV2BGR_I420 (128) = _IYUV   (FFmpeg
+ *                                                              yuv420p, PyAV, GStreamer I420, libcamera YUV420)
+ *   ADC_IMG_YV12  Y plane, then a V plane, then a U plane      OpenCV COLOR_YUV2BGR_YV12 (132)
+ *   ADC_IMG_P016  16-bit little-endian words: Y plane, then one plane of interleaved U V (NVDEC's high-bit-depth
+ *                 surface, FFmpeg p016le; also P010 and P012, whose samples are MSB-aligned in the same words)
+ * Colour encoding: any of these codes may be OR-ed with ADC_IMG_YUV_BT709 (ITU-R BT.709 instead of BT.601) and
+ * ADC_IMG_YUV_FULL_RANGE (Y, U, V over 0..255, JPEG / JFIF, instead of limited range).  No flag is BT.601 limited range.
+ * A flag on a format that is not YUV, or any other bit above 0xff, fails with ADC_ERR_ARG naming img->format, before
+ * the engine is checked.
+ * Conversion, per pixel from its own Y and the U, V of its chroma sample, all in int32 with arithmetic shifts,
+ * u = U - 128, v = V - 128, sat = clamp to 0..255:
+ *   limited range (OpenCV's 20-bit rule), y' = max(0, Y - 16) * 1220542, h = 1 << 19:
+ *     R = sat((y' + h + Rv*v) >> 20),  G = sat((y' + h + Gu*u + Gv*v) >> 20),  B = sat((y' + h + Bu*u) >> 20)
+ *   full range (OpenCV's 14-bit rule):
+ *     R = sat(Y + ((Rv*v + 8192) >> 14)),  G = sat(Y + ((Gu*u + Gv*v + 8192) >> 14)),  B = sat(Y + ((Bu*u + 8192) >> 14))
+ *                                      Rv        Gu       Gv       Bu
+ *   BT.601 limited (no flag)       1673527   -409993  -852492  2116026   = cv::cvtColor(frame, COLOR_YUV2BGR_<F>)
+ *   BT.709 limited                 1879825   -223607  -558796  2215014   = round(k * 2^20) of the exact BT.709
+ *                                                                          coefficients (Kr 0.2126, Kb 0.0722) times
+ *                                                                          255/224
+ *   BT.601 full range                22987     -5636   -11698    29049   = cv::cvtColor(ycrcb, COLOR_YCrCb2BGR) on
+ *                                                                          the pixels (Y, V, U)
+ *   BT.709 full range                25802     -3069    -7670    30402   = round(k * 2^14) of the exact coefficients
+ * Every intermediate fits in int32.  The BT.709 rules are within +-1 of the floating-point BT.709 matrix, rounded and
+ * saturated (limited range: for Y >= 16; below, Y - 16 clamps at 0 as in the BT.601 rule).  BT.601 limited range
+ * expands Y = 16..235 to 0..255: Y = U = V = 128 gives (130, 130, 130), and Y = U = V = 0 gives (0, 154, 0); the luma
+ * term of both limited-range rules is the same, so a grey pixel converts alike under BT.601 and BT.709.
+ * P016: every word is first reduced to 8 bits with the high-bit-depth rule at s = 8, to8(v) = min(255, (v + 127 +
+ * ((v >> 8) & 1)) >> 8) (convertTo(CV_8U, 1.0 / 256)), then the 8-bit rule of the frame's encoding applies.
  * Geometry (offsets in bytes, 64-bit; each view has its own base; image_stride as for every format):
  *   NV12 / NV21: luma of pixel (x, y) at base + i*image_stride + y*row_pitch + x; its chroma pair at
  *     base + i*image_stride + plane_pitch + (y >> 1)*row_pitch + 2*(x >> 1), U first for NV12, V first for NV21.
@@ -364,19 +385,38 @@ enum { ADC_IMG_BAYER_RGGB = 16, ADC_IMG_BAYER_GRBG = 17, ADC_IMG_BAYER_BGGR = 18
  *     Hs has plane_pitch = pitch * Hs).  Footprint: plane_pitch + ceil(H/2)*row_pitch.  plane_pitch is measured from the
  *     view's own base, so the right half of a side-by-side NV12 frame of even W is simply base + W; a top-bottom NV12
  *     pair cannot be expressed with one shared plane_pitch.
+ *   I420 / YV12: luma of pixel (x, y) at base + i*image_stride + y*row_pitch + x.  The chroma planes have row pitch
+ *     row_pitch / 2, so row_pitch must be even (ADC_ERR_ARG naming it otherwise, before the engine is checked); the
+ *     first (U for I420, V for YV12) starts at plane_pitch, the second ceil(H/2)*(row_pitch/2) bytes after the first,
+ *     and the sample of (x, y) is at (y >> 1)*(row_pitch/2) + (x >> 1) within its plane.  row_pitch: 0 = 2*ceil(W/2),
+ *     and at least that.  plane_pitch: 0 = H * row_pitch, and at least that.  Footprint: plane_pitch +
+ *     ceil(H/2)*row_pitch.  With tight pitches on an even frame this is OpenCV's (H*3/2, W) I420 Mat and FFmpeg's
+ *     contiguous yuv420p buffer.  A side-by-side I420 pair cannot be expressed with one shared plane_pitch: the
+ *     chroma rows of each half are not row_pitch / 2 apart.
+ *   P016: NV12's geometry in 16-bit words: luma word of (x, y) at base + i*image_stride + y*row_pitch + 2*x; its
+ *     chroma pair at base + i*image_stride + plane_pitch + (y >> 1)*row_pitch + 4*(x >> 1), U first.  row_pitch: 0 =
+ *     4*ceil(W/2), and at least that; plane_pitch: 0 = H * row_pitch, and at least that.  Footprint: plane_pitch +
+ *     ceil(H/2)*row_pitch.  On the device entries both base pointers, row_pitch, plane_pitch and image_stride must be
+ *     even (ADC_ERR_ARG naming the argument otherwise, before the engine is checked); the host entries take any
+ *     alignment, they upload the rows tightly.
  *   YUYV / UYVY / YVYU: pixel (x, y) is the Y0 (x even) or Y1 (x odd) of the macropixel at
  *     base + i*image_stride + y*row_pitch + 4*(x >> 1), with that macropixel's U and V.  row_pitch: 0 = 4*ceil(W/2),
  *     and at least that.  plane_pitch must be 0.  Footprint: H * row_pitch.
  * Semantics: a W x H view is matched exactly as if the caller had taken any even-sized frame holding the view at its
- * top-left, run cv::cvtColor(frame, COLOR_YUV2BGR_<F>) on it, cropped the result to W x H and passed that as packed BGR
- * (for even sizes: cvtColor on the view itself).  Chroma is sited at even positions relative to the view's own (0, 0),
- * so a crop of a larger frame must start at an even x (and, for NV12 / NV21, an even y): that is the caller's
+ * top-left, converted it with the rule above (without flags: cv::cvtColor(frame, COLOR_YUV2BGR_<F>); P016:
+ * convertTo(CV_8U, 1.0 / 256), then COLOR_YUV2BGR_NV12), cropped the result to W x H and passed that as packed BGR
+ * (for even sizes: the conversion of the view itself).  Chroma is sited at even positions relative to the view's own
+ * (0, 0), so a crop of a larger frame must start at an even x (and, for 4:2:0, an even y): that is the caller's
  * responsibility, as the pattern is for the Bayer formats.  Through the rectified entries the whole src_width x
- * src_height frame is converted first and that BGR frame is resampled; a neighbour outside the frame is BGR (0, 0, 0),
- * not the conversion of YUV (0, 0, 0).  Only the view's own samples are read: nothing past the last chroma byte of an
- * NV12 / NV21 view, nothing past 4*ceil(W/2) bytes of a packed 4:2:2 row.
- * Out of scope: three-plane 4:2:0 (I420 / YV12), BT.709, full range, 10- and 16-bit YUV (P010 / P016). */
+ * src_height frame is converted with its encoding first and that BGR frame is resampled; a neighbour outside the frame
+ * is BGR (0, 0, 0), not the conversion of YUV (0, 0, 0).  Only the view's own samples are read: nothing past the last
+ * chroma byte or word of a 4:2:0 view, nothing past ceil(W/2) bytes of an I420 / YV12 chroma row, nothing past
+ * 4*ceil(W/2) bytes of a packed 4:2:2 row.
+ * Out of scope: BT.2020 and HDR transfer functions, planar and semi-planar 4:2:2 and 4:4:4 (I422, NV16), packed 10-bit
+ * (v210, Y210), side-by-side I420. */
 enum { ADC_IMG_NV12 = 32, ADC_IMG_NV21 = 33, ADC_IMG_YUYV = 34, ADC_IMG_UYVY = 35, ADC_IMG_YVYU = 36 };
+enum { ADC_IMG_I420 = 38, ADC_IMG_YV12 = 39, ADC_IMG_P016 = 40 };
+enum { ADC_IMG_YUV_BT709 = 0x100, ADC_IMG_YUV_FULL_RANGE = 0x200 };
 /* High-bit-depth mono and Bayer frames, as GigE Vision / USB3 Vision cameras deliver them, reduced to 8 bits on the way
  * in.  The names are the GenICam PFNC pixel formats; five containers, each as mono and as the four Bayer patterns:
  *   ADC_IMG_MONO10   ADC_IMG_BAYER_{RG,GR,BG,GB}10    Mono10 / BayerRG10 ...: one sample per little-endian uint16,
@@ -430,15 +470,18 @@ enum {
     ADC_IMG_MONO12P = 84, ADC_IMG_BAYER_RG12P = 85, ADC_IMG_BAYER_GR12P = 86, ADC_IMG_BAYER_BG12P = 87, ADC_IMG_BAYER_GB12P = 88
 };
 typedef struct adc_image_desc {
-    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_*, the YUV and the high-bit-depth formats) */
+    int32_t format;        /* ADC_IMG_* (including ADC_IMG_BAYER_*, the YUV and the high-bit-depth formats; a YUV
+                              format OR-ed with ADC_IMG_YUV_BT709 / ADC_IMG_YUV_FULL_RANGE) */
     int32_t reserved;      /* must be zero */
     int64_t row_pitch;     /* bytes from one row to the next; 0 = tight (W * bytes per pixel; W for gray / Bayer / planar;
-                              2*ceil(W/2) for NV12 / NV21; 4*ceil(W/2) for YUYV / UYVY / YVYU; 2*W for the 16-bit
+                              2*ceil(W/2) for NV12 / NV21 / I420 / YV12; 4*ceil(W/2) for P016 and YUYV / UYVY /
+                              YVYU; 2*W for the 16-bit
                               containers; ceil(10*W/8) for 10p, ceil(12*W/8) for 12p) */
-    int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; NV12 / NV21: bytes
-                              from the luma plane to the chroma plane, 0 = H * row_pitch; other formats: must be 0 */
+    int64_t plane_pitch;   /* RGB_PLANAR: bytes from one channel plane to the next, 0 = H * row_pitch; NV12 / NV21 /
+                              P016: bytes from the luma plane to the chroma plane, I420 / YV12: to the first chroma
+                              plane, 0 = H * row_pitch; other formats: must be 0 */
     int64_t image_stride;  /* bytes from pair i's view to pair i+1's view, 0 = tight (H * row_pitch, or 3 * plane_pitch;
-                              plane_pitch + ceil(H/2) * row_pitch for NV12 / NV21) */
+                              plane_pitch + ceil(H/2) * row_pitch for NV12 / NV21 / I420 / YV12 / P016) */
 } adc_image_desc;          /* 32 bytes */
 
 /* adc_match_outputs_batch_device with the images described by `img` (NULL = tight packed BGR, the same call as
