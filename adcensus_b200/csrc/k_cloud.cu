@@ -77,7 +77,7 @@ k_point_cloud(int W, int N, int tiles, long long total, const float* __restrict_
                 const double ia = __drcp_rn(q_row(Q, 3, xd, yd, dd));
                 px[k] = coord(q_row(Q, 0, xd, yd, dd), ia);
                 py[k] = coord(q_row(Q, 1, xd, yd, dd), ia);
-                pz[k] = coord(q_row(Q, 2, xd, yd, dd), ia);
+                pz[k] = coord_z(Q, xd, yd, d, ia);
                 keep = isfinite(d) && isfinite(px[k]) && isfinite(py[k]) && isfinite(pz[k]) && z_min <= pz[k] &&
                        pz[k] <= z_max;
             }

@@ -3,7 +3,7 @@
 // One pass over n disparity maps: each pixel's f32 value is read once, and only the requested outputs are written
 // (include/adcensus_b200.h, DESIGN.md section 15):
 //   POINTS    cv::reprojectImageTo3D bit for bit: h_i = (((+0.0 + Q[i][0]*x) + Q[i][1]*y) + Q[i][2]*d) + Q[i][3] in
-//             double, P_c = (float)((double)(float)h_c * (1.0 / h_3))
+//             double, P_c = (float)((double)(float)h_c * (1.0 / h_3)); P_z = 10000 where d is FLT_MAX
 //   DEPTH     P_2 alone
 //   DISP_S16  saturate_cast<short>(d * 16) as x86 computes it, (min_disparity - 1) * 16 for +inf
 // The double arithmetic (q_row, coord) is in k_reproject.cuh, shared with the point clouds of k_cloud.cu.
@@ -53,7 +53,7 @@ k_reproject(int W, int N, long long n, const float* __restrict__ disp, const Adc
                 const int r = r0 + j, y = r / W, x = r - y * W;
                 const double xd = x, yd = y, dd = d;
                 const double ia = __drcp_rn(q_row(Q, 3, xd, yd, dd));
-                const float z = coord(q_row(Q, 2, xd, yd, dd), ia);
+                const float z = coord_z(Q, xd, yd, d, ia);
                 if (K & RP_DEPTH) depth[base + j] = z;
                 if (K & RP_POINTS) {
                     stage[3 * j] = coord(q_row(Q, 0, xd, yd, dd), ia);

@@ -20,3 +20,9 @@ static __device__ __forceinline__ double q_row(const AdcReprojQ& Q, int i, doubl
 static __device__ __forceinline__ float coord(double h, double ia) {
     return __double2float_rn(__dmul_rn((double)__double2float_rn(h), ia));
 }
+
+// Z: cv::reprojectImageTo3D replaces it by bigZ = 10000 wherever |d - minDisparity| <= FLT_EPSILON, and without
+// handleMissingValues its minDisparity is FLT_MAX, so a disparity of exactly FLT_MAX gets Z = 10000 whatever Q is
+static __device__ __forceinline__ float coord_z(const AdcReprojQ& Q, double x, double y, float d, double ia) {
+    return d == 3.40282347e+38f ? 10000.0f : coord(q_row(Q, 2, x, y, (double)d), ia);
+}

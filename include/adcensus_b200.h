@@ -583,7 +583,9 @@ int adc_match_rectified(adc_engine* e, const uint8_t* left, const uint8_t* right
  * which is OpenCV's: each coordinate is rounded to float twice (Vec3f /= double multiplies by the reciprocal), and the
  * +0.0 start turns a -0 first product into +0.  With a stereoRectify Q, column 2 of rows 0..2 is zero, so an invalid
  * (+inf) pixel gives 0 * inf = NaN in all three coordinates, exactly as OpenCV does; that is also the NaN-as-missing
- * convention of organised point clouds (PCL, Open3D).  NaN payloads are not specified.
+ * convention of organised point clouds (PCL, Open3D).  NaN payloads are not specified.  One exception, OpenCV's too:
+ * P_2 = 10000.0f where d is exactly FLT_MAX, whatever Q is (reprojectImageTo3D's bigZ for |d - minDisparity| <=
+ * FLT_EPSILON, where minDisparity is FLT_MAX without handleMissingValues).
  * DISP_S16: d = +inf gives (min_disparity - 1) * 16 saturated to int16 (the StereoMatcher invalid value, with the
  * engine's min_disparity); any other d gives cv::saturate_cast<short>(d * 16) as on x86: t = d * 16 rounded half to
  * even, saturated to [-32768, 32767] when it fits in int32, and -32768 otherwise, for NaN and for -inf.

@@ -8,7 +8,7 @@ INT16_MIN, INT16_MAX = -32768, 32767
 
 def points(disp: np.ndarray, Q) -> np.ndarray:
     """float32 [H][W][3]: h_i = (((+0.0 + Q[i][0]*x) + Q[i][1]*y) + Q[i][2]*d) + Q[i][3]*1.0 in double, one rounding per
-    operation; P_c = (float)((double)(float)h_c * (1.0 / h_3))."""
+    operation; P_c = (float)((double)(float)h_c * (1.0 / h_3)); P_z = 10000 where d is exactly FLT_MAX."""
     Q = np.asarray(Q).astype(np.float64)
     H, W = disp.shape
     ys, xs = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
@@ -16,7 +16,10 @@ def points(disp: np.ndarray, Q) -> np.ndarray:
     with np.errstate(all="ignore"):
         h = [(((np.zeros_like(d) + Q[i, 0] * xs) + Q[i, 1] * ys) + Q[i, 2] * d) + Q[i, 3] * 1.0 for i in range(4)]
         ia = 1.0 / h[3]
-        return np.stack([(h[c].astype(np.float32).astype(np.float64) * ia).astype(np.float32) for c in range(3)], -1)
+        P = np.stack([(h[c].astype(np.float32).astype(np.float64) * ia).astype(np.float32) for c in range(3)], -1)
+    # OpenCV's bigZ: Z = 10000 where |d - minDisparity| <= FLT_EPSILON, minDisparity = FLT_MAX without handleMissingValues
+    P[disp == np.finfo(np.float32).max, 2] = 10000.0
+    return P
 
 
 def depth(disp: np.ndarray, Q) -> np.ndarray:
