@@ -164,9 +164,11 @@ void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, cons
 // rectified ingestion (k_rectify.cu).  The engine's internal form of a view's remap table: one uint2 per output pixel,
 // .x = (u16)x0 | (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
 struct AdcRectGeom {
-    const uint2* map[2];   // left, right: [H][W] each
+    const uint2* map[2];   // left, right: [H][W] each (nullptr for a resize)
     int src_w, src_h;      // raw frame size
+    int type;              // the geometry: ADC_REMAP_* (through map) or ADC_RESIZE_* (k_resize.cu)
 };
+IMG_HD constexpr bool adc_is_resize(int type) { return type == ADC_RESIZE_AREA || type == ADC_RESIZE_LINEAR_EXACT; }
 // a view's adc_remap (map1 / map2 with byte pitches, device-readable, ADC_REMAP_F32 / ADC_REMAP_FIXED) -> out [H][W]
 void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1, long long pitch1, const void* map2,
                               long long pitch2, uint2* out, cudaStream_t st);
@@ -174,6 +176,10 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
 // resampled; S * ceil(N / 4 / II_GROUPS) < 2^31 (the grid's x)
 void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                                const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
+// resized ingestion (k_resize.cu): as adc_launch_rectify_ingest for a geometry r of an ADC_RESIZE_* type, whose
+// factors (AREA) the engine checked against dm.W x dm.H
+void adc_launch_resize_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                              const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
 // reprojection to 3-D (k_reproject.cu): n maps of dm.N pixels at disp -> the outputs whose pointer is not NULL (map i
 // at pixel i*N of each), Q row-major; s16_invalid = the DISP_S16 value of a +inf pixel.  One launch.
 struct AdcReprojQ { double q[16]; };

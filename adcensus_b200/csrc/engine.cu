@@ -116,7 +116,9 @@ struct adc_engine {
     int export_layout = ADC_COST_DHW, export_dtype = ADC_COST_F32;
     // image format of the last adc_match_images* call (adc_profile_kernel's ingestion timing)
     int img_format = ADC_IMG_RGB_PLANAR;
-    // rectification (adc_set_rectification): both views' maps in the internal form, [2][N]; nullptr = none set
+    // rectification (adc_set_rectification): its r->map_type, -1 = none set; for maps (ADC_REMAP_*) both views' maps in
+    // the internal form, [2][N], for a resize (ADC_RESIZE_*) nullptr
+    int rect_type = -1;
     uint2* rect_map = nullptr;
     int rect_src_w = 0, rect_src_h = 0;
     // raw frame format of the last adc_match_rectified* call (adc_profile_kernel's rectified ingestion timing)
@@ -559,15 +561,17 @@ int drain_lane(adc_engine* e, Lane& ln) {
 }
 
 // n pairs of views at left / right (pair i at byte i * g.image_stride; geometry g, resolved, over the raw frames of
-// `rect` or the engine's size) -> `bgr` as packed BGR [n][2][N*3] on st: a plain or rectified ingestion launch per
-// 65535 pairs (k_image_ingest's blockIdx.z is the pair).
+// `rect` or the engine's size) -> `bgr` as packed BGR [n][2][N*3] on st: a plain, rectified or resized ingestion launch
+// per 65535 pairs (k_image_ingest's blockIdx.z is the pair).
 void ingest_views(adc_engine* e, int n, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                   const AdcRectGeom* rect, uint8_t* bgr, cudaStream_t st) {
     for (int first = 0; first < n; first += 65535) {
         const int count = std::min(n - first, 65535);
         const long long off = (long long)first * g.image_stride;
         uint8_t* out = bgr + (size_t)first * 6 * e->P.dm.N;
-        if (rect) adc_launch_rectify_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
+        if (rect && adc_is_resize(rect->type))
+            adc_launch_resize_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
+        else if (rect) adc_launch_rectify_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
         else adc_launch_image_ingest(e->P.dm, count, left + off, right + off, g, out, st, &e->launches);
     }
 }
@@ -835,11 +839,11 @@ int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, int n
 // The rules the rectified entries add to the image entries' (after the engine check): a rectification is set, and
 // the descriptor's size-dependent rules hold for the raw frame size.
 int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, int n, AdcImageGeom* g, AdcRectGeom* r) {
-    if (!e->rect_map) return fail(ADC_ERR_ARG, "%s: no rectification is set (adc_set_rectification)", fn);
+    if (e->rect_type < 0) return fail(ADC_ERR_ARG, "%s: no rectification is set (adc_set_rectification)", fn);
     int rc = resolve_image(fn, e->rect_src_w, e->rect_src_h, img, n, g);
     if (rc) return rc;
     const size_t N = (size_t)e->P.dm.N;
-    *r = AdcRectGeom{{e->rect_map, e->rect_map + N}, e->rect_src_w, e->rect_src_h};
+    *r = AdcRectGeom{{e->rect_map, e->rect_map ? e->rect_map + N : nullptr}, e->rect_src_w, e->rect_src_h, e->rect_type};
     return ADC_OK;
 }
 
@@ -1449,13 +1453,22 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
 int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
     const char* fn = "adc_set_rectification";
     const bool f32 = r && r->map_type == ADC_REMAP_F32;
+    const bool resize = r && adc_is_resize(r->map_type);   // no maps: nothing to copy or convert
     const long long e1 = 4, e2 = f32 ? 4 : 2;   // bytes per element of map1 (float, int16 pair) and map2 (float, uint16)
     if (r) {
         if (r->src_width < 1 || r->src_width > 32767) return fail(ADC_ERR_ARG, "%s: r->src_width %d outside 1..32767", fn, r->src_width);
         if (r->src_height < 1 || r->src_height > 32767) return fail(ADC_ERR_ARG, "%s: r->src_height %d outside 1..32767", fn, r->src_height);
-        if (r->map_type != ADC_REMAP_F32 && r->map_type != ADC_REMAP_FIXED) return fail(ADC_ERR_ARG, "%s: r->map_type %d unknown", fn, r->map_type);
+        if (r->map_type != ADC_REMAP_F32 && r->map_type != ADC_REMAP_FIXED && !resize)
+            return fail(ADC_ERR_ARG, "%s: r->map_type %d unknown", fn, r->map_type);
         if (r->reserved != 0) return fail(ADC_ERR_ARG, "%s: r->reserved must be zero", fn);
-        for (int v = 0; v < 2; v++) {
+        for (int v = 0; v < 2 && resize; v++) {
+            const adc_remap& m = r->view[v];
+            if (m.map1) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1 must be NULL for a resize", fn, v);
+            if (m.map2) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2 must be NULL for a resize", fn, v);
+            if (m.map1_pitch) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1_pitch must be 0 for a resize", fn, v);
+            if (m.map2_pitch) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2_pitch must be 0 for a resize", fn, v);
+        }
+        for (int v = 0; v < 2 && !resize; v++) {
             const adc_remap& m = r->view[v];
             if (!m.map1) return fail(ADC_ERR_ARG, "%s: r->view[%d].map1 is NULL", fn, v);
             if (!m.map2) return fail(ADC_ERR_ARG, "%s: r->view[%d].map2 is NULL", fn, v);
@@ -1469,8 +1482,28 @@ int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
     }
     if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
     const long long W = e->W, H = e->H;
+    if (r && r->map_type == ADC_RESIZE_AREA) {
+        const long long kx = r->src_width / W, ky = r->src_height / H;
+        if (r->src_width < W || r->src_width % W)
+            return fail(ADC_ERR_ARG, "%s: r->src_width %d is not a multiple of W (%lld) for ADC_RESIZE_AREA", fn,
+                        r->src_width, W);
+        if (r->src_height < H || r->src_height % H)
+            return fail(ADC_ERR_ARG, "%s: r->src_height %d is not a multiple of H (%lld) for ADC_RESIZE_AREA", fn,
+                        r->src_height, H);
+        // cv::resize takes the integer-block rule only where its scale 1 / (W / src_width), in double, is the factor
+        // exactly; for 640 of the factors 1..4096 it is not, and OpenCV's general area path rounds differently
+        if (1.0 / ((double)W / r->src_width) != (double)kx)
+            return fail(ADC_ERR_ARG, "%s: r->src_width %d: the factor %lld is not exact in double (1 / (W / src_width)) "
+                        "for ADC_RESIZE_AREA", fn, r->src_width, kx);
+        if (1.0 / ((double)H / r->src_height) != (double)ky)
+            return fail(ADC_ERR_ARG, "%s: r->src_height %d: the factor %lld is not exact in double "
+                        "(1 / (H / src_height)) for ADC_RESIZE_AREA", fn, r->src_height, ky);
+        if (kx * ky > 4096)
+            return fail(ADC_ERR_ARG, "%s: r->src_width %d / W times r->src_height %d / H is more than 4096 for "
+                        "ADC_RESIZE_AREA", fn, r->src_width, r->src_height);
+    }
     long long p1[2] = {0, 0}, p2[2] = {0, 0};
-    if (r) {
+    if (r && !resize) {
         for (int v = 0; v < 2; v++) {
             const adc_remap& m = r->view[v];
             p1[v] = m.map1_pitch ? (long long)m.map1_pitch : W * e1;
@@ -1487,7 +1520,7 @@ int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
     uint2* maps = nullptr;
     void* tmp = nullptr;
     bool host[2][2] = {};
-    if (r) {
+    if (r && !resize) {
         bool any_host = false;
         for (int v = 0; v < 2; v++)
             for (int k = 0; k < 2; k++) {
@@ -1507,7 +1540,7 @@ int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
     }
     // join the engine's outstanding work (and whatever work of the caller's wrote device maps)
     cudaError_t err = cudaDeviceSynchronize();
-    for (int v = 0; r && v < 2 && err == cudaSuccess; v++) {
+    for (int v = 0; r && !resize && v < 2 && err == cudaSuccess; v++) {
         const adc_remap& m = r->view[v];
         const void* s1 = m.map1;
         const void* s2 = m.map2;
@@ -1534,6 +1567,7 @@ int adc_set_rectification(adc_engine* e, const adc_rectification* r) {
     }
     if (e->rect_map) CK(cudaFree(e->rect_map));
     e->rect_map = maps;
+    e->rect_type = r ? r->map_type : -1;
     e->rect_src_w = r ? r->src_width : 0;
     e->rect_src_h = r ? r->src_height : 0;
     return ADC_OK;
@@ -1903,17 +1937,20 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 bytes = 2.0 * adc_image_read_bytes(e->img_format, P.dm.W, P.dm.H) + 2 * 3.0 * N;
                 break;
             }
-            case 14: {  // volA's bytes taken as the wave's tight raw frames, resampled through the engine's maps
-                if (!e->rect_map) return fail(ADC_ERR_ARG, "adc_profile_kernel: no rectification is set (adc_set_rectification)");
+            case 14: {  // volA's bytes taken as the wave's tight raw frames, resampled through the engine's maps or resized
+                if (e->rect_type < 0) return fail(ADC_ERR_ARG, "adc_profile_kernel: no rectification is set (adc_set_rectification)");
                 AdcImageGeom g = adc_image_tight(e->rect_format, e->rect_src_w, e->rect_src_h);
                 const long long foot = g.image_stride;
                 if (2 * foot > P.dm.vol_stride * 4)
                     return fail(ADC_ERR_UNSUPPORTED, "adc_profile_kernel: a pair's raw frames (%lld bytes) exceed its share of a lane volume", 2 * foot);
                 g.image_stride = 2 * foot;
-                const AdcRectGeom rg{{e->rect_map, e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h};
+                const bool resize = adc_is_resize(e->rect_type);
+                const AdcRectGeom rg{{e->rect_map, resize ? nullptr : e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h,
+                                     e->rect_type};
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
                 ingest_views(e, w.S, src, src + foot, g, &rg, w.bgr, ln.st);
-                bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N + 2 * 8.0 * N / e->S;
+                bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N +
+                        (resize ? 0.0 : 2 * 8.0 * N / e->S);
                 break;
             }
             case 15:    // the cost computed from the wave's images and census words, summed as iteration 0's H pass into volA

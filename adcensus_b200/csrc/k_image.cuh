@@ -195,6 +195,27 @@ static __device__ __forceinline__ unsigned mosaic_px(const uint8_t* src, long lo
         mosaic_sample<F>(d, x, 1));
 }
 
+// Mosaics: the demosaiced pixels (x0 + (k & 1), y0 + (k >> 1)), k = 0..3, into s[k], where no clamp applies
+// (1 <= x0 <= w - 3, 1 <= y0 <= h - 3): their four 3x3 neighbourhoods are one 4x4 window of full-depth samples, loaded
+// once; each demosaic is reduced to 8 bits.
+template <int F>
+static __device__ __forceinline__ void mosaic_quad(const uint8_t* src, long long row_pitch, int x0, int y0,
+                                                   unsigned s[4]) {
+    int v[4][4];
+    const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch;
+#pragma unroll
+    for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) v[i][j] = mosaic_sample<F>(r0 + i * row_pitch, x0 - 1, j);
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const int dx = k & 1, dy = k >> 1;
+        s[k] = bayer_rule<img_pattern(F), img_shift(F)>(
+            x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
+            v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
+    }
+}
+
 // Pixel (x, y) of a w x h view at src in format F as B | G << 8 | R << 16: the demosaic of a mosaic, the conversion of
 // a YUV frame, a high-bit-depth mono sample reduced and repeated, or one of the one-pixel readers above.
 template <int F>
@@ -287,22 +308,10 @@ static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* 
         }
     };
     if constexpr (img_mosaic(F)) {
-        // when no clamp applies (1 <= x0, x0 + 1 <= sw - 2, likewise y0), the four 3x3 neighbourhoods are one 4x4
-        // window of full-depth samples, loaded once; each demosaic is reduced to 8 bits before the blend
+        // when no clamp applies (1 <= x0, x0 + 1 <= sw - 2, likewise y0), one 4x4 window serves all four
+        // neighbours; each demosaic is reduced to 8 bits before the blend
         if (x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
-            int v[4][4];
-            const uint8_t* r0 = src + (long long)(y0 - 1) * row_pitch;
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-#pragma unroll
-                for (int j = 0; j < 4; j++) v[i][j] = mosaic_sample<F>(r0 + i * row_pitch, x0 - 1, j);
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-                const int dx = k & 1, dy = k >> 1;
-                s[k] = bayer_rule<img_pattern(F), img_shift(F)>(
-                    x0 + dx, y0 + dy, v[1 + dy][1 + dx], v[dy][1 + dx], v[2 + dy][1 + dx], v[1 + dy][dx],
-                    v[1 + dy][2 + dx], v[dy][dx], v[dy][2 + dx], v[2 + dy][dx], v[2 + dy][2 + dx]);
-            }
+            mosaic_quad<F>(src, row_pitch, x0, y0, s);
         } else {
             each();
         }

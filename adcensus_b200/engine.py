@@ -214,6 +214,10 @@ def _image_pair_desc(left: np.ndarray, right: np.ndarray, fmt: int, H: int, W: i
 # rectification on the way in (adc_set_rectification, adc_match_rectified*): remap tables as cv2.initUndistortRectifyMap
 # returns them, float32 x / y planes or int16 (x, y) pairs + uint16 fractions
 REMAP_F32, REMAP_FIXED = 0, 1
+# resizing on the way in: the same entries over frames of another size, resized as cv2.resize with INTER_AREA (integer
+# downscale factors) or INTER_LINEAR_EXACT
+RESIZE_AREA, RESIZE_LINEAR_EXACT = 16, 17
+RESIZE_INTERPOLATIONS = {"area": RESIZE_AREA, "linear_exact": RESIZE_LINEAR_EXACT}
 
 
 class Remap(ctypes.Structure):
@@ -223,7 +227,7 @@ class Remap(ctypes.Structure):
 
 
 class Rectification(ctypes.Structure):
-    """adc_rectification: raw frame size, REMAP_* map type and both views' maps."""
+    """adc_rectification: raw frame size, REMAP_* map type and both views' maps, or a RESIZE_* type and no maps."""
     _fields_ = [("src_width", ctypes.c_int32), ("src_height", ctypes.c_int32), ("map_type", ctypes.c_int32),
                 ("reserved", ctypes.c_int32), ("view", Remap * 2)]
 
@@ -658,12 +662,26 @@ class Engine:
         _check(self._L.adc_set_rectification(self._h, ctypes.byref(r)))
         self.rect_src_size = (sw, sh)
 
+    def set_resize(self, src_size, interpolation="area"):
+        """Sets a resize as the geometry of the rectified entries: raw frames of src_size = (width, height) are converted
+        to BGR with their format's rule and resized to this engine's (width, height) as cv2.resize does with
+        INTER_AREA (interpolation "area": integer downscale factors that are exact in double as OpenCV computes them,
+        at most 4096 source pixels an output pixel) or
+        INTER_LINEAR_EXACT ("linear_exact": any sizes), bit for bit.  It replaces maps set with set_rectification, and
+        set_rectification(None) clears it.  match_rectified*, ingest_views(rectified=True) then take such frames."""
+        sw, sh = (int(v) for v in src_size)
+        t = RESIZE_INTERPOLATIONS.get(interpolation) if isinstance(interpolation, str) else int(interpolation)
+        if t is None:
+            raise ValueError(f"unknown interpolation {interpolation!r} (one of {sorted(RESIZE_INTERPOLATIONS)})")
+        _check(self._L.adc_set_rectification(self._h, ctypes.byref(Rectification(sw, sh, t, 0))))
+        self.rect_src_size = (sw, sh)
+
     def match_rectified(self, left, right, format="bgr", maps=(), volumes=(), layout="hwd", dtype="f32", cost=None,
                         cost_layout="hwd", cost_dtype=None, disparity=True):
         """match_images for raw frames: `left` / `right` are uint8 numpy views of the src_size frames given to
         set_rectification, in any IMG_* format and pitch, resampled through the maps on the way in.  The result is what
         match_outputs gives for cv2.remap(view, map1, map2, INTER_LINEAR, BORDER_CONSTANT, 0) of each view packed as
-        BGR."""
+        BGR; with a resize set (set_resize), for cv2.resize(view, (width, height), interpolation=...) instead."""
         if self.rect_src_size is None:
             raise AdcError("no rectification is set (set_rectification)")
         sw, sh = self.rect_src_size

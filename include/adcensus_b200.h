@@ -526,8 +526,33 @@ int adc_match_images(adc_engine* e, const uint8_t* left, const uint8_t* right, c
  *   the source byte at (x0 + dx, y0 + dy), or 0 for a neighbour outside the src_width x src_height frame.
  * Every map is [H][W] over the engine's output size; each map's rows may be pitched (bytes, 0 = tight).  The maps of
  * an F32 set and the map2 of a FIXED set are as cv::remap takes them; both map types are pinned to what cv::remap does
- * with that map (initUndistortRectifyMap's CV_16SC2 output is not convertMaps of its float output everywhere). */
+ * with that map (initUndistortRectifyMap's CV_16SC2 output is not convertMaps of its float output everywhere).
+ *
+ * Resizing on the way in: the same entries take frames of another size than W x H when the geometry set is a resize,
+ * map_type ADC_RESIZE_AREA or ADC_RESIZE_LINEAR_EXACT (no maps).  Each raw view is converted to 8-bit packed BGR at
+ * src_width x src_height with its format's rule, exactly as above (demosaic, YUV rule, depth reduction, gray ->
+ * (v, v, v)), and that frame is resized to W x H; the final map, the exported volumes and the side maps are bit for bit
+ * those of cv::resize(bgr, (W, H), interpolation = INTER_AREA / INTER_LINEAR_EXACT) followed by adc_match_images* on
+ * the result as tight packed BGR.  Channels are resized independently:
+ *   ADC_RESIZE_AREA (cv::INTER_AREA at integer factors, downscaling only): src_width = kx * W, src_height = ky * H,
+ *     kx * ky <= 4096, and each factor k exact in double as OpenCV computes it, 1.0 / ((double)W / src_width) == kx
+ *     and likewise ky.  That holds for 3456 of the factors 1..4096; the other 640 (49, 93, 98, 99, 103, ...) are
+ *     rejected, because OpenCV then takes its general area path, which rounds differently.  For every accepted pair,
+ *     with s the integer sum of an output pixel's kx x ky source block and n = kx * ky: out = (s + 2) >> 2 for
+ *     kx = ky = 2; otherwise out = round_half_even((float)s * (1.0f / n)) saturated to 255, both products in IEEE
+ *     float (1 x 1, unequal factors such as 2 x 3, and every other accepted factor).
+ *   ADC_RESIZE_LINEAR_EXACT (cv::INTER_LINEAR_EXACT, any sizes, up or down), separable; per axis with n_src -> n_dst
+ *     and d the output index: f = (d + 0.5) * scale - 0.5 with scale = 1.0 / ((double)n_dst / n_src), all in IEEE
+ *     double without fused multiply-add (scale is OpenCV's, the inverse of its inv_scale; (double)n_src / n_dst
+ *     differs from it in the last bit for some sizes, e.g. 49 -> 256, and then so can the output), i = floor(f),
+ *     c1 = round_half_even((f - i) * 256), c0 = 256 - c1; i < 0 gives i = 0, c1 = 0 and i >= n_src - 1 gives
+ *     i = n_src - 1, c1 = 0 (the border replicates; nothing outside the frame is read).  Per row
+ *     h = p[i] * c0x + p[i + 1] * c1x, and out = (h(y0) * c0y + h(y0 + 1) * c1y + 2^15) >> 16.
+ * cv::INTER_LINEAR itself is not offered: OpenCV's 8-bit path mixes vector and scalar rounding, so no one rule gives
+ * its results.  adc_match_rectified* and adc_ingest_views(rectified = 1) follow whichever geometry is set, maps or a
+ * resize; adc_profile_kernel id 14 times the resize ingestion while a resize is set. */
 enum { ADC_REMAP_F32 = 0, ADC_REMAP_FIXED = 1 };
+enum { ADC_RESIZE_AREA = 16, ADC_RESIZE_LINEAR_EXACT = 17 };
 typedef struct adc_remap {
     const void* map1;      /* F32: float x [H][W]; FIXED: int16 (x, y) [H][W][2] */
     const void* map2;      /* F32: float y [H][W]; FIXED: uint16 [H][W] */
@@ -537,7 +562,7 @@ typedef struct adc_remap {
 typedef struct adc_rectification {
     int32_t src_width;     /* raw frame size, each 1..32767 (OpenCV's coordinates are int16) */
     int32_t src_height;
-    int32_t map_type;      /* ADC_REMAP_* */
+    int32_t map_type;      /* ADC_REMAP_*, or ADC_RESIZE_* with every view's maps NULL and pitches 0 */
     int32_t reserved;      /* must be zero */
     adc_remap view[2];     /* left, right */
 } adc_rectification;       /* 80 bytes */
@@ -548,9 +573,13 @@ typedef struct adc_rectification {
  * made.  Synchronous: before the maps are replaced the device is synchronised, so that every earlier call, pipelined
  * or not, runs with the maps that were set when it was made.  Rules (each violation fails with ADC_ERR_ARG naming the
  * field; those that need no output size before the engine is checked): src_width and src_height in 1..32767;
- * map_type one of ADC_REMAP_*; reserved zero; no map pointer NULL; pitches not negative and, when not 0, at least a
- * row's bytes; map pointers and pitches aligned to their element (4 bytes for float, 2 for int16 / uint16).  A failed
- * allocation fails with ADC_ERR_NOMEM before anything changes.  adc_destroy frees the maps. */
+ * map_type one of ADC_REMAP_* or ADC_RESIZE_*; reserved zero; for maps, no map pointer NULL; pitches not negative
+ * and, when not 0, at least a row's bytes; map pointers and pitches aligned to their element (4 bytes for float, 2 for
+ * int16 / uint16).  For a resize every map pointer is NULL and every pitch 0, checked before the engine; after it, for
+ * ADC_RESIZE_AREA, src_width a multiple of W and src_height a multiple of H (naming the field; W x H itself is the
+ * factor 1 x 1), each factor exact in double (1.0 / ((double)W / src_width) == kx, naming r->src_width; likewise
+ * r->src_height) and kx * ky <= 4096.  A resize allocates nothing.  A failed allocation fails with ADC_ERR_NOMEM
+ * before anything changes.  adc_destroy frees the maps. */
 int adc_set_rectification(adc_engine* e, const adc_rectification* r);
 
 /* adc_match_images_batch_device / adc_match_images on raw frames: `img` (NULL = tight packed BGR) describes the raw
@@ -761,7 +790,8 @@ int adc_get_config(const adc_engine* e, adc_config* out);
  * engine's last adc_match_images* call, ADC_IMG_RGB_PLANAR if there was none, tight pitches; the source bytes of both
  * views + 2*3*N written per pair), 14 = rectified ingestion (format of the engine's last adc_match_rectified* call,
  * ADC_IMG_BGR if there was none, tight raw frames; needs a rectification set; per pair the bytes of both raw frames +
- * 2*3*N written, plus both views' internal maps, 2*8*N, once per wave), 15 = the AD-census cost computed inside the first
+ * 2*3*N written, plus both views' internal maps, 2*8*N, once per wave; while a resize is set the resize ingestion, per
+ * pair the bytes of both raw frames + 2*3*N written, no maps), 15 = the AD-census cost computed inside the first
  * horizontal arm sum, which the fused pipeline runs in place of ids 0 and 1 (per pair one volume written, 24*N bytes of
  * packed pixels and census words read, plus the horizontal window records), 16 = the scanline pass along -y with the WTA
  * as its epilogue, which the pipeline runs in place of ids 4 and 5 where nothing else reads the optimised volume (per pair
