@@ -1,9 +1,8 @@
 // adc_common.cuh -- shared declarations for the sm_90a AD-Census kernels.
 //
 // Data layout in HBM (per wave of S stereo pairs; every array is [S][...], pair index outermost):
-//   bgr      u8  [S][2][H][W][3]   left, right packed BGR: copied as the caller passes them, or written by the image
-//                                  ingestion kernel (k_image.cu) from another format / pitch, or by the rectified
-//                                  ingestion kernel (k_rectify.cu) from raw frames
+//   bgr      u8  [S][2][H][W][3]   left, right packed BGR: copied as the caller passes them, or written by the view
+//                                  ingestion kernel (k_image.cuh) from another format, pitch or source geometry
 //   gray     u8  [S][2][H][W]
 //   census   u64 [S][2][H][W]
 //   volA/B   f32 [S][H][W][Dp]     the two cost volumes, d fastest, Dp = D rounded up to 4 so that
@@ -156,30 +155,25 @@ size_t adc_cost_elem_bytes(int dtype);
 // ADC_COST_HWD / ADC_COST_DHW, element type ADC_COST_F32 / F16 / BF16 rounded to nearest even); dst aligned to its element
 void adc_launch_cost_export(const AdcParams& P, const AdcWave& w, const float* vol, void* dst, int layout, int dtype,
                             cudaStream_t st, unsigned long long* launches);
-// image ingestion (k_image.cu): S pairs of views at left / right (pair i at byte i*image_stride, format ADC_IMG_*,
-// pitches resolved: no zero defaults left; the formats, their geometry and adc_image_tight are in img_format.h) ->
-// bgr as packed BGR [S][2][N*3] (a wave's w.bgr, or a caller's views); S <= 65535 (the grid's z)
-void adc_launch_image_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                             uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
-// rectified ingestion (k_rectify.cu).  The engine's internal form of a view's remap table: one uint2 per output pixel,
-// .x = (u16)x0 | (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
+// The engine's internal form of a view's remap table (k_rectify.cu): one uint2 per output pixel, .x = (u16)x0 |
+// (u16)y0 << 16, .y = ax | ay << 5 (DESIGN.md section 14).
 struct AdcRectGeom {
     const uint2* map[2];   // left, right: [H][W] each (nullptr for a resize)
     int src_w, src_h;      // raw frame size
-    int type;              // the geometry: ADC_REMAP_* (through map) or ADC_RESIZE_* (k_resize.cu)
+    int type;              // the geometry: ADC_REMAP_* (through map) or ADC_RESIZE_* (factors checked against dm.W x dm.H)
 };
 IMG_HD constexpr bool adc_is_resize(int type) { return type == ADC_RESIZE_AREA || type == ADC_RESIZE_LINEAR_EXACT; }
 // a view's adc_remap (map1 / map2 with byte pitches, device-readable, ADC_REMAP_F32 / ADC_REMAP_FIXED) -> out [H][W]
 void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1, long long pitch1, const void* map2,
                               long long pitch2, uint2* out, cudaStream_t st);
-// S pairs of raw views at left / right (geometry g over src_w x src_h frames, pitches resolved) -> bgr [S][2][N*3],
-// resampled; S * ceil(N / 4 / II_GROUPS) < 2^31 (the grid's x)
-void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                               const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
-// resized ingestion (k_resize.cu): as adc_launch_rectify_ingest for a geometry r of an ADC_RESIZE_* type, whose
-// factors (AREA) the engine checked against dm.W x dm.H
-void adc_launch_resize_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                              const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
+// image ingestion (k_image.cu): S pairs of views at left / right (pair i at byte i*image_stride, format ADC_IMG_*,
+// pitches resolved: no zero defaults left; the formats, their geometry and adc_image_tight are in img_format.h) ->
+// bgr as packed BGR [S][2][N*3] (a wave's w.bgr, or a caller's views).  r == nullptr: views of the engine's size, read
+// in place; otherwise raw src_w x src_h frames, resampled through r's maps or resized.  One launch of at most
+// adc_view_ingest_max_pairs(dm) pairs.
+void adc_launch_view_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
+                            const AdcRectGeom* r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches);
+int adc_view_ingest_max_pairs(const AdcDims& dm);
 // reprojection to 3-D (k_reproject.cu): n maps of dm.N pixels at disp -> the outputs whose pointer is not NULL (map i
 // at pixel i*N of each), Q row-major; s16_invalid = the DISP_S16 value of a +inf pixel.  One launch.
 struct AdcReprojQ { double q[16]; };

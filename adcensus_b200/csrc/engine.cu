@@ -561,18 +561,15 @@ int drain_lane(adc_engine* e, Lane& ln) {
 }
 
 // n pairs of views at left / right (pair i at byte i * g.image_stride; geometry g, resolved, over the raw frames of
-// `rect` or the engine's size) -> `bgr` as packed BGR [n][2][N*3] on st: a plain, rectified or resized ingestion launch
-// per 65535 pairs (k_image_ingest's blockIdx.z is the pair).
+// `rect` or the engine's size) -> `bgr` as packed BGR [n][2][N*3] on st: one ingestion launch per
+// adc_view_ingest_max_pairs pairs.
 void ingest_views(adc_engine* e, int n, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
                   const AdcRectGeom* rect, uint8_t* bgr, cudaStream_t st) {
-    for (int first = 0; first < n; first += 65535) {
-        const int count = std::min(n - first, 65535);
+    const int chunk = adc_view_ingest_max_pairs(e->P.dm);
+    for (int first = 0; first < n; first += chunk) {
         const long long off = (long long)first * g.image_stride;
-        uint8_t* out = bgr + (size_t)first * 6 * e->P.dm.N;
-        if (rect && adc_is_resize(rect->type))
-            adc_launch_resize_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
-        else if (rect) adc_launch_rectify_ingest(e->P.dm, count, left + off, right + off, g, *rect, out, st, &e->launches);
-        else adc_launch_image_ingest(e->P.dm, count, left + off, right + off, g, out, st, &e->launches);
+        adc_launch_view_ingest(e->P.dm, std::min(n - first, chunk), left + off, right + off, g, rect,
+                               bgr + (size_t)first * 6 * e->P.dm.N, st, &e->launches);
     }
 }
 
@@ -836,14 +833,19 @@ int resolve_image(const char* fn, int w, int h, const adc_image_desc* img, int n
     return ADC_OK;
 }
 
+// The engine's rectification (set) as the ingestion kernel takes it.
+AdcRectGeom rect_geom(const adc_engine* e) {
+    const uint2* m = e->rect_map;
+    return AdcRectGeom{{m, m ? m + e->P.dm.N : nullptr}, e->rect_src_w, e->rect_src_h, e->rect_type};
+}
+
 // The rules the rectified entries add to the image entries' (after the engine check): a rectification is set, and
 // the descriptor's size-dependent rules hold for the raw frame size.
 int resolve_rectified(adc_engine* e, const char* fn, const adc_image_desc* img, int n, AdcImageGeom* g, AdcRectGeom* r) {
     if (e->rect_type < 0) return fail(ADC_ERR_ARG, "%s: no rectification is set (adc_set_rectification)", fn);
     int rc = resolve_image(fn, e->rect_src_w, e->rect_src_h, img, n, g);
     if (rc) return rc;
-    const size_t N = (size_t)e->P.dm.N;
-    *r = AdcRectGeom{{e->rect_map, e->rect_map ? e->rect_map + N : nullptr}, e->rect_src_w, e->rect_src_h, e->rect_type};
+    *r = rect_geom(e);
     return ADC_OK;
 }
 
@@ -1944,13 +1946,11 @@ int adc_profile_kernel(adc_engine* e, int32_t kernel_id, int32_t reps, float* av
                 if (2 * foot > P.dm.vol_stride * 4)
                     return fail(ADC_ERR_UNSUPPORTED, "adc_profile_kernel: a pair's raw frames (%lld bytes) exceed its share of a lane volume", 2 * foot);
                 g.image_stride = 2 * foot;
-                const bool resize = adc_is_resize(e->rect_type);
-                const AdcRectGeom rg{{e->rect_map, resize ? nullptr : e->rect_map + P.dm.N}, e->rect_src_w, e->rect_src_h,
-                                     e->rect_type};
+                const AdcRectGeom rg = rect_geom(e);
                 const uint8_t* src = reinterpret_cast<const uint8_t*>(w.volA);
                 ingest_views(e, w.S, src, src + foot, g, &rg, w.bgr, ln.st);
                 bytes = 2.0 * adc_image_read_bytes(e->rect_format, e->rect_src_w, e->rect_src_h) + 2 * 3.0 * N +
-                        (resize ? 0.0 : 2 * 8.0 * N / e->S);
+                        (adc_is_resize(e->rect_type) ? 0.0 : 2 * 8.0 * N / e->S);
                 break;
             }
             case 15:    // the cost computed from the wave's images and census words, summed as iteration 0's H pass into volA

@@ -1,7 +1,7 @@
 // img_format.h -- the image input formats (ADC_IMG_*, include/adcensus_b200.h): which codes exist, their family, the
 // parameters each family's reader takes, and the geometry and descriptor rules of a view.  The one place that knows
-// them: engine.cu asks it for the descriptor checks and the host staging, the dispatch of both ingestion kernels
-// (k_image.cu, k_rectify.cu) and their instantiations are generated from its list, and the readers (k_image.cuh) take
+// them: engine.cu asks it for the descriptor checks and the host staging, the dispatch of the ingestion kernel
+// (k_image.cu) and its instantiations are generated from its list, and the readers (k_image.cuh) take
 // their constants from it.  Plain C++ with no CUDA dependency, so g++ compiles it as well as nvcc.
 #pragma once
 
@@ -14,7 +14,7 @@
 #endif
 
 // Every format once, by family.  The family decides the reader and the translation unit that instantiates its
-// kernels: packed and planar u8 pixels (k_image.cu, k_rectify.cu), 8-bit Bayer mosaics (k_bayer.cu), YUV frames
+// kernels: packed and planar u8 pixels (k_image.cu), 8-bit Bayer mosaics (k_bayer.cu), YUV frames
 // (k_yuv.cu; k_yuv_video.cu and k_yuv_encodings.cu for the newer containers and the encoding flags) and the
 // high-bit-depth mono and Bayer frames (k_rawdepth.cu).
 #define ADC_IMG_PACKED_FORMATS(X) \

@@ -1,8 +1,10 @@
-// k_image.cuh -- the pieces the two image ingestion kernels share (k_image.cu: images in any format / pitch,
-// k_rectify.cu: raw frames resampled through remap tables): the per-format pixel readers, the one demosaic reader of
-// the 8-bit and high-bit-depth mosaics, the YUV conversion, the 10- / 12- / 16-bit sample readers with their depth
-// reduction, the store scheme that writes one view's packed BGR, and the kernels' launchers.  The formats and their
-// constants come from img_format.h.
+// k_image.cuh -- the view ingestion kernel k_view_ingest<F, G>: a caller's views in format F (any ADC_IMG_* code) and
+// source geometry G become packed BGR.  G says which source pixels an output pixel reads: its own pixel in place
+// (plain), four neighbours through a remap table (remap), its block (resize AREA) or four taps (resize LINEAR_EXACT).
+// Here are the per-format pixel readers, the one demosaic reader of the 8-bit and high-bit-depth mosaics, the YUV
+// conversion, the 10- / 12- / 16-bit sample readers with their depth reduction, the pixel rule of each geometry, the
+// store scheme that writes one view's packed BGR, and the kernel with its launcher.  The formats and their constants
+// come from img_format.h; the launch and its dispatch are in k_image.cu.
 //
 // The output of one view is a contiguous run of 3*N bytes.  A thread takes four consecutive pixels of it at a time:
 // 12 bytes, stored as three 32-bit words.  The view's run starts at an arbitrary byte phase (3*N*(2*pair + view) mod
@@ -267,29 +269,15 @@ __device__ __forceinline__ void store_view_bgr(uint8_t* __restrict__ o, int N, i
     }
 }
 
-// ---- the kernels (instantiated per format in the file of its family, see the end of this file) ----
+// ---- the source geometries: which source pixels an output pixel (x, y), p = y*W + x, reads ----
 
-// k_image.cu: pixel (x, y) of the view, read in place.
-template <int F>
-__global__ void __launch_bounds__(II_THREADS)
-k_image_ingest(int W, int H, int N, const uint8_t* __restrict__ left, const uint8_t* __restrict__ right,
-               long long row_pitch, long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
-    const int view = blockIdx.y, pair = blockIdx.z;
-    const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
-    uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
-    store_view_bgr(o, N, W, blockIdx.x,
-                   [&](int, int y, int x) { return view_px<F>(src, row_pitch, plane_pitch, W, H, x, y); });
-}
+// Plain: pixel (x, y) of the view, read in place (view_px).
 
-template <int F>
-void launch_image(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                  uint8_t* bgr, cudaStream_t st) {
-    const int groups = dm.N / 4;
-    dim3 grid(std::max(1, (groups + II_GROUPS - 1) / II_GROUPS), 2, S);
-    k_image_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.H, dm.N, left, right, g.row_pitch, g.plane_pitch, g.image_stride, bgr);
-}
-
-// One output pixel: the bilinear blend of the raw view `src` at map entry m, as B | G << 8 | R << 16.
+// Remap (ADC_REMAP_*): the bilinear blend of the raw view `src` at map entry m (k_rectify.cu's internal form), as
+// B | G << 8 | R << 16: the four neighbours of (x0, y0) weighted (32 - ax | ax) * (32 - ay | ay), (sum + 512) >> 10 per
+// channel.  When all four lie inside the frame (0 <= x0 < sw - 1, 0 <= y0 < sh - 1; never for a frame one pixel wide
+// or high) the loads are unconditional; otherwise each is loaded only if it is inside, so nothing outside a view's
+// frame is read.
 template <int F>
 static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* src, int sw, int sh, long long row_pitch,
                                                         long long plane_pitch) {
@@ -340,37 +328,149 @@ static __device__ __forceinline__ unsigned rectified_px(uint2 m, const uint8_t* 
     return out;
 }
 
+// The two resize rules are cv::resize's (include/adcensus_b200.h, DESIGN.md section 22):
+//   - ADC_RESIZE_AREA, integer factors kx = sw / W, ky = sh / H (each exact in double as OpenCV computes it, which the
+//     engine checks at set time): each output pixel sums its own kx x ky block, so every source pixel is read by
+//     exactly one output pixel; (s + 2) >> 2 for 2 x 2, round_half_even((float)s * (1.0f / n)) otherwise (n = kx * ky,
+//     the reciprocal rounded to float on the host);
+//   - ADC_RESIZE_LINEAR_EXACT, any sizes: per axis f = (d + 0.5) * scale - 0.5 in IEEE double (__dmul_rn / __dadd_rn:
+//     no fused multiply-add), scale = 1 / (n_dst / n_src) rounded on the host, i = floor(f), 8-bit weights
+//     c1 = round_half_even((f - i) * 256), c0 = 256 - c1, the index clamped into the frame with c1 = 0 at both
+//     borders; each thread computes its own taps, so there are no tables.  Four neighbours, all inside the frame, are
+//     blended as (h0 * c0y + h1 * c1y + 2^15) >> 16 with h = p[i] * c0x + p[i + 1] * c1x.
+
+// Per-channel sums of B | G << 8 | R << 16 pixels.
+struct Bgr3 {
+    int b = 0, g = 0, r = 0;
+    __device__ __forceinline__ void add(unsigned c) {
+        b += c & 255u;
+        g += c >> 8 & 255u;
+        r += c >> 16 & 255u;
+    }
+};
+
+// ADC_RESIZE_AREA: output pixel (x, y) from its kx x ky block.
 template <int F>
+static __device__ __forceinline__ unsigned area_px(const uint8_t* src, long long row_pitch, long long plane_pitch, int sw,
+                                                   int sh, int kx, int ky, float inv_n, int x, int y) {
+    Bgr3 s;
+    const int x0 = x * kx, y0 = y * ky;
+    if constexpr (img_mosaic(F)) {
+        // a 2 x 2 block of a mosaic away from the frame's edges: the four sites from one 4x4 window of samples
+        // (mosaic_quad) instead of four 3x3 neighbourhoods
+        if (kx == 2 && ky == 2 && x0 >= 1 && x0 <= sw - 3 && y0 >= 1 && y0 <= sh - 3) {
+            unsigned q[4];
+            mosaic_quad<F>(src, row_pitch, x0, y0, q);
+#pragma unroll
+            for (int k = 0; k < 4; k++) s.add(q[k]);
+            return (unsigned)((s.b + 2) >> 2) | (unsigned)((s.g + 2) >> 2) << 8 | (unsigned)((s.r + 2) >> 2) << 16;
+        }
+    }
+    for (int j = 0; j < ky; j++)
+        for (int i = 0; i < kx; i++) s.add(view_px<F>(src, row_pitch, plane_pitch, sw, sh, x0 + i, y0 + j));
+    if (kx == 2 && ky == 2)
+        return (unsigned)((s.b + 2) >> 2) | (unsigned)((s.g + 2) >> 2) << 8 | (unsigned)((s.r + 2) >> 2) << 16;
+    const auto q = [&](int v) { return (unsigned)min(255, __float2int_rn(__fmul_rn(__int2float_rn(v), inv_n))); };
+    return q(s.b) | q(s.g) << 8 | q(s.r) << 16;
+}
+
+// ADC_RESIZE_LINEAR_EXACT: the taps of destination index d on an axis of n source samples.
+struct Tap {
+    int i0, i1, c1;
+};
+static __device__ __forceinline__ Tap linear_tap(int d, double scale, int n) {
+    const double f = __dadd_rn(__dmul_rn((double)d + 0.5, scale), -0.5);
+    const double fl = floor(f);
+    int i = (int)fl, c1 = __double2int_rn(__dmul_rn(__dsub_rn(f, fl), 256.0));
+    if (i < 0) i = 0, c1 = 0;
+    if (i >= n - 1) i = n - 1, c1 = 0;
+    return Tap{i, min(i + 1, n - 1), c1};
+}
+
+template <int F>
+static __device__ __forceinline__ unsigned linear_px(const uint8_t* src, long long row_pitch, long long plane_pitch,
+                                                     int sw, int sh, double sx, double sy, int x, int y) {
+    const Tap tx = linear_tap(x, sx, sw), ty = linear_tap(y, sy, sh);
+    const unsigned p00 = view_px<F>(src, row_pitch, plane_pitch, sw, sh, tx.i0, ty.i0);
+    const unsigned p01 = view_px<F>(src, row_pitch, plane_pitch, sw, sh, tx.i1, ty.i0);
+    const unsigned p10 = view_px<F>(src, row_pitch, plane_pitch, sw, sh, tx.i0, ty.i1);
+    const unsigned p11 = view_px<F>(src, row_pitch, plane_pitch, sw, sh, tx.i1, ty.i1);
+    const int c0x = 256 - tx.c1, c0y = 256 - ty.c1;
+    unsigned out = 0;
+#pragma unroll
+    for (int c = 0; c < 24; c += 8) {
+        const int h0 = (int)(p00 >> c & 255u) * c0x + (int)(p01 >> c & 255u) * tx.c1;
+        const int h1 = (int)(p10 >> c & 255u) * c0x + (int)(p11 >> c & 255u) * tx.c1;
+        out |= (unsigned)((h0 * c0y + h1 * ty.c1 + (1 << 15)) >> 16) << c;
+    }
+    return out;
+}
+
+// The parameters of one geometry: the AREA factors and reciprocal, the LINEAR_EXACT scales.
+struct ResizeRule {
+    int kx, ky;
+    float inv_n;
+    double sx, sy;
+};
+
+// The source geometries of k_view_ingest.
+enum { VG_PLAIN, VG_REMAP, VG_AREA, VG_LINEAR };
+
+// Grid: blockIdx.y = view.  The resampling geometries take blockIdx.x = tile * S + pair: the S CTAs that read the same
+// stretch of a view's map are adjacent in launch order and run at the same time, so a wave reads each map from HBM once
+// and from L2 S - 1 times.  Plain reads nothing that pairs share and takes blockIdx.x = tile, blockIdx.z = pair: no
+// division in the block-index mapping, and a pair's views one after the other (the tile-outermost order measured gray
+// 23 % slower on H100).  Source offsets are 64-bit.
+// S pairs of views of sw x sh pixels at left / right (pair i at byte i*image_stride; plain views are the engine's
+// W x H, sh = H) -> bgr [S][2][N*3].  map_l / map_r are read by VG_REMAP only, `rule` by VG_AREA and VG_LINEAR only.
+template <int F, int G>
 __global__ void __launch_bounds__(II_THREADS)
-k_rectify_ingest(int W, int N, int S, int sw, int sh, const uint2* __restrict__ map_l, const uint2* __restrict__ map_r,
-                 const uint8_t* __restrict__ left, const uint8_t* __restrict__ right, long long row_pitch,
-                 long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
-    const int pair = blockIdx.x % S, tile = blockIdx.x / S, view = blockIdx.y;
+k_view_ingest(int W, int N, int S, int sw, int sh, ResizeRule rule, const uint2* __restrict__ map_l,
+              const uint2* __restrict__ map_r, const uint8_t* __restrict__ left, const uint8_t* __restrict__ right,
+              long long row_pitch, long long plane_pitch, long long image_stride, uint8_t* __restrict__ bgr) {
+    const bool plain = G == VG_PLAIN;
+    const int pair = plain ? blockIdx.z : blockIdx.x % S, tile = plain ? blockIdx.x : blockIdx.x / S, view = blockIdx.y;
     const uint8_t* src = (view ? right : left) + (long long)pair * image_stride;
     const uint2* map = view ? map_r : map_l;
     uint8_t* o = bgr + ((size_t)pair * 2 + view) * 3 * (size_t)N;
-    store_view_bgr(o, N, W, tile, [&](int p, int, int) {
-        return rectified_px<F>(__ldg(map + p), src, sw, sh, row_pitch, plane_pitch);
+    store_view_bgr(o, N, W, tile, [&](int p, int y, int x) {
+        if constexpr (G == VG_PLAIN) return view_px<F>(src, row_pitch, plane_pitch, W, sh, x, y);
+        else if constexpr (G == VG_REMAP) return rectified_px<F>(__ldg(map + p), src, sw, sh, row_pitch, plane_pitch);
+        else if constexpr (G == VG_AREA)
+            return area_px<F>(src, row_pitch, plane_pitch, sw, sh, rule.kx, rule.ky, rule.inv_n, x, y);
+        else return linear_px<F>(src, row_pitch, plane_pitch, sw, sh, rule.sx, rule.sy, x, y);
     });
 }
 
+// The arguments of one k_view_ingest launch, in the kernel's order.
+struct ViewIngest {
+    int W, N, S, sw, sh;
+    ResizeRule rule;
+    const uint2* map_l;
+    const uint2* map_r;
+    const uint8_t* left;
+    const uint8_t* right;
+    long long row_pitch, plane_pitch, image_stride;
+    uint8_t* bgr;
+};
+
 template <int F>
-void launch_rectify(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                    const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st) {
-    const int tiles = std::max(1, (dm.N / 4 + II_GROUPS - 1) / II_GROUPS);
-    dim3 grid((unsigned)(tiles * S), 2);
-    k_rectify_ingest<F><<<grid, II_THREADS, 0, st>>>(dm.W, dm.N, S, r.src_w, r.src_h, r.map[0], r.map[1], left, right,
-                                                     g.row_pitch, g.plane_pitch, g.image_stride, bgr);
+void launch_view_ingest(int G, dim3 grid, const ViewIngest& a, cudaStream_t st) {
+#define VI_LAUNCH(G)                                                                                                   \
+    k_view_ingest<F, G><<<grid, II_THREADS, 0, st>>>(a.W, a.N, a.S, a.sw, a.sh, a.rule, a.map_l, a.map_r, a.left,     \
+                                                     a.right, a.row_pitch, a.plane_pitch, a.image_stride, a.bgr)
+    switch (G) {
+        case VG_PLAIN: VI_LAUNCH(VG_PLAIN); break;
+        case VG_REMAP: VI_LAUNCH(VG_REMAP); break;
+        case VG_AREA: VI_LAUNCH(VG_AREA); break;
+        default: VI_LAUNCH(VG_LINEAR); break;
+    }
+#undef VI_LAUNCH
 }
 
-// The launchers of format F are instantiated in the file of F's family (img_format.h): II_IMAGE(F) / II_RECTIFY(F)
-// there, and nowhere else, so each file compiles only its own formats' kernels.
-#define II_IMAGE(F)                                                                                                    \
-    template void launch_image<F>(const AdcDims&, int, const uint8_t*, const uint8_t*, const AdcImageGeom&, uint8_t*,   \
-                                  cudaStream_t);
-#define II_RECTIFY(F)                                                                                                  \
-    template void launch_rectify<F>(const AdcDims&, int, const uint8_t*, const uint8_t*, const AdcImageGeom&,          \
-                                    const AdcRectGeom&, uint8_t*, cudaStream_t);
-#define II_EXTERN(F) extern II_IMAGE(F) extern II_RECTIFY(F)
+// The kernels of format F, all four geometries, are instantiated in the file of F's family (img_format.h):
+// II_VIEWS(F) there, and nowhere else, so each file compiles only its own formats' kernels.
+#define II_VIEWS(F) template void launch_view_ingest<F>(int, dim3, const ViewIngest&, cudaStream_t);
+#define II_EXTERN(F) extern II_VIEWS(F)
 ADC_IMG_CODES(II_EXTERN)
 #undef II_EXTERN

@@ -1,7 +1,6 @@
-// k_rawdepth.cu -- the high-bit-depth instantiations of the two image ingestion kernels (k_image.cuh): k_image_ingest
-// for adc_match_images* and k_rectify_ingest for adc_match_rectified*, one per format: five containers (16-bit words
-// holding 10, 12 or 16 significant bits; the PFNC 10p and 12p bit streams) x mono and the four Bayer patterns, all
-// reading through rd_sample, the mosaics through mosaic_px.  Container, depth and pattern are template constants, so
+// k_rawdepth.cu -- the high-bit-depth instantiations of the view ingestion kernel k_view_ingest (k_image.cuh), one per
+// format x source geometry: five containers (16-bit words holding 10, 12 or 16 significant bits; the PFNC 10p and 12p
+// bit streams) x mono and the four Bayer patterns, all reading through rd_sample, the mosaics through mosaic_px.  Container, depth and pattern are template constants, so
 // the shift of the depth reduction and the field width of the packed readers are immediates and the kernels take the
 // arguments every other format takes.
 //
@@ -13,5 +12,4 @@
 // see DESIGN.md section 19.
 #include "k_image.cuh"
 
-ADC_IMG_RAWDEPTH_FORMATS(II_IMAGE)
-ADC_IMG_RAWDEPTH_FORMATS(II_RECTIFY)
+ADC_IMG_RAWDEPTH_FORMATS(II_VIEWS)

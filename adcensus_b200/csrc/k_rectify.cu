@@ -1,4 +1,4 @@
-// k_rectify.cu -- rectification on the way in (adc_set_rectification, adc_match_rectified*).
+// k_rectify.cu -- rectification on the way in (adc_set_rectification): the conversion of remap tables.
 //
 // Set time: k_remap_convert turns a view's remap table, float (CV_32FC1 x / y planes) or fixed (CV_16SC2 + CV_16UC1),
 // into the engine's one internal form (adc_common.cuh AdcRectGeom): per output pixel the integer source corner
@@ -11,16 +11,8 @@
 //     [-2^20, 2^20] has x0 = +-32767 / -32768 after the int16 saturation, and since src_width, src_height <= 32767
 //     both neighbours x0 and x0 + 1 lie outside the frame: the border value 0 whichever way X saturated.
 //
-// Per wave: k_rectify_ingest<F> (k_image.cuh; dispatched here over every format of img_format.h, instantiated here for
-// the six formats of k_image.cu and in the family files for the others) makes one launch over the wave's pairs x 2
-// views.  For each output pixel it gathers the four neighbours of (x0, y0) from the raw view
-// through the format readers of k_image.cuh, weights them (32 - ax | ax) * (32 - ay | ay), and writes (sum + 512) >> 10
-// per channel with the store scheme of k_image.cuh.  When
-// all four neighbours lie inside the frame (0 <= x0 < src_width - 1, 0 <= y0 < src_height - 1; never for a frame one
-// pixel wide or high) the loads are unconditional; otherwise each neighbour is loaded only if it is inside, so nothing
-// outside a view's frame is read, and alpha bytes never are.  Source offsets are 64-bit.
-// Grid: blockIdx.x = tile * S + pair, blockIdx.y = view.  The S CTAs that read the same stretch of a view's map are
-// adjacent in launch order and run at the same time, so a wave reads each map from HBM once and from L2 S - 1 times.
+// Per wave the raw frames are resampled through these maps by k_view_ingest's remap geometry (k_image.cuh,
+// rectified_px).
 #include <algorithm>
 
 #include "adc_common.cuh"
@@ -67,15 +59,3 @@ void adc_launch_remap_convert(const AdcDims& dm, int map_type, const void* map1,
     if (map_type == ADC_REMAP_F32) k_remap_convert_f32<<<grid, RC_THREADS, 0, st>>>(dm.W, dm.N, m1, pitch1, m2, pitch2, out);
     else k_remap_convert_fixed<<<grid, RC_THREADS, 0, st>>>(dm.W, dm.N, m1, pitch1, m2, pitch2, out);
 }
-
-void adc_launch_rectify_ingest(const AdcDims& dm, int S, const uint8_t* left, const uint8_t* right, const AdcImageGeom& g,
-                               const AdcRectGeom& r, uint8_t* bgr, cudaStream_t st, unsigned long long* launches) {
-    switch (g.format) {
-#define RC_CASE(F) case F: launch_rectify<F>(dm, S, left, right, g, r, bgr, st); break;
-        ADC_IMG_CODES(RC_CASE)
-#undef RC_CASE
-    }
-    ++*launches;
-}
-
-ADC_IMG_PACKED_FORMATS(II_RECTIFY)

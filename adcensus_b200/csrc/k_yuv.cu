@@ -1,6 +1,5 @@
-// k_yuv.cu -- the YUV instantiations of the two image ingestion kernels (k_image.cuh): k_image_ingest for
-// adc_match_images* and k_rectify_ingest for adc_match_rectified*, one per format (NV12, NV21, YUYV, UYVY, YVYU), both
-// reading through yuv_px.
+// k_yuv.cu -- the YUV instantiations of the view ingestion kernel k_view_ingest (k_image.cuh): one per format (NV12,
+// NV21, YUYV, UYVY, YVYU) x source geometry, all reading through yuv_px.
 //
 // Plain ingestion: each thread converts four consecutive output pixels, one luma and two chroma byte loads each;
 // neighbouring lanes take neighbouring pixels, so a warp's luma loads cover one contiguous stretch of a row and its
@@ -9,5 +8,4 @@
 // neighbour outside the frame is 0.  No shared memory: see DESIGN.md section 18.
 #include "k_image.cuh"
 
-ADC_IMG_YUV_FORMATS(II_IMAGE)
-ADC_IMG_YUV_FORMATS(II_RECTIFY)
+ADC_IMG_YUV_FORMATS(II_VIEWS)

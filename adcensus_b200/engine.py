@@ -783,8 +783,8 @@ class Engine:
     def ingest_views_batch_device(self, n: int, d_left: int, d_right: int, d_views: int, image=None, rectified=False,
                                   stream: int = 0):
         """Device pointers (ints): n pairs described by `image` (an ImageDesc, None = tight packed BGR), plain or through
-        the rectification, written to d_views as packed BGR [n][2][H][W][3].  One launch per 65535 pairs enqueued on
-        `stream` without synchronising."""
+        the rectification, written to d_views as packed BGR [n][2][H][W][3].  One launch per 65535 pairs (fewer for
+        an engine of more than 2^27 pixels) enqueued on `stream` without synchronising."""
         _check(self._L.adc_ingest_views_batch_device(self._h, n, d_left, d_right,
                                                      None if image is None else ctypes.byref(image),
                                                      1 if rectified else 0, d_views, stream))

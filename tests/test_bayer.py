@@ -3,14 +3,13 @@ cv2.cvtColor(raw, COLOR_Bayer*2BGR) followed by the packed-BGR entry point, with
 
 CPU: the numpy restatement (bayer_testlib) against live cv2.cvtColor with IPP on and off (skipped without OpenCV) and
 against the committed fixture, composed with rectify_testlib's cv2.remap (never skipped); the argument rules that need
-no engine; the constants; the Bayer instantiations' register / local-memory figures.
+no engine; the constants.
 GPU: Cone mosaiced with every pattern against the CPU oracle on the restated demosaic; synthetic batches (odd sizes,
 crops at even and odd offsets, row pitch > W, image stride > footprint, several waves with a partial last one, pipelined
 and not) against adc_match_outputs_batch_device on the restated images, every output; the single-pair host entries;
 raw frames through both map types, larger and smaller than the engine, 1 x 1 and 2 x N; launch counts.
 """
 import ctypes
-import re
 
 import numpy as np
 import pytest
@@ -140,18 +139,6 @@ def test_bayer_constants():
     assert (d.format, d.row_pitch, d.plane_pitch) == (A.IMG_BAYER_GRBG, 40, 0)
     with pytest.raises(ValueError):
         A.engine._image_view_desc(np.zeros((8, 27, 3), np.uint8), A.IMG_BAYER_RGGB, 8, 27)
-
-
-def test_bayer_kernels_use_no_local_memory():
-    """ptxas -v on k_bayer.cu: the four plain and four rectified Bayer instantiations have no stack frame and no
-    spills."""
-    assert "k_bayer.cu" in (ROOT / "adcensus_b200" / "csrc" / "Makefile").read_text()
-    report = E.ptxas_report(ROOT / "adcensus_b200" / "csrc" / "k_bayer.cu")
-    assert len(report) == 8 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
-                                    for f in report.values()), report
-    for k in ("k_image_ingest", "k_rectify_ingest"):
-        codes = [re.search(rf"{k}ILi(\d+)E", name) for name, f in report.items() if f["regs"] is not None]
-        assert sorted(int(c.group(1)) for c in codes if c) == [16, 17, 18, 19], (k, sorted(report))
 
 
 # ---- GPU ------------------------------------------------------------------------------------------

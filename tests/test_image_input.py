@@ -3,7 +3,7 @@ read in place and matched exactly as the same pixels packed as BGR.
 
 CPU: the argument rules (on a NULL engine, before any device work), the descriptor's layout and the constants, the numpy
 packing helper against hand-built images, the gray golden cases (recorded from the unmodified reference) against the C
-restatement, k_image's register / local-memory figures.
+restatement.
 GPU: every colour format on Cone through both entry points (the reference's map, the packed-BGR call's matching cost);
 the gray golden cases; side-by-side, stacked, cropped and gray batches through the batched entry with several waves per
 lane; image strides past 2^31 bytes; the unchanged default path; the size-dependent argument rules.
@@ -152,13 +152,6 @@ def test_gray_golden_restatement():
                     assert m.sum() >= 4 * w and (a[m] == 127).all(), name
         orc.close()
     assert golden["synth_gray_odd"]["width"] % 2 == 1
-
-
-def test_image_kernel_uses_no_local_memory():
-    """ptxas -v on k_image.cu: no stack frame and no spills in any of the six instantiations."""
-    report = E.ptxas_report(T.REPO / "adcensus_b200" / "csrc" / "k_image.cu")
-    assert len(report) == 6 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
-                                    for f in report.values()), report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------

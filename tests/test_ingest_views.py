@@ -1,13 +1,20 @@
 """The views as the engine matches them (adc_ingest_views, adc_ingest_views_batch_device): the packed BGR views stage 1
 reads, for every format family, plain and through the rectification, handed to the caller; and the camera path from raw
-frames to a coloured point cloud.
+frames to a coloured point cloud; and the ingestion kernel itself.
 
+CPU: ptxas -v on every file that instantiates the ingestion kernel: each family file holds k_view_ingest for its own
+codes x the four source geometries, every ADC_IMG_* code once per geometry across them, none with a stack frame, spills
+or local memory; k_rectify.cu only its two map conversions.
 GPU: views of BGRA side-by-side frames, planar RGB, NV12, YUYV, BayerRG8, Mono12 and BayerRG12p, plain and rectified,
 with row pitches and image strides above tight and odd offsets, against the numpy restatements of the formats and of
 cv::remap; the same views fed back as packed BGR match to the same final maps as the raw-format call; the host entry;
-the rectified call without a rectification; launch counts; raw BayerRG12p frames through ingest_views, the rectified
-match and a point cloud coloured by the left views, against the host chain restated in numpy.
+the rectified call without a rectification; launch counts; batches of more pairs than one launch takes, plain and
+resized, against the restatements; raw BayerRG12p frames through ingest_views, the rectified match and a point cloud
+coloured by the left views, against the host chain restated in numpy.
 """
+import re
+from concurrent.futures import ThreadPoolExecutor
+
 import numpy as np
 import pytest
 
@@ -15,11 +22,54 @@ import adc_testlib as T
 import bayer_testlib as B
 import cloud_testlib as C
 import engine_testlib as E
+import images_testlib as IT
 import rawdepth_testlib as RD
 import rectify_testlib as R
+import resize_testlib as RS
 import yuv_testlib as Y
+import yuv_video_testlib as V
 
 FORMATS = ["bgra", "rgb_planar", "nv12", "yuyv", "bayer_rggb", "mono12", "bayer_rg12p"]
+CSRC = T.REPO / "adcensus_b200" / "csrc"
+GEOMETRIES = 4   # k_view_ingest's G: plain, remap, area, linear-exact
+
+# The file that instantiates k_view_ingest for each code: the family files of img_format.h.
+FAMILY_FILES = {
+    "k_image.cu": sorted(IT.CODE.values()),
+    "k_bayer.cu": sorted(B.CODE.values()),
+    "k_yuv.cu": sorted(Y.CODE.values()),
+    "k_yuv_encodings.cu": sorted(c | e for c in Y.CODE.values() for e in V.ENC.values() if e),
+    "k_yuv_video.cu": sorted(c | e for c in V.CODE.values() for e in V.ENC.values()),
+    "k_rawdepth.cu": sorted(RD.CODE.values()),
+}
+
+
+def test_ingestion_kernels_use_no_local_memory():
+    """ptxas -v on each file that instantiates k_view_ingest<F, G> and on k_rectify.cu: no function has a stack frame,
+    spills or local memory; each family file holds exactly its own codes x the four geometries, so that every code of
+    ADC_IMG_CODES is instantiated once per geometry (268 kernels); k_rectify.cu holds its two map conversions only."""
+    mk = (CSRC / "Makefile").read_text()
+    files = [*FAMILY_FILES, "k_rectify.cu"]
+    assert all(f in mk for f in files)
+    with ThreadPoolExecutor(len(files)) as ex:
+        reports = dict(zip(files, ex.map(lambda f: E.ptxas_report(CSRC / f), files)))
+    for f, report in reports.items():
+        assert all((k["stack"], k["spill_stores"], k["spill_loads"], k["lmem"]) == (0, 0, 0, 0)
+                   for k in report.values()), (f, report)
+    conv = reports.pop("k_rectify.cu")
+    assert sorted(n for n, k in conv.items() if k["regs"] is not None) == sorted(conv) and len(conv) == 2
+    assert all("k_remap_convert_" in n for n in conv), sorted(conv)
+    every = []
+    for f, codes in FAMILY_FILES.items():
+        kernels = [n for n, k in reports[f].items() if k["regs"] is not None]
+        got = [re.fullmatch(r"_Z\d+k_view_ingestILi(\d+)ELi(\d+)E.*", n) for n in kernels]
+        assert all(got), (f, kernels)
+        got = sorted((int(m.group(1)), int(m.group(2))) for m in got)
+        assert got == sorted((c, g) for c in codes for g in range(GEOMETRIES)), f
+        every += got
+    want = sorted((RS.CODE[f] | e, g) for f in RS.CODE for e in ([0] + [e for e in V.ENC.values() if e]
+                                                                  if f in V.ALL else [0]) for g in range(GEOMETRIES))
+    assert sorted(every) == want and len(every) == 268
 
 
 def _frame(rng, fmt, W, H):
@@ -165,6 +215,44 @@ def test_errors_and_launch_counts():
     c0 = eng.launch_count
     eng.ingest_views(np.zeros((H, W, 3), np.uint8), np.zeros((H, W, 3), np.uint8), "bgr")
     assert eng.launch_count == c0 + 1
+    eng.close()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("geometry", ["plain", "area", "linear_exact"])
+@pytest.mark.parametrize("fmt", ["bgr", "bayer_rggb"])
+def test_more_pairs_than_one_launch(fmt, geometry):
+    """65535 + 9 pairs of 8 x 4 views through adc_ingest_views_batch_device, plain and resized (2 x 2 AREA, 13 x 7
+    LINEAR_EXACT): two launches, and every pair equals the restatement of its frames (the format's conversion, then the
+    resize).  Pair i takes frames i mod 509 and (i + 254) mod 509 of 509 distinct random frames, so a pair read from or
+    written to another pair's place fewer than 509 pairs away, in either launch, shows."""
+    import adcensus_b200 as A
+    torch, dev = E.cuda()
+    W, H, n, P = 8, 4, 65535 + 9, 509
+    sw, sh = {"plain": (W, H), "area": (2 * W, 2 * H), "linear_exact": (13, 7)}[geometry]
+    rng = np.random.default_rng(len(fmt) + len(geometry))
+    eng = E.engine(W, H, T.default_option(max_disparity=4), wave_pairs=2, lanes=1)
+    if geometry != "plain":
+        eng.set_resize((sw, sh), geometry)
+    frames = [RS.random_frame(rng, fmt, sw, sh) for _ in range(P)]
+    want = [RS.decode(f, fmt, sw, sh) for f in frames]
+    if geometry != "plain":
+        want = [RS.resize(b, W, H, RS.AREA if geometry == "area" else RS.LINEAR_EXACT) for b in want]
+    want = np.stack(want)
+    raw = np.stack([np.ascontiguousarray(f).reshape(-1) for f in frames])   # tight frames, one per row
+    li = np.arange(n) % P
+    ri = (li + P // 2) % P
+    left, right = (torch.from_numpy(raw[k]).to(dev) for k in (li, ri))
+    views, intact = E.guarded(6 * n * W * H, torch.uint8, 3, 5, 0xee)
+    c0 = eng.launch_count
+    eng.ingest_views_batch_device(n, left.data_ptr(), right.data_ptr(), views.data_ptr(),
+                                  A.image_desc(fmt, 0, 0, raw.shape[1]), geometry != "plain",
+                                  torch.cuda.current_stream().cuda_stream)
+    assert eng.launch_count == c0 + 2
+    torch.cuda.synchronize()
+    assert intact(), "a guard of the views was overwritten"
+    got = views.cpu().numpy().reshape(n, 2, H, W, 3)
+    assert np.array_equal(got[:, 0], want[li]) and np.array_equal(got[:, 1], want[ri])
     eng.close()
 
 

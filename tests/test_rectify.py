@@ -4,7 +4,7 @@ packed-BGR entry point.
 
 CPU: the numpy restatement (rectify_testlib) against cv2.remap on random, realistic and degenerate cases for both map
 types (skipped without OpenCV) and against the committed fixture (never skipped); the argument rules that need no
-engine; the structs' layout and the constants; k_rectify's register / local-memory figures.
+engine; the structs' layout and the constants.
 GPU: Cone through initUndistortRectifyMap maps of a made-up rig (both map types, sources smaller than, equal to and
 larger than W x H, every format tight / pitched / cropped) against the restated images; identity maps against
 adc_match_images; batches with several waves per lane, pipelined and not, with guard bytes; image strides past 2^31;
@@ -181,15 +181,6 @@ def test_map_builders_python():
         _remap((mx[:, :6], my[:, :6]), 5, 7)
     with pytest.raises(ValueError):
         _remap((mx[:, ::2], my[:, ::2]), 5, 4)
-
-
-def test_rectify_kernel_uses_no_local_memory():
-    """ptxas -v on k_rectify.cu: no stack frame and no spills in the six ingestion instantiations and the two map
-    conversions."""
-    report = E.ptxas_report(T.REPO / "adcensus_b200" / "csrc" / "k_rectify.cu")
-    assert len(report) == 8 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
-                                    for f in report.values()), report
-    assert sum(f["regs"] is not None and "k_rectify_ingest" in name for name, f in report.items()) == 6, report
 
 
 # ---- GPU ------------------------------------------------------------------------------------------

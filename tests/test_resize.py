@@ -3,8 +3,7 @@ size than the engine's, converted with their format's rule and resized as cv::re
 
 CPU: the numpy restatement (resize_testlib) against live cv2.resize (every AREA factor 1..10 x 1..10 and the largest
 accepted, every accepted 1-D AREA factor 1..4096 on half-way samples, every 1-D LINEAR_EXACT size pair 1..512, random 2-D sizes, the BASELINE shapes, 1 / 3 / 4 channels) and
-against the committed fixture; the argument rules that need no engine; the header's and the binding's constants; the
-new kernels' register / local-memory figures.
+against the committed fixture; the argument rules that need no engine; the header's and the binding's constants.
 GPU: Cone through the full pipeline from larger and smaller frames against the packed-BGR call on the restated
 images; adc_ingest_views_batch_device for every ADC_IMG_* code and encoding under both rules (tight, pitched,
 side-by-side, odd sizes, one-pixel-wide and -high sources, other bytes of the buffer changed); batched device and host
@@ -12,7 +11,6 @@ entries, pipelined and not, the host staging fallback, a poisoned engine, geomet
 the rules that need an engine; profile id 14.
 """
 import ctypes
-import re
 
 import numpy as np
 import pytest
@@ -23,7 +21,6 @@ import rectify_testlib as R
 import resize_testlib as RS
 
 ROOT = T.REPO
-CSRC = ROOT / "adcensus_b200" / "csrc"
 MAPS = ["wta_left", "wta_right", "outliers", "min_cost", "peak_ratio"]
 VOLS = ["cost", "aggr", "opt"]
 GOLDEN = T.GOLDEN_DIR / "golden_resize_cases.npz"
@@ -174,18 +171,6 @@ def test_resize_constants():
     assert ctypes.sizeof(A.Rectification) == 80 and A.Rectification.map_type.offset == 8
     r = A.Rectification(900, 750, A.RESIZE_AREA, 0)
     assert (r.view[0].map1, r.view[1].map2, r.view[0].map1_pitch) == (None, None, 0)
-
-
-def test_resize_kernels_use_no_local_memory():
-    """ptxas -v on k_resize.cu: one kernel per format code x rule, none with a stack frame, spills or local memory."""
-    assert "k_resize.cu" in (CSRC / "Makefile").read_text()
-    report = E.ptxas_report(CSRC / "k_resize.cu")
-    kernels = {n: f for n, f in report.items() if f["regs"] is not None}
-    assert all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0) for f in report.values())
-    got = sorted((int(m.group(2)), int(m.group(1))) for m in
-                 (re.search(r"k_resize_ingestILi(\d+)ELi(\d+)E", n) for n in kernels) if m)
-    want = sorted((t, RS.CODE[f] | e) for f, e in CODES for t in (RS.AREA, RS.LINEAR_EXACT))
-    assert len(kernels) == len(got) == 2 * len(CODES) == 134 and got == want
 
 
 # ---- GPU ------------------------------------------------------------------------------------------

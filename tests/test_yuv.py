@@ -4,7 +4,7 @@ with or without rectification.
 
 CPU: the numpy restatement (yuv_testlib) against live cv2.cvtColor with the optimised paths on and off (skipped without
 OpenCV) and against the committed fixture, composed with rectify_testlib's cv2.remap (never skipped); the argument
-rules that need no engine; the constants and the view parser; the YUV instantiations' register / local-memory figures.
+rules that need no engine; the constants and the view parser.
 GPU: Cone in every format through a 450 x 376 surface against the CPU oracle on the restated decode; synthetic batches
 (odd sizes, row pitch, plane pitch and image stride above their minimums, several waves with a partial last one,
 pipelined and not), even-offset crops and side-by-side frames against adc_match_outputs_batch_device on the restated
@@ -12,7 +12,6 @@ images, every output; the single-pair host entries; raw frames through both map 
 engine, odd, 1 x 1 and 1 x N; the size-dependent rule violations; launch counts.
 """
 import ctypes
-import re
 
 import numpy as np
 import pytest
@@ -187,18 +186,6 @@ def test_yuv_constants():
             P(frame[1:8, 4:29], fmt, 7, 25)
         with pytest.raises(ValueError):
             P(np.zeros((7, 26), np.uint8), fmt, 7, 26)
-
-
-def test_yuv_kernels_use_no_local_memory():
-    """ptxas -v on k_yuv.cu: the five plain and five rectified YUV instantiations report their registers and have no
-    stack frame and no spills."""
-    assert "k_yuv.cu" in (ROOT / "adcensus_b200" / "csrc" / "Makefile").read_text()
-    report = E.ptxas_report(ROOT / "adcensus_b200" / "csrc" / "k_yuv.cu")
-    assert len(report) == 10 and all((f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0)
-                                     for f in report.values()), report
-    for k in ("k_image_ingest", "k_rectify_ingest"):
-        codes = [re.search(rf"{k}ILi(\d+)E", name) for name, f in report.items() if f["regs"] is not None]
-        assert sorted(int(c.group(1)) for c in codes if c) == [32, 33, 34, 35, 36], (k, sorted(report))
 
 
 # ---- GPU ------------------------------------------------------------------------------------------

@@ -5,7 +5,7 @@ cvtColor where OpenCV has the rule) followed by the packed-BGR entry point, with
 CPU: the restatement against the committed fixture (composed with rectify_testlib's remap) and against live cv2 (skipped
 without OpenCV); every encoding on all 2^24 (Y, U, V) triples (BT.601 limited against yuv_testlib, full range against
 cv2, BT.709 within +-1 of the floating-point matrix); the argument rules that need no engine; the header's, the
-kernels' and the binding's constants; the view parser; the new instantiations' register / local-memory figures.
+kernels' and the binding's constants; the view parser.
 GPU: every container x encoding through the image, rectified and ingest-views entries, host and device (batches with
 odd sizes, pitches and strides above their minimums, several waves, pipelined and not), side-by-side halves and
 even-offset crops, guard bytes after each view, a poisoned engine, the size rules and launch counts.
@@ -267,22 +267,6 @@ def test_view_parser():
             P(frame[:, :37], fmt, 9, 37)
     d = P(np.zeros((8, 50, 2), np.uint8)[1:8, 4:30], A.IMG_UYVY | A.IMG_YUV_FULL_RANGE, 7, 25)
     assert (d.format, d.row_pitch, d.plane_pitch) == (A.IMG_UYVY | A.IMG_YUV_FULL_RANGE, 100, 0)
-
-
-def test_new_kernels_use_no_local_memory():
-    """ptxas -v: k_yuv_video.cu holds I420, YV12 and P016 in all four encodings and k_yuv_encodings.cu the formats of
-    k_yuv.cu under the three flagged encodings, plain and rectified; none has a stack frame or spills."""
-    mk = (CSRC / "Makefile").read_text()
-    flagged = [e for e in V.ENC.values() if e]
-    for src, codes in (("k_yuv_video.cu", sorted(c | e for c in V.CODE.values() for e in V.ENC.values())),
-                       ("k_yuv_encodings.cu", sorted(c | e for c in Y.CODE.values() for e in flagged))):
-        assert src in mk
-        report = E.ptxas_report(CSRC / src)
-        assert len(report) == 2 * len(codes) and all(
-            (f["stack"], f["spill_stores"], f["spill_loads"], f["lmem"]) == (0, 0, 0, 0) for f in report.values()), report
-        for k in ("k_image_ingest", "k_rectify_ingest"):
-            got = [re.search(rf"{k}ILi(\d+)E", name) for name, f in report.items() if f["regs"] is not None]
-            assert sorted(int(c.group(1)) for c in got if c) == codes, (src, k)
 
 
 # ---- GPU ------------------------------------------------------------------------------------------
