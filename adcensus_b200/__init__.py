@@ -25,6 +25,8 @@ from .engine import (IMG_MONO10, IMG_BAYER_RG10, IMG_BAYER_GR10, IMG_BAYER_BG10,
 from .engine import (IMG_I420, IMG_YV12, IMG_P016, YUV_VIDEO_FORMATS, IMG_YUV_BT709, IMG_YUV_FULL_RANGE,  # noqa: F401
                      YUV_ENCODINGS)
 from .engine import RESIZE_AREA, RESIZE_LINEAR_EXACT, RESIZE_INTERPOLATIONS  # noqa: F401
+from .engine import (COLORMAPS, COLORMAP_NONE, PREVIEW_MINMAX, PREVIEW_FIXED, PREVIEW_FORMATS,  # noqa: F401
+                     PreviewParams, preview_params, preview_shape)
 from .build import build_library  # noqa: F401
 
 __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "TAP", "lib_path",
@@ -41,4 +43,6 @@ __all__ = ["ADCensusOption", "ADCensusStereo", "AdcError", "Engine", "STAGE", "T
            "IMG_I420", "IMG_YV12", "IMG_P016", "YUV_VIDEO_FORMATS", "IMG_YUV_BT709", "IMG_YUV_FULL_RANGE", "YUV_ENCODINGS",
            "image_desc", "REMAP_F32", "REMAP_FIXED", "Remap", "Rectification", "REPROJ_POINTS", "REPROJ_DEPTH",
            "REPROJ_DISP_S16", "REPROJ_KINDS", "ReprojectOut", "SPECKLE_S16", "SPECKLE_F32", "SPECKLE_TYPES",
-           "SpeckleParams", "CloudOut", "RESIZE_AREA", "RESIZE_LINEAR_EXACT", "RESIZE_INTERPOLATIONS"]
+           "SpeckleParams", "CloudOut", "RESIZE_AREA", "RESIZE_LINEAR_EXACT", "RESIZE_INTERPOLATIONS",
+           "COLORMAPS", "COLORMAP_NONE", "PREVIEW_MINMAX", "PREVIEW_FIXED", "PREVIEW_FORMATS", "PreviewParams",
+           "preview_params", "preview_shape"]

@@ -206,6 +206,22 @@ struct AdcSpeckle {
 // uint32 sizes.  Four launches.
 void adc_launch_speckles(const AdcDims& dm, long long n, bool f32, void* maps, void* work, const AdcSpeckle& p,
                          cudaStream_t st, unsigned long long* launches);
+// previews (k_preview.cu): n maps of dm.N pixels at maps -> n frames of dst_w x dst_h at dst (frame i at byte
+// i*image_stride, format ADC_IMG_BGR / BGRA / RGBA / GRAY / NV12 / NV21 / I420 / YV12, pitches resolved).  work
+// non-NULL = MINMAX: 2*n uint32 zeroed in stream order before the call, (alpha, beta) unused; NULL = FIXED with the
+// float (alpha, beta).  inv_x / inv_y = 1.0 / ((double)dst_w / W), 1.0 / ((double)dst_h / H).  Two launches (MINMAX)
+// or one.
+struct AdcPreviewArgs {
+    uint8_t* dst;
+    unsigned* work;
+    long long row_pitch, plane_pitch, image_stride;
+    double inv_x, inv_y;
+    float alpha, beta;
+    int format, colormap, dst_w, dst_h;
+    uint8_t invalid[3];
+};
+void adc_launch_preview(const AdcDims& dm, long long n, const float* maps, const AdcPreviewArgs& a, cudaStream_t st,
+                        unsigned long long* launches);
 void adc_launch_diffmaps(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 void adc_launch_arms(const AdcParams& P, const AdcWave& w, cudaStream_t st, unsigned long long* launches);
 // one 1-D pass of the cross aggregation: horizontal (dir=0) or vertical (dir=1) ordered sums,

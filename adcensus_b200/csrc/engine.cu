@@ -22,6 +22,7 @@
 #include <vector>
 
 #include "../../include/adcensus_b200.h"
+#include "../../include/adcensus_b200_preview.h"
 #include "adc_common.cuh"
 #include "ca_plan.h"
 #include "so_plan.h"
@@ -43,6 +44,9 @@ static_assert(sizeof(adc_speckle_params) == 32 && offsetof(adc_speckle_params, m
               offsetof(adc_speckle_params, reserved) == 24, "adc_speckle_params layout (include/adcensus_b200.h)");
 static_assert(sizeof(adc_reproject_out) == 16 && offsetof(adc_reproject_out, kind) == 8 &&
               offsetof(adc_reproject_out, reserved) == 12, "adc_reproject_out layout (include/adcensus_b200.h)");
+static_assert(sizeof(adc_preview_params) == 48 && offsetof(adc_preview_params, alpha) == 8 &&
+              offsetof(adc_preview_params, dst_width) == 24 && offsetof(adc_preview_params, invalid_bgr) == 32 &&
+              offsetof(adc_preview_params, reserved) == 40, "adc_preview_params layout (include/adcensus_b200_preview.h)");
 static_assert(sizeof(adc_cloud_out) == 48 && offsetof(adc_cloud_out, colors) == 8 && offsetof(adc_cloud_out, pixels) == 16 &&
               offsetof(adc_cloud_out, counts) == 24 && offsetof(adc_cloud_out, capacity) == 32 &&
               offsetof(adc_cloud_out, reserved) == 40, "adc_cloud_out layout (include/adcensus_b200.h)");
@@ -1160,6 +1164,93 @@ int cloud_enqueue(adc_engine* e, long long n, const float* disp, const double* Q
     return ADC_OK;
 }
 
+// The output formats of the previews.
+bool preview_format(int f) {
+    switch (f) {
+        case ADC_IMG_BGR: case ADC_IMG_BGRA: case ADC_IMG_RGBA: case ADC_IMG_GRAY:
+        case ADC_IMG_NV12: case ADC_IMG_NV21: case ADC_IMG_I420: case ADC_IMG_YV12: return true;
+        default: return false;
+    }
+}
+
+// The rules of the preview entries that need no engine (device: the alignment rules too).
+int check_preview_args(const char* fn, int n, const float* maps, const adc_preview_params* p, const void* dst,
+                       const adc_image_desc* desc, const void* work, bool device) {
+    if (!p) return fail(ADC_ERR_ARG, "%s: p is NULL", fn);
+    if (p->colormap < ADC_COLORMAP_NONE || p->colormap >= ADC_COLORMAP_COUNT)
+        return fail(ADC_ERR_ARG, "%s: p->colormap %d unknown (ADC_COLORMAP_NONE or 0..%d)", fn, p->colormap,
+                    ADC_COLORMAP_COUNT - 1);
+    if (p->range != ADC_PREVIEW_MINMAX && p->range != ADC_PREVIEW_FIXED)
+        return fail(ADC_ERR_ARG, "%s: p->range %d unknown", fn, p->range);
+    if (!std::isfinite(p->alpha)) return fail(ADC_ERR_ARG, "%s: p->alpha is not finite", fn);
+    if (!std::isfinite(p->beta)) return fail(ADC_ERR_ARG, "%s: p->beta is not finite", fn);
+    if (p->range == ADC_PREVIEW_MINMAX && (p->alpha != 0 || p->beta != 0))
+        return fail(ADC_ERR_ARG, "%s: p->alpha and p->beta must be 0 with ADC_PREVIEW_MINMAX", fn);
+    for (int i = 0; i < 5; i++)
+        if (p->reserved_[i]) return fail(ADC_ERR_ARG, "%s: p->reserved_ must be zero", fn);
+    if (p->reserved != 0) return fail(ADC_ERR_ARG, "%s: p->reserved must be zero", fn);
+    const int format = desc ? desc->format : ADC_IMG_BGR;
+    if (!preview_format(format))
+        return fail(ADC_ERR_ARG, "%s: dst->format %d is not a preview format (BGR, BGRA, RGBA, GRAY, NV12, NV21, I420, "
+                    "YV12, without flags)", fn, format);
+    const bool yuv = img_yuv420(format);
+    if (p->dst_width < 0 || p->dst_width > 32767)
+        return fail(ADC_ERR_ARG, "%s: p->dst_width %d outside 0..32767", fn, p->dst_width);
+    if (p->dst_height < 0 || p->dst_height > 32767)
+        return fail(ADC_ERR_ARG, "%s: p->dst_height %d outside 0..32767", fn, p->dst_height);
+    if (yuv && p->dst_width % 2) return fail(ADC_ERR_ARG, "%s: p->dst_width %d must be even for a 4:2:0 format", fn, p->dst_width);
+    if (yuv && p->dst_height % 2) return fail(ADC_ERR_ARG, "%s: p->dst_height %d must be even for a 4:2:0 format", fn, p->dst_height);
+    int rc = check_image_desc(fn, desc);
+    if (rc) return rc;
+    if (!maps) return fail(ADC_ERR_ARG, "%s: maps is NULL", fn);
+    if (!dst) return fail(ADC_ERR_ARG, "%s: dst is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (device && (uintptr_t)maps % 4) return fail(ADC_ERR_ARG, "%s: maps are not 4-byte aligned", fn);
+    if (device && (uintptr_t)work % 4) return fail(ADC_ERR_ARG, "%s: work is not 4-byte aligned", fn);
+    return ADC_OK;
+}
+
+// The rules of the preview entries after the engine check: the frame size (0 = the engine's; even for 4:2:0) and the
+// descriptor's size-dependent rules for n frames.  `a` receives everything but the pointers.
+int resolve_preview(const adc_engine* e, const char* fn, int n, const adc_preview_params* p, const adc_image_desc* desc,
+                    AdcPreviewArgs* a) {
+    const int w = p->dst_width ? p->dst_width : e->W, h = p->dst_height ? p->dst_height : e->H;
+    const int format = desc ? desc->format : ADC_IMG_BGR;
+    if (img_yuv420(format) && (w % 2 || h % 2))
+        return fail(ADC_ERR_ARG, "%s: the frame size %d x %d (0 = the engine's) must be even for a 4:2:0 format", fn, w, h);
+    adc_image_desc d = desc ? *desc : adc_image_desc{};
+    AdcImageGeom g;
+    int rc = resolve_image(fn, w, h, &d, std::max(n, 1), &g);
+    if (rc) return rc;
+    *a = AdcPreviewArgs{};
+    a->row_pitch = g.row_pitch;
+    a->plane_pitch = g.plane_pitch;
+    a->image_stride = g.image_stride;
+    a->inv_x = 1.0 / ((double)w / e->W);
+    a->inv_y = 1.0 / ((double)h / e->H);
+    a->alpha = (float)p->alpha;
+    a->beta = (float)p->beta;
+    a->format = format;
+    a->colormap = p->colormap;
+    a->dst_w = w;
+    a->dst_h = h;
+    memcpy(a->invalid, p->invalid_bgr, 3);
+    return ADC_OK;
+}
+
+size_t preview_work_bytes(long long n) { return 8 * (size_t)n; }
+
+// Renders n maps at device address maps into the frames at dst on st; work (MINMAX) is zeroed first.
+int preview_enqueue(adc_engine* e, long long n, const float* maps, AdcPreviewArgs a, bool minmax, void* dst, void* work,
+                    cudaStream_t st) {
+    a.dst = static_cast<uint8_t*>(dst);
+    a.work = minmax ? static_cast<unsigned*>(work) : nullptr;
+    if (minmax) CK(cudaMemsetAsync(work, 0, preview_work_bytes(n), st));
+    adc_launch_preview(e->P.dm, n, maps, a, st, &e->launches);
+    CK(cudaGetLastError());
+    return ADC_OK;
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -1793,6 +1884,74 @@ int adc_point_cloud(adc_engine* e, const float* disp, const double Q[16], const 
     CK(cudaMemcpy(out->points, o.points, 12 * kept, cudaMemcpyDeviceToHost));
     if (out->colors) CK(cudaMemcpy(out->colors, o.colors, 3 * kept, cudaMemcpyDeviceToHost));
     if (out->pixels) CK(cudaMemcpy(out->pixels, o.pixels, 4 * kept, cudaMemcpyDeviceToHost));
+    return ADC_OK;
+}
+
+int adc_preview_workspace_bytes(const adc_engine* e, int32_t n, size_t* out) {
+    const char* fn = "adc_preview_workspace_bytes";
+    if (!out) return fail(ADC_ERR_ARG, "%s: out is NULL", fn);
+    if (n < 0) return fail(ADC_ERR_ARG, "%s: n %d is negative", fn, n);
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    *out = preview_work_bytes(n);
+    return ADC_OK;
+}
+
+int adc_preview_batch_device(adc_engine* e, int32_t n, const float* d_maps, const adc_preview_params* p, void* d_dst,
+                             const adc_image_desc* dst, void* d_work, size_t work_bytes, void* stream) {
+    const char* fn = "adc_preview_batch_device";
+    int rc = check_preview_args(fn, n, d_maps, p, d_dst, dst, d_work, true);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcPreviewArgs a;
+    if ((rc = resolve_preview(e, fn, n, p, dst, &a))) return rc;
+    const bool minmax = p->range == ADC_PREVIEW_MINMAX;
+    if (minmax && work_bytes < preview_work_bytes(n))
+        return fail(ADC_ERR_ARG, "%s: work_bytes %zu below the %zu bytes of %d maps", fn, work_bytes, preview_work_bytes(n), n);
+    if (n == 0) return ADC_OK;
+    if (minmax && !d_work) return fail(ADC_ERR_ARG, "%s: work is NULL", fn);
+    CK(cudaSetDevice(e->cfg.device));
+    return preview_enqueue(e, n, d_maps, a, minmax, d_dst, d_work, (cudaStream_t)stream);
+}
+
+int adc_preview(adc_engine* e, const float* map, const adc_preview_params* p, void* dst, const adc_image_desc* desc) {
+    const char* fn = "adc_preview";
+    int rc = check_preview_args(fn, 1, map, p, dst, desc, nullptr, false);
+    if (rc) return rc;
+    if (!e) return fail(ADC_ERR_ARG, "%s: engine is NULL", fn);
+    AdcPreviewArgs a;
+    if ((rc = resolve_preview(e, fn, 1, p, desc, &a))) return rc;
+    if ((rc = idle_lane0(e))) return rc;
+    Lane& ln = e->lanes[0];
+    const size_t N = (size_t)e->P.dm.N;
+    // the frame is rendered tightly into the staging, then each plane's rows are copied to the caller's pitches
+    const AdcImageGeom tight = adc_image_tight(a.format, a.dst_w, a.dst_h);
+    AdcPreviewArgs t = a;
+    t.row_pitch = tight.row_pitch;
+    t.plane_pitch = tight.plane_pitch;
+    t.image_stride = tight.image_stride;
+    float* d_map = nullptr;
+    uint8_t* d_frame = nullptr;
+    void* work = nullptr;
+    rc = grow_stage(e, fn, "the map and its preview", [&](Carver& c) {
+        work = c.take<unsigned>(2);
+        d_map = c.take<float>(N);
+        d_frame = c.take<uint8_t>((size_t)tight.image_stride);
+    });
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(d_map, map, N * sizeof(float), cudaMemcpyHostToDevice, ln.st));
+    if ((rc = preview_enqueue(e, 1, d_map, t, p->range == ADC_PREVIEW_MINMAX, d_frame, work, ln.st))) return rc;
+    const int format = a.format;
+    const long long row_bytes = img_row_pitch(format, a.dst_w);
+    for (int c = 0; c < img_planes(format); c++) {
+        uint8_t* to = static_cast<uint8_t*>(dst) + img_plane_offset(format, c, a.dst_h, a.row_pitch, a.plane_pitch);
+        const uint8_t* from = d_frame + img_plane_offset(format, c, a.dst_h, t.row_pitch, t.plane_pitch);
+        CK(cudaMemcpy2DAsync(to, (size_t)img_plane_row_pitch(format, c, a.row_pitch), from,
+                             (size_t)img_plane_row_pitch(format, c, t.row_pitch),
+                             (size_t)img_plane_row_pitch(format, c, row_bytes), (size_t)img_plane_rows(format, c, a.dst_h),
+                             cudaMemcpyDeviceToHost, ln.st));
+    }
+    CK(cudaStreamSynchronize(ln.st));
+    CK(cudaGetLastError());
     return ADC_OK;
 }
 

@@ -307,6 +307,46 @@ class SpeckleParams(ctypes.Structure):
 assert ctypes.sizeof(SpeckleParams) == 32
 
 
+# previews (adc_preview*): colormap names -> cv2.COLORMAP_* values ("none" = gray), the range rules, the output formats
+COLORMAP_NONE = -1
+COLORMAPS = {"none": COLORMAP_NONE, "autumn": 0, "bone": 1, "jet": 2, "winter": 3, "rainbow": 4, "ocean": 5, "summer": 6,
+             "spring": 7, "cool": 8, "hsv": 9, "pink": 10, "hot": 11, "parula": 12, "magma": 13, "inferno": 14,
+             "plasma": 15, "viridis": 16, "cividis": 17, "twilight": 18, "twilight_shifted": 19, "turbo": 20,
+             "deepgreen": 21}
+PREVIEW_MINMAX, PREVIEW_FIXED = 0, 1
+PREVIEW_FORMATS = {"bgr": IMG_BGR, "bgra": IMG_BGRA, "rgba": IMG_RGBA, "gray": IMG_GRAY, "nv12": IMG_NV12,
+                   "nv21": IMG_NV21, "i420": IMG_I420, "yv12": IMG_YV12}
+
+
+class PreviewParams(ctypes.Structure):
+    """adc_preview_params: colormap (COLORMAPS value), range (PREVIEW_*), alpha / beta (FIXED), frame size (0 = the
+    engine's), the colour of invalid pixels (B, G, R) and reserved zeros."""
+    _fields_ = [("colormap", ctypes.c_int32), ("range", ctypes.c_int32), ("alpha", ctypes.c_double),
+                ("beta", ctypes.c_double), ("dst_width", ctypes.c_int32), ("dst_height", ctypes.c_int32),
+                ("invalid_bgr", ctypes.c_uint8 * 3), ("reserved_", ctypes.c_uint8 * 5), ("reserved", ctypes.c_int64)]
+
+
+assert ctypes.sizeof(PreviewParams) == 48
+
+
+def preview_params(colormap="turbo", value_range=None, size=None, invalid=(0, 0, 0)) -> PreviewParams:
+    """A PreviewParams from a colormap name or value, value_range None (MINMAX over the valid pixels) or (alpha, beta)
+    (FIXED: convertTo's scale and shift), size None (the engine's) or (width, height), and the invalid colour (B, G, R)."""
+    cm = _code(COLORMAPS, colormap, "colormap") if isinstance(colormap, str) else int(colormap)
+    w, h = (0, 0) if size is None else (int(size[0]), int(size[1]))
+    rng, a, b = (PREVIEW_MINMAX, 0.0, 0.0) if value_range is None else \
+        (PREVIEW_FIXED, float(value_range[0]), float(value_range[1]))
+    return PreviewParams(cm, rng, a, b, w, h, (ctypes.c_uint8 * 3)(*[int(v) for v in invalid]))
+
+
+def preview_shape(format, width: int, height: int):
+    """The numpy shape of one tight preview frame: [h][w][3] BGR, [h][w][4] BGRA / RGBA, [h][w] gray, [h * 3 / 2][w]
+    for the 4:2:0 formats (OpenCV's I420 / YV12 Mat, NV12 / NV21 alike)."""
+    f = _code(PREVIEW_FORMATS, format, "preview format") if isinstance(format, str) else int(format)
+    return {IMG_BGR: (height, width, 3), IMG_BGRA: (height, width, 4), IMG_RGBA: (height, width, 4),
+            IMG_GRAY: (height, width)}.get(f, (height * 3 // 2, width))
+
+
 class CloudOut(ctypes.Structure):
     """adc_cloud_out: the destinations of a point cloud (points, colors or None, pixels or None, counts), the points
     per map they hold (capacity) and a reserved zero."""
@@ -399,6 +439,10 @@ def load_library() -> ctypes.CDLL:
     L.adc_point_cloud_batch_device.argtypes = [vp, i32, f32p, ctypes.POINTER(ctypes.c_double), u8p, ctypes.c_int64,
                                                ctypes.c_float, ctypes.c_float, ctypes.POINTER(CloudOut), vp,
                                                ctypes.c_size_t, vp]
+    L.adc_preview_workspace_bytes.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_size_t)]
+    L.adc_preview.argtypes = [vp, f32p, ctypes.POINTER(PreviewParams), vp, ctypes.POINTER(ImageDesc)]
+    L.adc_preview_batch_device.argtypes = [vp, i32, f32p, ctypes.POINTER(PreviewParams), vp, ctypes.POINTER(ImageDesc),
+                                           vp, ctypes.c_size_t, vp]
     L.adc_debug_get.argtypes = [vp, i32, vp, ctypes.c_size_t]
     L.adc_debug_get.restype = ctypes.c_size_t
     L.adc_debug_counters.argtypes = [vp, ctypes.POINTER(ctypes.c_int32 * 16)]
@@ -831,6 +875,42 @@ class Engine:
         _check(self._L.adc_point_cloud_batch_device(self._h, n, d_disp, _q_matrix(Q), d_bgr or None, int(bgr_stride),
                                                     float(z_range[0]), float(z_range[1]), ctypes.byref(out), d_work,
                                                     work_bytes, stream))
+
+    # ---- previews (adc_preview*) ---------------------------------------------------------------------------
+    def preview(self, map, colormap="turbo", value_range=None, size=None, format="bgr", invalid=(0, 0, 0)) -> np.ndarray:
+        """One float32 [H][W] map (final map, side map, depth; non-finite = invalid) rendered as a tight 8-bit frame of
+        preview_shape(format, *size): cv2.normalize(NORM_MINMAX over the valid pixels; value_range (alpha, beta) =
+        convertTo(CV_8U, alpha, beta) instead) -> cv2.applyColorMap(colormap; "none" = gray) -> invalid pixels set to
+        `invalid` (B, G, R) -> cv2.resize(size = (width, height), INTER_NEAREST; None = the engine's size) ->
+        cv2.cvtColor(COLOR_BGR2<format>), bit for bit."""
+        H, W = self.height, self.width
+        m = np.ascontiguousarray(map, np.float32)
+        if m.shape != (H, W):
+            raise ValueError(f"expected a map of shape {(H, W)}, got {m.shape}")
+        p = preview_params(colormap, value_range, size, invalid)
+        f = _code(PREVIEW_FORMATS, format, "preview format") if isinstance(format, str) else int(format)
+        out = np.empty(preview_shape(f, p.dst_width or W, p.dst_height or H), np.uint8)
+        _check(self._L.adc_preview(self._h, m.ctypes.data, ctypes.byref(p), out.ctypes.data,
+                                   ctypes.byref(ImageDesc(f, 0, 0, 0, 0))))
+        return out
+
+    def preview_workspace_bytes(self, n: int) -> int:
+        """Bytes of device workspace that preview_batch_device needs for n maps with MINMAX (8 per map)."""
+        out = ctypes.c_size_t()
+        _check(self._L.adc_preview_workspace_bytes(self._h, n, ctypes.byref(out)))
+        return int(out.value)
+
+    def preview_batch_device(self, n: int, d_maps: int, d_dst: int, image=None, colormap="turbo", value_range=None,
+                             size=None, invalid=(0, 0, 0), d_work: int = 0, work_bytes: int = 0, stream: int = 0):
+        """Device pointers (ints): n float32 maps of H*W at d_maps rendered as preview() renders them into n frames at
+        d_dst described by `image` (an ImageDesc of a preview format, e.g. image_desc("nv12", row_pitch=...), None =
+        tight BGR); MINMAX needs work_bytes >= preview_workspace_bytes(n) at d_work.  A memset and two launches
+        (MINMAX) or one launch (FIXED) enqueued on `stream` without synchronising; in pipelined mode the maps must be
+        joined on `stream` first."""
+        p = preview_params(colormap, value_range, size, invalid)
+        _check(self._L.adc_preview_batch_device(self._h, n, d_maps, ctypes.byref(p), d_dst,
+                                                None if image is None else ctypes.byref(image), d_work or None,
+                                                work_bytes, stream))
 
     def match_batch(self, lefts, rights) -> np.ndarray:
         """lefts/rights: arrays [n][H][W][3] (or sequences of images).  Host memory in, host memory out."""
